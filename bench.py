@@ -1,17 +1,21 @@
 #!/usr/bin/env python
-"""bench.py -- LLaMA-7B Q4_0 tokens/sec on B200 (BASELINE.json metric): decode@1 (default line) and prefill@512 (--metric prefill).
+"""bench.py -- LLaMA-7B Q4_0 tokens/sec on H100 (BASELINE.json metric): decode@1 (default line) and prefill@512 (--metric prefill).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--metric decode|prefill]    our arm (N>1: torchrun, one replica per GPU)
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--metric decode|prefill] [--dump-outputs DIR]    our arm (N>1: torchrun, one replica per GPU)
   python bench.py --impl reference [--metric decode|prefill] [...]                  the reference's own ggml CPU path, FULL 32-layer model
 
 A "step" is one pass of the hot path over one batch: one decode token (Llama::evaluate with 1 token) at n_past = 512 on a
 synthetic, device-generated LLaMA-7B Q4_0 model (BASELINE.json configs[1]).  Every headline number is measured on the CONFORMANT
 path: kernels that reproduce the reference's AVX2 operation order, logits bit-identical to the reference CPU path (DESIGN.md §2).
-The order-free kernels (B200_SESSION_FAST) are reported beside it under "fast_mode" and labelled non-conformant.  `value` is measured with inputs resident in
+`value` is measured with inputs resident in
 HBM (token id and logits stay on the device); `e2e` goes through the host-buffer call (b200_session_evaluate: token H2D,
 logits D2H, sync) every step.  Timing: CUDA events on the backend's stream, W >= 3 warm-up steps, the 3.7 GB of weights
-are far larger than the 126 MB L2 so every step streams them from HBM.  Multi-GPU (the path does not need to shard: 7B fits
+are far larger than the 50 MB L2 so every step streams them from HBM.  Multi-GPU (the path does not need to shard: 7B fits
 one GPU) = N independent replicas, no data-path collective, "scaling": "weak".
+
+--dump-outputs DIR writes, after the timed steps, what the timed path computed in its last step: the last-row logits a caller of
+Llama::evaluate receives, DIR/logits.npy (float32 [1, n_vocab]).  Weights (seeded device synthesis) and prompt (seeded generator)
+are the same on every run with the same arguments, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -38,8 +42,28 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         j = json.load(open(p))
-        return dict(hbm_gbs=j["hbm_gbs"], bf16_tflops=j["bf16_tflops"], bf16_sustained=j.get("bf16_tflops_sustained", j["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source="fallback")
+        return dict(hbm_gbs=j["hbm_gbs"], bf16_tflops=j["bf16_tflops"], bf16_sustained=j.get("bf16_tflops_sustained", j["bf16_tflops"]),
+                    hbm_source="MEASURED_PEAKS.json (burst copy)", bf16_source="MEASURED_PEAKS.json (cuBLAS bf16, sustained)")
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- the denominators, not reached rates
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0,
+                hbm_source="H100 SXM data sheet (HBM3, 700 W card)", bf16_source="H100 SXM data sheet (dense BF16, 700 W card)")
+
+
+def device_logits_last_row(L, sess, n, n_vocab, device):
+    """The last row of the session's device-resident logits after an evaluate of n tokens, copied to the host.  The library links the CUDA
+    runtime statically; torch's runtime shares the device's primary context, so it can copy from the library's pointer."""
+    import torch
+    ptr = L.b200_session_device_logits(sess._s) + (n - 1) * n_vocab * 4
+
+    class _Dev:
+        __cuda_array_interface__ = {"shape": (1, n_vocab), "typestr": "<f4", "data": (ptr, False), "version": 3}
+    return torch.as_tensor(_Dev(), device=f"cuda:{device}").cpu().numpy()
+
+
+def dump_outputs(path, **arrays):
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), np.ascontiguousarray(a, np.float32))
 
 
 def algorithmic_bytes_per_token(hp, n_past, blk=18):
@@ -59,7 +83,7 @@ def prefill_flops(hp, n):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region (read-only queries)."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index):
@@ -215,7 +239,7 @@ def cpu_reference(metric, steps, warmup, log=lambda *a: None, weights=None, gpu=
 
 
 def cuda_reference(args, steps, warmup, log):
-    """Prior art on the same box: the reference's own CUDA backend -- LC/ggml-cuda.cu compiled UNMODIFIED for sm_100 with cuBLAS (oracle/Makefile `refcuda`),
+    """Prior art on the same box: the reference's own CUDA backend -- LC/ggml-cuda.cu compiled UNMODIFIED for sm_90 with cuBLAS (oracle/Makefile `refcuda`),
     driven by the reference's ggml graph executor through the LLaMA graph exactly as llm-base does with ModelParameters::use_gpu (all layers offloaded):
     dequantize + cuBLAS for batches (LC/ggml-cuda.cu:3121-3160), mul_mat_vec_q / dp4a for single tokens (:1807-1843).  Timed on the host clock around
     evaluate (the executor synchronises per node).  Checker-side code; nothing of it is linked into the product."""
@@ -250,7 +274,7 @@ def cuda_reference(args, steps, warmup, log):
     return {"impl": "reference-cuda", "metric": METRIC_PREFILL if prefill_metric else METRIC, "value": val, "unit": "tokens/s", "n_gpus": 1, "steps": steps, "warmup": warmup,
             "ms_per_step": (best[1] if prefill_metric else best[0]) * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "reference CUDA kernels: dp4a mat-vec on Q8_1 activations (decode), dequantize -> cuBLAS (prefill)", "data": "synthetic",
-            "config": {"workload": "LLaMA-7B Q4_0, the reference's own CUDA backend (LC/ggml-cuda.cu recompiled for sm_100) under its ggml graph executor", "n_layer": args.layers,
+            "config": {"workload": "LLaMA-7B Q4_0, the reference's own CUDA backend (LC/ggml-cuda.cu recompiled for sm_90) under its ggml graph executor", "n_layer": args.layers,
                        "host_threads": best[2]},
             "decode_tokens_per_s": 1.0 / best[0], "prefill_tokens_per_s": N_PAST / best[1], "prefill_ms": best[1] * 1e3,
             "e2e": {"value": val, "unit": "tokens/s", "h2d_bytes_per_step": 4 * (N_PAST if prefill_metric else 1), "d2h_bytes_per_step": 4 * hp["n_vocab"] * (N_PAST if prefill_metric else 1)},
@@ -340,6 +364,8 @@ def tp_main(args, rank, local_rank, world, steps, warmup, emit, log):
 
     with ClockSampler(local_rank) as clk:
         ms_dev = timed(steps)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, logits=device_logits_last_row(L, sess, 1, hp["n_vocab"], local_rank))
         for _ in range(3):
             sess.rewind(N_PAST); L.b200_session_evaluate(sess._s, one.ctypes.data, 1, logits.ctypes.data, 0)
         barrier()
@@ -414,12 +440,13 @@ def main():
     ap.add_argument("--steps", type=int, default=None)
     ap.add_argument("--warmup", type=int, default=None)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference", "reference-cuda"],
-                    help="reference = the reference's ggml CPU path; reference-cuda = the reference's own CUDA backend (LC/ggml-cuda.cu recompiled for sm_100, oracle/_ref) on this GPU")
+                    help="reference = the reference's ggml CPU path; reference-cuda = the reference's own CUDA backend (LC/ggml-cuda.cu recompiled for sm_90, oracle/_ref) on this GPU")
     ap.add_argument("--metric", default="decode", choices=["decode", "prefill"], help="which half of BASELINE.json's metric the JSON line reports")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--layers", type=int, default=32, help="debug only: anything but 32 is NOT the benchmark config")
     ap.add_argument("--parallel", default="tp", choices=["tp", "replicas"], help="N > 1: tensor-parallel row split of ONE model (strong scaling, default) or N independent replicas")
     ap.add_argument("--model", default="7b-q4_0", choices=["7b-q4_0", "13b-q5_1"], help="13b-q5_1 = BASELINE.json configs[3] (tensor-parallel decode only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="after the timed steps, write the last step's logits as DIR/logits.npy (float32)")
     args = ap.parse_args()
     # stdout carries exactly ONE line (the JSON); libraries that print to fd 1 (e.g. NCCL's version banner) are sent to stderr
     sys.stdout.flush()
@@ -512,6 +539,8 @@ def main():
             L.b200_session_evaluate_device(sess._s, None, N_PAST)
         pf_dev = L.b200_timing_end_ms()
         barrier()
+        if prefill_metric and args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, logits=device_logits_last_row(L, sess, N_PAST, hp["n_vocab"], local_rank))
         t0 = time.perf_counter()
         L.b200_timing_begin()
         for _ in range(p_steps):                                      # e2e: host token ids in (2 KB), last-row logits out (128 KB), sync, every step
@@ -531,7 +560,7 @@ def main():
     gemm = None
     if rank == 0:
         L.b200_op_bench_mul_mat.argtypes = [C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.POINTER(C.c_float)]
-        impl = 7 if os.environ.get("B200_PREFILL_GEMM", "tc5") != "mma" else 6
+        impl = 7 if os.environ.get("B200_PREFILL_GEMM", "wgmma") != "mma" else 6
         e, f, v = hp["n_embd"], hp["n_ff"], hp["n_vocab"]
         tot_ms, tot_fl, n_l = 0.0, 0.0, 0
         for K, N, cnt, B in ((e, 3 * e, hp["n_layer"], N_PAST), (e, e, hp["n_layer"], N_PAST), (e, 2 * f, hp["n_layer"], N_PAST), (f, e, hp["n_layer"], N_PAST)):
@@ -545,16 +574,18 @@ def main():
                "e2e": {"value": world * N_PAST / (pf_e2e / p_steps * 1e-3), "unit": "tokens/s", "h2d_bytes_per_step": 4 * N_PAST, "d2h_bytes_per_step": 4 * hp["n_vocab"],
                        "ms_per_step": pf_e2e / p_steps},
                "step_roofline": {"bound": "tensor", "flops_per_step": fl, "achieved": fl / (pf_ms * 1e-3) / 1e12, "peak": pk["bf16_sustained"], "unit": "TFLOP/s",
-                                 "frac": fl / (pf_ms * 1e-3) / 1e12 / pk["bf16_sustained"], "peak_source": pk["source"] + " (cuBLAS bf16, sustained)"},
+                                 "frac": fl / (pf_ms * 1e-3) / 1e12 / pk["bf16_sustained"], "peak_source": pk["bf16_source"]},
                "clocks": pf_clocks,
                "note": "conformant (bit-exact) path; includes attention; lm_head on the last row only (OutputRequest without all_logits) -- the reference computes all 512 rows"}
     if gemm:
-        # exact-order floor: 9 fp32 operations per (token, row, 32-block) -- the reference's own rounding sequence -- on 148 SMs x 128 lanes
-        fp32_floor_ms = 9.0 * gemm["flops"] / 64.0 / (148 * 128 * (pf_clocks.get("sm_mhz") or 1965.0) * 1e6) * 1e3
-        prefill["roofline"] = {"bound": "tensor", "kernel": ("mm_exact_tc5_kernel<Q4_0> (tcgen05.mma + TMEM + TMA)" if gemm["impl"] == 7 else "mm_exact_mma_kernel<Q4_0> (mma.sync)") +
+        # exact-order floor: 9 fp32 operations per (token, row, 32-block) -- the reference's own rounding sequence -- on every SM x 128 lanes
+        n_sm = C.c_int32(0)
+        assert L.b200_device_info(C.byref(n_sm), None, None) == 0
+        fp32_floor_ms = 9.0 * gemm["flops"] / 64.0 / (n_sm.value * 128 * (pf_clocks.get("sm_mhz") or pf_clocks.get("sm_max_mhz") or 1980.0) * 1e6) * 1e3
+        prefill["roofline"] = {"bound": "tensor", "kernel": ("mm_exact_tc5_kernel<Q4_0> (wgmma + TMA)" if gemm["impl"] == 7 else "mm_exact_mma_kernel<Q4_0> (mma.sync)") +
                                f": the {gemm['launches']} per-layer weight GEMMs of one 512-token pass, timed alone on operands of the same shapes",
                                "achieved": gemm["flops"] / (gemm["ms"] * 1e-3) / 1e12, "peak": pk["bf16_sustained"], "unit": "TFLOP/s",
-                               "frac": gemm["flops"] / (gemm["ms"] * 1e-3) / 1e12 / pk["bf16_sustained"], "peak_source": pk["source"] + " (cuBLAS bf16, sustained)",
+                               "frac": gemm["flops"] / (gemm["ms"] * 1e-3) / 1e12 / pk["bf16_sustained"], "peak_source": pk["bf16_source"],
                                "traffic": None, "launches": gemm["launches"], "ms_per_pass": gemm["ms"], "share_of_step": gemm["ms"] / pf_ms,
                                "exact_order_fp32_floor_ms": fp32_floor_ms, "frac_of_exact_order_floor": fp32_floor_ms / gemm["ms"],
                                "note": "useful flops 2*B*N*K; the bit-exact kernel runs block-diagonal MMAs (4x the useful tensor work) and is bound by the reference's ordered fp32 chain, not the tensor pipe"}
@@ -579,6 +610,8 @@ def main():
             L.b200_session_evaluate_device(sess._s, None, 1)
         ms_dev = L.b200_timing_end_ms()
         barrier()
+        if not prefill_metric and args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, logits=device_logits_last_row(L, sess, 1, hp["n_vocab"], local_rank))
         # e2e arm: host token in, host logits out, every step
         logits = np.empty(hp["n_vocab"], np.float32)
         for _ in range(3):
@@ -619,9 +652,8 @@ def main():
         "e2e": {"value": world * d_steps / (ms_e2e * 1e-3), "unit": "tokens/s", "h2d_bytes_per_step": 4, "d2h_bytes_per_step": 4 * hp["n_vocab"], "ms_per_step": ms_e2e / d_steps},
         "roofline": {"bound": "hbm", "kernel": "mmv_exact_stream_kernel<Q4_0> (the stand-alone form of the mmv_fused_kernel<Q4_0,EPI> instances of the decode graph: same core loop, "
                                              "no fused epilogue): all 129 weight mat-vecs of the model back to back, timed alone (93% of a token's bytes)",
-                     "achieved": probe_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": probe_gbs / pk["hbm_gbs"], "peak_source": pk["source"] + " (burst copy)",
-                     # ncu --set full (profiles/r01h_mmv_fused.ncu-rep): dram__bytes_read of a mat-vec launch = 1.0015 x its algorithmic bytes, no writes to speak of
-                     "traffic": nbytes.value / max(1, nl.value) * 1.0015, "traffic_source": "ncu dram__bytes_read+write per launch, scaled from the captured w13 launch (50.80 MB vs 50.72 MB algorithmic)",
+                     "achieved": probe_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": probe_gbs / pk["hbm_gbs"], "peak_source": pk["hbm_source"],
+                     "traffic": None,
                      "launches": int(nl.value), "avg_launch_us": ms_probe * 1e3 / max(1, nl.value),
                      "algorithmic_bytes_per_launch": nbytes.value / max(1, nl.value)},
         "step_roofline": {"bound": "hbm", "bytes_per_token": tok_bytes, "weights": wbytes, "kv": kvbytes, "achieved_gbs": tok_bytes / (ms_dev / d_steps * 1e-3) / 1e9,
@@ -636,7 +668,7 @@ def main():
         "dtype": "u8/s8 block dots -> f32 (Q4_0 weights x Q8_0 activations)", "data": "synthetic",
         "config": {"workload": workload, "n_layer": hp["n_layer"], "n_ctx": 2048,
                    "kv_cache": "f16", "parallelism": f"{world} independent replica(s), no collective",
-                   "l2": "inputs larger than L2: 3.7 GB of weights streamed per step vs 126 MB L2",
+                   "l2": "inputs larger than L2: 3.7 GB of weights streamed per step vs 50 MB L2",
                    "weights": "random-init, generated on device (N(0,1/K) -> Q4_0 by the reference's quantizer rule)"},
         "e2e": main_part["e2e"],
         "gpu_launches": (pf_launches if prefill_metric else launches_per_step) * steps,

@@ -13,7 +13,7 @@
  *   InferenceSession::feed_prompt   crates/llm-base/src/inference_session.rs:299-350 (chunks of n_batch, ContextFull)
  *
  * Where the per-node seam (ggml_b200.h) replays the reference's graph one node per call, this front end owns the whole
- * forward pass: a static schedule of fused sm_100a kernels (captured as a CUDA graph for decode), weights and KV cache
+ * forward pass: a static schedule of fused sm_90a kernels (captured as a CUDA graph for decode), weights and KV cache
  * resident in HBM.  Both front ends run the same kernels and are held to the same parity bar.
  *
  * Threading / device contract: one process drives ONE device (b200_init picks it; multi-GPU = one process per GPU, see b200_llama_new_tp), and
@@ -217,7 +217,7 @@ int  b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);
 /* quantize_row_q8_K (LC/k_quants.c:1133-1183) of B rows of K floats -> B * K/256 block_q8_K {f32 d; i8 qs[256]; i16 bsums[16]} (292 bytes each), bit-exact */
 int  b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_out);
-enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = EXACT; TC5 = tcgen05/TMEM/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->tcgen05 GEMM (mmq_tc5.cu, non-conformant) */
+enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = EXACT; TC5 = the tensor-core prefill GEMMs (the name predates the sm_90a port): wgmma/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->wgmma GEMM (mmq_tc5.cu, non-conformant) */
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,4 @@
-"""llm_b200 -- B200-native quantized-inference backend behind the rustformers/llm accelerator seam.
+"""llm_b200 -- H100-native quantized-inference backend behind the rustformers/llm accelerator seam.
 
 The product is the C-ABI shared library llm_b200/libllm_b200.so (sources in llm_b200/csrc, headers in include/):
   * include/ggml_b200.h : the ggml_cuda_* seam the reference's ggml.c and crates/ggml call (drop-in boundary)

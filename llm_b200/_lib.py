@@ -35,7 +35,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(f"{LIB_PATH} is not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                          "(nvcc, sm_100a). llm_b200 has no CPU fallback.")
+                          "(nvcc, sm_90a). llm_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp, i32, i64, sz = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t
     L.b200_init.argtypes = [C.c_int]

@@ -1,4 +1,4 @@
-// llm_b200/csrc/common.cuh -- shared device/host helpers for the B200 (sm_100a) ggml backend.
+// llm_b200/csrc/common.cuh -- shared device/host helpers for the H100 (sm_90a) ggml backend.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

@@ -1,9 +1,8 @@
 // llm_b200/csrc/decode.cu -- one decoded token = ONE persistent cooperative kernel (Llama::evaluate with a single token,
 // crates/models/llama/src/lib.rs:144-368), bit-exact with the reference's CPU path.
 //
-// Why: at batch 1 the 7B graph is ~129 weight mat-vecs of 1.5-8 us each plus ~400 tiny row ops; launched one by one the GPU
-// spends more time filling and draining pipelines than streaming weights (profiles/r01_notes.md: 2.5 TB/s inside the mat-vecs,
-// 0.9 TB/s per token).  Here every CTA stays resident for the whole token:
+// Why: at batch 1 the 7B graph is ~129 weight mat-vecs of a few microseconds each plus ~400 tiny row ops; launched one by one the GPU
+// spends more time filling and draining pipelines than streaming weights.  Here every CTA stays resident for the whole token:
 //   * its producer warp walks the model's weight matrices in graph order and keeps the shared-memory ring full with cp.async;
 //     weights do not depend on activations, so streaming continues while the compute warps wait at a phase boundary or run attention;
 //   * its 4 compute warps execute the graph phase by phase, separated by grid-wide barriers (6 per layer):

@@ -11,7 +11,7 @@
 //   7 mmv<RES>         w2 h + inpFF                                                           (:332-334)
 // Everything that depends on the position reads n_past from DEVICE memory, so the captured graph is valid for every token; the
 // last node increments it.  All arithmetic is the bit-exact arithmetic of exact.cu / rowops.cu (same device functions as decode.cu).
-// What was tried on top of this and measured slower (PDL, norm fusion, tiled weights + TMA, L2 prefetch, ...): profiles/r01_notes.md.
+// Variants that were tried on top of this and not kept: norm fusion, tiled weights + TMA, L2 prefetch.
 #include <cooperative_groups.h>
 #include <stdlib.h>
 
@@ -35,9 +35,8 @@ namespace {
 
 // Programmatic dependent launch.  Every kernel of the chain touches nothing a predecessor writes (and writes nothing at all) before
 // `pdl_wait`; what runs ahead of the wait only reads the constant weights (the producer warp of the next mat-vec fills its ring).
-// WHERE the dependents are released matters (B200, LLaMA-7B decode, ms/token): trigger at kernel entry 2.41 (the successors sit on SM
-// resources the running kernel's tail needs), no PDL 1.757, trigger after the last tile is consumed 1.729, trigger from the producer warp
-// as soon as every byte of the CTA is requested 1.705 -> that is the default.
+// WHERE the dependents are released matters: triggered at kernel entry, the successors sit on SM resources the running kernel's tail needs;
+// the default triggers from the producer warp as soon as every byte of the CTA is requested (B200_PDL_EARLY=0: after the last tile is consumed).
 // tuning aid: per-launch timeline (DecodeParams::prof), see b200_session_decode_timeline
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ void prof_begin(unsigned long long *p) { if (p && threadIdx.x == 0) { const unsigned long long t = gtime(); atomicMin(p, t); atomicMax(p + 3 * B200_PROF_SLOTS, t); } }
@@ -140,7 +139,7 @@ __device__ __forceinline__ void norm_pack_body(const float *__restrict__ x, cons
     prof_end(prof);
 }
 // Two entry points: the single-GPU kernel does not carry the 24 bytes of TpSync, so its argument block stays inside ONE 64-byte line of the constant bank
-// (56 B; with them, 80 B, the 4-CTA kernel measured +0.2..0.4 us per launch, 64 launches per token: profiles/r02m_timeline*.txt).
+// (56 B; with them, 80 B, every one of the 64 launches per token reads one more line).
 __global__ void __launch_bounds__(256) norm_pack_kernel(const float *__restrict__ x, const float *__restrict__ gain, int4 *__restrict__ pack,
                                                         int e, float eps, int q81, int off, int scale16, unsigned long long *prof) {
     norm_pack_body<false>(x, gain, pack, e, eps, q81, off, scale16, prof, TpSync{});
@@ -157,7 +156,7 @@ struct MmvArgs {
     const int4 *xpack;            // input records
     float *dst; const float *addend;                       // EPI_RES / EPI_LOGITS
     // Two pointer groups that no launch uses together share their 32 bytes: the argument block (QWeight 72 B + this struct) then stays within four 64-byte
-    // lines of the constant bank (248 B; 280 B with both groups measured +0.2..0.4 us on every launch of the decode graph, profiles/r02_notes.md).
+    // lines of the constant bank (248 B; 280 B with both groups, one more line read on every launch of the decode graph).
     union {
         struct { float *q; __half *K, *V; const float2 *rope_cs; };                            // EPI_QKV (LLaMA: RoPE + KV store)
         // EPI_BIAS: dst = ((W x + bias) [+ add1]) [+ add2] in that order (ggml_add nodes of gptneox lib.rs:200,302,308-325); EPI_GELU: gelu(W x + bias) quantized
@@ -598,7 +597,7 @@ void launch_mmv(const QWeight &w, MmvArgs A, cudaStream_t st) {
     constexpr int G = EPI == EPI_SILU ? 2 : 1;
     const int64_t groups = ((w.N + ROWS - 1) / ROWS + G - 1) / G;
     // Ring depth: the deepest ring that still keeps every row group resident at once (more bytes in flight per CTA: the small matrices
-    // -- 128 groups for 148 SMs -- are bound by HBM round trips per CTA, not by bandwidth); never deeper than one group's chunk count.
+    // -- 128 groups for 132 SMs -- are bound by HBM round trips per CTA, not by bandwidth); never deeper than one group's chunk count.
     const int chunks = (int)((w.nb + CB - 1) / CB) * G;
     const int base = SST < depth_cap ? SST : depth_cap;
     int nst = base;

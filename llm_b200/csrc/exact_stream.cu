@@ -5,11 +5,11 @@
 //     row) into a 4-stage shared-memory ring with 16-byte cp.async and signals each stage through an mbarrier
 //     (cp.async.mbarrier.arrive): the compute warps never touch global memory for weights.  The kernel is persistent: a CTA walks
 //     several row tiles and the ring keeps streaming across them.  (v1 used one cp.async.bulk per row and per plane: 64 TMA requests
-//     of 64..512 B per stage cost ~60 cycles each and capped the SM at ~9 GB/s -- profiles/r01_notes.md.)
+//     of 64..512 B per stage made the request rate, not the bytes, the limit of an SM.)
 //   * 4 compute warps (4 threads per row: thread w owns AVX lanes w and w+4 == packed word w of every block) walk the blocks
 //     IN ORDER out of shared memory: 3 LDS + 3 unpack + 2 dp4a + 2 i2f + 1 cvt + 1 fmul + 2 fma per block;
 //   * the quantized activation row is re-packed once per mat-vec (quantize_act_pack) into 16-byte records per (block, word).
-// Algorithmic bytes per row of K weights: K/32 * {18, 20, 22, 24, 34}; each is read exactly once (ncu: dram bytes == algorithmic).
+// Algorithmic bytes per row of K weights: K/32 * {18, 20, 22, 24, 34}; each is read exactly once.
 #include "stream_core.cuh"
 
 namespace b200 {

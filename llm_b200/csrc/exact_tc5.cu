@@ -1,25 +1,15 @@
-// llm_b200/csrc/exact_tc5.cu -- bit-exact ggml_mul_mat for a batch of activation rows (prefill) on Blackwell's 5th-generation tensor cores:
-// TMA-staged activations, tcgen05.mma into TMEM, tcgen05.ld epilogue, warp-specialised, one CTA per SM.
+// llm_b200/csrc/exact_tc5.cu -- bit-exact ggml_mul_mat for a batch of activation rows (prefill) on Hopper's warpgroup tensor cores:
+// TMA-staged activations, wgmma.mma_async from shared-memory descriptors into registers, warp-specialised, one CTA per SM.
 //
-// What has to come out (AVX2 build of ggml_vec_dot_q*_q8_*, LC/ggml.c:2434-2457, 2561-2590, 2700-2737, 2841-2879, 2953-2977; driver :10526-10572):
-// per output (token t, row n) eight f32 lane accumulators; for every 32-element block b IN ORDER
+// Per output (token t, row n) the reference keeps eight f32 lane accumulators; for every 32-element block b IN ORDER
 //     acc_L = fma(d_w[n,b] * d_x[t,b], (float)S_L, acc_L),   S_L = sum_{e<4} w[4L+e] * x[4L+e]   (integers)
-// then ((a0+a4)+(a2+a6)) + ((a1+a5)+(a3+a7))  (+ summs = fma chain of m_w * s_x for Q4_1 / Q5_1).
+// then ((a0+a4)+(a2+a6)) + ((a1+a5)+(a3+a7)) (+ the fma chain of m_w * s_x for Q4_1 / Q5_1).  The S_L come from wgmma with a BLOCK-DIAGONAL
+// B operand (DESIGN.md section 4): per half-block and warpgroup, A = 64 tokens x 16 Q8 quants, B = (16 rows x 4 lanes) x 16 weights, column
+// (n, l) non-zero only at elements 4l..4l+3, scale-d = 0, so D[t][(n, l)] = S_{4h+l} exactly.  Column c = 8i + 2q + e of the fragment
+// (q = lane % 4) is row 4(i/2) + q, lane 2(i%2) + e: a thread holds all eight lanes of its rows.
 //
-// The eight S_L of a (token, row, block) are produced by the tensor core with a BLOCK-DIAGONAL B operand (same idea as exact_mma.cu, now in
-// tcgen05 form): for one half-block (16 elements = one kind::f16 K step)
-//     A = 128 tokens x 16 elements (the Q8 quants as f16, exact)            -- M = 128  = TMEM lanes
-//     B = (32 rows x 4 lanes) x 16 elements, column (n, l) non-zero only at elements 4l..4l+3 (the integer weights as f16, exact)   -- N = 128
-//     D[t][(n, l)] = S_{4h+l}  exactly (|S| < 2^17; accumulate is OFF: every MMA is a fresh product)
-// Two MMAs (halves h = 0, 1) per block fill 256 TMEM columns = all eight partial dots of 128 tokens x 32 rows; TMEM holds two such blocks
-// (512 columns) so the tensor core runs one block ahead of the epilogue.  What stays on the CUDA cores is precisely the reference's rounding
-// sequence: one f32 product and eight ordered fmas per (token, row, block) = the bound of this kernel (fp32 pipe), see DESIGN.md section 4.
-//
-// Warp roles (384 threads):  warp 0   : TMA producer  -- cp.async.bulk.tensor of the f16 activations [128 tokens x 64 elements], 128B swizzle
-//                            warp 1   : MMA issuer    -- one thread: tcgen05.mma x 4 per stage, tcgen05.commit to the stage / TMEM barriers
-//                            warps 2-3: expanders     -- packed weights (L2) -> block-diagonal f16 B operands in shared memory + f32 scales
-//                            warps 4-11: epilogue     -- tcgen05.ld, the ordered fp32 chains (packed fma.rn.f32x2), final hsum, store
-// A thread of the epilogue IS a token (TMEM lane): it owns 16 rows x 8 lanes of accumulators; d_x is its private scalar, d_w is warp-uniform.
+// Warps: 0 TMA producer (f16 activations [128 tokens x 64], 128B swizzle, + scales); 2-3 expanders (packed weights -> block-diagonal f16
+// B operands + f32 scales); 4-11 two consumer warpgroups (tokens 0-63 / 64-127) sharing each stage's B: wgmma, the ordered fp32 chains, store.
 #include <string.h>
 
 #include "kernels.cuh"
@@ -31,19 +21,19 @@ namespace {
 
 using namespace tc5;
 
-constexpr int TM = 128, TN = 32, NST = 4, DWR = 2 * NST + 4;     // tokens / rows per CTA, pipeline stages (2 blocks each), scale ring (blocks)
+constexpr int TM = 128, TN = 32, NST = 4;                         // tokens / rows per CTA, pipeline stages (2 blocks each)
 constexpr int A_STAGE = TM * 64 * 2;                              // 16 KB: [128 tokens][64 elements] f16, 128-byte rows, swizzled
 constexpr int B_LBO = 128, B_SBO = 272;                           // K-adjacent core matrices contiguous; 8-column groups 272 B apart (the expanders' 8-byte
                                                                   // stores then spread over the banks: 2-way instead of 8-way conflicts with 256)
-constexpr int B_HALF = 16 * B_SBO;                                // one block-diagonal operand (N = 128 columns x K = 16), no swizzle
+constexpr int B_HALF = 16 * B_SBO;                                // one block-diagonal operand (N = 128 columns = 32 rows x 4 lanes, K = 16), no swizzle
 constexpr int B_STAGE = 4 * B_HALF;                               // [block j][half h]
-constexpr int XR = NST + 2, X_STAGE = TM * 16;                    // ring of per-stage activation scales: [token] float4 {d, aux} x 2 blocks
+constexpr int W_STAGE = 2 * 2 * TN * 4;                           // weight scales of the stage: [block j][d | m][32 rows] f32
+constexpr int X_STAGE = TM * 16;                                  // activation scales of the stage: [token] float4 {d, aux} x 2 blocks
 constexpr int NTHREADS = 384;
-// setmaxnreg re-splits the CTA's OWN register pool (what the launch allocated: 384 threads x 168, the __launch_bounds__(384, 1) cap); a split that asks
-// for more than the pool never completes (the kernel hangs in USETMAXREG.TRY_ALLOC)
-constexpr int PROD_REGS = 56, EPI_REGS = 224;
-static_assert(128 * PROD_REGS + 256 * EPI_REGS <= NTHREADS * 168, "register split exceeds the CTA's pool");
-constexpr int SMEM_BYTES = 1024 + NST * (A_STAGE + B_STAGE) + DWR * TN * 8 + XR * X_STAGE + 256;
+// setmaxnreg re-splits the CTA's own register pool (what the launch allocated: 384 threads x 168, the __launch_bounds__(384, 1) cap)
+constexpr int PROD_REGS = 56, CONS_REGS = 224;
+static_assert(128 * PROD_REGS + 256 * CONS_REGS <= NTHREADS * 168, "register split exceeds the CTA's pool");
+constexpr int SMEM_BYTES = 1024 + NST * (A_STAGE + B_STAGE + W_STAGE + X_STAGE) + 128;
 
 template <int TYPE> struct Tc {
     static constexpr bool MIN = (TYPE == T_Q4_1 || TYPE == T_Q5_1), QH = (TYPE == T_Q5_0 || TYPE == T_Q5_1), Q8 = (TYPE == T_Q8_0);
@@ -65,40 +55,32 @@ struct WRaw { uint4 q; uint32_t dm; uint32_t qh; };               // one (row, b
 
 template <int TYPE>
 __global__ void __launch_bounds__(NTHREADS, 1) mm_exact_tc5_kernel(const __grid_constant__ CUtensorMap tmap_x, const QWeight w, const float4 *__restrict__ xdt,
-                                                                   float *__restrict__ dst, int64_t ldd, int64_t B, const float *__restrict__ addend, int64_t lda) {
+                                                                     float *__restrict__ dst, int64_t ldd, int64_t B, const float *__restrict__ addend, int64_t lda) {
     using T = Tc<TYPE>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;                     // 128B-swizzled tiles need 1024-byte alignment
     uint8_t *const sptr = smem_raw + (sbase - smem_u32(smem_raw));
-    const uint32_t sA = sbase, sB = sbase + NST * A_STAGE, sW = sB + NST * B_STAGE, sX = sW + DWR * TN * 8, sBar = sX + XR * X_STAGE;
+    const uint32_t sA = sbase, sB = sbase + NST * A_STAGE, sX = sB + NST * (B_STAGE + W_STAGE), sBar = sX + NST * X_STAGE;
     uint8_t *const pB = sptr + NST * A_STAGE;
-    float2 *const pW = (float2 *)(sptr + NST * (A_STAGE + B_STAGE));
-    const float4 *const pX = (const float4 *)(sptr + NST * (A_STAGE + B_STAGE) + DWR * TN * 8);
-    uint32_t *const pTmem = (uint32_t *)(sptr + NST * (A_STAGE + B_STAGE) + DWR * TN * 8 + XR * X_STAGE + 128);
+    float *const pW = (float *)(sptr + NST * (A_STAGE + B_STAGE));
+    const float4 *const pX = (const float4 *)(sptr + NST * (A_STAGE + B_STAGE + W_STAGE));
     auto bar_a_full = [&](int s) { return sBar + 8 * s; };
     auto bar_b_full = [&](int s) { return sBar + 8 * (NST + s); };
     auto bar_empty = [&](int s) { return sBar + 8 * (2 * NST + s); };
-    auto bar_t_full = [&](int i) { return sBar + 8 * (3 * NST + i); };
-    auto bar_t_empty = [&](int i) { return sBar + 8 * (3 * NST + 2 + i); };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t n_base = (int64_t)blockIdx.x * TN, m_base = (int64_t)blockIdx.y * TM;
     const int nb = (int)w.nb, nstage = nb / 2;
 
-    // ---- set-up: zero the operand buffers (the off-diagonal zeros are written once), barriers, TMEM ----
+    // ---- set-up: zero the operand buffers (the off-diagonal zeros are written once), barriers ----
     for (int i = tid; i < NST * B_STAGE / 16; i += NTHREADS) ((uint4 *)pB)[i] = make_uint4(0u, 0u, 0u, 0u);
     fence_proxy_async_smem();
     if (tid == 0) {
         tma_prefetch_desc(&tmap_x);
-        for (int s = 0; s < NST; s++) { mbar_init(bar_a_full(s), 1); mbar_init(bar_b_full(s), 64); mbar_init(bar_empty(s), 1); }
-        for (int i = 0; i < 2; i++) { mbar_init(bar_t_full(i), 1); mbar_init(bar_t_empty(i), 8); }
+        for (int s = 0; s < NST; s++) { mbar_init(bar_a_full(s), 1); mbar_init(bar_b_full(s), 64); mbar_init(bar_empty(s), 8); }
         fence_barrier_init();
     }
-    if (warp == 1) { tmem_alloc(smem_u32(pTmem), 512); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *pTmem;
     bool dead = false;
 
     if (warp < 4) {
@@ -112,38 +94,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) mm_exact_tc5_kernel(const __grid_
                     mbar_wait(bar_empty(slot), par ^ 1, dead);
                     mbar_expect_tx(bar_a_full(slot), A_STAGE + x_bytes);
                     tma_load_2d(sA + slot * A_STAGE, &tmap_x, st * 64, (int)m_base, bar_a_full(slot));
-                    // {d, aux} of this stage's two blocks for the tile's tokens: one contiguous piece of the block-pair-major scale array.  Ring of
-                    // NST + 2 stages: slot st % XR is rewritten only after the MMAs of stage st - NST completed, i.e. after the epilogue has finished
-                    // stage st - NST - 1 (the tensor core cannot run further ahead than the two TMEM buffers)
-                    bulk_load(sX + (st % XR) * X_STAGE, xdt + ((size_t)st * B + m_base), x_bytes, bar_a_full(slot));
+                    // {d, aux} of this stage's two blocks for the tile's tokens: one contiguous piece of the block-pair-major scale array
+                    bulk_load(sX + slot * X_STAGE, xdt + ((size_t)st * B + m_base), x_bytes, bar_a_full(slot));
                 }
             }
-        } else if (warp == 1) {
-            // ================= MMA issuer =================
-            if (lane == 0) {
-                constexpr uint32_t idesc = make_idesc_f16(128, 128);
-                for (int st = 0; st < nstage; st++) {
-                    const int slot = st % NST; const uint32_t par = (st / NST) & 1;
-                    mbar_wait(bar_a_full(slot), par, dead);
-                    mbar_wait(bar_b_full(slot), par, dead);
-                    tc_fence_after();
-#pragma unroll
-                    for (int j = 0; j < 2; j++) {
-                        const int blk = 2 * st + j, buf = blk & 1;
-                        mbar_wait(bar_t_empty(buf), ((blk >> 1) & 1) ^ 1, dead);
-                        tc_fence_after();
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-                            const uint64_t ad = make_smem_desc(sA + slot * A_STAGE + j * 64 + h * 32, 16, 1024, LAYOUT_SW128);
-                            const uint64_t bd = make_smem_desc(sB + slot * B_STAGE + (j * 2 + h) * B_HALF, B_LBO, B_SBO, LAYOUT_NONE);
-                            mma_f16_ss(tmem + buf * 256 + h * 128, ad, bd, idesc, 0u);
-                        }
-                        tc_commit(bar_t_full(buf));
-                    }
-                    tc_commit(bar_empty(slot));
-                }
-            }
-        } else {
+        } else if (warp >= 2) {
             // ================= expanders: thread (row r, half h) =================
             const int et = tid - 64, r = et >> 1, h = et & 1;
             const int64_t n = n_base + r < w.N ? n_base + r : w.N - 1;
@@ -157,11 +112,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) mm_exact_tc5_kernel(const __grid_
                 x.qh = T::QH ? h_ptr[blk] : 0u;
                 return x;
             };
-            // column (r, l) of half h: non-zero K slots 4l..4l+3  ->  8 bytes at this offset inside the 4 KB operand
+            // column (r, l) of half h: non-zero K slots 4l..4l+3  ->  8 bytes at this offset inside the operand.  Column index inside the
+            // 64-column operand of row slice r / 16: 16 (r % 16 / 4) + 8 (l / 2) + 2 (r % 4) + l % 2 (the fragment order of the header comment)
             uint32_t col_off[4];
 #pragma unroll
-            for (int l = 0; l < 4; l++) col_off[l] = (uint32_t)((r >> 1) * B_SBO + (l >> 1) * B_LBO + (4 * (r & 1) + l) * 16 + (l & 1) * 8);
-            int wslot = 0;                                                                             // scale-ring slot of the block being expanded
+            for (int l = 0; l < 4; l++) {
+                const uint32_t c = (uint32_t)(64 * (r >> 4) + 16 * ((r & 15) >> 2) + 8 * (l >> 1) + 2 * (r & 3) + (l & 1));
+                col_off[l] = (c >> 3) * B_SBO + (l >> 1) * B_LBO + (c & 7) * 16 + (l & 1) * 8;
+            }
             auto expand = [&](const WRaw &x, int slot, int j) {
                 uint8_t *out = pB + slot * B_STAGE + (j * 2 + h) * B_HALF;
                 const uint32_t qw[4] = {x.q.x, x.q.y, x.q.z, x.q.w};
@@ -178,130 +136,106 @@ __global__ void __launch_bounds__(NTHREADS, 1) mm_exact_tc5_kernel(const __grid_
                     f.y = bytes_to_half2(v, 0x4342u, T::OFF);
                     *(uint2 *)(out + col_off[l]) = f;
                 }
-                if (h == 0) {                                                                          // f32 scales, two planes: d[DWR][32] | m[DWR][32]
-                    float *pd = (float *)pW;
-                    if (T::MIN) { __half2 hh; memcpy(&hh, &x.dm, 4); pd[wslot * TN + r] = __low2float(hh); pd[DWR * TN + wslot * TN + r] = __high2float(hh); }
-                    else pd[wslot * TN + r] = __half2float(__ushort_as_half((unsigned short)x.dm));
+                if (h == 0) {                                                                          // f32 scales: [slot][j][d | m][32 rows]
+                    float *pd = pW + (slot * 2 + j) * 2 * TN;
+                    if (T::MIN) { __half2 hh; memcpy(&hh, &x.dm, 4); pd[r] = __low2float(hh); pd[TN + r] = __high2float(hh); }
+                    else pd[r] = __half2float(__ushort_as_half((unsigned short)x.dm));
                 }
             };
-            WRaw c0[2], c1[2];                                                                     // two stages in flight
-            if (nstage > 0) { c0[0] = fetch(0); c0[1] = fetch(1); }
-            if (nstage > 1) { c1[0] = fetch(2); c1[1] = fetch(3); }
-            for (int st = 0; st < nstage; st += 2) {
-#pragma unroll
-                for (int u = 0; u < 2; u++) {
-                    const int s2 = st + u;
-                    if (s2 >= nstage) break;
-                    const int slot = s2 % NST; const uint32_t par = (s2 / NST) & 1;
-                    mbar_wait(bar_empty(slot), par ^ 1, dead);
-                    WRaw *cur = u ? c1 : c0;
-                    expand(cur[0], slot, 0); if (++wslot == DWR) wslot = 0;
-                    expand(cur[1], slot, 1); if (++wslot == DWR) wslot = 0;
-                    if (s2 + 2 < nstage) { cur[0] = fetch(2 * (s2 + 2)); cur[1] = fetch(2 * (s2 + 2) + 1); }
-                    fence_proxy_async_smem();
-                    mbar_arrive(bar_b_full(slot));
-                }
+            WRaw cur[2];                                                                           // the next stage's blocks are in flight while
+            if (nstage > 0) { cur[0] = fetch(0); cur[1] = fetch(1); }                              // this one waits for its ring slot
+            for (int st = 0; st < nstage; st++) {
+                const int slot = st % NST; const uint32_t par = (st / NST) & 1;
+                mbar_wait(bar_empty(slot), par ^ 1, dead);
+                expand(cur[0], slot, 0);
+                expand(cur[1], slot, 1);
+                if (st + 1 < nstage) { cur[0] = fetch(2 * (st + 1)); cur[1] = fetch(2 * (st + 1) + 1); }
+                fence_proxy_async_smem();
+                mbar_arrive(bar_b_full(slot));
             }
         }
     } else {
-        // ================= epilogue: thread = token (TMEM lane), 16 rows x 8 lanes =================
-        // Software pipeline over "chunks" (4 rows = 2 x 16 TMEM columns): iteration g waits for the loads of chunk g (issued one iteration
-        // earlier), issues the loads of chunk g + 1 -- tcgen05.ld and the rows' weight scales -- and only then runs the fp32 chain of chunk g,
-        // so the TMEM / shared-memory latency hides behind 20 arithmetic instructions of the same warp (and the SM's other 7 epilogue warps).
-        reg_alloc<EPI_REGS>();
-        const int q = warp & 3, ch = (warp - 4) >> 2, tok = q * 32 + lane;
-        const int64_t m = m_base + tok;
-        const uint32_t t_lane = tmem + ((uint32_t)(q * 32) << 16) + ch * 64;
-        float2 acc[16][4];
-        float summs[16];
+        // ================= consumers: warpgroup g = tokens 64g .. 64g+63 of the tile, all 32 rows =================
+        // thread: tokens tok0, tok0 + 8; rows 16 s + 4 jj + q (row slice s, jj < 4), all eight lanes of each
+        reg_alloc<CONS_REGS>();
+        const int g = (warp >> 2) - 1, q = lane & 3;
+        const int tok0 = g * 64 + (warp & 3) * 16 + (lane >> 2);
+        float acc[2][4][2][8];
+        float summs[2][4][2];
+        float d[2][32];
 #pragma unroll
-        for (int r = 0; r < 16; r++) { summs[r] = 0.f;
+        for (int s = 0; s < 2; s++)
 #pragma unroll
-            for (int p = 0; p < 4; p++) acc[r][p] = make_float2(0.f, 0.f); }
+            for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+                for (int u = 0; u < 2; u++) {
+                    summs[s][jj][u] = 0.f;
+#pragma unroll
+                    for (int L = 0; L < 8; L++) acc[s][jj][u][L] = 0.f;
+                }
+#pragma unroll
+        for (int i = 0; i < 32; i++) { d[0][i] = 0.f; d[1][i] = 0.f; }
 
-        // chunk = 8 rows x 4 lanes of ONE half-block = one 32-column tcgen05.ld (the wide loads use the TMEM read port best: profiles/r02_notes.md);
-        // order per block: (rows 0-7, lanes 0-3), (rows 0-7, lanes 4-7), (rows 8-15, lanes 0-3), (rows 8-15, lanes 4-7)
-        uint32_t dA[32], dB[32];                                                                   // TMEM staging, double-buffered
-        float4 wd[2], wm[2];                                                                       // d (and m) of the chunk pair's 8 rows
-        float sc[8];                                                                               // d_w * d_x of those rows (shared by the two halves)
-        const float *pWd = (const float *)pW, *pWm = pWd + DWR * TN;                               // scale ring as two planes: d[DWR][32] | m[DWR][32]
-        int wslot = 0, xslot = 0;                                                                  // ring positions of the block / stage being LOADED next
-        // The barrier probe of a block's first load is hoisted one chunk ahead of its use (`probe`): an mbarrier try_wait takes ~100 cycles to answer even when
-        // the phase is already complete, and issued early it answers behind the fp32 chain of the previous chunk instead of in front of the TMEM load.
-        bool rdy = false;
-        auto probe = [&](int blk) { rdy = dead || mbar_try_wait(bar_t_full(blk & 1), (blk >> 1) & 1); };
-        auto issue = [&](int blk, int c, uint32_t (&d)[32]) {                                     // c = 0..3 as listed above
-            const int buf = blk & 1;
-            if (c == 0) { if (!rdy) mbar_wait(bar_t_full(buf), (blk >> 1) & 1, dead); tc_fence_after(); }
-            tmem_ld_x32(t_lane + buf * 256 + (c & 1) * 128 + (c >> 1) * 32, d);
-        };
-        auto load_w = [&](int slot, int c2) {                                                     // rows 8 c2 .. 8 c2 + 7 of the block in ring slot `slot`
-            const float4 *pd = (const float4 *)(pWd + slot * TN + ch * 16 + c2 * 8);
-            wd[0] = pd[0]; wd[1] = pd[1];
-            if (T::MIN) { const float4 *pm = (const float4 *)(pWm + slot * TN + ch * 16 + c2 * 8); wm[0] = pm[0]; wm[1] = pm[1]; }
-        };
-        auto compute = [&](int c, const uint32_t (&d)[32], float dx, float sx) {
-            const int h = c & 1, r0 = (c >> 1) * 8;
-            if (h == 0) {
-                const float dws[8] = {wd[0].x, wd[0].y, wd[0].z, wd[0].w, wd[1].x, wd[1].y, wd[1].z, wd[1].w};
+        for (int st = 0; st < nstage; st++) {
+            const int slot = st % NST; const uint32_t par = (st / NST) & 1;
+            mbar_wait(bar_a_full(slot), par, dead);
+            mbar_wait(bar_b_full(slot), par, dead);
 #pragma unroll
-                for (int rr = 0; rr < 8; rr++) sc[rr] = __fmul_rn(dws[rr], dx);
-                if (T::MIN) {
-                    const float mws[8] = {wm[0].x, wm[0].y, wm[0].z, wm[0].w, wm[1].x, wm[1].y, wm[1].z, wm[1].w};
+            for (int j = 0; j < 2; j++) {
+                const float2 x0 = ((const float2 *)(pX + slot * TM + tok0))[j], x1 = ((const float2 *)(pX + slot * TM + tok0 + 8))[j];
+                const float dx[2] = {x0.x, x1.x}, sx[2] = {x0.y, x1.y};
+                const float *pd = pW + (slot * 2 + j) * 2 * TN, *pm = pd + TN;
 #pragma unroll
-                    for (int rr = 0; rr < 8; rr++) summs[r0 + rr] = __fmaf_rn(mws[rr], sx, summs[r0 + rr]);
+                for (int s = 0; s < 2; s++) {
+                    wgmma_fence();
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const uint64_t ad = make_smem_desc(sA + slot * A_STAGE + g * 64 * 128 + j * 64 + h * 32, 16, 1024, LAYOUT_SW128);
+                        const uint64_t bd = make_smem_desc(sB + slot * B_STAGE + (j * 2 + h) * B_HALF + s * 8 * B_SBO, B_LBO, B_SBO, LAYOUT_NONE);
+                        wgmma_m64n64k16(d[h], ad, bd, 0u);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(d[0]); fence_regs(d[1]);
+#pragma unroll
+                    for (int jj = 0; jj < 4; jj++) {
+                        const int row = 16 * s + 4 * jj + q;
+                        const float dw = pd[row];
+                        const float mw = T::MIN ? pm[row] : 0.f;
+#pragma unroll
+                        for (int u = 0; u < 2; u++) {
+                            const float sc = __fmul_rn(dw, dx[u]);
+                            if (T::MIN) summs[s][jj][u] = __fmaf_rn(mw, sx[u], summs[s][jj][u]);
+#pragma unroll
+                            for (int h = 0; h < 2; h++)
+#pragma unroll
+                                for (int il = 0; il < 2; il++)
+#pragma unroll
+                                    for (int e = 0; e < 2; e++)
+                                        acc[s][jj][u][4 * h + 2 * il + e] = __fmaf_rn(sc, d[h][4 * (2 * jj + il) + 2 * u + e], acc[s][jj][u][4 * h + 2 * il + e]);
+                        }
+                    }
                 }
             }
-#pragma unroll
-            for (int rr = 0; rr < 8; rr++) {
-                const float2 s2 = make_float2(sc[rr], sc[rr]);
-                acc[r0 + rr][2 * h] = ffma2(s2, make_float2(__uint_as_float(d[rr * 4 + 0]), __uint_as_float(d[rr * 4 + 1])), acc[r0 + rr][2 * h]);
-                acc[r0 + rr][2 * h + 1] = ffma2(s2, make_float2(__uint_as_float(d[rr * 4 + 2]), __uint_as_float(d[rr * 4 + 3])), acc[r0 + rr][2 * h + 1]);
-            }
-        };
-        auto release = [&](int blk) {                                                              // every column of the block's buffer is in registers
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_t_empty(blk & 1));
-        };
-        auto next_w = [&]() { int s0 = wslot; if (++wslot == DWR) wslot = 0; return s0; };
-
-        int ws = 0;                                                                                // ring slot of the block being computed
-        if (nstage > 0) { issue(0, 0, dA); ws = next_w(); load_w(ws, 0); }
-        for (int st = 0; st < nstage; st++) {
-            // the scales of this stage (landed with the stage's activations, before its MMAs ran)
-            const float4 xd = pX[xslot * TM + tok];
-            if (++xslot == XR) xslot = 0;
-            const bool more = st + 1 < nstage;
-            const int b0 = 2 * st, b1 = 2 * st + 1;
-            // the weight scales of rows 8-15 are fetched once compute(0) has turned rows 0-7's into sc[]; the next block's only after its tmem_full wait
-            // (the expander wrote them before the MMAs the barrier reports)
-            tc_wait_ld(); issue(b0, 1, dB); compute(0, dA, xd.x, xd.y); load_w(ws, 1);
-            tc_wait_ld(); issue(b0, 2, dA); compute(1, dB, xd.x, xd.y);
-            tc_wait_ld(); issue(b0, 3, dB); probe(b1); compute(2, dA, xd.x, xd.y);
-            tc_wait_ld(); release(b0); issue(b1, 0, dA); ws = next_w(); load_w(ws, 0); compute(3, dB, xd.x, xd.y);
-            tc_wait_ld(); issue(b1, 1, dB); compute(0, dA, xd.z, xd.w); load_w(ws, 1);
-            tc_wait_ld(); issue(b1, 2, dA); compute(1, dB, xd.z, xd.w);
-            tc_wait_ld(); issue(b1, 3, dB); if (more) probe(b1 + 1); compute(2, dA, xd.z, xd.w);
-            tc_wait_ld(); release(b1); if (more) { issue(b1 + 1, 0, dA); ws = next_w(); load_w(ws, 0); } compute(3, dB, xd.z, xd.w);
+            __syncwarp();                                                                          // the stage's operands and scales are consumed
+            if (lane == 0) mbar_arrive(bar_empty(slot));
         }
         // hsum_float_8 (LC/ggml.c:608-616): ((a0+a4)+(a2+a6)) + ((a1+a5)+(a3+a7)), then + summs
-        if (m < B) {
-            float *out = dst + (size_t)m * ldd + n_base + ch * 16;
-            const float *add = addend ? addend + (size_t)m * lda + n_base + ch * 16 : nullptr;
 #pragma unroll
-            for (int r = 0; r < 16; r++) {
-                const float a0 = acc[r][0].x, a1 = acc[r][0].y, a2 = acc[r][1].x, a3 = acc[r][1].y;
-                const float a4 = acc[r][2].x, a5 = acc[r][2].y, a6 = acc[r][3].x, a7 = acc[r][3].y;
-                float v = __fadd_rn(__fadd_rn(__fadd_rn(a0, a4), __fadd_rn(a2, a6)), __fadd_rn(__fadd_rn(a1, a5), __fadd_rn(a3, a7)));
-                if (T::MIN) v = __fadd_rn(v, summs[r]);
-                if (n_base + ch * 16 + r < w.N) out[r] = add ? __fadd_rn(v, add[r]) : v;
-            }
-        }
+        for (int s = 0; s < 2; s++)
+#pragma unroll
+            for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+                for (int u = 0; u < 2; u++) {
+                    const int64_t m = m_base + tok0 + 8 * u, n = n_base + 16 * s + 4 * jj + q;
+                    if (m < B && n < w.N) {
+                        const float *a = acc[s][jj][u];
+                        float v = __fadd_rn(__fadd_rn(__fadd_rn(a[0], a[4]), __fadd_rn(a[2], a[6])), __fadd_rn(__fadd_rn(a[1], a[5]), __fadd_rn(a[3], a[7])));
+                        if (T::MIN) v = __fadd_rn(v, summs[s][jj][u]);
+                        dst[(size_t)m * ldd + n] = addend ? __fadd_rn(v, addend[(size_t)m * lda + n]) : v;
+                    }
+                }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem, 512); }
 }
 
 // quantize_act with the quants written as fp16 in plain row-major [B][K] (the TMA source), same arithmetic as quantize_act_kernel (quant.cu)

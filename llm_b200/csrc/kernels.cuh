@@ -1,4 +1,4 @@
-// llm_b200/csrc/kernels.cuh -- launchers of the hand-written sm_100a kernels (plain pointers, explicit stream).
+// llm_b200/csrc/kernels.cuh -- launchers of the hand-written sm_90a kernels (plain pointers, explicit stream).
 // Used by both front ends: the ggml_cuda_* seam (seam.cu) and the native session runtime (session.cu).
 #pragma once
 #include "common.cuh"
@@ -43,14 +43,14 @@ inline size_t xh_bytes(int64_t K, int64_t B) { return (size_t)((B + 15) / 16 * 1
 void quantize_act_f16(int vdt, const float *x, int64_t ldx, __half *xh, float2 *ds, int64_t K, int64_t B, cudaStream_t st);
 void mul_mat_q_exact_mma(const QWeight &w, const __half *xh, const float2 *xds, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
 
-// ---- exact_tc5.cu : the same bit-exact batched mat-mul on tcgen05 tensor cores (TMA-staged activations, TMEM accumulators) ------------
+// ---- exact_tc5.cu : the same bit-exact batched mat-mul on wgmma tensor cores (TMA-staged activations, register accumulators) ------------
 // xh = fp16 quants, plain row-major [B][K] (16-byte aligned; the TMA source); xds as above
 void quantize_act_f16_rm(int vdt, const float *x, int64_t ldx, __half *xh, float2 *ds, int64_t K, int64_t B, cudaStream_t st);
 bool prefill_gemm_tc5();         // session.cu: B200_PREFILL_GEMM != "mma" (the default)
 int exact_tc5_check_timeout();   // debugging aid of the op-level entry points: non-zero if a pipeline barrier of the kernel ever timed out
 void mul_mat_q_exact_tc5(const QWeight &w, const __half *xh, const float2 *xds, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
 
-// ---- mmq_tc5.cu : order-free (NON-conformant) fused dequant -> tcgen05 GEMM, f16 operands, f32 accumulation over K in TMEM --------------------
+// ---- mmq_tc5.cu : order-free (NON-conformant) fused dequant -> wgmma GEMM, f16 operands, f32 accumulation over K in registers --------------------
 void cvt_act_f16(const float *x, int64_t ldx, __half *xh, int64_t K, int64_t B, cudaStream_t st);      // f32 rows -> fp16 row-major [B][K]
 void mul_mat_q_fast_tc5(const QWeight &w, const __half *xh, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
 int fast_tc5_check_timeout();

@@ -1,18 +1,17 @@
 // llm_b200/csrc/mmq_tc5.cu -- the north star's named kernel in its order-free ("fast", NON-conformant) form: fused per-32-element-block
-// dequant -> tcgen05 tensor-core GEMM with TMA staging, f32 accumulation over the whole K in TMEM.
+// dequant -> wgmma tensor-core GEMM with TMA staging, f32 accumulation over the whole K in registers.
 //
 //   dst[t][n] = sum_k f16(x[t][k]) * f16(d_w[n][k/32] * (q[n][k] - off) (+ m_w))          (the reference's CUDA prefill does dequantize -> cublasSgemm in
 //                                                                                          TF32: LC/ggml-cuda.cu:3121-3160, dequant :1308-1327)
 // Why it is only the fast mode: the reference's CPU result depends on the AVX2 operation order (DESIGN.md section 2); this kernel rounds activations and
-// dequantized weights to fp16 and lets the tensor core sum 4096+ terms in its own order -- ~1e-3 per mat-mul, ~1e-2 on logits.  The conformant tcgen05
+// dequantized weights to fp16 and lets the tensor core sum 4096+ terms in its own order -- ~1e-3 per mat-mul, ~1e-2 on logits.  The conformant wgmma
 // kernel is exact_tc5.cu; this one shows what the tensor pipe does when the fp32 chain is not the bound.
 //
-// CTA = 128 tokens (M, TMEM lanes) x 256 weight rows (N, TMEM columns), K stepped 64 elements per pipeline stage:
-//   warp 0      TMA producer: activations f16 [128 tokens x 64] (128B swizzle), one cp.async.bulk.tensor per stage
-//   warp 1      MMA issuer: 4 x tcgen05.mma.kind::f16 (M128 N256 K16) per stage, accumulate in TMEM; tcgen05.commit frees the stage
-//   warps 6-21  dequant: thread = (weight row, block of the stage); packed nibbles (+ fifth bits) -> f16 via the 0x6400 magic, one HFMA2 per pair applies d (and m), written as the
-//               128B-swizzled K-major B operand (the scale d is the row-block's fp16 scalar in a register, broadcast by the HFMA2 operand)
-//   warps 2-5   epilogue: tcgen05.ld 32 columns at a time, f32 stores (+ addend)
+// CTA = 128 tokens (M) x 128 weight rows (N), K stepped 64 elements per pipeline stage:
+//   warp 0       TMA producer: activations f16 [128 tokens x 64] (128B swizzle), one cp.async.bulk.tensor per stage
+//   warps 4-11   two consumer warpgroups (tokens 0-63 / 64-127): 4 x wgmma.m64n128k16 per stage, accumulators in registers, f32 stores (+ addend)
+//   warps 12-19  dequant: thread = (weight row, block of the stage); packed nibbles (+ fifth bits) -> f16 via the 0x6400 magic, one HFMA2 per pair applies d
+//                (and m), written as the 128B-swizzled K-major B operand
 #include <string.h>
 
 #include "kernels.cuh"
@@ -24,11 +23,10 @@ namespace {
 
 using namespace tc5;
 
-constexpr int FM = 128, FN = 256, FST = 4;
+constexpr int FM = 128, FN = 128, FST = 4;
 constexpr int FA = FM * 128, FB = FN * 128;                       // bytes per stage: [rows][64 f16] = 128-byte rows, swizzled
-constexpr int FTHREADS = 704;                                    // TMA + MMA + 4 epilogue + 16 dequant warps (one (row, block) per thread and stage: the dequant
-                                                                  // is ~2.7 instructions per weight and needs the warps to hide its own latencies, profiles/r02_notes.md)
-constexpr int FSMEM = 1024 + FST * (FA + FB) + 256;
+constexpr int FTHREADS = 640;                                    // TMA warpgroup + 2 consumer warpgroups + 2 dequant warpgroups
+constexpr int FSMEM = 1024 + FST * (FA + FB) + 128;
 
 template <int TYPE> struct Fq {
     static constexpr bool MIN = (TYPE == T_Q4_1 || TYPE == T_Q5_1), QH = (TYPE == T_Q5_0 || TYPE == T_Q5_1), Q8 = (TYPE == T_Q8_0);
@@ -50,18 +48,16 @@ __device__ __forceinline__ uint32_t deq2(uint32_t v, uint32_t sel, uint32_t off_
 
 template <int TYPE>
 __global__ void __launch_bounds__(FTHREADS, 1) mm_fast_tc5_kernel(const __grid_constant__ CUtensorMap tmap_x, const QWeight w, float *__restrict__ dst, int64_t ldd, int64_t B,
-                                                                  const float *__restrict__ addend, int64_t lda) {
+                                                                    const float *__restrict__ addend, int64_t lda) {
     using T = Fq<TYPE>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t *const sptr = smem_raw + (sbase - smem_u32(smem_raw));
     const uint32_t sA = sbase, sB = sbase + FST * FA, sBar = sB + FST * FB;
     uint8_t *const pB = sptr + FST * FA;
-    uint32_t *const pTmem = (uint32_t *)(sptr + FST * (FA + FB) + 128);
     auto bar_a = [&](int s) { return sBar + 8 * s; };
     auto bar_b = [&](int s) { return sBar + 8 * (FST + s); };
     auto bar_e = [&](int s) { return sBar + 8 * (2 * FST + s); };
-    const uint32_t bar_done = sBar + 8 * 3 * FST;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t n_base = (int64_t)blockIdx.x * FN, m_base = (int64_t)blockIdx.y * FM;
@@ -69,15 +65,10 @@ __global__ void __launch_bounds__(FTHREADS, 1) mm_fast_tc5_kernel(const __grid_c
 
     if (tid == 0) {
         tma_prefetch_desc(&tmap_x);
-        for (int s = 0; s < FST; s++) { mbar_init(bar_a(s), 1); mbar_init(bar_b(s), 512); mbar_init(bar_e(s), 1); }
-        mbar_init(bar_done, 1);
+        for (int s = 0; s < FST; s++) { mbar_init(bar_a(s), 1); mbar_init(bar_b(s), 2 * FN); mbar_init(bar_e(s), 8); }
         fence_barrier_init();
     }
-    if (warp == 1) { tmem_alloc(smem_u32(pTmem), 256); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *pTmem;
     bool dead = false;
 
     if (warp == 0) {
@@ -89,27 +80,9 @@ __global__ void __launch_bounds__(FTHREADS, 1) mm_fast_tc5_kernel(const __grid_c
                 tma_load_2d(sA + slot * FA, &tmap_x, st * 64, (int)m_base, bar_a(slot));
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc_f16(FM, FN);
-            for (int st = 0; st < nstage; st++) {
-                const int slot = st % FST; const uint32_t par = (st / FST) & 1;
-                mbar_wait(bar_a(slot), par, dead);
-                mbar_wait(bar_b(slot), par, dead);
-                tc_fence_after();
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    const uint64_t ad = make_smem_desc(sA + slot * FA + k * 32, 16, 1024, LAYOUT_SW128);
-                    const uint64_t bd = make_smem_desc(sB + slot * FB + k * 32, 16, 1024, LAYOUT_SW128);
-                    mma_f16_ss(tmem, ad, bd, idesc, (st > 0 || k > 0) ? 1u : 0u);
-                }
-                tc_commit(bar_e(slot));
-            }
-            tc_commit(bar_done);
-        }
-    } else if (warp >= 6) {
+    } else if (warp >= 12) {
         // ================= dequant: thread = (weight row of the tile, block j of the stage) =================
-        const int r = (tid - 192) & 255, j = (tid - 192) >> 8;
+        const int r = (tid - 384) & (FN - 1), j = (tid - 384) / FN;
         const int64_t n = n_base + r < w.N ? n_base + r : w.N - 1;
         const uint8_t *q_ptr = w.qs + (size_t)n * nb * T::QS;
         const uint8_t *d_ptr = (const uint8_t *)w.dm + (size_t)n * nb * T::DM;
@@ -123,7 +96,7 @@ __global__ void __launch_bounds__(FTHREADS, 1) mm_fast_tc5_kernel(const __grid_c
             return x;
         };
         const uint32_t row_off = (uint32_t)r * 128u, sw = (uint32_t)(r & 7);
-        auto expand = [&](const Raw &x, int slot, int j) {
+        auto expand = [&](const Raw &x, int slot) {
             uint8_t *row = pB + slot * FB + row_off;
             const __half dh = __ushort_as_half((unsigned short)(x.dm & 0xffffu));
             const __half2 d2 = __half2half2(dh);
@@ -147,48 +120,64 @@ __global__ void __launch_bounds__(FTHREADS, 1) mm_fast_tc5_kernel(const __grid_c
                 *(uint4 *)(row + (((uint32_t)(4 * j + c) ^ sw) << 4)) = f;
             }
         };
-        Raw c0, c1, c2, c3;                                                                        // four stages in flight
+        Raw c0, c1;                                                                                // two stages in flight
         if (nstage > 0) c0 = fetch(j);
         if (nstage > 1) c1 = fetch(2 + j);
-        if (nstage > 2) c2 = fetch(4 + j);
-        if (nstage > 3) c3 = fetch(6 + j);
-        for (int st = 0; st < nstage; st += 4) {
+        for (int st = 0; st < nstage; st += 2) {
 #pragma unroll
-            for (int u = 0; u < 4; u++) {
+            for (int u = 0; u < 2; u++) {
                 const int s2 = st + u;
                 if (s2 >= nstage) break;
                 const int slot = s2 % FST; const uint32_t par = (s2 / FST) & 1;
                 mbar_wait(bar_e(slot), par ^ 1, dead);
-                Raw &cur = u == 0 ? c0 : u == 1 ? c1 : u == 2 ? c2 : c3;
-                expand(cur, slot, j);
-                if (s2 + 4 < nstage) cur = fetch(2 * (s2 + 4) + j);
+                Raw &cur = u == 0 ? c0 : c1;
+                expand(cur, slot);
+                if (s2 + 2 < nstage) cur = fetch(2 * (s2 + 2) + j);
                 fence_proxy_async_smem();
                 mbar_arrive(bar_b(slot));
             }
         }
-    } else if (warp >= 2) {
-        // ================= epilogue (4 consecutive warps cover the 4 TMEM lane quarters) =================
-        const int q = warp & 3;
-        const int64_t m = m_base + q * 32 + lane;
-        mbar_wait(bar_done, 0, dead);
-        tc_fence_after();
-#pragma unroll 1
-        for (int g = 0; g < FN / 32; g++) {
-            uint32_t v[32];
-            tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + g * 32, v);
-            tc_wait_ld();
-            if (m < B) {
-                float *out = dst + (size_t)m * ldd + n_base + g * 32;
-                const float *add = addend ? addend + (size_t)m * lda + n_base + g * 32 : nullptr;
+    } else if (warp >= 4) {
+        // ================= consumers: warpgroup g = tokens 64g .. 64g+63 of the tile, all 128 rows =================
+        const int g = (warp >> 2) - 1;
+        float acc[64];
 #pragma unroll
-                for (int i = 0; i < 32; i++)
-                    if (n_base + g * 32 + i < w.N) out[i] = add ? __uint_as_float(v[i]) + add[i] : __uint_as_float(v[i]);
+        for (int i = 0; i < 64; i++) acc[i] = 0.f;
+        for (int st = 0; st < nstage; st++) {
+            const int slot = st % FST; const uint32_t par = (st / FST) & 1;
+            mbar_wait(bar_a(slot), par, dead);
+            mbar_wait(bar_b(slot), par, dead);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const uint64_t ad = make_smem_desc(sA + slot * FA + g * 64 * 128 + k * 32, 16, 1024, LAYOUT_SW128);
+                const uint64_t bd = make_smem_desc(sB + slot * FB + k * 32, 16, 1024, LAYOUT_SW128);
+                wgmma_m64n128k16(acc, ad, bd, (st > 0 || k > 0) ? 1u : 0u);
             }
+            wgmma_commit();
+            // the previous stage's MMAs are complete once at most this stage's group is pending: release its slot
+            wgmma_wait<1>();
+            if (st > 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_e((st - 1) % FST)); }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        // fragment: rows (tokens) 16 (warp % 4) + lane / 4 (+ 8), columns 8i + 2 (lane % 4) + {0, 1}
+        const int64_t m0 = m_base + g * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+            const int64_t m = m0 + 8 * u;
+            if (m >= B) continue;
+            float *out = dst + (size_t)m * ldd + n_base;
+            const float *add = addend ? addend + (size_t)m * lda + n_base : nullptr;
+#pragma unroll
+            for (int i = 0; i < 16; i++)
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int c = 8 * i + 2 * (lane & 3) + e;
+                    if (n_base + c < w.N) out[c] = add ? acc[4 * i + 2 * u + e] + add[c] : acc[4 * i + 2 * u + e];
+                }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem, 256); }
 }
 
 __global__ void __launch_bounds__(256) cvt_act_f16_kernel(const float *__restrict__ x, int64_t ldx, __half *__restrict__ xh, int64_t K, int64_t total) {

@@ -1,4 +1,4 @@
-// llm_b200/csrc/neox.cu -- native host runtime for GPT-NeoX and GPT-2 (include/llm_b200.h: b200_neox_*): model + InferenceSession on the B200.
+// llm_b200/csrc/neox.cu -- native host runtime for GPT-NeoX and GPT-2 (include/llm_b200.h: b200_neox_*): model + InferenceSession on the GPU.
 //
 // Mirrors   GptNeoX::new / TensorLoader         crates/models/gptneox/src/lib.rs:36-140
 //           GptNeoX::evaluate (the graph)       crates/models/gptneox/src/lib.rs:156-350   (feed-forward: :487-515)
@@ -6,7 +6,7 @@
 //                                                                                               sequential residual, lm_head optional -> tied to wte)
 //           InferenceSession::compute           crates/llm-base/src/inference_session.rs:114-295
 // Batches (prefill) run node by node on the bit-exact kernels of this directory (LayerNorm, bias adds, RoPE mode 2 on n_rot of the head size, gelu table,
-// exact quantized mat-muls incl. the tcgen05 GEMM, exact f16 attention mat-muls); single tokens run the fused 8-kernels-per-layer schedule of
+// exact quantized mat-muls incl. the wgmma GEMM, exact f16 attention mat-muls); single tokens run the fused 8-kernels-per-layer schedule of
 // decode_ops.cu::neox_decode_enqueue from one CUDA graph per context bucket.  Logits are bit-identical to the reference's CPU path (tests/test_gpu_neox.py).
 #include <string.h>
 

@@ -1,4 +1,4 @@
-// llm_b200/csrc/seam.cu -- the ggml_cuda_* C ABI (include/ggml_b200.h) served by the B200 kernels.
+// llm_b200/csrc/seam.cu -- the ggml_cuda_* C ABI (include/ggml_b200.h) served by the project's CUDA kernels.
 //
 // This is the per-node, drop-in front end: the reference's graph executor (LC/ggml.c:14584-14591) calls
 // ggml_cuda_compute_forward for every node and the Rust side (crates/ggml/src/tensor.rs, accelerator/mod.rs) manages
@@ -171,7 +171,7 @@ void op_mul_mat(const ggml_tensor *src0, const ggml_tensor *src1, ggml_tensor *d
         const int64_t ldx = is_contiguous(src1) ? K : (int64_t)(src1->nb[1] / 4);
         if (B >= 16 && !R.fast) {                                       // prefill: bit-exact, block dots on tensor cores
             __half *xh = (__half *)R.op_arena.get((size_t)xh_bytes(K, B), st);
-            if (prefill_gemm_tc5() && B >= 96) {                        // tcgen05 / TMEM / TMA kernel (exact_tc5.cu)
+            if (prefill_gemm_tc5() && B >= 96) {                        // wgmma / TMA kernel (exact_tc5.cu)
                 quantize_act_f16_rm(vec_dot_type(src0->type), x, ldx, xh, xds, K, B, st);
                 mul_mat_q_exact_tc5(w, xh, xds, d, N, B, nullptr, 0, st);
             } else {

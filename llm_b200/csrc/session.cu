@@ -1,4 +1,4 @@
-// llm_b200/csrc/session.cu -- native host runtime (include/llm_b200.h): Llama model + InferenceSession on the B200.
+// llm_b200/csrc/session.cu -- native host runtime (include/llm_b200.h): Llama model + InferenceSession on the GPU.
 //
 // Mirrors, in C++ over the kernels of this directory, what the reference does in Rust over ggml:
 //   Llama::new / TensorLoader          crates/models/llama/src/lib.rs:43-140
@@ -130,7 +130,7 @@ namespace {
 struct Launches { int n = 0; };
 }  // namespace
 void silu_mul_rows(const float *h13, float *out, int64_t f, int64_t n, cudaStream_t st);
-// B200_PREFILL_GEMM=mma selects the round-1 mma.sync kernel for every batch size (default: tcgen05 for batches >= 96 tokens)
+// B200_PREFILL_GEMM=mma selects the round-1 mma.sync kernel for every batch size (default: wgmma for batches >= 96 tokens)
 namespace b200 {
 bool prefill_gemm_tc5() {
     static int v = -1;
@@ -151,7 +151,7 @@ void matmul(b200_session *s, const QWeight &w, const float *x, float *dst, int64
         return;
     }
     if (!fast && B >= 16) {                          // prefill: bit-exact, block dots on tensor cores
-        if (prefill_gemm_tc5() && B >= 96) {         // tcgen05 / TMEM / TMA kernel: 128-token tiles (exact_tc5.cu)
+        if (prefill_gemm_tc5() && B >= 96) {         // wgmma / TMA kernel: 128-token tiles (exact_tc5.cu)
             quantize_act_f16_rm(vec_dot_type(w.type), x, w.K, s->xh, s->xds, w.K, B, st);
             mul_mat_q_exact_tc5(w, s->xh, s->xds, dst, ldd, B, addend, lda, st);
         } else {                                     // mma.sync kernel: 64-token tiles, better for short batches (exact_mma.cu)
@@ -165,7 +165,7 @@ void matmul(b200_session *s, const QWeight &w, const float *x, float *dst, int64
     if (!fast)       mul_mat_q_exact(w, s->xq, s->xds, dst, ldd, B, addend, lda, st);
     else if (B == 1) mul_mat_vec_q(w, s->xq, s->xds, dst, addend, st);
     else if (B < 16) mul_mat_q_simple(w, s->xq, s->xds, dst, ldd, B, addend, lda, st);
-    else if (prefill_gemm_tc5() && B >= 64) { cvt_act_f16(x, w.K, s->xh, w.K, B, st); mul_mat_q_fast_tc5(w, s->xh, dst, ldd, B, addend, lda, st); }   // fused dequant -> tcgen05 GEMM
+    else if (prefill_gemm_tc5() && B >= 64) { cvt_act_f16(x, w.K, s->xh, w.K, B, st); mul_mat_q_fast_tc5(w, s->xh, dst, ldd, B, addend, lda, st); }   // fused dequant -> wgmma GEMM
     else             mul_mat_q(w, s->xq, s->xds, dst, ldd, B, addend, lda, st);
     L.n += 2;
 }

@@ -32,8 +32,8 @@ template <int TYPE, int ROWS = SR, int CB = SCB> struct St {
 
 // int -> float without the conversion unit: the block dots start from the accumulator seed 0x4B400000 (the bits of 12582912.0f = 1.5 * 2^23), so the
 // integer result, read as a float, is exactly 12582912 + s for |s| < 2^22 (here |s| <= 4 * 128 * 127 + seeds), and one FADD on the FMA pipe returns
-// exactly (float)s.  The I2F of the straightforward form runs on the quarter-rate XU pipe, which measured ~50 % busy in the mat-vec steady state
-// (profiles/r01h_mmv_fused.ncu-rep: sm__inst_executed_pipe_xu 37 % of the elapsed time including the ramp) with the FMA pipe at 15 %.
+// exactly (float)s.  The I2F of the straightforward form runs on the quarter-rate XU pipe, which would otherwise be the busiest pipe of the
+// mat-vec steady state while the FMA pipe idles.
 constexpr int I2F_MAGIC = 0x4B400000;
 __device__ __forceinline__ float i2f_magic(int biased) { return __fadd_rn(__int_as_float(biased), -12582912.0f); }
 

@@ -1,6 +1,6 @@
-// llm_b200/csrc/tc5.cuh -- thin inline-PTX wrappers of the Blackwell (sm_100a) machinery used by the tcgen05 GEMMs:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05.mma / .commit / .ld, TMEM allocation, setmaxnreg, packed f32x2 arithmetic.
-// Descriptor bit layouts follow the PTX ISA 8.6 "tcgen05 matrix / instruction descriptor" tables.
+// llm_b200/csrc/tc5.cuh -- thin inline-PTX wrappers of the Hopper (sm_90a) machinery used by the wgmma GEMMs:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma.mma_async with shared-memory descriptors, setmaxnreg.
+// Descriptor bit layout: PTX ISA "Matrix Descriptor Format" for wgmma (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -22,9 +22,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
     asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     return ok != 0;
 }
-// Spin with a watchdog: a protocol bug must not hang the GPU box (a hang is a strike).  After ~1 s without progress the thread records
+// Spin with a watchdog: a protocol bug must not hang the GPU.  After ~1 s without progress the thread records
 // (bar, parity, block, thread) in g_timeout, turns "dead" (all its later waits return at once) and the kernel runs to completion with
-// garbage results; the host reads g_timeout (tc5_check_timeout) in the op-level entry points and the tests.
+// garbage results; the host reads g_timeout (check_timeout) in the op-level entry points and the tests.
 static __device__ unsigned int g_timeout[8];   // one copy per translation unit (each kernel file has its own *_check_timeout)
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, bool &dead) {
     if (dead || mbar_try_wait(bar, parity)) return;
@@ -37,7 +37,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, bool &d
         }
     }
 }
-// generic-proxy writes to shared memory -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy writes to shared memory -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- TMA ----------------------------------------------------------------------------------------------------------------------
@@ -50,66 +50,46 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void *src, uint32_
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-// ---- TMEM / tcgen05 -------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t cols) { asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols) : "memory"); }
-__device__ __forceinline__ void tmem_relinquish() { asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) { asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// all previously issued tcgen05.mma of this thread complete -> one arrival on `bar` (implies fence::before_thread_sync)
-__device__ __forceinline__ void tc_commit(uint32_t bar) { asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory"); }
-// D[tmem] (+)= A[smem] * B[smem], f16/bf16 inputs, f32 accumulate; issued by ONE thread
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// Shared-memory matrix descriptor (K-major operands).  Canonical layouts in 16-byte units (cute/atom/mma_traits_sm100.hpp):
+// ---- wgmma ----------------------------------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (K-major operands).  Canonical layouts in 16-byte units (cute/atom/mma_traits_sm90_gmma.hpp):
 //   no swizzle : ((8,n),2):((1,SBO),LBO)   -- 8 rows x 16 B core matrices; LBO = stride between the two K halves, SBO = between 8-row groups
 //   128B swizzle: ((8,n),2):((8,SBO),1)    -- rows of 128 B, 16-byte chunk c of row r at chunk (c ^ (r & 7)); SBO = 1024 B; LBO unused
-constexpr uint64_t LAYOUT_NONE = 0, LAYOUT_SW128 = 2;
+constexpr uint64_t LAYOUT_NONE = 0, LAYOUT_SW128 = 1;
 __host__ __device__ inline uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint64_t layout) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) |
-           (1ull << 46) /* descriptor version (Blackwell) */ | (layout << 61);
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (layout << 62);
 }
-// Instruction descriptor, kind::f16: D f32, A/B f16 (bf16 = 1), both K-major, dense
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int ab_format = 0) {
-    return (1u << 4) | ((uint32_t)ab_format << 7) | ((uint32_t)ab_format << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// wgmma issue protocol of a warpgroup: fence (orders earlier register / shared-memory accesses before the async reads), the MMAs,
+// commit them as one group, wait until at most N groups are pending
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads of wgmma accumulators above the wait that makes them valid
+template <int R> __device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32 bit, x32 columns: thread i of warp w reads TMEM lane 32*(w%4)+i, columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-                 "%24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-                   "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-                   "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, f16 inputs from shared memory (K-major descriptors), f32 accumulators in registers.
+// Thread `lane` of warp w of the warpgroup holds rows 16w + lane/4 (d[4i], d[4i+1]) and 16w + lane/4 + 8 (d[4i+2], d[4i+3]), columns 8i + 2(lane%4) + {0, 1}.
+// Operand lists: SM90_OPS(t) names %t0 .. %t9, SM90_ACC8(i) binds d[i .. i+7] read-write.
+#define SM90_OPS(t) "%" #t "0, %" #t "1, %" #t "2, %" #t "3, %" #t "4, %" #t "5, %" #t "6, %" #t "7, %" #t "8, %" #t "9"
+#define SM90_OPS0 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9"
+#define SM90_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define SM90_ACC32(i) SM90_ACC8(i), SM90_ACC8(i + 8), SM90_ACC8(i + 16), SM90_ACC8(i + 24)
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\twgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+                 SM90_OPS0 ", " SM90_OPS(1) ", " SM90_OPS(2) ", %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : SM90_ACC32(0) : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-                   "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
+// the same with N = 128 (64 accumulators per thread, i < 16)
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\twgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+                 SM90_OPS0 ", " SM90_OPS(1) ", " SM90_OPS(2) ", " SM90_OPS(3) ", " SM90_OPS(4) ", " SM90_OPS(5) ", %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : SM90_ACC32(0), SM90_ACC32(32) : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
 template <int N> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-
-// Blackwell packed fp32: two IEEE round-to-nearest fmas / muls per instruction (per-lane results identical to fmaf / fmul)
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\tfma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-}
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-    float2 d;
-    asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmul.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (the library links cudart statically and not libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,

@@ -13,7 +13,7 @@
 // aligned 8-byte store is single-copy atomic, so a consumer that polls a unit until its tag equals the expected one has the payload -- the low-latency
 // protocol NCCL calls LL.  tag = epoch * (n_layer + 1) + layer stamp + 1, epoch = tokens decoded so far: monotonic, nothing is ever reset, and a unit is
 // only rewritten after every rank consumed its previous content (the next write of a buffer needs results that depend on all ranks having read it).
-// Measured alternative (round 2, profiles/r02_notes.md): plain stores + __threadfence_system() + a per-kernel flag cost ~14 us per exchanging kernel.
+// The alternative -- plain stores + __threadfence_system() + a per-kernel flag -- puts a system-scope fence and a flag round trip into every exchanging kernel.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,9 +33,9 @@ struct TpCtx {                 // kernel argument (POD); world == 1: single GPU,
                                    // 2 = additionally store to the local slab only: the time is compute alone
     int relax = 0;                 // bit 0: the norm kernels, bit 1: the mat-vecs fed by exchanged records -- kernels whose every dependence on their predecessor
                                    // travels through tagged units may skip griddepcontrol.wait (which also waits for the predecessor's peer stores to be
-                                   // acknowledged across NVLink).  Measured (profiles/r02_notes.md, r02l-r02o): compute alone falls from 1.86 to 1.42 ms / token (7B, 2 GPUs),
-                                   // but the early-resident pollers take issue slots and L2 bandwidth from the producers and the token gets no faster
-                                   // (2.02 / 2.09 / 2.09 ms for 0 / 1 / 3): default 0 = every kernel waits for its predecessor grid.  B200_TP_RELAX overrides.
+                                   // acknowledged across NVLink).  Compute alone gets faster that way,
+                                   // but the early-resident pollers take issue slots and L2 bandwidth from the producers and the token need not get faster:
+                                   // default 0 = every kernel waits for its predecessor grid.  B200_TP_RELAX overrides.
 };
 
 // what one kernel instance reads / writes (baked into the CUDA graph; the epoch is read from device memory)
@@ -83,7 +83,7 @@ __device__ __forceinline__ void tp_wait_sample(const TpCtx &T, int buf, int64_t 
     (void)tp_get(T, buf, unit, tag);
 }
 // Two units per 16-byte load, for consumers that read many units: issue ALL the loads first (tp_ld2), then check the tags (tp_fix2) -- the polling branch
-// of tp_get serialises a thread's loads at one L2 round trip each (measured: 6.8 us to gather w2's input records that way, profiles/r02_notes.md).
+// of tp_get serialises a thread's loads at one L2 round trip each.
 __device__ __forceinline__ uint4 tp_ld2(const TpCtx &T, int buf, int64_t pair) {
     const uint4 *src = (const uint4 *)(T.peer[T.rank] + T.off[buf]) + pair;
     uint4 v;

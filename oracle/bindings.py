@@ -421,6 +421,13 @@ class OracleLlama:
             return logits, tap
         return logits
 
+    def eval_into(self, tokens, logits):
+        """same, into a caller-owned [n, n_vocab] f32 buffer (the CPU arm of bench.py when oracle/_ref is not built)"""
+        tokens = np.ascontiguousarray(tokens, np.int32)
+        rc = self.orc.lib.or_llama_eval(self.m, _p(tokens), tokens.size, _p(logits))
+        assert rc == 0, rc
+        return logits
+
     def eval_tap(self, tokens, il, stage, count):
         """eval and return (logits, flat f32 tap of `count` floats taken at (layer il, stage)); see llama_oracle.c"""
         tokens = np.ascontiguousarray(tokens, np.int32)

@@ -16,7 +16,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: takes more than a few seconds")
 
 
@@ -37,7 +37,7 @@ def orc():
 
 @pytest.fixture(scope="session")
 def ref():
-    """The reference's own compiled ggml.c (oracle/_ref). Built here when /root/reference exists; prebuilt on the GPU box."""
+    """The reference's own compiled ggml.c (oracle/_ref), built by __graft_entry__.build() where the reference sources are present."""
     from oracle import bindings as B
     if not B.have_ref("ref"):
         if os.path.exists("/root/reference/crates/ggml/sys/llama-cpp/ggml.c"):

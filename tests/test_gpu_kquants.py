@@ -7,12 +7,7 @@ from oracle import bindings as B
 
 pytestmark = pytest.mark.gpu
 
-# Q4_K / Q5_K / Q6_K ran bit-exact on a B200 (profiles/r02n_kquant_tests.log).  Q2_K / Q3_K were added after the round's GPU budget was spent: their layout and
-# operation order are pinned on the CPU (tests/test_oracle_kquants.py: the numpy restatement the kernel was written from; tests/test_kquants_lane_arithmetic.py: the
-# kernel's own word-level index / mask / dp4a / shuffle expressions restated in Python), the CUDA code itself has not met
-# hardware yet -- non-strict xfail keeps a first-run surprise from stopping the suite under `-x`; an XPASS is the expected outcome.
-_UNRUN = pytest.mark.xfail(strict=False, reason="Q2_K / Q3_K kernels not yet run on a GPU (round-2 GPU budget exhausted); CPU restatement pinned")
-KTYPES = [pytest.param(n, t, marks=_UNRUN) if n in ("q2_K", "q3_K") else (n, t) for n, t in B.KQUANT_TYPES.items()]
+KTYPES = list(B.KQUANT_TYPES.items())
 
 
 @pytest.fixture(scope="module")

@@ -52,7 +52,7 @@ def test_neox_native_vs_reference(orc, cfg, name):
 @pytest.mark.parametrize("name", ["q4_0", "q5_1"])
 def test_neox_20b_geometry_two_layers(orc, name):
     """BASELINE.json configs[4] geometry: n_embd 6144, 64 heads of 96, n_rot 24, vocab 50432, parallel residual; 2 layers.
-    Prefill 130 tokens (tcgen05 GEMM path, batch >= 96) + decode steps across the 256 bucket edge."""
+    Prefill 130 tokens (wgmma GEMM path, batch >= 96) + decode steps across the 256 bucket edge."""
     from llm_b200.neox import GptNeoX
     t = B.QUANT_TYPES[name]
     hp, tens = synth.make_neox(dict(synth.NEOX_CONFIGS["neox-20b"], n_layer=2, n_ctx=512), t, orc.quantize)

@@ -95,7 +95,7 @@ def test_mul_mat_tensor_core_bit_exact(L, orc, name, t, K, N, Bn):
 @pytest.mark.parametrize("K,N,Bn", [(4096, 200, 128), (256, 33, 16), (704, 100, 40), (11008, 48, 37), (4096, 17, 300), (64, 16, 129), (2048, 130, 512),
                                      (5120, 96, 257), (128, 32, 1)])
 def test_mul_mat_tcgen05_bit_exact(L, orc, name, t, K, N, Bn):
-    """prefill GEMM on the 5th-generation tensor cores (TMA-staged activations, block-diagonal tcgen05.mma into TMEM, tcgen05.ld epilogue;
+    """prefill GEMM on the warpgroup tensor cores (TMA-staged activations, block-diagonal wgmma.mma_async into registers;
     exact_tc5.cu): same bits as ggml_compute_forward_mul_mat, for every format, ragged N / token counts and K tails of the stage ring"""
     rng = np.random.default_rng(K * 13 + N + t)
     w = (rng.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32)
@@ -156,7 +156,7 @@ def test_weight_quantizer_bit_exact(L, orc, name, t):
 @pytest.mark.parametrize("name,t", TYPES)
 @pytest.mark.parametrize("K,N,Bn", [(4096, 256, 128), (704, 100, 40), (11008, 300, 200), (2048, 513, 512), (64, 16, 129)])
 def test_mul_mat_fast_tcgen05_vs_oracle(L, orc, name, t, K, N, Bn):
-    """fused dequant -> tcgen05 GEMM (mmq_tc5.cu), the order-free fast mode: fp16 operands, f32 accumulation in TMEM.  Held to 2e-3 of the row scale
+    """fused dequant -> wgmma GEMM (mmq_tc5.cu), the order-free fast mode: fp16 operands, f32 accumulation in registers.  Held to 2e-3 of the row scale
     (it is NOT the conformant path: activations are not Q8-quantized and the summation order is the tensor core's)"""
     rng = np.random.default_rng(K * 17 + N + t)
     w = (rng.standard_normal((N, K)) / np.sqrt(K)).astype(np.float32)

@@ -1,7 +1,7 @@
-// tools/membench.cu -- micro-benchmark behind the weight layout decision (profiles/r01_notes.md): how fast can a ring of shared-memory
+// tools/membench.cu -- micro-benchmark behind the weight layout decision: how fast can a ring of shared-memory
 // stages be filled from HBM when a stage is (A) 32 row segments of 256 B at the row pitch of a [N][K/32][16 B] plane (16-byte cp.async
 // by one producer warp) versus (B) one contiguous 9 KB region fetched by a single bulk (TMA) copy.  No arithmetic: consumers only
-// wait for the stage and hand it back.   nvcc -arch=sm_100a -O3 -o membench tools/membench.cu && ./membench
+// wait for the stage and hand it back.   nvcc -arch=sm_90a -O3 -o membench tools/membench.cu && ./membench
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

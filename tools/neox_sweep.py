@@ -1,7 +1,7 @@
 """BASELINE.json configs[4]: quant-format sweep Q4_0 / Q4_1 / Q5_0 / Q5_1 / Q8_0 on GPT-NeoX-20B geometry (44 layers, n_embd 6144, 64 heads of 96, n_rot 24,
-vocab 50432), one B200: decode@1 at n_past = 512 through the native fused schedule (8 kernels per layer from one CUDA graph), device-resident, CUDA events;
-tokens/s, ms/token and the fraction of the measured HBM roofline (every weight byte once + the f16 KV cache read).  Weights are generated on the device.
-Usage: python tools/neox_sweep.py [--layers 44] [--steps 32] [--formats q4_0,q8_0] > profiles/r02_neox20b_sweep.json"""
+vocab 50432), one H100: decode@1 at n_past = 512 through the native fused schedule (8 kernels per layer from one CUDA graph), device-resident, CUDA events;
+tokens/s, ms/token and the fraction of the HBM roofline (every weight byte once + the f16 KV cache read).  Weights are generated on the device.
+Usage: python tools/neox_sweep.py [--layers 44] [--steps 32] [--formats q4_0,q8_0] > neox20b_sweep.json"""
 import argparse
 import ctypes as C
 import json
@@ -26,7 +26,7 @@ def main():
     ap.add_argument("--steps", type=int, default=32)
     ap.add_argument("--formats", default="q4_0,q4_1,q5_0,q5_1,q8_0")
     args = ap.parse_args()
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0}
+    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 3350.0}   # H100 SXM data sheet
     L = _lib.lib()
     out = []
     for name in args.formats.split(","):
@@ -38,7 +38,7 @@ def main():
         s = m.start_session(512)
         toks = np.random.default_rng(7).integers(0, hp["n_vocab"], N_PAST + 1, dtype=np.int32)
         L.b200_timing_begin()
-        s.evaluate(toks[:N_PAST])                              # prefill@512 (node-by-node exact kernels incl. the tcgen05 GEMM); fills the KV cache
+        s.evaluate(toks[:N_PAST])                              # prefill@512 (node-by-node exact kernels incl. the wgmma GEMM); fills the KV cache
         pf_ms = L.b200_timing_end_ms()
         logits = s.evaluate(toks[N_PAST:N_PAST + 1])
         assert np.isfinite(logits).all()
@@ -60,7 +60,7 @@ def main():
         print(json.dumps(rec), flush=True)
         out.append(rec)
         s.close(); m.close()
-    print(json.dumps({"config": "GPT-NeoX-20B geometry, decode batch=1 n_past=512, 1 x B200, conformant (bit-exact) kernels", "results": out}))
+    print(json.dumps({"config": "GPT-NeoX-20B geometry, decode batch=1 n_past=512, 1 x H100, conformant (bit-exact) kernels", "results": out}))
 
 
 if __name__ == "__main__":

@@ -1,6 +1,6 @@
 """Kernel-only timing of the prefill weight mat-muls (7B shapes, 512 tokens) for the exact kernels: mma.sync (exact_mma.cu, impl 6)
-vs tcgen05 (exact_tc5.cu, impl 7) [and the order-free int8 kernel, impl 3].  Prints ms, useful TFLOP/s (2*B*N*K) and the fp32-pipe
-fraction (9 fp32 ops per token*row*block on 148 SMs x 128 lanes).  Usage: python tools/prefill_gemm_bench.py [wtype] [B]"""
+vs wgmma (exact_tc5.cu, impl 7) [and the order-free int8 kernel, impl 3].  Prints ms, useful TFLOP/s (2*B*N*K) and the fp32-pipe
+fraction (9 fp32 ops per token*row*block on every SM x 128 lanes at the SM clock given, default the H100's 1980 MHz boost).  Usage: python tools/prefill_gemm_bench.py [wtype] [B] [impls] [sm_mhz]"""
 import ctypes as C
 import sys
 
@@ -10,6 +10,9 @@ from llm_b200 import _lib
 L = _lib.lib()
 L.b200_op_bench_mul_mat.argtypes = [C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.POINTER(C.c_float)]
 L.b200_init(0)
+n_sm = C.c_int32(0)
+assert L.b200_device_info(C.byref(n_sm), None, None) == 0
+sm_hz = (float(sys.argv[4]) if len(sys.argv) > 4 else 1980.0) * 1e6
 wtype = int(sys.argv[1]) if len(sys.argv) > 1 else 2
 B = int(sys.argv[2]) if len(sys.argv) > 2 else 512
 impls = [int(a) for a in sys.argv[3].split(",")] if len(sys.argv) > 3 else [6, 7]
@@ -20,7 +23,7 @@ for name, K, N in shapes:
         ms = C.c_float()
         rc = L.b200_op_bench_mul_mat(wtype, K, N, B, impl, 10, C.byref(ms))
         fl = 2.0 * B * N * K
-        fp32 = 9.0 * B * N * (K // 32) / (148 * 128 * 1.965e9)
+        fp32 = 9.0 * B * N * (K // 32) / (n_sm.value * 128 * sm_hz)
         print(f"{name:8s} K={K:6d} N={N:6d} B={B} impl={impl} rc={rc} {ms.value:8.3f} ms  {fl / ms.value / 1e9:8.1f} TFLOP/s  fp32-pipe floor {fp32 * 1e3:6.3f} ms ({fp32 * 1e3 / ms.value:5.2f})", flush=True)
         tot[impl] += ms.value * (32 if name != "lm_head" else 1)
 for impl in impls:
