@@ -15,6 +15,7 @@
 #include <cooperative_groups.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <array>
 #include <map>
 #include <vector>
@@ -167,7 +168,7 @@ struct MmvArgs {
     int4 *xpack_out; const uint16_t *lut_silu;
     int q81, off, scale16;
     int *n_past_inc;              // EPI_LOGITS: the last node of the token increments InferenceSession::n_past on the device
-    int nst;                      // ring depth chosen by launch_mmv
+    int nst;                      // ring depth chosen by mmv_plan
     int pdl_early;                // trigger the dependents from the producer warp once every byte is requested (B200_PDL_EARLY, default 1)
     unsigned long long *prof;
     // tensor-parallel decode (tp.cuh): this rank owns rows [row0, row0 + w.N) of the full matrix; results go to buffer dst_buf of every rank
@@ -471,17 +472,43 @@ __global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict
     __half *q16 = p16 + nlay;
     __half *vs = (__half *)(sm + (((size_t)nlay * 6 + (size_t)hd * 2 + 127) & ~(size_t)127));
     pdl_trigger();                                              // the successor (wo) only needs shared memory beside us: let it prefetch its tiles now
+    // Ahead of the wait: n_past and the KV cache below it.  Of these, this token's kernels write only cache position n_past of each layer (the
+    // qkv node).  The older positions were written by earlier tokens or the prefill, n_past by the previous token's last kernel or by a
+    // stream-ordered copy after a rewind -- all of it complete before this token's first kernel (the embedding row, a plain stream-ordered launch
+    // without the programmatic attribute, decode_ops_t / neox_ops_t) starts, and so before any kernel chained behind it by PDL, this one included.
+    // So the old cache -- the whole HBM traffic of this kernel -- streams while the qkv node still runs; q, the K row at n_past and the V chunk
+    // holding it are read after the wait.
+    const int p = __ldcg(n_past), n_kv = p + 1;
+    const int np = n_kv & ~31;
+    const int64_t vrow0 = (int64_t)(hk * hd + c0) * n_ctx;
+    const int cold = p / 8;                                      // 16-byte V chunks per row wholly before position p
+    for (int i = tid; i < 32 * cold; i += ATH) {                 // V rows of this CTA's 32 channels: consumed after the soft_max
+        const int rr = i / cold, cc = i - rr * cold;
+        cp16(smem_u32(vs + rr * vstride + cc * 8), Vl + vrow0 + (int64_t)rr * n_ctx + cc * 8);
+    }
+    const int per = (n_kv + per_head - 1) / per_head, j0 = part * per, j1 = n_kv < j0 + per ? n_kv : j0 + per;   // this CTA's KQ positions
+    const int nvec = hd / 32;                                    // 16-byte loads per thread per position (chunks i = 0..nvec-1)
+    constexpr int PU = 4;                                        // positions per quad per pass: up to 4 * nvec 16-byte loads in flight per thread
+    int4 kv[PU][4];
+    auto krow_of = [&](int j) { return Kl + (int64_t)(j < j1 ? j : j0) * gqa + hk * hd + 8 * u; };
+#pragma unroll
+    for (int pu = 0; pu < PU; pu++) {                            // the first pass's K rows below p
+        const int j = j0 + pu * (ATH / 4) + (tid >> 2);
+        const __half *krow = krow_of(j);
+#pragma unroll
+        for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = j < j1 && j < p ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+    }
     pdl_wait();
     float qv = 0.f;
-    if (tid < hd) qv = __ldcg(q + h * hd + tid);               // in flight together with the n_past load (hd <= 256 = ATH)
-    const int n_kv = __ldcg(n_past) + 1;
-    const int np = n_kv & ~31;
-
-    {   // V rows of this CTA's 32 channels: all copies in flight now, consumed after the soft_max
-        const int cpr = (n_kv + 7) / 8;                          // 16-byte chunks per row
-        for (int i = tid; i < 32 * cpr; i += ATH) {
-            const int rr = i / cpr, cc = i - rr * cpr;
-            cp16(smem_u32(vs + rr * vstride + cc * 8), Vl + (int64_t)(hk * hd + c0 + rr) * n_ctx + cc * 8);
+    if (tid < hd) qv = __ldcg(q + h * hd + tid);               // hd <= 256 = ATH
+    if (tid < 32) cp16(smem_u32(vs + tid * vstride + cold * 8), Vl + vrow0 + (int64_t)tid * n_ctx + cold * 8);
+#pragma unroll
+    for (int pu = 0; pu < PU; pu++) {
+        const int j = j0 + pu * (ATH / 4) + (tid >> 2);
+        if (j == p && j < j1) {
+            const __half *krow = krow_of(j);
+#pragma unroll
+            for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = __ldcg((const int4 *)(krow + 32 * i));
         }
     }
     if (tid < hd) q16[tid] = __float2half_rn(qv);
@@ -492,17 +519,15 @@ __global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict
 
     // ---- KQ for this CTA's share of the positions ----
     {
-        const int per = (n_kv + per_head - 1) / per_head, j0 = part * per, j1 = n_kv < j0 + per ? n_kv : j0 + per;
-        const int nvec = hd / 32;                                // 16-byte loads per thread per position (chunks i = 0..nvec-1)
-        constexpr int PU = 4;                                    // positions per quad per pass: up to 4 * nvec 16-byte loads in flight per thread
         for (int jb = j0; jb < j1; jb += PU * (ATH / 4)) {
-            int4 kv[PU][4];
+            if (jb != j0) {                                      // later passes (contexts beyond 4 * ATH / 4 positions per CTA)
 #pragma unroll
-            for (int pu = 0; pu < PU; pu++) {
-                const int j = jb + pu * (ATH / 4) + (tid >> 2);
-                const __half *krow = Kl + (int64_t)(j < j1 ? j : j0) * gqa + hk * hd + 8 * u;
+                for (int pu = 0; pu < PU; pu++) {
+                    const int j = jb + pu * (ATH / 4) + (tid >> 2);
+                    const __half *krow = krow_of(j);
 #pragma unroll
-                for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = j < j1 ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+                    for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = j < j1 ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+                }
             }
 #pragma unroll
             for (int pu = 0; pu < PU; pu++) {
@@ -572,43 +597,123 @@ __global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict
     prof_end(prof);
 }
 
-template <int TYPE, int EPI, bool TP = false>
-void launch_mmv(const QWeight &w, MmvArgs A, cudaStream_t st) {
-    constexpr int ROWS = SR, CB = SCB;
+// ---- ring and grid plan of the decode mat-vecs ------------------------------------------------------------------------------------------------
+// What one CTA takes from an SM while it is resident: shared memory (static + dynamic + the per-CTA reservation), registers as the SM allocates
+// them (per warp, in units of 256), threads.  Footprints add up: a + b = both resident on one SM.
+struct CtaFootprint {
+    int smem = 0, regs = 0, threads = 0, ctas = 0;
+    CtaFootprint operator+(const CtaFootprint &o) const { return {smem + o.smem, regs + o.regs, threads + o.threads, ctas + o.ctas}; }
+};
+struct SmLimits { int sms, smem, reserved, regs, threads, ctas; double hbm_bytes_per_ns; };   // per SM; hbm: the SM's share of the device's peak
+const SmLimits &sm_limits() {
+    static SmLimits L{};
+    if (!L.sms) {
+        int dev; B200_CHECK(cudaGetDevice(&dev));
+        auto at = [&](cudaDeviceAttr a) { int v; B200_CHECK(cudaDeviceGetAttribute(&v, a, dev)); return v; };
+        L.sms = at(cudaDevAttrMultiProcessorCount); L.smem = at(cudaDevAttrMaxSharedMemoryPerMultiprocessor);
+        L.reserved = at(cudaDevAttrReservedSharedMemoryPerBlock); L.regs = at(cudaDevAttrMaxRegistersPerMultiprocessor);
+        L.threads = at(cudaDevAttrMaxThreadsPerMultiProcessor); L.ctas = at(cudaDevAttrMaxBlocksPerMultiprocessor);
+        // memory clock (kHz) x bus width (bits) x 2 (double data rate): 3.35 TB/s on an H100 SXM, 25 GB/s per SM
+        L.hbm_bytes_per_ns = (double)at(cudaDevAttrMemoryClockRate) * 1e3 * at(cudaDevAttrGlobalMemoryBusWidth) / 8.0 * 2.0 / 1e9 / L.sms;
+    }
+    return L;
+}
+template <typename... KArgs>
+CtaFootprint footprint_of(void (*kern)(KArgs...), int threads, size_t dyn_smem) {
+    cudaFuncAttributes fa;
+    B200_CHECK(cudaFuncGetAttributes(&fa, (const void *)kern));
+    const int warps = (threads + 31) / 32;
+    return {(int)(fa.sharedSizeBytes + dyn_smem) + sm_limits().reserved, warps * ((fa.numRegs * 32 + 255) / 256 * 256), warps * 32, 1};
+}
+
+// Loaded HBM latency one CTA's weight ring has to cover.  Not a device attribute: a figure fitted on one H100 80GB HBM3 at a 400 W power limit,
+// where capping every ring of the 7B decode graph at 6 Q4_0 stages (61 KB) streams as fast as 8 or 12, 4 stages is slower, and w13 at 3 stages
+// x 2 CTAs per SM takes 1.7x as long: ~2.4 us at that SM's 25 GB/s share (the share itself is derived from the device, sm_limits).
+constexpr double kLoadedLatencyNs = 2400.0;
+
+struct MmvPlan { int nst = 0, grid = 0, smem = 0; CtaFootprint cta; };
+
+// the most row groups one SM streams when CTA b runs on SM b mod sms and takes groups b, b + grid, ...  A model, not a guarantee: on an idle
+// GPU the block scheduler fills the SMs in CTA order, but CTAs launched under a predecessor's tail land wherever SMs free up first, so with
+// CTAs of unequal share (qkv: 264 CTAs, the first 120 with 2 groups) an SM can end up with more than its fair share.  Placement never
+// changes results, only how evenly the bytes are spread.
+int64_t max_groups_per_sm(int64_t groups, int64_t grid, int sms) {
+    int64_t worst = 0;
+    for (int s = 0; s < sms && s < grid; s++) {
+        int64_t t = 0;
+        for (int64_t b = s; b < grid; b += sms) t += (groups - b + grid - 1) / grid;
+        worst = t > worst ? t : worst;
+    }
+    return worst;
+}
+
+// Ring depth and grid of one mat-vec, computed once per (matrix shape, successor).  `succ` is what the node launched after this one needs
+// on an SM: with room left for it, its CTAs become resident while this kernel's tail runs and start their own loads under it (the mat-vec
+// producer warp streams weights ahead of griddepcontrol.wait; the attention kernel the older KV cache).  The plan:
+//   * one wave, balanced: no SM streams more row groups than ceil(groups / SMs);
+//   * k CTAs per SM plus one successor CTA fit the SM's shared memory, registers, threads and CTA slots;
+//   * every CTA's ring, as deep as that room allows, holds at least HBM-share x latency bytes (or the CTA's whole share of the matrix):
+//     the depth beyond that lets a node bank weights while its predecessor still runs;
+//   * the most CTAs per SM that meet this, and at least 2 where the row groups allow: the four consumer warps of one CTA retire about
+//     30 GB/s of Q4_0 weights (wo, w2), barely the SM's HBM share;
+//   * if no such plan leaves room for the successor, the plan ignores it.
+template <int TYPE, int EPI, bool TP>
+const MmvPlan &mmv_plan(const QWeight &w, const CtaFootprint &succ) {
     using T = St<TYPE>;
-    static int smem_set = 0, sms = 0, depth_cap = -1;
-    static std::map<int, std::array<int, SST_MAX + 1>> occ_by_nb;
-    if (!sms) { int dev; B200_CHECK(cudaGetDevice(&dev)); B200_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)); }
+    auto kern = mmv_fused_kernel<TYPE, EPI, TP>;
+    static std::map<std::array<int64_t, 5>, MmvPlan> plans;
+    static int smem_set = 0, depth_cap = -1;
+    const std::array<int64_t, 5> key{w.N, w.nb, succ.smem, succ.regs, succ.threads};
+    auto it = plans.find(key);
+    if (it != plans.end()) return it->second;
+    const SmLimits &L = sm_limits();
     if (depth_cap < 0) { const char *e = getenv("B200_RING_DEPTH"); depth_cap = e ? atoi(e) : SST_MAX; if (depth_cap < 2) depth_cap = 2; if (depth_cap > SST_MAX) depth_cap = SST_MAX; }
     auto smem_of = [&](int nst) { return 256 + T::ring_bytes(nst) + (int)w.nb * 64 + 256; };
     if (smem_of(SST_MAX) > smem_set) {
         const int want = smem_of(SST_MAX) < 227 * 1024 ? smem_of(SST_MAX) : 227 * 1024;
-        B200_CHECK(cudaFuncSetAttribute(mmv_fused_kernel<TYPE, EPI, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, want));
+        B200_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, want));
         smem_set = smem_of(SST_MAX);
     }
-    auto it = occ_by_nb.find((int)w.nb);
-    if (it == occ_by_nb.end()) {                                          // CTAs per SM for every ring depth at this activation length
-        std::array<int, SST_MAX + 1> o{};
-        for (int nst = 2; nst <= SST_MAX; nst++)
-            if (smem_of(nst) <= 227 * 1024) B200_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o[nst], mmv_fused_kernel<TYPE, EPI, TP>, STHREADS, smem_of(nst)));
-        it = occ_by_nb.emplace((int)w.nb, o).first;
-    }
-    const std::array<int, SST_MAX + 1> &occ = it->second;
+    const CtaFootprint base = footprint_of(kern, STHREADS, 0);
     constexpr int G = EPI == EPI_SILU ? 2 : 1;
-    const int64_t groups = ((w.N + ROWS - 1) / ROWS + G - 1) / G;
-    // Ring depth: the deepest ring that still keeps every row group resident at once (more bytes in flight per CTA: the small matrices
-    // -- 128 groups for 132 SMs -- are bound by HBM round trips per CTA, not by bandwidth); never deeper than one group's chunk count.
-    const int chunks = (int)((w.nb + CB - 1) / CB) * G;
-    const int base = SST < depth_cap ? SST : depth_cap;
-    int nst = base;
-    B200_ASSERT(occ[nst] > 0);
-    const int64_t need = groups < (int64_t)sms * occ[base] ? groups : (int64_t)sms * occ[base];
-    for (int c = base + 1; c <= depth_cap && c <= chunks; c++)
-        if (occ[c] > 0 && (int64_t)sms * occ[c] >= need) nst = c;
-    A.nst = nst;
+    const int64_t groups = ((w.N + SR - 1) / SR + G - 1) / G;
+    const int chunks = (int)((w.nb + SCB - 1) / SCB) * G;              // ring stages per row group
+    const int64_t fair = (groups + L.sms - 1) / L.sms;
+    const int min_stages = (int)(L.hbm_bytes_per_ns * kLoadedLatencyNs / T::STAGE_BYTES + 0.999);
+    const int min_k = fair < 2 ? (int)fair : 2;
+    MmvPlan best;
+    for (int pass = 0; pass < 3 && !best.nst; pass++) {              // 2: last resort, any ring that runs
+        const CtaFootprint room = pass == 0 ? succ : CtaFootprint{};
+        for (int k = (int)(fair < L.ctas ? fair : L.ctas); k >= (pass < 2 ? min_k : 1) && !best.nst; k--) {
+            const int64_t grid = groups < (int64_t)L.sms * k ? groups : (int64_t)L.sms * k;
+            if (max_groups_per_sm(groups, grid, L.sms) > fair) continue;
+            const int per_cta = (int)((groups + grid - 1) / grid) * chunks;
+            int nst = 0;
+            for (int c = 2; c <= depth_cap && c <= (per_cta > 2 ? per_cta : 2); c++) {
+                if (smem_of(c) > 227 * 1024) break;
+                int occ = 0;
+                B200_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, STHREADS, smem_of(c)));
+                CtaFootprint one = base;
+                one.smem += smem_of(c);
+                const CtaFootprint all = CtaFootprint{k * one.smem, k * one.regs, k * one.threads, k} + room;
+                if (occ < k || all.smem > L.smem || all.regs > L.regs || all.threads > L.threads || all.ctas > L.ctas) break;
+                nst = c;
+            }
+            const int need = pass == 2 ? 2 : std::min({min_stages, per_cta, depth_cap});
+            if (nst < need || nst < 2) continue;
+            best.nst = nst; best.grid = (int)grid; best.smem = smem_of(nst);
+            best.cta = base; best.cta.smem += best.smem;
+        }
+    }
+    B200_ASSERT(best.nst > 0);
+    return plans.emplace(key, best).first->second;
+}
+
+template <int TYPE, int EPI, bool TP = false>
+void launch_mmv(const QWeight &w, MmvArgs A, const MmvPlan &plan, cudaStream_t st) {
+    A.nst = plan.nst;
     { static int pe = -1; if (pe < 0) { const char *e = getenv("B200_PDL_EARLY"); pe = e ? atoi(e) : 1; } A.pdl_early = pe; }
-    const int64_t slots = (int64_t)sms * occ[nst];
-    launch_k<1>(mmv_fused_kernel<TYPE, EPI, TP>, dim3((unsigned)(groups < slots ? groups : slots)), dim3(STHREADS), (size_t)smem_of(nst), st, w, A);
+    launch_k<1>(mmv_fused_kernel<TYPE, EPI, TP>, dim3((unsigned)plan.grid), dim3(STHREADS), (size_t)plan.smem, st, w, A);
 }
 
 // dynamic shared memory opt-in of the cluster attention kernel: one high-water mark for both instantiations (the attribute is per function, not per caller)
@@ -664,6 +769,8 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         else { (void)S; launch_k(norm_pack_kernel, grid, block, 0, st, x, gain, xpack_a, e, P.eps, q81, off, s16, pr()); }
         n++;
     };
+    // the token boundary: a plain launch (no programmatic attribute), so nothing of this token starts before the previous token has completed --
+    // attn_fused_kernel reads n_past and the older KV cache ahead of its griddepcontrol.wait on that guarantee
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     if (tp) { launch_k(tp_spread_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.x, e); n++; }
     // attention: one cluster launch per layer (default) or the two-kernel variant (B200_ATTN_FUSED=0, or head sizes a cluster cannot cover)
@@ -676,13 +783,23 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
     static size_t sv_set = 48 * 1024;
     if (sv_smem > sv_set) { B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem)); sv_set = sv_smem; }
+    // mat-vec plans, each leaving room for what follows it (planned from the successor backwards; every layer has the same shapes): the norm
+    // kernels release their dependents at entry, so beside wo and w2 there has to be room for the norm AND the next mat-vec
+    const CtaFootprint f_norm = TP ? footprint_of(norm_pack_tp_kernel, 256, 0) : footprint_of(norm_pack_kernel, 256, 0);
+    const CtaFootprint f_attn = fused_attn ? footprint_of(attn_fused_kernel<TP>, ATH, fa_smem)
+                                           : footprint_of(P.hd == 128 ? attn_kq_kernel<128> : attn_kq_kernel<64>, 128, 0);
+    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_QKV, TP>(layers[0].wqkv, f_attn);
+    const MmvPlan &p_w2 = mmv_plan<TYPE, EPI_RES, TP>(layers[0].w2, f_norm + p_qkv.cta);
+    const MmvPlan &p_w13 = mmv_plan<TYPE, EPI_SILU, TP>(layers[0].w13, p_w2.cta);
+    const MmvPlan &p_wo = mmv_plan<TYPE, EPI_RES, TP>(layers[0].wo, f_norm + p_w13.cta);
+    const MmvPlan &p_out = mmv_plan<TYPE, EPI_LOGITS, TP>(P.output, CtaFootprint{});
     for (int il = 0; il < P.n_layer; il++) {
         const DecodeLayer &L = layers[il];
         const unsigned v = (unsigned)il + 1;                     // flag value of this layer's exchanges (tp.cuh)
         launch_norm(P.x, L.attn_norm, ts(TPB_X, (unsigned)il, -1, 0, -1, 0));
         MmvArgs A{}; A.xpack = xpack_a; A.q = P.q; A.K = L.K; A.V = L.V; A.rope_cs = P.rope_cs; A.rope_half = P.rope_half; A.hd = P.hd; A.e = e_loc; A.gqa = P.gqa;
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
-        A.prof = pr(); launch_mmv<TYPE, EPI_QKV, TP>(L.wqkv, A, st); n++;
+        A.prof = pr(); launch_mmv<TYPE, EPI_QKV, TP>(L.wqkv, A, p_qkv, st); n++;
         if (fused_attn) {
             cudaLaunchConfig_t cfg{};
             cfg.gridDim = dim3(P.n_head * (P.hd / 32)); cfg.blockDim = dim3(ATH); cfg.dynamicSmemBytes = fa_smem; cfg.stream = st;
@@ -705,19 +822,19 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         }
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.ff; Bo.addend = P.x;
         Bo.ts = ts(TPB_XD, v, TPB_X, (unsigned)il, TPB_FF, v); Bo.row0 = tp ? P.row0_e : 0;
-        Bo.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.wo, Bo, st); n++;
+        Bo.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.wo, Bo, p_wo, st); n++;
         launch_norm(P.ff, L.ffn_norm, ts(TPB_FF, v, -1, 0, -1, 0));
         MmvArgs C{}; C.xpack = xpack_a; C.xpack_out = P.xpack_f; C.lut_silu = P.lut_silu; C.q81 = q81; C.off = off; C.scale16 = s16;
         C.ts = ts(-1, 0, -1, 0, TPB_XF, v); C.row0 = tp ? P.row0_w13 : 0;
-        C.prof = pr(); launch_mmv<TYPE, EPI_SILU, TP>(L.w13, C, st); n++;
+        C.prof = pr(); launch_mmv<TYPE, EPI_SILU, TP>(L.w13, C, p_w13, st); n++;
         MmvArgs D{}; D.xpack = P.xpack_f; D.dst = P.x; D.addend = P.ff;
         D.ts = ts(TPB_XF, v, TPB_FF, v, TPB_X, v); D.row0 = tp ? P.row0_e : 0;
-        D.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.w2, D, st); n++;
+        D.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.w2, D, p_w2, st); n++;
     }
     launch_norm(P.x, P.norm, ts(TPB_X, (unsigned)P.n_layer, -1, 0, -1, 0));
     MmvArgs Z{}; Z.xpack = xpack_a; Z.dst = P.logits; Z.addend = nullptr; Z.n_past_inc = P.n_past;
     Z.ts = ts(-1, 0, -1, 0, TPB_LOGITS, 0); Z.row0 = tp ? P.row0_v : 0;
-    Z.prof = pr(); launch_mmv<TYPE, EPI_LOGITS, TP>(P.output, Z, st); n++;
+    Z.prof = pr(); launch_mmv<TYPE, EPI_LOGITS, TP>(P.output, Z, p_out, st); n++;
     if (tp) {                                                    // gathered logits -> the plain array the host reads; then the epoch moves on
         launch_k(tp_collect_kernel, dim3((P.n_vocab_full + 255) / 256), dim3(256), 0, st, P.logits, P.n_vocab_full); n++;
         launch_k(tp_bump_kernel, dim3(1), dim3(32), 0, st); n++;
@@ -815,6 +932,8 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     const int q81 = has_min(TYPE) ? 1 : 0, off = TYPE == T_Q5_0 ? 16 : 0, s16 = TYPE == T_Q4_0 ? 1 : 0;
     const int e = P.e;
     int n = 0;
+    // the token boundary: a plain launch (no programmatic attribute), so nothing of this token starts before the previous token has completed --
+    // attn_fused_kernel reads n_past and the older KV cache ahead of its griddepcontrol.wait on that guarantee
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
@@ -823,11 +942,17 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     attn_fused_reserve(fa_smem);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
+    const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
+    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wqkv, footprint_of(neox_rope_store_kernel, 256, 0) + footprint_of(attn_fused_kernel<false>, ATH, fa_smem));
+    const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
+    const MmvPlan &p_fc = mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta);
+    const MmvPlan &p_dense = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wdense, f_ln + p_fc.cta);
+    const MmvPlan &p_head = mmv_plan<TYPE, EPI_BIAS, false>(P.lm_head, CtaFootprint{});
     for (int il = 0; il < P.n_layer; il++) {
         const NeoxLayer &L = layers[il];
         launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;          // :192-196
         MmvArgs A{}; A.xpack = P.xpack_a; A.dst = P.qkv; A.bias = L.bqkv;
-        launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, st); n++;                                                                                      // :199-200
+        launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, p_qkv, st); n++;                                                                                      // :199-200
         launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, L.K, L.V, (const int *)P.n_past, P.rope_cs, P.rope_half,
                  P.gpt2 ? 0 : P.n_rot, P.hd, e, P.n_ctx, P.gpt2 ? P.hd : 3 * P.hd, P.gpt2 ? e : P.hd, P.gpt2 ? 2 * e : 2 * P.hd); n++;               // :205-247
         {
@@ -846,18 +971,18 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         }
         // attention.dense (+bias); sequential residual: ff_in = that + inpL                                                                    :301-312
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out; Bo.bias = L.bdense; Bo.add1 = P.parallel_residual ? nullptr : P.x;
-        launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, st); n++;
+        launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;
         // mlp: LayerNorm of inpL (parallel residual) or of ff_in                                                                                :313-316 / ffn
         launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)(P.parallel_residual ? P.x : P.attn_out), L.ln2_g, L.ln2_b, P.xpack_a, e, q81, off, s16); n++;
         MmvArgs C{}; C.xpack = P.xpack_a; C.xpack_out = P.xpack_f; C.bias = L.bfc; C.lut_gelu = P.lut_gelu; C.q81 = q81; C.off = off; C.scale16 = s16;
-        launch_mmv<TYPE, EPI_GELU>(L.wfc, C, st); n++;
+        launch_mmv<TYPE, EPI_GELU>(L.wfc, C, p_fc, st); n++;
         // parallel: inpL = ((proj + bias) + attn) + inpL; sequential: inpL = (proj + bias) + ff_in                                              :317-325
         MmvArgs D{}; D.xpack = P.xpack_f; D.dst = P.x; D.bias = L.bproj; D.add1 = P.attn_out; D.add2 = P.parallel_residual ? P.x : nullptr;
-        launch_mmv<TYPE, EPI_BIAS>(L.wproj, D, st); n++;
+        launch_mmv<TYPE, EPI_BIAS>(L.wproj, D, p_proj, st); n++;
     }
     launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16); n++;                     // :332-334
     MmvArgs Z{}; Z.xpack = P.xpack_a; Z.dst = P.logits; Z.n_past_inc = P.n_past;
-    launch_mmv<TYPE, EPI_BIAS>(P.lm_head, Z, st); n++;                                                                                        // :342
+    launch_mmv<TYPE, EPI_BIAS>(P.lm_head, Z, p_head, st); n++;                                                                                        // :342
     B200_CHECK(cudaGetLastError());
     if (launches) *launches = n;
 }
