@@ -1,5 +1,7 @@
-// llm_b200/csrc/decode.h -- parameters of the one-launch-per-token decode kernel (decode.cu)
+// llm_b200/csrc/decode.h -- parameters of the decode schedules (decode.cu, decode_ops.cu) and the sessions' cache of decode graphs
 #pragma once
+#include <functional>
+#include <utility>
 #include <vector>
 
 #include "kernels.cuh"
@@ -70,5 +72,28 @@ bool launch_decode(const DecodeParams &P, int wtype, cudaStream_t st, int *grid_
 
 // default decode schedule: 8 fused kernels per layer on `st` (decode_ops.cu); position read from *P.n_past on the device
 void decode_ops_enqueue(const DecodeParams &P, const std::vector<DecodeLayer> &layers, int wtype, int n_kv_bucket, int4 *xpack_a, cudaStream_t st, int *launches);
+
+// A session's decode graphs (decode_ops.cu): one per context bucket of 256 positions, and the device copy of n_past the schedules read.
+struct DecodeGraphCache {
+    std::vector<std::pair<int, cudaGraphExec_t>> graphs;   // (n_kv bucket, instantiated graph)
+    bool warm = false;                  // the first step runs eagerly (it sets kernel attributes), later ones replay a graph
+    int nodes = 0;                      // launches of one step
+    int *d_n_past = nullptr, *h_n_past = nullptr;          // device word, pinned staging word
+    int dev_n_past = -1;                // value currently held by *d_n_past (-1: unknown)
+
+    DecodeGraphCache();                 // allocates the n_past words
+    ~DecodeGraphCache();                // drop() and frees them
+    DecodeGraphCache(const DecodeGraphCache &) = delete;
+    DecodeGraphCache &operator=(const DecodeGraphCache &) = delete;
+
+    // uploads n_past if the device copy is stale (after a prefill or a rewind)
+    void sync_n_past(int n_past, cudaStream_t st);
+    // one decode step at position n_kv - 1 (its last kernel increments *d_n_past): enqueue(bucket, st, &nodes) enqueues the schedule for up to
+    // `bucket` positions.  Runs it eagerly on the first step or when replay is false, else replays (capturing on first use) the bucket's graph.
+    // Returns the step's launch count.
+    int run(int n_kv, int n_ctx, bool replay, const std::function<void(int, cudaStream_t, int *)> &enqueue, cudaStream_t st);
+    // destroys every graph (they hold kernel arguments that changed)
+    void drop();
+};
 
 }  // namespace b200

@@ -724,6 +724,28 @@ static void attn_fused_reserve(size_t bytes) {
     B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
+// dynamic shared memory of attn_fused_kernel for nlay positions and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
+size_t attn_fused_smem(int nlay, int hd) {
+    return (((size_t)nlay * 6 + (size_t)hd * 2 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 32) * 2;
+}
+// one cluster of hd/32 CTAs per head; a programmatic dependent of its predecessor unless B200_PDL clears bit 1
+template <bool TP>
+void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const __half *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
+                       float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                       unsigned long long *prof, const TpSync &S, int head0) {
+    const size_t smem = attn_fused_smem(nlay, hd);
+    attn_fused_reserve(smem);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(n_head * (hd / 32)); cfg.blockDim = dim3(ATH); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute at[2];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = hd / 32; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = (pdl_mask() & 2) ? 2 : 1;
+    B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+                                  q81, off, scale16, prof, S, head0));
+}
 
 // tensor-parallel helpers (tp.cuh).  spread: the embedding row every rank computed for itself -> the X exchange buffer's unit form (stamp 0);
 // collect: the gathered logits units -> the plain f32 logits array the host reads; bump: the token is complete, the epoch moves on.
@@ -776,10 +798,9 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     // attention: one cluster launch per layer (default) or the two-kernel variant (B200_ATTN_FUSED=0, or head sizes a cluster cannot cover)
     static const bool fused_env = !(getenv("B200_ATTN_FUSED") && getenv("B200_ATTN_FUSED")[0] == '0');
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
-    const size_t fa_smem = (((size_t)nlay * 6 + (size_t)P.hd * 2 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 32) * 2;
+    const size_t fa_smem = attn_fused_smem(nlay, P.hd);
     const bool fused_attn = (fused_env || tp) && P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && fa_smem <= 227 * 1024;
     B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue
-    if (fused_attn) attn_fused_reserve(fa_smem);
     const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
     static size_t sv_set = 48 * 1024;
     if (sv_smem > sv_set) { B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem)); sv_set = sv_smem; }
@@ -801,17 +822,8 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
         A.prof = pr(); launch_mmv<TYPE, EPI_QKV, TP>(L.wqkv, A, p_qkv, st); n++;
         if (fused_attn) {
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(P.n_head * (P.hd / 32)); cfg.blockDim = dim3(ATH); cfg.dynamicSmemBytes = fa_smem; cfg.stream = st;
-            cudaLaunchAttribute at[2];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = P.hd / 32; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            at[1].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = at; cfg.numAttrs = (pdl_mask() & 2) ? 2 : 1;
-            B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, (const float *)P.q, (const __half *)L.K, (const __half *)L.V, P.xpack_d, (const int *)P.n_past,
-                                          (const uint16_t *)P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, nlay, q81, off, s16, pr(),
-                                          ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0));
+            launch_attn_fused<TP>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, nlay, q81, off, s16, pr(),
+                                  ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0);
             n++;
         } else {
             launch_k(P.hd == 128 ? attn_kq_kernel<128> : attn_kq_kernel<64>, dim3((n_kv_bucket + 63) / 64, P.n_head), dim3(128), 0, st,
@@ -937,9 +949,8 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
-    const size_t fa_smem = (((size_t)nlay * 6 + (size_t)P.hd * 2 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 32) * 2;
+    const size_t fa_smem = attn_fused_smem(nlay, P.hd);
     B200_ASSERT(P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && fa_smem <= 227 * 1024 && e <= 8192);
-    attn_fused_reserve(fa_smem);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
@@ -955,20 +966,8 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, p_qkv, st); n++;                                                                                      // :199-200
         launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, L.K, L.V, (const int *)P.n_past, P.rope_cs, P.rope_half,
                  P.gpt2 ? 0 : P.n_rot, P.hd, e, P.n_ctx, P.gpt2 ? P.hd : 3 * P.hd, P.gpt2 ? e : P.hd, P.gpt2 ? 2 * e : 2 * P.hd); n++;               // :205-247
-        {
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(P.n_head * (P.hd / 32)); cfg.blockDim = dim3(ATH); cfg.dynamicSmemBytes = fa_smem; cfg.stream = st;
-            cudaLaunchAttribute at[2];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = P.hd / 32; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            at[1].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = at; cfg.numAttrs = (pdl_mask() & 2) ? 2 : 1;
-            B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<false>, (const float *)P.q, (const __half *)L.K, (const __half *)L.V, P.xpack_d, (const int *)P.n_past,
-                                          (const uint16_t *)P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, nlay, q81, off, s16,
-                                          (unsigned long long *)nullptr, S, 0));                                                           // :250-298
-            n++;
-        }
+        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, nlay, q81, off, s16,
+                                 nullptr, S, 0); n++;                                                                                     // :250-298
         // attention.dense (+bias); sequential residual: ff_in = that + inpL                                                                    :301-312
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out; Bo.bias = L.bdense; Bo.add1 = P.parallel_residual ? nullptr : P.x;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;
@@ -1018,6 +1017,53 @@ void decode_ops_enqueue(const DecodeParams &P, const std::vector<DecodeLayer> &l
         case T_Q8_0: if (tp) decode_ops_t<T_Q8_0, true>(P, layers, n_kv_bucket, xpack_a, st, launches); else decode_ops_t<T_Q8_0, false>(P, layers, n_kv_bucket, xpack_a, st, launches); break;
         default: B200_ASSERT(!"decode_ops_enqueue: unsupported weight type");
     }
+}
+
+DecodeGraphCache::DecodeGraphCache() {
+    B200_CHECK(cudaMalloc(&d_n_past, sizeof(int)));
+    B200_CHECK(cudaMallocHost(&h_n_past, sizeof(int)));
+}
+DecodeGraphCache::~DecodeGraphCache() {
+    drop();
+    B200_CHECK(cudaFree(d_n_past));
+    B200_CHECK(cudaFreeHost(h_n_past));
+}
+
+void DecodeGraphCache::sync_n_past(int n_past, cudaStream_t st) {
+    if (dev_n_past == n_past) return;
+    B200_CHECK(cudaStreamSynchronize(st));      // the pinned staging word may still be in flight
+    *h_n_past = n_past;
+    B200_CHECK(cudaMemcpyAsync(d_n_past, h_n_past, sizeof(int), cudaMemcpyHostToDevice, st));
+    dev_n_past = n_past;
+}
+
+int DecodeGraphCache::run(int n_kv, int n_ctx, bool replay, const std::function<void(int, cudaStream_t, int *)> &enqueue, cudaStream_t st) {
+    sync_n_past(n_kv - 1, st);
+    const int bucket = std::min((n_kv + 255) / 256 * 256, n_ctx);
+    if (!warm || !replay) {
+        enqueue(bucket, st, &nodes);
+        warm = true;
+    } else {
+        cudaGraphExec_t exec = nullptr;
+        for (auto &g : graphs) if (g.first == bucket) exec = g.second;
+        if (!exec) {
+            cudaGraph_t graph;
+            B200_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+            enqueue(bucket, st, &nodes);
+            B200_CHECK(cudaStreamEndCapture(st, &graph));
+            B200_CHECK(cudaGraphInstantiate(&exec, graph, 0));
+            B200_CHECK(cudaGraphDestroy(graph));
+            graphs.emplace_back(bucket, exec);
+        }
+        B200_CHECK(cudaGraphLaunch(exec, st));
+    }
+    dev_n_past = n_kv;
+    return nodes;
+}
+
+void DecodeGraphCache::drop() {
+    for (auto &g : graphs) cudaGraphExecDestroy(g.second);
+    graphs.clear();
 }
 
 }  // namespace b200

@@ -1,5 +1,5 @@
 // llm_b200/csrc/kernels.cuh -- launchers of the hand-written sm_90a kernels (plain pointers, explicit stream).
-// Used by both front ends: the ggml_cuda_* seam (seam.cu) and the native session runtime (session.cu).
+// Used by all three front ends: the ggml_cuda_* seam (seam.cu) and the native LLaMA (session.cu) and GPT-NeoX / GPT-2 (neox.cu) sessions.
 #pragma once
 #include "common.cuh"
 
@@ -33,7 +33,7 @@ void mul_mat_q(const QWeight &w, const int8_t *xq, const float2 *xds, float *dst
 // cross-check implementation (CUDA cores, dp4a), same contract
 void mul_mat_q_simple(const QWeight &w, const int8_t *xq, const float2 *xds, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
 
-// ---- exact.cu : bit-exact (AVX2 operation order) versions; the DEFAULT of both front ends -----------------------------------------
+// ---- exact.cu : bit-exact (AVX2 operation order) versions; the DEFAULT of every front end -----------------------------------------
 // same contract as mul_mat_q for any B >= 1; results are bit-identical to ggml_compute_forward_mul_mat on the reference's x86 build
 void mul_mat_q_exact(const QWeight &w, const int8_t *xq, const float2 *xds, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
 
@@ -46,7 +46,6 @@ void mul_mat_q_exact_mma(const QWeight &w, const __half *xh, const float2 *xds, 
 // ---- exact_tc5.cu : the same bit-exact batched mat-mul on wgmma tensor cores (TMA-staged activations, register accumulators) ------------
 // xh = fp16 quants, plain row-major [B][K] (16-byte aligned; the TMA source); xds as above
 void quantize_act_f16_rm(int vdt, const float *x, int64_t ldx, __half *xh, float2 *ds, int64_t K, int64_t B, cudaStream_t st);
-bool prefill_gemm_tc5();         // session.cu: B200_PREFILL_GEMM != "mma" (the default)
 int exact_tc5_check_timeout();   // debugging aid of the op-level entry points: non-zero if a pipeline barrier of the kernel ever timed out
 void mul_mat_q_exact_tc5(const QWeight &w, const __half *xh, const float2 *xds, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
 
@@ -60,6 +59,15 @@ bool mmv_exact_stream_supported(const QWeight &w);
 // bit-faithful activation quantizer emitting 16-byte records per (block, word): see exact_stream.cu
 void quantize_act_pack(int wtype, const float *x, int4 *pack, int64_t K, cudaStream_t st);
 void mul_mat_vec_q_exact_stream(const QWeight &w, const int4 *xpack, float *dst, const float *addend, cudaStream_t st);
+
+// ---- mul_mat.cu : the bit-exact ggml_mul_mat of every front end -------------------------------------------------------------------------
+bool prefill_gemm_tc5();         // B200_PREFILL_GEMM != "mma" (the default)
+// activation buffers for B rows of K: xq [B][K] int8, xds [B][K/32], xpack (K/32) * 64 bytes, xh xh_bytes(K, B)
+struct ExactActs { int8_t *xq; float2 *xds; int4 *xpack; __half *xh; };
+// dst[b*ldd + n] (+ addend[b*lda + n]) for B rows of x (row stride ldx): quantizes x and runs the exact kernel for B -- the streaming mat-vec
+// (B == 1), the wgmma GEMM (B >= 96, prefill_gemm_tc5()), the mma.sync GEMM (B >= 16) or exact.cu.  Returns the number of launches (2).
+int mul_mat_exact_auto(const QWeight &w, const float *x, int64_t ldx, int64_t B, float *dst, int64_t ldd, const float *addend, int64_t lda,
+                       const ExactActs &a, cudaStream_t st);
 
 // ---- kquants.cu : Q4_K / Q5_K / Q6_K weights x Q8_K activations, bit-exact with ggml_vec_dot_q*_K_q8_K (AVX2 build) -------------------------
 size_t q8k_bytes(int64_t K, int64_t B);

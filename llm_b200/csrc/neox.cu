@@ -39,18 +39,17 @@ struct b200_neox_model {
 
 struct b200_neox_session {
     b200_neox_model *m = nullptr;
-    int n_batch = 0, n_past = 0, dev_n_past = -1, last_launches = 0, graph_nodes = 0;
+    int n_batch = 0, n_past = 0, last_launches = 0;
     __half *memory_k = nullptr, *memory_v = nullptr;            // [n_layer][n_ctx][e], [n_layer][e][n_ctx]
     int32_t *d_tokens = nullptr, *h_tokens = nullptr;
     float *x = nullptr, *cur = nullptr, *qkv = nullptr, *kq = nullptr, *attn = nullptr, *h4 = nullptr, *hact = nullptr, *t = nullptr, *logits = nullptr, *h_logits = nullptr;
     float *qdec = nullptr;
     int8_t *xq = nullptr; float2 *xds = nullptr; int4 *xpack = nullptr; __half *xh = nullptr;
     int4 *xpack_a = nullptr, *xpack_d = nullptr, *xpack_f = nullptr;
-    int *d_n_past = nullptr, *h_n_past = nullptr;
-    bool decode_ok = false, decode_warm = false;
+    bool decode_ok = false;
     std::vector<NeoxLayer> dl;
     NeoxParams dp;
-    std::vector<std::pair<int, cudaGraphExec_t>> graphs;
+    DecodeGraphCache decode;
 };
 
 bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
@@ -103,26 +102,6 @@ bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
 
 namespace {
 
-// ggml_mul_mat(w, x) for B rows: INIT-phase quantization + the bit-exact kernel for the batch size
-void matmul(b200_neox_session *s, const QWeight &w, const float *x, float *dst, int64_t ldd, int64_t B, cudaStream_t st, int &n) {
-    if (B == 1 && mmv_exact_stream_supported(w)) {
-        quantize_act_pack(w.type, x, s->xpack, w.K, st);
-        mul_mat_vec_q_exact_stream(w, s->xpack, dst, nullptr, st);
-    } else if (B >= 16) {
-        if (prefill_gemm_tc5() && B >= 96) {
-            quantize_act_f16_rm(vec_dot_type(w.type), x, w.K, s->xh, s->xds, w.K, B, st);
-            mul_mat_q_exact_tc5(w, s->xh, s->xds, dst, ldd, B, nullptr, 0, st);
-        } else {
-            quantize_act_f16(vec_dot_type(w.type), x, w.K, s->xh, s->xds, w.K, B, st);
-            mul_mat_q_exact_mma(w, s->xh, s->xds, dst, ldd, B, nullptr, 0, st);
-        }
-    } else {
-        quantize_act(vec_dot_type(w.type), x, w.K, s->xq, s->xds, w.K, B, st);
-        mul_mat_q_exact(w, s->xq, s->xds, dst, ldd, B, nullptr, 0, st);
-    }
-    n += 2;
-}
-
 void forward(b200_neox_session *s, int n, bool all_rows) {
     b200_neox_model *m = s->m;
     const b200_neox_hparams &hp = m->hp;
@@ -130,35 +109,13 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     const int e = hp.n_embd, hd = m->hd, n_head = hp.n_head, n_ctx = hp.context_size, n_past = s->n_past, n_kv = n_past + n;
     int L = 0;
     if (n == 1 && s->decode_ok) {
-        if (s->dev_n_past != n_past) {
-            B200_CHECK(cudaStreamSynchronize(st));
-            *s->h_n_past = n_past;
-            B200_CHECK(cudaMemcpyAsync(s->d_n_past, s->h_n_past, sizeof(int), cudaMemcpyHostToDevice, st));
-        }
-        int bucket = ((n_kv + 255) / 256) * 256; if (bucket > n_ctx) bucket = n_ctx;
-        int nodes = 0;
-        if (!s->decode_warm) {
-            neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, &nodes);
-            s->decode_warm = true; s->graph_nodes = nodes;
-        } else {
-            cudaGraphExec_t exec = nullptr;
-            for (auto &g : s->graphs) if (g.first == bucket) exec = g.second;
-            if (!exec) {
-                cudaGraph_t graph;
-                B200_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-                neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, &nodes);
-                B200_CHECK(cudaStreamEndCapture(st, &graph));
-                B200_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-                B200_CHECK(cudaGraphDestroy(graph));
-                s->graphs.emplace_back(bucket, exec);
-                s->graph_nodes = nodes;
-            }
-            B200_CHECK(cudaGraphLaunch(exec, st));
-        }
-        s->dev_n_past = n_past + 1;
-        s->last_launches = s->graph_nodes; s->n_past += 1;
+        s->last_launches = s->decode.run(n_kv, n_ctx, true, [s, &hp](int bucket, cudaStream_t st, int *nodes) {
+            neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
+        }, st);
+        s->n_past += 1;
         return;
     }
+    const ExactActs acts{s->xq, s->xds, s->xpack, s->xh};
     const float kq_scale = 1.0f / sqrtf((float)e / (float)n_head);                                                  // :270-273
     const bool g2 = m->gpt2(), parallel = !g2 && hp.use_parallel_residual;
     const RopeTable *rope = g2 ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, hd, n_ctx);
@@ -171,7 +128,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         const b200_neox_model::Layer &ly = m->layers[il];
         __half *Kl = s->memory_k + (size_t)il * n_ctx * e, *Vl = s->memory_v + (size_t)il * n_ctx * e;
         layer_norm(s->x, s->cur, ly.ln1_g, ly.ln1_b, e, n, st); L++;                                                  // :192-196
-        matmul(s, ly.wqkv, s->cur, s->qkv, ld3, n, st, L);                                                             // :199
+        L += mul_mat_exact_auto(ly.wqkv, s->cur, e, n, s->qkv, ld3, nullptr, 0, acts, st);                                // :199
         add_f32(s->qkv, ly.bqkv, s->qkv, (int64_t)n * ld3, ld3, st); L++;                                             // :200
         if (!g2) {   // RoPE mode 2 in place on q and k                                                                       :205-228
             rope_f32(s->qkv, s->qkv, hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
@@ -188,15 +145,15 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         soft_max(s->kq, s->kq, n_kv, (int64_t)n_head * n, n, kq_scale, true, n_past, true, true, st); L++;            // :270-279
         mul_mat_f16_exact(Vl, n_kv, hd, n_head, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2, s->kq, n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
                           s->cur, (int64_t)e * 4, (int64_t)hd * 4, -1, st); L++;                                      // :282-298
-        matmul(s, ly.wdense, s->cur, s->attn, e, n, st, L);                                                            // :301
+        L += mul_mat_exact_auto(ly.wdense, s->cur, e, n, s->attn, e, nullptr, 0, acts, st);                               // :301
         add_f32(s->attn, ly.bdense, s->attn, (int64_t)n * e, e, st); L++;                                             // :302
         const float *ff_in = s->x;
         if (!parallel) { add_f32(s->attn, s->x, s->attn, (int64_t)n * e, (int64_t)n * e, st); L++; ff_in = s->attn; }   // :308-309 / gpt2 :279
         layer_norm(ff_in, s->cur, ly.ln2_g, ly.ln2_b, e, n, st); L++;                                                 // feed_forward :487-493
-        matmul(s, ly.wfc, s->cur, s->h4, 4 * (int64_t)e, n, st, L);
+        L += mul_mat_exact_auto(ly.wfc, s->cur, e, n, s->h4, 4 * (int64_t)e, nullptr, 0, acts, st);
         add_f32(s->h4, ly.bfc, s->h4, (int64_t)n * 4 * e, 4 * (int64_t)e, st); L++;
         unary_lut(UNARY_GELU, s->h4, s->hact, (int64_t)n * 4 * e, st); L++;
-        matmul(s, ly.wproj, s->hact, s->t, e, n, st, L);
+        L += mul_mat_exact_auto(ly.wproj, s->hact, 4 * (int64_t)e, n, s->t, e, nullptr, 0, acts, st);
         add_f32(s->t, ly.bproj, s->t, (int64_t)n * e, e, st); L++;
         add_f32(s->t, s->attn, s->t, (int64_t)n * e, (int64_t)n * e, st); L++;                                        // parallel: ffn + attn; sequential: ffn + ff_in
         if (parallel) { add_f32(s->t, s->x, s->x, (int64_t)n * e, (int64_t)n * e, st); L++; }        // :324
@@ -204,11 +161,11 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     }
     if (all_rows || n == 1) {
         layer_norm(s->x, s->cur, m->lnf_g, m->lnf_b, e, n, st); L++;                                                   // :332-334
-        matmul(s, m->lm_head, s->cur, s->logits, hp.n_vocab, n, st, L);                                                // :342
+        L += mul_mat_exact_auto(m->lm_head, s->cur, e, n, s->logits, hp.n_vocab, nullptr, 0, acts, st);                   // :342
     } else {
         const size_t last = (size_t)(n - 1);
         layer_norm(s->x + last * e, s->cur + last * e, m->lnf_g, m->lnf_b, e, 1, st); L++;
-        matmul(s, m->lm_head, s->cur + last * e, s->logits + last * hp.n_vocab, hp.n_vocab, 1, st, L);
+        L += mul_mat_exact_auto(m->lm_head, s->cur + last * e, e, 1, s->logits + last * hp.n_vocab, hp.n_vocab, nullptr, 0, acts, st);
     }
     s->last_launches = L;
     s->n_past += n;
@@ -319,7 +276,6 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     B200_CHECK(cudaMalloc(&s->xpack, (4 * e / QK) * 64)); B200_CHECK(cudaMalloc(&s->xh, xh_bytes(4 * e, B)));
     B200_CHECK(cudaMalloc(&s->qdec, e * 4));
     B200_CHECK(cudaMalloc(&s->xpack_a, (e / QK) * 64)); B200_CHECK(cudaMalloc(&s->xpack_d, (e / QK) * 64)); B200_CHECK(cudaMalloc(&s->xpack_f, (4 * e / QK) * 64));
-    B200_CHECK(cudaMalloc(&s->d_n_past, sizeof(int))); B200_CHECK(cudaMallocHost(&s->h_n_past, sizeof(int)));
     const RopeTable *rt_ = m->gpt2() ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, m->hd, (int)n_ctx);
     s->dl.resize(hp.n_layer);
     for (int il = 0; il < hp.n_layer; il++) {
@@ -331,7 +287,7 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     P.n_layer = hp.n_layer; P.e = (int)e; P.hd = m->hd; P.n_head = hp.n_head; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab; P.n_rot = hp.n_rot;
     P.parallel_residual = !m->gpt2() && hp.use_parallel_residual; P.gpt2 = m->gpt2() ? 1 : 0; P.wpe = m->wpe; P.wte = m->wte; P.lm_head = m->lm_head; P.lnf_g = m->lnf_g; P.lnf_b = m->lnf_b;
     P.kq_scale = 1.0f / sqrtf((float)e / (float)hp.n_head); P.rope_cs = rt_ ? rt_->cs : nullptr; P.rope_half = rt_ ? rt_->half : 0;
-    P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens; P.n_past = s->d_n_past;
+    P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens; P.n_past = s->decode.d_n_past;
     P.x = s->x; P.qkv = s->qkv; P.q = s->qdec; P.attn_out = s->attn; P.logits = s->logits;
     P.xpack_a = s->xpack_a; P.xpack_d = s->xpack_d; P.xpack_f = s->xpack_f;
     QWeight p1; p1.nb = (int64_t)e / QK; QWeight p2; p2.nb = 4 * (int64_t)e / QK;
@@ -380,14 +336,12 @@ int b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, f
 void b200_neox_session_free(b200_neox_session *s) {
     if (!s) return;
     B200_CHECK(cudaStreamSynchronize(rt().stream));
-    for (auto &g : s->graphs) cudaGraphExecDestroy(g.second);
     void *dev[] = {s->memory_k, s->memory_v, s->d_tokens, s->x, s->cur, s->qkv, s->kq, s->attn, s->h4, s->hact, s->t, s->logits, s->xq, s->xds, s->xpack, s->xh, s->qdec,
-                   s->xpack_a, s->xpack_d, s->xpack_f, s->d_n_past};
+                   s->xpack_a, s->xpack_d, s->xpack_f};
     for (void *p : dev) if (p) B200_CHECK(cudaFree(p));
     if (s->h_tokens) B200_CHECK(cudaFreeHost(s->h_tokens));
     if (s->h_logits) B200_CHECK(cudaFreeHost(s->h_logits));
-    if (s->h_n_past) B200_CHECK(cudaFreeHost(s->h_n_past));
-    delete s;
+    delete s;                                           // the decode graphs and n_past words go with s->decode
 }
 
 }  // extern "C"

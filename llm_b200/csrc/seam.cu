@@ -3,8 +3,8 @@
 // This is the per-node, drop-in front end: the reference's graph executor (LC/ggml.c:14584-14591) calls
 // ggml_cuda_compute_forward for every node and the Rust side (crates/ggml/src/tensor.rs, accelerator/mod.rs) manages
 // buffers through transform_tensor / assign_buffers*.  Semantics follow LC/ggml-cuda.cu:3807-4135 (what the callers rely
-// on), the mechanism is ours: weights are re-laid out into 16-byte planes at upload, mat-muls run the integer-exact
-// kernels of mmvq.cu / mmq.cu, row ops run rowops.cu.  Single device per process (GGML_BACKEND_GPU_SPLIT is rejected: the
+// on), the mechanism is ours: weights are re-laid out into 16-byte planes at upload, mat-muls run the bit-exact
+// kernels mul_mat.cu picks (B200_FAST=1: those of mmvq.cu / mmq.cu), row ops run rowops.cu.  Single device per process (GGML_BACKEND_GPU_SPLIT is rejected: the
 // reference's Rust API can never produce it, crates/llm-base/src/model/mod.rs:244-250).
 #include <string.h>
 
@@ -160,33 +160,19 @@ void op_mul_mat(const ggml_tensor *src0, const ggml_tensor *src1, ggml_tensor *d
         }
         const float *x = (const float *)src_dev(src1);
         float *d = (float *)dst_dev(dst);
-        if (B == 1 && !R.fast && mmv_exact_stream_supported(w)) {      // decode: bit-exact streaming mat-vec
-            int4 *pack = (int4 *)R.op_arena.get((size_t)(K / QK) * 64, st);
-            quantize_act_pack(src0->type, x, pack, K, st);
-            mul_mat_vec_q_exact_stream(w, pack, d, nullptr, st);
-            dst_finish(dst, d);
-            return;
-        }
-        float2 *xds = (float2 *)R.op_arena.get((size_t)B * (K / QK) * sizeof(float2), st);
         const int64_t ldx = is_contiguous(src1) ? K : (int64_t)(src1->nb[1] / 4);
-        if (B >= 16 && !R.fast) {                                       // prefill: bit-exact, block dots on tensor cores
-            __half *xh = (__half *)R.op_arena.get((size_t)xh_bytes(K, B), st);
-            if (prefill_gemm_tc5() && B >= 96) {                        // wgmma / TMA kernel (exact_tc5.cu)
-                quantize_act_f16_rm(vec_dot_type(src0->type), x, ldx, xh, xds, K, B, st);
-                mul_mat_q_exact_tc5(w, xh, xds, d, N, B, nullptr, 0, st);
-            } else {
-                quantize_act_f16(vec_dot_type(src0->type), x, ldx, xh, xds, K, B, st);
-                mul_mat_q_exact_mma(w, xh, xds, d, N, B, nullptr, 0, st);
-            }
-            dst_finish(dst, d);
-            return;
-        }
         int8_t *xq = (int8_t *)R.op_arena.get((size_t)B * K, st);
-        quantize_act(vec_dot_type(src0->type), x, ldx, xq, xds, K, B, st);
-        if (!R.fast)     mul_mat_q_exact(w, xq, xds, d, N, B, nullptr, 0, st);
-        else if (B == 1) mul_mat_vec_q(w, xq, xds, d, nullptr, st);
-        else if (B < 16) mul_mat_q_simple(w, xq, xds, d, N, B, nullptr, 0, st);
-        else             mul_mat_q(w, xq, xds, d, N, B, nullptr, 0, st);
+        float2 *xds = (float2 *)R.op_arena.get((size_t)B * (K / QK) * sizeof(float2), st);
+        if (!R.fast) {
+            int4 *xpack = (int4 *)R.op_arena.get((size_t)(K / QK) * 64, st);
+            __half *xh = (__half *)R.op_arena.get(xh_bytes(K, B), st);
+            mul_mat_exact_auto(w, x, ldx, B, d, N, nullptr, 0, {xq, xds, xpack, xh}, st);
+        } else {
+            quantize_act(vec_dot_type(src0->type), x, ldx, xq, xds, K, B, st);
+            if (B == 1)      mul_mat_vec_q(w, xq, xds, d, nullptr, st);
+            else if (B < 16) mul_mat_q_simple(w, xq, xds, d, N, B, nullptr, 0, st);
+            else             mul_mat_q(w, xq, xds, d, N, B, nullptr, 0, st);
+        }
         dst_finish(dst, d);
         return;
     }

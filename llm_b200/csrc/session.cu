@@ -81,15 +81,12 @@ struct b200_session {
     // debug taps (tests): copy one intermediate buffer of (layer, stage) aside during forward()
     // one-launch-per-token decode kernel (decode.cu)
     unsigned long long *d_prof = nullptr;
-    DecodeLayer *d_layers = nullptr; unsigned int *d_bar = nullptr; int *d_n_past = nullptr; int *h_n_past = nullptr;
+    DecodeLayer *d_layers = nullptr; unsigned int *d_bar = nullptr;
     float *qbuf = nullptr, *attn = nullptr; int4 *xpack_d = nullptr, *xpack_f = nullptr;
-    int dev_n_past = -1;             // value currently held by *d_n_past (-1: unknown)
     bool mega_ok = false; int mega_grid = 0;
     std::vector<DecodeLayer> h_layers;                 // host copy of the layer table (kernel arguments of the decode graph)
     int4 *xpack_a = nullptr;
-    bool decode_warm = false;                          // first decode step runs eagerly (sets kernel attributes), later ones replay a graph
-    std::vector<std::pair<int, cudaGraphExec_t>> graphs;   // (n_kv bucket, instantiated graph)
-    int graph_nodes = 0;
+    DecodeGraphCache decode;                           // the decode graphs and the device copy of n_past they read
     DecodeParams dp;
     int tap_layer = -2, tap_stage = 0;
     float *tap = nullptr; size_t tap_cap = 0, tap_count = 0;
@@ -130,40 +127,15 @@ namespace {
 struct Launches { int n = 0; };
 }  // namespace
 void silu_mul_rows(const float *h13, float *out, int64_t f, int64_t n, cudaStream_t st);
-// B200_PREFILL_GEMM=mma selects the round-1 mma.sync kernel for every batch size (default: wgmma for batches >= 96 tokens)
-namespace b200 {
-bool prefill_gemm_tc5() {
-    static int v = -1;
-    if (v < 0) { const char *e = getenv("B200_PREFILL_GEMM"); v = (e && !strcmp(e, "mma")) ? 0 : 1; }
-    return v != 0;
-}
-}  // namespace b200
 
 namespace {
 
 // ggml_mul_mat(w, x): quantize the f32 activation rows (the INIT phase of ggml_compute_forward_mul_mat) and multiply
 void matmul(b200_session *s, const QWeight &w, const float *x, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda,
             cudaStream_t st, Launches &L, bool fast) {
-    if (B == 1 && !fast && mmv_exact_stream_supported(w)) {
-        quantize_act_pack(w.type, x, s->xpack, w.K, st);
-        mul_mat_vec_q_exact_stream(w, s->xpack, dst, addend, st);
-        L.n += 2;
-        return;
-    }
-    if (!fast && B >= 16) {                          // prefill: bit-exact, block dots on tensor cores
-        if (prefill_gemm_tc5() && B >= 96) {         // wgmma / TMA kernel: 128-token tiles (exact_tc5.cu)
-            quantize_act_f16_rm(vec_dot_type(w.type), x, w.K, s->xh, s->xds, w.K, B, st);
-            mul_mat_q_exact_tc5(w, s->xh, s->xds, dst, ldd, B, addend, lda, st);
-        } else {                                     // mma.sync kernel: 64-token tiles, better for short batches (exact_mma.cu)
-            quantize_act_f16(vec_dot_type(w.type), x, w.K, s->xh, s->xds, w.K, B, st);
-            mul_mat_q_exact_mma(w, s->xh, s->xds, dst, ldd, B, addend, lda, st);
-        }
-        L.n += 2;
-        return;
-    }
+    if (!fast) { L.n += mul_mat_exact_auto(w, x, w.K, B, dst, ldd, addend, lda, {s->xq, s->xds, s->xpack, s->xh}, st); return; }
     quantize_act(vec_dot_type(w.type), x, w.K, s->xq, s->xds, w.K, B, st);
-    if (!fast)       mul_mat_q_exact(w, s->xq, s->xds, dst, ldd, B, addend, lda, st);
-    else if (B == 1) mul_mat_vec_q(w, s->xq, s->xds, dst, addend, st);
+    if (B == 1)      mul_mat_vec_q(w, s->xq, s->xds, dst, addend, st);
     else if (B < 16) mul_mat_q_simple(w, s->xq, s->xds, dst, ldd, B, addend, lda, st);
     else if (prefill_gemm_tc5() && B >= 64) { cvt_act_f16(x, w.K, s->xh, w.K, B, st); mul_mat_q_fast_tc5(w, s->xh, dst, ldd, B, addend, lda, st); }   // fused dequant -> wgmma GEMM
     else             mul_mat_q(w, s->xq, s->xds, dst, ldd, B, addend, lda, st);
@@ -186,43 +158,21 @@ void forward(b200_session *s, int n, bool all_rows = true) {
     const bool fast = !tp && (s->cfg.flags & B200_SESSION_FAST) != 0;
     if (tp && (n != 1 || !s->tp_connected)) { fprintf(stderr, "llm_b200: tensor-parallel sessions decode one token per step, after b200_session_tp_connect\n"); exit(1); }
     if (n == 1 && s->mega_ok && !fast && (tp || (!(s->cfg.flags & B200_SESSION_UNFUSED) && s->tap_layer == -2))) {
-        if (s->dev_n_past != n_past) {                 // after a prefill / rewind the device copy of n_past is stale
-            B200_CHECK(cudaStreamSynchronize(st));      // (the pinned staging word may still be in flight)
-            *s->h_n_past = n_past;
-            B200_CHECK(cudaMemcpyAsync(s->d_n_past, s->h_n_past, sizeof(int), cudaMemcpyHostToDevice, st));
-        }
         if (!tp && (s->cfg.flags & B200_SESSION_MEGA)) {
             // experimental: the whole token in one persistent cooperative kernel (decode.cu)
+            s->decode.sync_n_past(n_past, st);
             if (launch_decode(s->dp, hp.wtype, st, &s->mega_grid)) {
-                s->dev_n_past = n_past + 1;
+                s->decode.dev_n_past = n_past + 1;      // the kernel increments it
                 s->last_launches = 1; s->last_n = 1; s->n_past += 1;
                 return;
             }
             s->mega_ok = false;
         } else {
             // default: 7 fused kernels per layer, replayed from one CUDA graph per token (decode_ops.cu)
-            int bucket = ((n_kv + 255) / 256) * 256; if (bucket > n_ctx) bucket = n_ctx;
-            int nodes = 0;
-            if (!s->decode_warm || (s->cfg.flags & B200_SESSION_NO_GRAPH)) {
-                decode_ops_enqueue(s->dp, s->h_layers, hp.wtype, bucket, s->xpack_a, st, &nodes);
-                s->decode_warm = true; s->graph_nodes = nodes;
-            } else {
-                cudaGraphExec_t exec = nullptr;
-                for (auto &g : s->graphs) if (g.first == bucket) exec = g.second;
-                if (!exec) {
-                    cudaGraph_t graph;
-                    B200_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-                    decode_ops_enqueue(s->dp, s->h_layers, hp.wtype, bucket, s->xpack_a, st, &nodes);
-                    B200_CHECK(cudaStreamEndCapture(st, &graph));
-                    B200_CHECK(cudaGraphInstantiate(&exec, graph, 0));
-                    B200_CHECK(cudaGraphDestroy(graph));
-                    s->graphs.emplace_back(bucket, exec);
-                    s->graph_nodes = nodes;
-                }
-                B200_CHECK(cudaGraphLaunch(exec, st));
-            }
-            s->dev_n_past = n_past + 1;
-            s->last_launches = s->graph_nodes; s->last_n = 1; s->n_past += 1;
+            s->last_launches = s->decode.run(n_kv, n_ctx, !(s->cfg.flags & B200_SESSION_NO_GRAPH), [s, &hp](int bucket, cudaStream_t st, int *nodes) {
+                decode_ops_enqueue(s->dp, s->h_layers, hp.wtype, bucket, s->xpack_a, st, nodes);
+            }, st);
+            s->last_n = 1; s->n_past += 1;
             return;
         }
     }
@@ -528,6 +478,18 @@ void b200_model_free(b200_model *m) {
     delete m;
 }
 
+// the layer table of the decode schedules: each layer's weights and its slice of the KV cache (gqa_loc: this rank's cache width, all of it on one GPU)
+static std::vector<DecodeLayer> decode_layers(const b200_session *s) {
+    const b200_model *m = s->m;
+    const size_t slice = (size_t)m->hp.context_size * m->gqa_loc;
+    std::vector<DecodeLayer> hl(m->hp.n_layer);
+    for (int il = 0; il < m->hp.n_layer; il++) {
+        const Layer &L = m->layers[il];
+        hl[il] = DecodeLayer{L.wqkv, L.wo, L.w13, L.w2, L.attention_norm, L.ffn_norm, s->memory_k + il * slice, s->memory_v + il * slice};
+    }
+    return hl;
+}
+
 // ---- tensor-parallel session: decode only (prompts are fed token by token), activations that cross GPUs live in ONE exchange slab -------------
 static b200_session *start_session_tp(b200_session *s) {
     b200_model *m = s->m;
@@ -548,8 +510,6 @@ static b200_session *start_session_tp(b200_session *s) {
     B200_CHECK(cudaEventCreateWithFlags(&s->tokens_uploaded, cudaEventDisableTiming));
     B200_CHECK(cudaMalloc(&s->qbuf, (size_t)m->e_loc * 4));
     B200_CHECK(cudaMalloc(&s->xpack_a, (e / QK) * 64));
-    B200_CHECK(cudaMalloc(&s->d_n_past, sizeof(int)));
-    B200_CHECK(cudaMallocHost(&s->h_n_past, sizeof(int)));
     B200_CHECK(cudaMalloc(&s->d_prof, B200_PROF_SLOTS * 8 * sizeof(unsigned long long)));
     B200_CHECK(cudaMemset(s->d_prof, 0, B200_PROF_SLOTS * 8 * sizeof(unsigned long long)));
     // the exchange slab: arrays of 8-byte {word, tag} units (tp.cuh) -- x | ff | attention records | ffn records | logits, 256-byte aligned pieces
@@ -572,22 +532,14 @@ static b200_session *start_session_tp(b200_session *s) {
     B200_CHECK(cudaMalloc(&s->logits, V * 4));                            // the gathered logits, plain f32 for the host
     s->ff = nullptr; s->xpack_d = nullptr; s->xpack_f = nullptr;
     const RopeTable &rt_ = rope_table(hp.n_rot, 0, hp.rope_freq_base, hp.rope_freq_scale, m->hd, (int)n_ctx);
-    {
-        std::vector<DecodeLayer> hl(hp.n_layer);
-        for (int il = 0; il < hp.n_layer; il++) {
-            const Layer &L = m->layers[il];
-            hl[il] = DecodeLayer{L.wqkv, L.wo, L.w13, L.w2, L.attention_norm, L.ffn_norm,
-                                 s->memory_k + (size_t)il * n_ctx * gqa, s->memory_v + (size_t)il * n_ctx * gqa};
-        }
-        s->h_layers = hl;
-    }
+    s->h_layers = decode_layers(s);
     DecodeParams &P = s->dp;
     P.layers = nullptr; P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
     P.e = (int)e; P.f = m->f_loc; P.hd = m->hd; P.gqa = m->gqa_loc; P.n_head = hp.n_head / G; P.n_head_kv = hp.n_head_kv / G; P.n_ctx = (int)n_ctx; P.n_vocab = m->v_loc;
     P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f;
     P.rope_cs = rt_.cs; P.rope_half = rt_.half;
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
-    P.token = s->d_tokens; P.n_past = s->d_n_past;
+    P.token = s->d_tokens; P.n_past = s->decode.d_n_past;
     P.x = s->x; P.q = s->qbuf; P.kq = nullptr; P.attn = nullptr; P.ff = s->ff; P.h13 = nullptr; P.logits = s->logits;
     P.xpack_d = s->xpack_d; P.xpack_f = s->xpack_f; P.bar = nullptr; P.scratch_bytes = 0;
     P.e_loc = m->e_loc; P.head0 = r * (hp.n_head / G); P.n_vocab_full = hp.n_vocab;
@@ -640,26 +592,16 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     B200_CHECK(cudaMalloc(&s->attn, e * 4));
     B200_CHECK(cudaMalloc(&s->d_bar, 2 * sizeof(unsigned int)));
     B200_CHECK(cudaMemset(s->d_bar, 0, 2 * sizeof(unsigned int)));
-    B200_CHECK(cudaMalloc(&s->d_n_past, sizeof(int)));
-    B200_CHECK(cudaMallocHost(&s->h_n_past, sizeof(int)));
-    {
-        std::vector<DecodeLayer> hl(hp.n_layer);
-        for (int il = 0; il < hp.n_layer; il++) {
-            const Layer &L = m->layers[il];
-            hl[il] = DecodeLayer{L.wqkv, L.wo, L.w13, L.w2, L.attention_norm, L.ffn_norm,
-                                 s->memory_k + (size_t)il * n_ctx * gqa, s->memory_v + (size_t)il * n_ctx * gqa};
-        }
-        s->h_layers = hl;
-        B200_CHECK(cudaMalloc(&s->d_layers, hl.size() * sizeof(DecodeLayer)));
-        B200_CHECK(cudaMemcpy(s->d_layers, hl.data(), hl.size() * sizeof(DecodeLayer), cudaMemcpyHostToDevice));
-    }
+    s->h_layers = decode_layers(s);
+    B200_CHECK(cudaMalloc(&s->d_layers, s->h_layers.size() * sizeof(DecodeLayer)));
+    B200_CHECK(cudaMemcpy(s->d_layers, s->h_layers.data(), s->h_layers.size() * sizeof(DecodeLayer), cudaMemcpyHostToDevice));
     DecodeParams &P = s->dp;
     P.layers = s->d_layers; P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
     P.e = (int)e; P.f = (int)f; P.hd = m->hd; P.gqa = m->gqa; P.n_head = hp.n_head; P.n_head_kv = hp.n_head_kv; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab;
     P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f;
     P.rope_cs = rt_.cs; P.rope_half = rt_.half;
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
-    P.token = s->d_tokens; P.n_past = s->d_n_past;
+    P.token = s->d_tokens; P.n_past = s->decode.d_n_past;
     P.x = s->x; P.q = s->qbuf; P.kq = s->kq; P.attn = s->attn; P.ff = s->ff; P.h13 = s->h13; P.logits = s->logits;
     P.bar = s->d_bar;
     B200_CHECK(cudaMalloc(&s->xpack_d, (e / QK) * 64));
@@ -832,8 +774,7 @@ int b200_session_tp_set_nowait(b200_session *s, int32_t nowait) {     // measure
     B200_CHECK(cudaStreamSynchronize(rt().stream));
     s->dp.tp.nowait = nowait < 0 ? 0 : nowait > 2 ? 2 : nowait;
     decode_set_tp(s->dp.tp, rt().stream);
-    for (auto &g : s->graphs) cudaGraphExecDestroy(g.second);
-    s->graphs.clear();
+    s->decode.drop();
     return B200_OK;
 }
 int32_t b200_session_tp_timeouts(b200_session *s) {      // number of flag waits that gave up (a peer stopped): must be 0
@@ -847,19 +788,17 @@ int32_t b200_session_tp_timeouts(b200_session *s) {      // number of flag waits
 void b200_session_free(b200_session *s) {
     if (!s) return;
     B200_CHECK(cudaStreamSynchronize(rt().stream));
-    if (s->h_n_past) B200_CHECK(cudaFreeHost(s->h_n_past));
-    for (auto &g : s->graphs) cudaGraphExecDestroy(g.second);
     if (s->tp_slab) {                                    // tensor-parallel session: the exchange slab and the peers' mappings
         for (int p = 0; p < TP_MAX; p++) if (s->tp_peer_map[p]) cudaIpcCloseMemHandle(s->tp_peer_map[p]);
         B200_CHECK(cudaFree(s->tp_slab)); B200_CHECK(cudaFree(s->tp_state));
     }
-    void *dev[] = {s->xpack_a, s->xpack_d, s->xpack_f, s->d_prof, s->d_layers, s->d_bar, s->d_n_past, s->qbuf, s->attn, s->tap, s->memory_k, s->memory_v, s->d_tokens, s->x, s->cur, s->ff, s->qkv, s->kq, s->h13, s->hmul, s->logits, s->xq, s->xds, s->xpack, s->xh, s->topk};
+    void *dev[] = {s->xpack_a, s->xpack_d, s->xpack_f, s->d_prof, s->d_layers, s->d_bar, s->qbuf, s->attn, s->tap, s->memory_k, s->memory_v, s->d_tokens, s->x, s->cur, s->ff, s->qkv, s->kq, s->h13, s->hmul, s->logits, s->xq, s->xds, s->xpack, s->xh, s->topk};
     for (void *p : dev) if (p) B200_CHECK(cudaFree(p));
     if (s->h_tokens) B200_CHECK(cudaFreeHost(s->h_tokens));
     if (s->h_logits) B200_CHECK(cudaFreeHost(s->h_logits));
     if (s->h_topk) B200_CHECK(cudaFreeHost(s->h_topk));
     if (s->tokens_uploaded) B200_CHECK(cudaEventDestroy(s->tokens_uploaded));
-    delete s;
+    delete s;                                           // the decode graphs and n_past words go with s->decode
 }
 
 // ---- single-op entry points on host buffers ---------------------------------------------------------------------------------
