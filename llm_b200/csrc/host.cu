@@ -1,0 +1,106 @@
+// llm_b200/csrc/host.cu -- tensor slots and session state shared by the LLaMA and GPT-NeoX / GPT-2 runtimes (host.h)
+#include <string.h>
+
+#include "../../include/llm_b200.h"
+#include "host.h"
+
+namespace b200 {
+
+QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows) {
+    QWeight v = w;
+    v.N = nrows;
+    v.qs = w.qs + (size_t)row0 * w.nb * qs_bytes(w.type);
+    if (w.qh) v.qh = w.qh + (size_t)row0 * w.nb;
+    v.dm = (const uint8_t *)w.dm + (size_t)row0 * w.nb * (has_min(w.type) ? 4 : 2);
+    v.base = nullptr;
+    return v;
+}
+
+int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes) {
+    Runtime &R = rt();
+    if (s.is_q) {
+        if (type != s.q.type || nbytes != s.bytes()) return B200_ERR_TENSOR_SHAPE;
+        R.op_arena.reset();
+        void *raw = R.op_arena.get(nbytes, R.stream);
+        B200_CHECK(cudaMemcpyAsync(raw, host, nbytes, cudaMemcpyHostToDevice, R.stream));
+        if (!s.chunk) repack_weights(s.q, raw, R.stream);
+        else {
+            const size_t piece = (size_t)s.chunk * s.q.nb * ggml_block_bytes(type);
+            for (int64_t c = 0; c * s.chunk < s.rows; c++)
+                repack_weights(row_view(s.q, c * s.stride + s.row0, s.chunk), (const char *)raw + c * piece, R.stream);
+        }
+        B200_CHECK(cudaStreamSynchronize(R.stream));
+    } else {
+        if (type != T_F32 || nbytes != s.bytes()) return B200_ERR_TENSOR_SHAPE;
+        B200_CHECK(cudaMemcpy(s.f, host, nbytes, cudaMemcpyHostToDevice));
+        B200_CHECK(cudaDeviceSynchronize());   // legacy-stream copy/memset: not ordered with our non-blocking stream, and a pageable H2D cudaMemcpy may return before its DMA lands
+    }
+    return B200_OK;
+}
+
+int read_slot(const Slot &s, void *host, size_t nbytes) {
+    Runtime &R = rt();
+    if (nbytes != s.bytes()) return B200_ERR_TENSOR_SHAPE;
+    if (s.is_q) {
+        R.op_arena.reset();
+        void *raw = R.op_arena.get(nbytes, R.stream);
+        if (!s.chunk) unpack_weights(s.q, raw, R.stream);
+        else {
+            const size_t piece = (size_t)s.chunk * s.q.nb * ggml_block_bytes(s.q.type);
+            for (int64_t c = 0; c * s.chunk < s.rows; c++)
+                unpack_weights(row_view(s.q, c * s.stride + s.row0, s.chunk), (char *)raw + c * piece, R.stream);
+        }
+        B200_CHECK(cudaMemcpyAsync(host, raw, nbytes, cudaMemcpyDeviceToHost, R.stream));
+        B200_CHECK(cudaStreamSynchronize(R.stream));
+    } else {
+        B200_CHECK(cudaStreamSynchronize(R.stream));
+        B200_CHECK(cudaMemcpy(host, s.f, nbytes, cudaMemcpyDeviceToHost));
+    }
+    return B200_OK;
+}
+
+void SessionCore::start(int n_batch_, int n_ctx_, int n_vocab_, size_t kv_elems) {
+    n_batch = n_batch_; n_ctx = n_ctx_; n_vocab = n_vocab_;
+    memory_k = device_zeros<__half>(kv_elems * 2);              // offload_no_scratch zero-fills (LC/ggml-cuda.cu:3967-3973)
+    memory_v = device_zeros<__half>(kv_elems * 2);
+    d_tokens = device_alloc<int32_t>((size_t)n_batch * 4);
+    h_tokens = pinned_alloc<int32_t>((size_t)n_batch * 4);
+    h_logits = pinned_alloc<float>((size_t)n_batch * n_vocab * 4);
+    cudaEvent_t ev;
+    B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    tokens_uploaded.reset(ev);
+}
+
+int SessionCore::admit(int n) const {
+    if (n < 1 || n > n_batch) return B200_ERR_BAD_ARG;
+    if (n_past + n > n_ctx) return B200_ERR_CONTEXT_FULL;
+    return B200_OK;
+}
+
+int SessionCore::stage_tokens(const int32_t *tokens, int n) {
+    for (int i = 0; i < n; i++) if (tokens[i] < 0 || tokens[i] >= n_vocab) return B200_ERR_BAD_ARG;
+    cudaStream_t st = rt().stream;
+    B200_CHECK(cudaEventSynchronize(tokens_uploaded.get()));   // the previous (feed-only) call may still be reading the staging buffer
+    memcpy(h_tokens.get(), tokens, (size_t)n * 4);
+    B200_CHECK(cudaMemcpyAsync(d_tokens.get(), h_tokens.get(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaEventRecord(tokens_uploaded.get(), st));
+    return B200_OK;
+}
+
+void SessionCore::copy_logits(float *out, const float *logits, int n, bool all_rows) {
+    if (!out) return;
+    cudaStream_t st = rt().stream;
+    const size_t V = n_vocab, rows = all_rows ? n : 1;
+    const float *src = all_rows ? logits : logits + (size_t)(n - 1) * V;
+    B200_CHECK(cudaMemcpyAsync(h_logits.get(), src, rows * V * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    memcpy(out, h_logits.get(), rows * V * 4);
+}
+
+int SessionCore::set_n_past(int v) {
+    if (v < 0 || v > n_past) return B200_ERR_BAD_ARG;
+    n_past = v;
+    return B200_OK;
+}
+
+}  // namespace b200

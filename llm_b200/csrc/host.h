@@ -1,0 +1,109 @@
+// llm_b200/csrc/host.h -- host plumbing shared by the LLaMA (session.cu) and GPT-NeoX / GPT-2 (neox.cu) runtimes: owned device and pinned
+// buffers, the weight slab and its named tensor slots, seeded synthesis, and the state every session keeps (KV cache, token / logits staging).
+#pragma once
+#include <memory>
+#include <type_traits>
+#include <vector>
+
+#include "decode.h"
+#include "kernels.cuh"
+#include "runtime.h"
+
+namespace b200 {
+
+// ---- owned allocations: one cudaMalloc / cudaMallocHost / event each, released with the struct that holds the handle ---------------
+struct DeviceFree { void operator()(void *p) const { B200_CHECK(cudaFree(p)); } };
+struct PinnedFree { void operator()(void *p) const { B200_CHECK(cudaFreeHost(p)); } };
+struct EventDestroy { void operator()(cudaEvent_t e) const { B200_CHECK(cudaEventDestroy(e)); } };
+template <class T> using DeviceBuf = std::unique_ptr<T, DeviceFree>;
+template <class T> using PinnedBuf = std::unique_ptr<T, PinnedFree>;
+using Event = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDestroy>;
+
+template <class T> DeviceBuf<T> device_alloc(size_t bytes) { void *p = nullptr; B200_CHECK(cudaMalloc(&p, bytes)); return DeviceBuf<T>((T *)p); }
+// the memset runs on the legacy stream: the caller orders it before the backend's non-blocking stream (cudaDeviceSynchronize)
+template <class T> DeviceBuf<T> device_zeros(size_t bytes) { DeviceBuf<T> b = device_alloc<T>(bytes); B200_CHECK(cudaMemset(b.get(), 0, bytes)); return b; }
+template <class T> PinnedBuf<T> pinned_alloc(size_t bytes) { void *p = nullptr; B200_CHECK(cudaMallocHost(&p, bytes)); return PinnedBuf<T>((T *)p); }
+
+QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows);   // rows [row0, row0+nrows) of a planes matrix
+
+// ---- the weights of one model -------------------------------------------------------------------------------------------------
+// One pass over a model's tensors in slab order: the sizing pass (base == nullptr) only advances `off`, the placing pass also points each tensor
+// into the slab. Quantized matrices take qweight_layout's bytes, f32 vectors are padded to 256 bytes.
+struct SlabCarver {
+    int wtype; char *base;
+    size_t off = 0, streamed = 0;       // streamed: GGML bytes of every matrix carved
+    void q(QWeight &w, int64_t K, int64_t N) {
+        off += qweight_layout(w, wtype, K, N, base ? base + off : nullptr);
+        streamed += (size_t)N * (K / QK) * ggml_block_bytes(wtype);
+    }
+    void f(float *&p, int64_t n) { if (base) p = (float *)(base + off); off += ((size_t)n * 4 + 255) & ~(size_t)255; }
+};
+
+// The k-th tensor drawn gets seed + 0x1000003 * k, so a model's synthetic weights depend on the order of the draws.
+struct SeedSeq {
+    uint64_t seed; cudaStream_t st; uint64_t id = 0;
+    uint64_t next() { return seed + 0x1000003ull * (++id); }
+    void q(const QWeight &w) { synth_qweight(w, next(), st); }                       // N(0, 1/K) quantized by the reference's rule
+    void gain(float *p, int64_t n) { synth_gain(p, n, next(), st); }                 // 1 + 0.1 N(0,1)
+    void bias(float *p, int64_t n) { synth_gain(p, n, next(), st); scale_shift_f32(p, n, 0.1f, -0.1f, st); }   // 0.01 N(0,1)
+};
+
+// One HBM slab holding every weight, and which of the model's named tensors have been loaded into it.
+struct Weights {
+    DeviceBuf<char> slab;
+    size_t slab_bytes = 0, weight_bytes = 0;    // weight_bytes: what one forward pass streams (the front end takes out the gathered-only embedding)
+    std::vector<uint8_t> loaded;                // per tensor slot
+    int n_loaded = 0;
+
+    // layout(SlabCarver &) carves the tensors: run once to size the slab, then once more to place them in it
+    template <class Layout> void carve(int wtype, int n_slots, Layout &&layout) {
+        SlabCarver size{wtype, nullptr};
+        layout(size);
+        slab_bytes = size.off;
+        slab = device_alloc<char>(slab_bytes);
+        SlabCarver place{wtype, slab.get()};
+        layout(place);
+        weight_bytes = place.streamed;
+        loaded.assign(n_slots, 0);
+    }
+    void mark(int id) { if (!loaded[id]) { loaded[id] = 1; n_loaded++; } }
+    bool all_loaded() const { return n_loaded == (int)loaded.size(); }
+    // seeded synthetic weights generated in HBM (bench): draw(SeedSeq &) fills every tensor
+    template <class Draw> void synthesize(uint64_t seed, Draw &&draw) {
+        SeedSeq seq{seed, rt().stream};
+        draw(seq);
+        B200_CHECK(cudaStreamSynchronize(rt().stream));
+        loaded.assign(loaded.size(), 1);
+        n_loaded = (int)loaded.size();
+    }
+};
+
+// Where a named tensor lives in the slab: a quantized matrix `q` or `n` floats at `f`.
+// chunk > 0: the tensor's rows live in `chunk`-row pieces, piece c at rows [c * stride + row0, + chunk) of the matrix `q`
+// (LLaMA's w1 / w3 are interleaved in 32-row pieces inside w13 so that 64 consecutive rows hold both factors of 32 silu*mul outputs)
+struct Slot {
+    QWeight q; float *f = nullptr; int64_t n = 0; bool is_q = false; int chunk = 0; int64_t row0 = 0, stride = 0, rows = 0;
+    int64_t q_rows() const { return chunk ? rows : q.N; }
+    size_t bytes() const { return is_q ? (size_t)q_rows() * q.nb * ggml_block_bytes(q.type) : (size_t)n * 4; }
+};
+int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes);   // GGML blocks (repacked on the GPU) or f32; B200_OK / B200_ERR_TENSOR_SHAPE
+int read_slot(const Slot &s, void *host, size_t nbytes);                       // the inverse: GGML blocks or f32 back to the host
+
+// ---- what every session keeps: the f16 KV cache, the position, token and logits staging, the decode graphs -------------------------
+struct SessionCore {
+    int n_batch = 0, n_ctx = 0, n_vocab = 0;
+    int n_past = 0, last_launches = 0;
+    DeviceBuf<__half> memory_k, memory_v;
+    DeviceBuf<int32_t> d_tokens; PinnedBuf<int32_t> h_tokens;
+    PinnedBuf<float> h_logits;          // n_batch rows of n_vocab
+    Event tokens_uploaded;              // guards reuse of h_tokens by the next evaluate()
+    DecodeGraphCache decode;            // the decode graphs and the device copy of n_past they read
+
+    void start(int n_batch, int n_ctx, int n_vocab, size_t kv_elems);   // zero-filled KV cache of kv_elems f16 values each for K and V
+    int admit(int n) const;             // B200_ERR_BAD_ARG unless 1 <= n <= n_batch, B200_ERR_CONTEXT_FULL if n more positions do not fit
+    int stage_tokens(const int32_t *tokens, int n);   // validates the ids and uploads them to d_tokens
+    void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)
+    int set_n_past(int v);
+};
+
+}  // namespace b200

@@ -14,42 +14,31 @@
 #include <vector>
 
 #include "../../include/llm_b200.h"
-#include "decode.h"
-#include "kernels.cuh"
-#include "runtime.h"
+#include "host.h"
 
 using namespace b200;
 
-struct b200_neox_model {
+struct b200_neox_model : Weights {
     b200_neox_hparams hp;
     int hd = 0;
-    char *slab = nullptr;
-    size_t slab_bytes = 0, weight_bytes = 0;
     QWeight wte, lm_head;
     float *lnf_g = nullptr, *lnf_b = nullptr, *wpe = nullptr;     // wpe: GPT-2 learned positions [n_ctx][e] f32
     bool gpt2() const { return hp.arch == 1; }
     struct Layer { QWeight wqkv, wdense, wfc, wproj; float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj; };
     std::vector<Layer> layers;
-    std::vector<uint8_t> loaded;
-    int n_loaded = 0;
     int n_slots() const { return 4 + 12 * hp.n_layer + (gpt2() && hp.has_lm_head ? 1 : 0); }   // GPT-2: slot 3 = wpe, lm_head (if present) last
-    struct Slot { QWeight q; float *f = nullptr; int64_t n = 0; bool is_q = false; };
     bool lookup(const char *name, Slot &s, int &id);
 };
 
-struct b200_neox_session {
+struct b200_neox_session : SessionCore {   // memory_k [n_layer][n_ctx][e], memory_v [n_layer][e][n_ctx]
     b200_neox_model *m = nullptr;
-    int n_batch = 0, n_past = 0, last_launches = 0;
-    __half *memory_k = nullptr, *memory_v = nullptr;            // [n_layer][n_ctx][e], [n_layer][e][n_ctx]
-    int32_t *d_tokens = nullptr, *h_tokens = nullptr;
-    float *x = nullptr, *cur = nullptr, *qkv = nullptr, *kq = nullptr, *attn = nullptr, *h4 = nullptr, *hact = nullptr, *t = nullptr, *logits = nullptr, *h_logits = nullptr;
-    float *qdec = nullptr;
-    int8_t *xq = nullptr; float2 *xds = nullptr; int4 *xpack = nullptr; __half *xh = nullptr;
-    int4 *xpack_a = nullptr, *xpack_d = nullptr, *xpack_f = nullptr;
+    DeviceBuf<float> x, cur, qkv, kq, attn, h4, hact, t, logits;
+    DeviceBuf<float> qdec;
+    DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh;
+    DeviceBuf<int4> xpack_a, xpack_d, xpack_f;
     bool decode_ok = false;
     std::vector<NeoxLayer> dl;
     NeoxParams dp;
-    DecodeGraphCache decode;
 };
 
 bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
@@ -115,57 +104,57 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         s->n_past += 1;
         return;
     }
-    const ExactActs acts{s->xq, s->xds, s->xpack, s->xh};
+    const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()};
     const float kq_scale = 1.0f / sqrtf((float)e / (float)n_head);                                                  // :270-273
     const bool g2 = m->gpt2(), parallel = !g2 && hp.use_parallel_residual;
     const RopeTable *rope = g2 ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, hd, n_ctx);
     const int64_t ld3 = 3 * (int64_t)e;
     // where q / k / v of head h live inside a row of the fused projection: NeoX per head [q | k | v], GPT-2 the three thirds of the row
     const int64_t hs = g2 ? hd : 3 * hd, koff = g2 ? e : hd, voff = g2 ? 2 * (int64_t)e : 2 * hd;
-    get_rows_q(m->wte, s->d_tokens, s->x, n, st); L++;                                                               // :178
-    if (g2) { add_f32(s->x, m->wpe + (size_t)n_past * e, s->x, (int64_t)n * e, (int64_t)n * e, st); L++; }             // gpt2 lib.rs:164-172: + wpe[n_past + i]
+    get_rows_q(m->wte, s->d_tokens.get(), s->x.get(), n, st); L++;                                                               // :178
+    if (g2) { add_f32(s->x.get(), m->wpe + (size_t)n_past * e, s->x.get(), (int64_t)n * e, (int64_t)n * e, st); L++; }             // gpt2 lib.rs:164-172: + wpe[n_past + i]
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &ly = m->layers[il];
-        __half *Kl = s->memory_k + (size_t)il * n_ctx * e, *Vl = s->memory_v + (size_t)il * n_ctx * e;
-        layer_norm(s->x, s->cur, ly.ln1_g, ly.ln1_b, e, n, st); L++;                                                  // :192-196
-        L += mul_mat_exact_auto(ly.wqkv, s->cur, e, n, s->qkv, ld3, nullptr, 0, acts, st);                                // :199
-        add_f32(s->qkv, ly.bqkv, s->qkv, (int64_t)n * ld3, ld3, st); L++;                                             // :200
+        __half *Kl = s->memory_k.get() + (size_t)il * n_ctx * e, *Vl = s->memory_v.get() + (size_t)il * n_ctx * e;
+        layer_norm(s->x.get(), s->cur.get(), ly.ln1_g, ly.ln1_b, e, n, st); L++;                                                  // :192-196
+        L += mul_mat_exact_auto(ly.wqkv, s->cur.get(), e, n, s->qkv.get(), ld3, nullptr, 0, acts, st);                                // :199
+        add_f32(s->qkv.get(), ly.bqkv, s->qkv.get(), (int64_t)n * ld3, ld3, st); L++;                                             // :200
         if (!g2) {   // RoPE mode 2 in place on q and k                                                                       :205-228
-            rope_f32(s->qkv, s->qkv, hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
-            rope_f32(s->qkv + koff, s->qkv + koff, hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
+            rope_f32(s->qkv.get(), s->qkv.get(), hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
+            rope_f32(s->qkv.get() + koff, s->qkv.get() + koff, hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
         }
         {   // k -> cache rows n_past.., v -> cache columns (transposed; GPT-2's v_trans copy of every evaluate is this layout)       :231-247
             StridedDesc sk{{hd, n_head, n, 1}, {4, hs * 4, ld3 * 4, 0}}, dk{{hd, n_head, n, 1}, {2, (int64_t)hd * 2, (int64_t)e * 2, 0}};
-            cpy_strided(s->qkv + koff, T_F32, sk, Kl + (size_t)n_past * e, T_F16, dk, st); L++;
+            cpy_strided(s->qkv.get() + koff, T_F32, sk, Kl + (size_t)n_past * e, T_F16, dk, st); L++;
             StridedDesc dv{{hd, n_head, n, 1}, {(int64_t)n_ctx * 2, (int64_t)hd * n_ctx * 2, 2, 0}};
-            cpy_strided(s->qkv + voff, T_F32, sk, Vl + n_past, T_F16, dv, st); L++;
+            cpy_strided(s->qkv.get() + voff, T_F32, sk, Vl + n_past, T_F16, dv, st); L++;
         }
-        mul_mat_f16_exact(Kl, hd, n_kv, n_head, (int64_t)e * 2, (int64_t)hd * 2, s->qkv, n, n_head, ld3 * 4, hs * 4,
-                          s->kq, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st); L++;                          // :250-267
-        soft_max(s->kq, s->kq, n_kv, (int64_t)n_head * n, n, kq_scale, true, n_past, true, true, st); L++;            // :270-279
-        mul_mat_f16_exact(Vl, n_kv, hd, n_head, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2, s->kq, n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
-                          s->cur, (int64_t)e * 4, (int64_t)hd * 4, -1, st); L++;                                      // :282-298
-        L += mul_mat_exact_auto(ly.wdense, s->cur, e, n, s->attn, e, nullptr, 0, acts, st);                               // :301
-        add_f32(s->attn, ly.bdense, s->attn, (int64_t)n * e, e, st); L++;                                             // :302
-        const float *ff_in = s->x;
-        if (!parallel) { add_f32(s->attn, s->x, s->attn, (int64_t)n * e, (int64_t)n * e, st); L++; ff_in = s->attn; }   // :308-309 / gpt2 :279
-        layer_norm(ff_in, s->cur, ly.ln2_g, ly.ln2_b, e, n, st); L++;                                                 // feed_forward :487-493
-        L += mul_mat_exact_auto(ly.wfc, s->cur, e, n, s->h4, 4 * (int64_t)e, nullptr, 0, acts, st);
-        add_f32(s->h4, ly.bfc, s->h4, (int64_t)n * 4 * e, 4 * (int64_t)e, st); L++;
-        unary_lut(UNARY_GELU, s->h4, s->hact, (int64_t)n * 4 * e, st); L++;
-        L += mul_mat_exact_auto(ly.wproj, s->hact, 4 * (int64_t)e, n, s->t, e, nullptr, 0, acts, st);
-        add_f32(s->t, ly.bproj, s->t, (int64_t)n * e, e, st); L++;
-        add_f32(s->t, s->attn, s->t, (int64_t)n * e, (int64_t)n * e, st); L++;                                        // parallel: ffn + attn; sequential: ffn + ff_in
-        if (parallel) { add_f32(s->t, s->x, s->x, (int64_t)n * e, (int64_t)n * e, st); L++; }        // :324
-        else { B200_CHECK(cudaMemcpyAsync(s->x, s->t, (size_t)n * e * 4, cudaMemcpyDeviceToDevice, st)); }
+        mul_mat_f16_exact(Kl, hd, n_kv, n_head, (int64_t)e * 2, (int64_t)hd * 2, s->qkv.get(), n, n_head, ld3 * 4, hs * 4,
+                          s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st); L++;                          // :250-267
+        soft_max(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, kq_scale, true, n_past, true, true, st); L++;            // :270-279
+        mul_mat_f16_exact(Vl, n_kv, hd, n_head, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2, s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
+                          s->cur.get(), (int64_t)e * 4, (int64_t)hd * 4, -1, st); L++;                                      // :282-298
+        L += mul_mat_exact_auto(ly.wdense, s->cur.get(), e, n, s->attn.get(), e, nullptr, 0, acts, st);                               // :301
+        add_f32(s->attn.get(), ly.bdense, s->attn.get(), (int64_t)n * e, e, st); L++;                                             // :302
+        const float *ff_in = s->x.get();
+        if (!parallel) { add_f32(s->attn.get(), s->x.get(), s->attn.get(), (int64_t)n * e, (int64_t)n * e, st); L++; ff_in = s->attn.get(); }   // :308-309 / gpt2 :279
+        layer_norm(ff_in, s->cur.get(), ly.ln2_g, ly.ln2_b, e, n, st); L++;                                                 // feed_forward :487-493
+        L += mul_mat_exact_auto(ly.wfc, s->cur.get(), e, n, s->h4.get(), 4 * (int64_t)e, nullptr, 0, acts, st);
+        add_f32(s->h4.get(), ly.bfc, s->h4.get(), (int64_t)n * 4 * e, 4 * (int64_t)e, st); L++;
+        unary_lut(UNARY_GELU, s->h4.get(), s->hact.get(), (int64_t)n * 4 * e, st); L++;
+        L += mul_mat_exact_auto(ly.wproj, s->hact.get(), 4 * (int64_t)e, n, s->t.get(), e, nullptr, 0, acts, st);
+        add_f32(s->t.get(), ly.bproj, s->t.get(), (int64_t)n * e, e, st); L++;
+        add_f32(s->t.get(), s->attn.get(), s->t.get(), (int64_t)n * e, (int64_t)n * e, st); L++;                                        // parallel: ffn + attn; sequential: ffn + ff_in
+        if (parallel) { add_f32(s->t.get(), s->x.get(), s->x.get(), (int64_t)n * e, (int64_t)n * e, st); L++; }        // :324
+        else { B200_CHECK(cudaMemcpyAsync(s->x.get(), s->t.get(), (size_t)n * e * 4, cudaMemcpyDeviceToDevice, st)); }
     }
     if (all_rows || n == 1) {
-        layer_norm(s->x, s->cur, m->lnf_g, m->lnf_b, e, n, st); L++;                                                   // :332-334
-        L += mul_mat_exact_auto(m->lm_head, s->cur, e, n, s->logits, hp.n_vocab, nullptr, 0, acts, st);                   // :342
+        layer_norm(s->x.get(), s->cur.get(), m->lnf_g, m->lnf_b, e, n, st); L++;                                                   // :332-334
+        L += mul_mat_exact_auto(m->lm_head, s->cur.get(), e, n, s->logits.get(), hp.n_vocab, nullptr, 0, acts, st);                   // :342
     } else {
         const size_t last = (size_t)(n - 1);
-        layer_norm(s->x + last * e, s->cur + last * e, m->lnf_g, m->lnf_b, e, 1, st); L++;
-        L += mul_mat_exact_auto(m->lm_head, s->cur + last * e, e, 1, s->logits + last * hp.n_vocab, hp.n_vocab, nullptr, 0, acts, st);
+        layer_norm(s->x.get() + last * e, s->cur.get() + last * e, m->lnf_g, m->lnf_b, e, 1, st); L++;
+        L += mul_mat_exact_auto(m->lm_head, s->cur.get() + last * e, e, 1, s->logits.get() + last * hp.n_vocab, hp.n_vocab, nullptr, 0, acts, st);
     }
     s->last_launches = L;
     s->n_past += n;
@@ -184,26 +173,18 @@ b200_neox_model *b200_neox_new(const b200_neox_hparams *hp) {
     const int e = hp->n_embd, v = hp->n_vocab, t = hp->wtype;
     m->hd = e / hp->n_head;
     m->layers.resize(hp->n_layer);
-    for (int pass = 0; pass < 2; pass++) {
-        size_t off = 0;
-        auto cq = [&](QWeight &w, int64_t K, int64_t N) {
-            off += qweight_layout(w, t, K, N, pass ? m->slab + off : nullptr);
-            if (pass) m->weight_bytes += (size_t)N * (K / QK) * ggml_block_bytes(t);
-        };
-        auto cf = [&](float *&p, int64_t n) { if (pass) p = (float *)(m->slab + off); off += ((size_t)n * 4 + 255) & ~(size_t)255; };
-        cq(m->wte, e, v);
-        if (!m->gpt2() || hp->has_lm_head) cq(m->lm_head, e, v);
-        cf(m->lnf_g, e); cf(m->lnf_b, e);
-        if (m->gpt2()) cf(m->wpe, (int64_t)hp->context_size * e);
+    m->carve(t, m->n_slots(), [m, hp, e, v](SlabCarver &c) {
+        c.q(m->wte, e, v);
+        if (!m->gpt2() || hp->has_lm_head) c.q(m->lm_head, e, v);
+        c.f(m->lnf_g, e); c.f(m->lnf_b, e);
+        if (m->gpt2()) c.f(m->wpe, (int64_t)hp->context_size * e);
         for (auto &L : m->layers) {
-            cf(L.ln1_g, e); cf(L.ln1_b, e); cf(L.ln2_g, e); cf(L.ln2_b, e); cf(L.bqkv, 3 * e); cf(L.bdense, e); cf(L.bfc, 4 * e); cf(L.bproj, e);
-            cq(L.wqkv, e, 3 * e); cq(L.wdense, e, e); cq(L.wfc, e, 4 * e); cq(L.wproj, 4 * e, e);
+            c.f(L.ln1_g, e); c.f(L.ln1_b, e); c.f(L.ln2_g, e); c.f(L.ln2_b, e); c.f(L.bqkv, 3 * e); c.f(L.bdense, e); c.f(L.bfc, 4 * e); c.f(L.bproj, e);
+            c.q(L.wqkv, e, 3 * e); c.q(L.wdense, e, e); c.q(L.wfc, e, 4 * e); c.q(L.wproj, 4 * e, e);
         }
-        if (!pass) { m->slab_bytes = off; B200_CHECK(cudaMalloc(&m->slab, off)); }
-    }
+    });
     if (m->gpt2() && !hp->has_lm_head) m->lm_head = m->wte;              // tied output projection (gpt2 lib.rs:319-320): wte is streamed as the lm_head
     else m->weight_bytes -= (size_t)v * (e / QK) * ggml_block_bytes(t);  // the embedding table is gathered from, not streamed
-    m->loaded.assign(m->n_slots(), 0);
     return m;
 }
 
@@ -211,85 +192,64 @@ size_t b200_neox_weight_bytes(b200_neox_model *m) { return m ? m->weight_bytes :
 
 int b200_neox_load_tensor(b200_neox_model *m, const char *name, int32_t type, const void *host_data, size_t nbytes) {
     if (!m || !name || !host_data) return B200_ERR_BAD_ARG;
-    b200_neox_model::Slot s; int id;
+    Slot s; int id;
     if (!m->lookup(name, s, id)) return B200_ERR_UNKNOWN_TENSOR;
-    Runtime &R = rt();
-    if (s.is_q) {
-        if (type != s.q.type || nbytes != (size_t)s.q.N * s.q.nb * ggml_block_bytes(type)) return B200_ERR_TENSOR_SHAPE;
-        R.op_arena.reset();
-        void *raw = R.op_arena.get(nbytes, R.stream);
-        B200_CHECK(cudaMemcpyAsync(raw, host_data, nbytes, cudaMemcpyHostToDevice, R.stream));
-        repack_weights(s.q, raw, R.stream);
-        B200_CHECK(cudaStreamSynchronize(R.stream));
-    } else {
-        if (type != T_F32 || nbytes != (size_t)s.n * 4) return B200_ERR_TENSOR_SHAPE;
-        B200_CHECK(cudaMemcpy(s.f, host_data, nbytes, cudaMemcpyHostToDevice));
-        B200_CHECK(cudaDeviceSynchronize());
-    }
-    if (!m->loaded[id]) { m->loaded[id] = 1; m->n_loaded++; }
-    return B200_OK;
+    const int rc = load_slot(s, type, host_data, nbytes);
+    if (rc == B200_OK) m->mark(id);
+    return rc;
 }
 
-// seeded synthetic weights generated in HBM (bench): N(0, 1/K) quantized by the reference's rule, LayerNorm gains 1 + 0.1 N(0,1), biases = gains - 1 (small)
+// seeded synthetic weights generated in HBM (bench): LayerNorm gains 1 + 0.1 N(0,1), biases = gains - 1 (small)
 int b200_neox_synthesize(b200_neox_model *m, uint64_t seed) {
     if (!m) return B200_ERR_BAD_ARG;
-    cudaStream_t st = rt().stream;
-    uint64_t id = 0;
-    auto q = [&](const QWeight &w) { synth_qweight(w, seed + 0x1000003ull * (++id), st); };
-    auto g = [&](float *p, int64_t n) { synth_gain(p, n, seed + 0x1000003ull * (++id), st); };
-    auto b = [&](float *p, int64_t n) { synth_gain(p, n, seed + 0x1000003ull * (++id), st); scale_shift_f32(p, n, 0.1f, -0.1f, st); };   // 0.01 N(0,1)
-    const int e = m->hp.n_embd;
-    q(m->wte); if (!m->gpt2() || m->hp.has_lm_head) q(m->lm_head); g(m->lnf_g, e); b(m->lnf_b, e);
-    if (m->gpt2()) b(m->wpe, (int64_t)m->hp.context_size * e);
-    for (auto &L : m->layers) {
-        g(L.ln1_g, e); b(L.ln1_b, e); g(L.ln2_g, e); b(L.ln2_b, e); b(L.bqkv, 3 * e); b(L.bdense, e); b(L.bfc, 4 * e); b(L.bproj, e);
-        q(L.wqkv); q(L.wdense); q(L.wfc); q(L.wproj);
-    }
-    B200_CHECK(cudaStreamSynchronize(st));
-    m->loaded.assign(m->n_slots(), 1); m->n_loaded = m->n_slots();
+    const int64_t e = m->hp.n_embd;
+    m->synthesize(seed, [m, e](SeedSeq &r) {
+        r.q(m->wte); if (!m->gpt2() || m->hp.has_lm_head) r.q(m->lm_head); r.gain(m->lnf_g, e); r.bias(m->lnf_b, e);
+        if (m->gpt2()) r.bias(m->wpe, (int64_t)m->hp.context_size * e);
+        for (auto &L : m->layers) {
+            r.gain(L.ln1_g, e); r.bias(L.ln1_b, e); r.gain(L.ln2_g, e); r.bias(L.ln2_b, e); r.bias(L.bqkv, 3 * e); r.bias(L.bdense, e); r.bias(L.bfc, 4 * e); r.bias(L.bproj, e);
+            r.q(L.wqkv); r.q(L.wdense); r.q(L.wfc); r.q(L.wproj);
+        }
+    });
     return B200_OK;
 }
 
 void b200_neox_free(b200_neox_model *m) {
     if (!m) return;
     B200_CHECK(cudaStreamSynchronize(rt().stream));
-    if (m->slab) B200_CHECK(cudaFree(m->slab));
-    delete m;
+    delete m;                                           // the slab goes with it
 }
 
 b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) {
     if (!m || n_batch < 1) return nullptr;
-    if (m->n_loaded != m->n_slots()) { fprintf(stderr, "llm_b200: neox start_session: %d of %d tensors loaded\n", m->n_loaded, m->n_slots()); return nullptr; }
+    if (!m->all_loaded()) { fprintf(stderr, "llm_b200: neox start_session: %d of %d tensors loaded\n", m->n_loaded, m->n_slots()); return nullptr; }
     b200_neox_session *s = new b200_neox_session();
-    s->m = m; s->n_batch = n_batch;
+    s->m = m;
     const b200_neox_hparams &hp = m->hp;
     const size_t e = hp.n_embd, B = n_batch, n_ctx = hp.context_size, V = hp.n_vocab;
-    const size_t kv = (size_t)hp.n_layer * n_ctx * e;
-    B200_CHECK(cudaMalloc(&s->memory_k, kv * 2)); B200_CHECK(cudaMalloc(&s->memory_v, kv * 2));
-    B200_CHECK(cudaMemset(s->memory_k, 0, kv * 2)); B200_CHECK(cudaMemset(s->memory_v, 0, kv * 2));
-    B200_CHECK(cudaMalloc(&s->d_tokens, B * 4)); B200_CHECK(cudaMallocHost(&s->h_tokens, B * 4));
-    B200_CHECK(cudaMalloc(&s->x, B * e * 4)); B200_CHECK(cudaMalloc(&s->cur, B * e * 4)); B200_CHECK(cudaMalloc(&s->qkv, B * 3 * e * 4));
-    B200_CHECK(cudaMalloc(&s->kq, (size_t)hp.n_head * B * n_ctx * 4)); B200_CHECK(cudaMalloc(&s->attn, B * e * 4));
-    B200_CHECK(cudaMalloc(&s->h4, B * 4 * e * 4)); B200_CHECK(cudaMalloc(&s->hact, B * 4 * e * 4)); B200_CHECK(cudaMalloc(&s->t, B * e * 4));
-    B200_CHECK(cudaMalloc(&s->logits, B * V * 4)); B200_CHECK(cudaMallocHost(&s->h_logits, B * V * 4));
-    B200_CHECK(cudaMalloc(&s->xq, B * 4 * e)); B200_CHECK(cudaMalloc(&s->xds, B * (4 * e / QK) * sizeof(float2)));
-    B200_CHECK(cudaMalloc(&s->xpack, (4 * e / QK) * 64)); B200_CHECK(cudaMalloc(&s->xh, xh_bytes(4 * e, B)));
-    B200_CHECK(cudaMalloc(&s->qdec, e * 4));
-    B200_CHECK(cudaMalloc(&s->xpack_a, (e / QK) * 64)); B200_CHECK(cudaMalloc(&s->xpack_d, (e / QK) * 64)); B200_CHECK(cudaMalloc(&s->xpack_f, (4 * e / QK) * 64));
+    s->start(n_batch, hp.context_size, hp.n_vocab, (size_t)hp.n_layer * n_ctx * e);
+    s->x = device_alloc<float>(B * e * 4); s->cur = device_alloc<float>(B * e * 4); s->qkv = device_alloc<float>(B * 3 * e * 4);
+    s->kq = device_alloc<float>((size_t)hp.n_head * B * n_ctx * 4); s->attn = device_alloc<float>(B * e * 4);
+    s->h4 = device_alloc<float>(B * 4 * e * 4); s->hact = device_alloc<float>(B * 4 * e * 4); s->t = device_alloc<float>(B * e * 4);
+    s->logits = device_alloc<float>(B * V * 4);
+    s->xq = device_alloc<int8_t>(B * 4 * e); s->xds = device_alloc<float2>(B * (4 * e / QK) * sizeof(float2));
+    s->xpack = device_alloc<int4>((4 * e / QK) * 64); s->xh = device_alloc<__half>(xh_bytes(4 * e, B));
+    s->qdec = device_alloc<float>(e * 4);
+    s->xpack_a = device_alloc<int4>((e / QK) * 64); s->xpack_d = device_alloc<int4>((e / QK) * 64); s->xpack_f = device_alloc<int4>((4 * e / QK) * 64);
     const RopeTable *rt_ = m->gpt2() ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, m->hd, (int)n_ctx);
     s->dl.resize(hp.n_layer);
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &L = m->layers[il];
         s->dl[il] = NeoxLayer{L.wqkv, L.wdense, L.wfc, L.wproj, L.ln1_g, L.ln1_b, L.ln2_g, L.ln2_b, L.bqkv, L.bdense, L.bfc, L.bproj,
-                              s->memory_k + (size_t)il * n_ctx * e, s->memory_v + (size_t)il * n_ctx * e};
+                              s->memory_k.get() + (size_t)il * n_ctx * e, s->memory_v.get() + (size_t)il * n_ctx * e};
     }
     NeoxParams &P = s->dp;
     P.n_layer = hp.n_layer; P.e = (int)e; P.hd = m->hd; P.n_head = hp.n_head; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab; P.n_rot = hp.n_rot;
     P.parallel_residual = !m->gpt2() && hp.use_parallel_residual; P.gpt2 = m->gpt2() ? 1 : 0; P.wpe = m->wpe; P.wte = m->wte; P.lm_head = m->lm_head; P.lnf_g = m->lnf_g; P.lnf_b = m->lnf_b;
     P.kq_scale = 1.0f / sqrtf((float)e / (float)hp.n_head); P.rope_cs = rt_ ? rt_->cs : nullptr; P.rope_half = rt_ ? rt_->half : 0;
-    P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens; P.n_past = s->decode.d_n_past;
-    P.x = s->x; P.qkv = s->qkv; P.q = s->qdec; P.attn_out = s->attn; P.logits = s->logits;
-    P.xpack_a = s->xpack_a; P.xpack_d = s->xpack_d; P.xpack_f = s->xpack_f;
+    P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
+    P.x = s->x.get(); P.qkv = s->qkv.get(); P.q = s->qdec.get(); P.attn_out = s->attn.get(); P.logits = s->logits.get();
+    P.xpack_a = s->xpack_a.get(); P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
     QWeight p1; p1.nb = (int64_t)e / QK; QWeight p2; p2.nb = 4 * (int64_t)e / QK;
     s->decode_ok = m->hd % 32 == 0 && m->hd <= 128 && e % 128 == 0 && e <= 8192 && n_ctx % 8 == 0 && mmv_exact_stream_supported(p1) && mmv_exact_stream_supported(p2) &&
                    !getenv("B200_NEOX_UNFUSED");
@@ -298,50 +258,31 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
 }
 
 int32_t b200_neox_n_past(const b200_neox_session *s) { return s ? s->n_past : -1; }
-int b200_neox_set_n_past(b200_neox_session *s, int32_t n_past) {
-    if (!s || n_past < 0 || n_past > s->n_past) return B200_ERR_BAD_ARG;
-    s->n_past = n_past;
-    return B200_OK;
-}
+int b200_neox_set_n_past(b200_neox_session *s, int32_t n_past) { return s ? s->set_n_past(n_past) : B200_ERR_BAD_ARG; }
 int32_t b200_neox_last_launches(const b200_neox_session *s) { return s ? s->last_launches : 0; }
 int b200_neox_sync(b200_neox_session *s) { if (!s) return B200_ERR_BAD_ARG; B200_CHECK(cudaStreamSynchronize(rt().stream)); return B200_OK; }
 
 // tokens already in HBM (left there by the last b200_neox_evaluate), logits stay in HBM
 int b200_neox_evaluate_device(b200_neox_session *s, int32_t n) {
-    if (!s || n < 1 || n > s->n_batch) return B200_ERR_BAD_ARG;
-    if (s->n_past + n > s->m->hp.context_size) return B200_ERR_CONTEXT_FULL;
+    if (!s) return B200_ERR_BAD_ARG;
+    if (const int rc = s->admit(n)) return rc;
     forward(s, n, true);
     return B200_OK;
 }
 
 int b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits) {
-    if (!s || !tokens || n < 1 || n > s->n_batch) return B200_ERR_BAD_ARG;
-    if (s->n_past + n > s->m->hp.context_size) return B200_ERR_CONTEXT_FULL;
-    for (int i = 0; i < n; i++) if (tokens[i] < 0 || tokens[i] >= s->m->hp.n_vocab) return B200_ERR_BAD_ARG;
-    cudaStream_t st = rt().stream;
-    B200_CHECK(cudaStreamSynchronize(st));
-    memcpy(s->h_tokens, tokens, (size_t)n * 4);
-    B200_CHECK(cudaMemcpyAsync(s->d_tokens, s->h_tokens, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    if (!s || !tokens) return B200_ERR_BAD_ARG;
+    if (const int rc = s->admit(n)) return rc;
+    if (const int rc = s->stage_tokens(tokens, n)) return rc;
     forward(s, n, all_logits != 0);
-    if (logits_out) {
-        const size_t V = s->m->hp.n_vocab, rows = all_logits ? n : 1;
-        const float *src = all_logits ? s->logits : s->logits + (size_t)(n - 1) * V;
-        B200_CHECK(cudaMemcpyAsync(s->h_logits, src, rows * V * 4, cudaMemcpyDeviceToHost, st));
-        B200_CHECK(cudaStreamSynchronize(st));
-        memcpy(logits_out, s->h_logits, rows * V * 4);
-    }
+    s->copy_logits(logits_out, s->logits.get(), n, all_logits != 0);
     return B200_OK;
 }
 
 void b200_neox_session_free(b200_neox_session *s) {
     if (!s) return;
     B200_CHECK(cudaStreamSynchronize(rt().stream));
-    void *dev[] = {s->memory_k, s->memory_v, s->d_tokens, s->x, s->cur, s->qkv, s->kq, s->attn, s->h4, s->hact, s->t, s->logits, s->xq, s->xds, s->xpack, s->xh, s->qdec,
-                   s->xpack_a, s->xpack_d, s->xpack_f};
-    for (void *p : dev) if (p) B200_CHECK(cudaFree(p));
-    if (s->h_tokens) B200_CHECK(cudaFreeHost(s->h_tokens));
-    if (s->h_logits) B200_CHECK(cudaFreeHost(s->h_logits));
-    delete s;                                           // the decode graphs and n_past words go with s->decode
+    delete s;                                           // every buffer, the decode graphs and n_past words go with it
 }
 
 }  // extern "C"

@@ -1,0 +1,181 @@
+// llm_b200/csrc/ops.cu -- single-op entry points on host buffers (include/llm_b200.h: b200_op_*): one kernel family per call, for tests and
+// kernel benchmarks
+#include <vector>
+
+#include "../../include/llm_b200.h"
+#include "kernels.cuh"
+#include "runtime.h"
+
+using namespace b200;
+
+namespace {
+
+// The activation operand of the batched mat-mul implementations: the tensor-core GEMMs read f16 rows (EXACT_TC5 / EXACT_MMA with the Q8 block
+// scales in xds), every other implementation reads Q8 blocks (xq, xds).
+struct Acts { int8_t *xq; float2 *xds; __half *xh; };
+
+void prepare(int32_t impl, int32_t wtype, const float *dx, int64_t K, int64_t B, const Acts &a, cudaStream_t st) {
+    if (impl == B200_MM_FAST_TC5) cvt_act_f16(dx, K, a.xh, K, B, st);
+    else if (impl == B200_MM_EXACT_TC5) quantize_act_f16_rm(vec_dot_type(wtype), dx, K, a.xh, a.xds, K, B, st);
+    else if (impl == B200_MM_EXACT_MMA) quantize_act_f16(vec_dot_type(wtype), dx, K, a.xh, a.xds, K, B, st);
+    else quantize_act(vec_dot_type(wtype), dx, K, a.xq, a.xds, K, B, st);
+}
+
+// FAST_TC5, EXACT_TC5, EXACT_MMA, or else the Q8 GEMM (mmq.cu)
+void run(int32_t impl, const QWeight &w, const Acts &a, float *dd, int64_t N, int64_t B, cudaStream_t st) {
+    if (impl == B200_MM_FAST_TC5) mul_mat_q_fast_tc5(w, a.xh, dd, N, B, nullptr, 0, st);
+    else if (impl == B200_MM_EXACT_TC5) mul_mat_q_exact_tc5(w, a.xh, a.xds, dd, N, B, nullptr, 0, st);
+    else if (impl == B200_MM_EXACT_MMA) mul_mat_q_exact_mma(w, a.xh, a.xds, dd, N, B, nullptr, 0, st);
+    else mul_mat_q(w, a.xq, a.xds, dd, N, B, nullptr, 0, st);
+}
+
+// B200_ERR_IO if a pipeline barrier of the wgmma kernel `impl` ever timed out (call after the stream is synchronized)
+int check_timeout(int32_t impl) {
+    if (impl == B200_MM_EXACT_TC5 && exact_tc5_check_timeout() != 0) return B200_ERR_IO;
+    if (impl == B200_MM_FAST_TC5 && fast_tc5_check_timeout() != 0) return B200_ERR_IO;
+    return B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200_op_quantize_act(int32_t vdt, const float *x, int64_t K, int64_t B, int8_t *qs_out, float *d_out, float *aux_out) {
+    if (!x || K % QK || (vdt != T_Q8_0 && vdt != T_Q8_1)) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    const size_t nblk = (size_t)B * (K / QK);
+    float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
+    int8_t *dq = (int8_t *)R.op_arena.get((size_t)B * K, st);
+    float2 *dds = (float2 *)R.op_arena.get(nblk * sizeof(float2), st);
+    B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
+    quantize_act(vdt, dx, K, dq, dds, K, B, st);
+    std::vector<float2> h(nblk);
+    B200_CHECK(cudaMemcpyAsync(qs_out, dq, (size_t)B * K, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaMemcpyAsync(h.data(), dds, nblk * sizeof(float2), cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    for (size_t i = 0; i < nblk; i++) { if (d_out) d_out[i] = h[i].x; if (aux_out) aux_out[i] = h[i].y; }
+    return B200_OK;
+}
+
+int b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_out) {      // quantize_row_q8_K of B rows -> B * K/256 block_q8_K (292 bytes each)
+    if (!x || !blocks_out || K % 256) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
+    void *xq = R.op_arena.get(q8k_bytes(K, B), st);
+    B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
+    quantize_act_q8k(dx, K, xq, K, B, st);
+    B200_CHECK(cudaMemcpyAsync(blocks_out, xq, q8k_bytes(K, B), cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
+int b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl) {
+    if (is_kquant(wtype)) {                              // Q2_K .. Q6_K: one exact kernel (kquants.cu); `impl` must be AUTO or EXACT
+        if (!w_ggml || !x || !dst || K % 256 || (impl != B200_MM_AUTO && impl != B200_MM_EXACT)) return B200_ERR_BAD_ARG;
+        Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+        cudaStream_t st = R.stream;
+        const size_t raw_bytes = (size_t)N * (K / 256) * kquant_block_bytes(wtype);
+        void *raw = R.op_arena.get(raw_bytes, st);
+        float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
+        float *dd = (float *)R.op_arena.get((size_t)B * N * 4, st);
+        void *xq = R.op_arena.get(q8k_bytes(K, B), st);
+        B200_CHECK(cudaMemcpyAsync(raw, w_ggml, raw_bytes, cudaMemcpyHostToDevice, st));
+        B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
+        quantize_act_q8k(dx, K, xq, K, B, st);
+        mul_mat_kq_exact(wtype, raw, xq, dd, N, K, N, B, nullptr, 0, st);
+        B200_CHECK(cudaMemcpyAsync(dst, dd, (size_t)B * N * 4, cudaMemcpyDeviceToHost, st));
+        B200_CHECK(cudaStreamSynchronize(st));
+        return B200_OK;
+    }
+    if (!is_quant(wtype) || !w_ggml || !x || !dst || K % 64) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    const size_t raw_bytes = (size_t)N * (K / QK) * ggml_block_bytes(wtype);
+    void *raw = R.op_arena.get(raw_bytes, st);
+    B200_CHECK(cudaMemcpyAsync(raw, w_ggml, raw_bytes, cudaMemcpyHostToDevice, st));
+    QWeight w;
+    const size_t pb = qweight_layout(w, wtype, K, N, nullptr);
+    qweight_layout(w, wtype, K, N, R.op_arena.get(pb, st));
+    repack_weights(w, raw, st);
+    if (impl == B200_MM_AUTO) impl = B200_MM_EXACT;
+    float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
+    float *dd = (float *)R.op_arena.get((size_t)B * N * 4, st);
+    Acts a{};
+    a.xq = (int8_t *)R.op_arena.get((size_t)B * K, st);
+    a.xds = (float2 *)R.op_arena.get((size_t)B * (K / QK) * sizeof(float2), st);
+    if (impl == B200_MM_EXACT_MMA) a.xh = (__half *)R.op_arena.get(xh_bytes(K, B), st);
+    else if (impl == B200_MM_EXACT_TC5 || impl == B200_MM_FAST_TC5) a.xh = (__half *)R.op_arena.get((size_t)B * K * 2 + 16, st);
+    B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
+    prepare(impl, wtype, dx, K, B, a, st);
+    if (impl == B200_MM_EXACT_STREAM) {
+        if (!mmv_exact_stream_supported(w)) return B200_ERR_BAD_ARG;
+        int4 *pack = (int4 *)R.op_arena.get((size_t)(K / QK) * 64, st);
+        for (int64_t b = 0; b < B; b++) { quantize_act_pack(wtype, dx + b * K, pack, K, st); mul_mat_vec_q_exact_stream(w, pack, dd + b * N, nullptr, st); }
+    } else if (impl == B200_MM_EXACT) mul_mat_q_exact(w, a.xq, a.xds, dd, N, B, nullptr, 0, st);
+    else if (impl == B200_MM_VEC) { for (int64_t b = 0; b < B; b++) mul_mat_vec_q(w, a.xq + b * K, a.xds + b * (K / QK), dd + b * N, nullptr, st); }
+    else if (impl == B200_MM_SIMPLE) mul_mat_q_simple(w, a.xq, a.xds, dd, N, B, nullptr, 0, st);
+    else {
+        run(impl, w, a, dd, N, B, st);
+        B200_CHECK(cudaStreamSynchronize(st));
+        if (const int rc = check_timeout(impl)) return rc;
+    }
+    B200_CHECK(cudaMemcpyAsync(dst, dd, (size_t)B * N * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
+// ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} on the GPU (crates/llm-base/src/quantize.rs:320-414 calls them per tensor): f32 rows in, GGML blocks out
+int b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int64_t N, void *ggml_blocks_out) {
+    if (!is_quant(wtype) || !w_host || !ggml_blocks_out || K % QK) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    float *dw = (float *)R.op_arena.get((size_t)N * K * 4, st);
+    B200_CHECK(cudaMemcpyAsync(dw, w_host, (size_t)N * K * 4, cudaMemcpyHostToDevice, st));
+    QWeight w;
+    const size_t pb = qweight_layout(w, wtype, K, N, nullptr);
+    qweight_layout(w, wtype, K, N, R.op_arena.get(pb, st));
+    quantize_weights(w, dw, st);
+    const size_t raw_bytes = (size_t)N * (K / QK) * ggml_block_bytes(wtype);
+    void *raw = R.op_arena.get(raw_bytes, st);
+    unpack_weights(w, raw, st);
+    B200_CHECK(cudaMemcpyAsync(ggml_blocks_out, raw, raw_bytes, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
+// Kernel-only timing of one weight mat-mul on device-resident synthetic operands (seeded random weights and activations): used by
+// tools/prefill_gemm_bench.py and bench.py's prefill roofline; impl = B200_MM_EXACT_MMA / B200_MM_EXACT_TC5 / B200_MM_TENSOR
+int b200_op_bench_mul_mat(int32_t wtype, int64_t K, int64_t N, int64_t B, int32_t impl, int32_t iters, float *ms_out) {
+    if (!is_quant(wtype) || K % 64 || !ms_out || iters < 1) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    QWeight w;
+    const size_t pb = qweight_layout(w, wtype, K, N, nullptr);
+    void *base = R.op_arena.get(pb, st);
+    qweight_layout(w, wtype, K, N, base);
+    synth_qweight(w, 777u, st);
+    float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
+    float *dd = (float *)R.op_arena.get((size_t)B * N * 4, st);
+    Acts a;
+    a.xds = (float2 *)R.op_arena.get((size_t)B * (K / QK) * sizeof(float2), st);
+    a.xh = (__half *)R.op_arena.get(xh_bytes(K, B) + 16, st);
+    a.xq = (int8_t *)R.op_arena.get((size_t)B * K, st);
+    synth_gain(dx, B * K, 12345u, st);
+    prepare(impl, wtype, dx, K, B, a, st);
+    for (int i = 0; i < 2; i++) run(impl, w, a, dd, N, B, st);
+    cudaEvent_t e0, e1;
+    B200_CHECK(cudaEventCreate(&e0)); B200_CHECK(cudaEventCreate(&e1));
+    B200_CHECK(cudaEventRecord(e0, st));
+    for (int i = 0; i < iters; i++) run(impl, w, a, dd, N, B, st);
+    B200_CHECK(cudaEventRecord(e1, st));
+    B200_CHECK(cudaEventSynchronize(e1));
+    float ms = 0.f;
+    B200_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+    *ms_out = ms / iters;
+    B200_CHECK(cudaEventDestroy(e0)); B200_CHECK(cudaEventDestroy(e1));
+    return check_timeout(impl);
+}
+
+}  // extern "C"

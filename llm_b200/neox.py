@@ -10,18 +10,11 @@ from typing import Dict
 import numpy as np
 
 from . import _lib
-from .session import ContextFull
+from .session import _check, _Native
 
 
 class NeoxHparams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_vocab", "n_embd", "n_head", "n_layer", "n_rot", "use_parallel_residual", "wtype", "context_size", "arch", "has_lm_head")]
-
-
-def _check(rc, what):
-    if rc == -1:
-        raise ContextFull(what)
-    if rc != 0:
-        raise RuntimeError(f"{what} failed with code {rc}")
 
 
 def _bind(L):
@@ -48,10 +41,11 @@ def _bind(L):
     return L
 
 
-class GptNeoX:
+class GptNeoX(_Native):
     """hyperparameters: n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype"""
 
     ARCH = 0
+    _HANDLE, _FREE = "_m", "b200_neox_free"
 
     def __init__(self, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray] = None, context_size: int = None, device: int = 0):
         self.L = _bind(_lib.lib())
@@ -78,17 +72,6 @@ class GptNeoX:
     def start_session(self, n_batch: int = 8) -> "NeoxSession":
         return NeoxSession(self, n_batch)
 
-    def close(self):
-        if getattr(self, "_m", None):
-            self.L.b200_neox_free(self._m)
-            self._m = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class Gpt2(GptNeoX):
     """KnownModel for GPT-2 (crates/models/gpt2/src/lib.rs): hyperparameters n_vocab, n_ctx, n_embd, n_head, n_layer, wtype; tensors "model/wte",
@@ -97,7 +80,9 @@ class Gpt2(GptNeoX):
     ARCH = 1
 
 
-class NeoxSession:
+class NeoxSession(_Native):
+    _HANDLE, _FREE = "_s", "b200_neox_session_free"
+
     def __init__(self, model: GptNeoX, n_batch: int):
         self.model, self.L = model, model.L
         self._s = self.L.b200_neox_start_session(model._m, n_batch)
@@ -124,14 +109,3 @@ class NeoxSession:
 
     def sync(self):
         self.L.b200_neox_sync(self._s)
-
-    def close(self):
-        if getattr(self, "_s", None):
-            self.L.b200_neox_session_free(self._s)
-            self._s = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

@@ -65,8 +65,27 @@ def _check(rc, what):
         raise RuntimeError(f"{what} failed with code {rc}")
 
 
-class Llama:
+class _Native:
+    """Owner of one native handle (attribute `_HANDLE`, released by the library function `_FREE`): close() frees it once, and so does
+    garbage collection."""
+    _HANDLE, _FREE = "", ""
+
+    def close(self):
+        h = getattr(self, self._HANDLE, None)
+        if h:
+            getattr(self.L, self._FREE)(h)
+            setattr(self, self._HANDLE, None)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Llama(_Native):
     """KnownModel for LLaMA.  `hyperparameters` is a dict with n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff, wtype."""
+    _HANDLE, _FREE = "_m", "b200_model_free"
 
     def __init__(self, hyperparameters: Dict[str, int], params: ModelParameters = None, tensors: Dict[str, np.ndarray] = None,
                  device: int = 0):
@@ -116,19 +135,10 @@ class Llama:
     def context_size(self) -> int:
         return self.params.context_size
 
-    def close(self):
-        if getattr(self, "_m", None):
-            self.L.b200_model_free(self._m)
-            self._m = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+class InferenceSession(_Native):
+    _HANDLE, _FREE = "_s", "b200_session_free"
 
-
-class InferenceSession:
     def __init__(self, model: Llama, config: InferenceSessionConfig):
         self.model, self.config, self.L = model, config, model.L
         cfg = _lib.SessionConfig(n_batch=config.n_batch, flags=config.flags)
@@ -186,14 +196,3 @@ class InferenceSession:
     @property
     def last_launches(self) -> int:
         return self.L.b200_session_last_launches(self._s)
-
-    def close(self):
-        if getattr(self, "_s", None):
-            self.L.b200_session_free(self._s)
-            self._s = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
