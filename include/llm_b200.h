@@ -204,6 +204,8 @@ int  b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, 
 int  b200_neox_evaluate_device(b200_neox_session *s, int32_t n);       /* tokens of the last evaluate stay in HBM, logits stay in HBM */
 int32_t b200_neox_n_past(const b200_neox_session *s);
 int  b200_neox_set_n_past(b200_neox_session *s, int32_t n_past);
+/* raw f16 KV cache bytes, which = 0 memory_k [n_layer][n_ctx][n_embd], 1 memory_v [n_layer][n_embd][n_ctx] (V by channel, also for GPT-2) */
+int  b200_neox_read_kv(b200_neox_session *s, int32_t which, void *host_out, size_t nbytes);
 int32_t b200_neox_last_launches(const b200_neox_session *s);
 int  b200_neox_sync(b200_neox_session *s);
 void b200_neox_session_free(b200_neox_session *s);

@@ -70,14 +70,18 @@ bool decode_supported(const DecodeParams &P, int wtype);
 // cooperative launch on `st`; returns false if the kernel cannot be made resident (caller falls back to the per-op schedule)
 bool launch_decode(const DecodeParams &P, int wtype, cudaStream_t st, int *grid_out);
 
+// whether attn_fused_kernel's shared memory for a bucket of nlay positions (a multiple of 64) and head size hd fits the 227 KB opt-in limit:
+// true up to nlay = 3264 for every hd <= 128.  Past it LLaMA decodes with the two-kernel attention and GPT-NeoX / GPT-2 per op.
+bool attn_fused_fits(int nlay, int hd);
+
 // default decode schedule: 8 fused kernels per layer on `st` (decode_ops.cu); position read from *P.n_past on the device
 void decode_ops_enqueue(const DecodeParams &P, const std::vector<DecodeLayer> &layers, int wtype, int n_kv_bucket, int4 *xpack_a, cudaStream_t st, int *launches);
 
 // A session's decode graphs (decode_ops.cu): one per context bucket of 256 positions, and the device copy of n_past the schedules read.
 struct DecodeGraphCache {
-    std::vector<std::pair<int, cudaGraphExec_t>> graphs;   // (n_kv bucket, instantiated graph)
+    struct Graph { int bucket; cudaGraphExec_t exec; int nodes; };   // nodes: the step's launches (buckets past 3264 positions launch more)
+    std::vector<Graph> graphs;
     bool warm = false;                  // the first step runs eagerly (it sets kernel attributes), later ones replay a graph
-    int nodes = 0;                      // launches of one step
     int *d_n_past = nullptr, *h_n_past = nullptr;          // device word, pinned staging word
     int dev_n_past = -1;                // value currently held by *d_n_past (-1: unknown)
 
@@ -86,7 +90,9 @@ struct DecodeGraphCache {
     DecodeGraphCache(const DecodeGraphCache &) = delete;
     DecodeGraphCache &operator=(const DecodeGraphCache &) = delete;
 
-    // uploads n_past if the device copy is stale (after a prefill or a rewind)
+    // the context bucket a step at position n_kv - 1 runs in: n_kv rounded up to 256 positions, at most n_ctx
+    static int bucket(int n_kv, int n_ctx);
+    // uploads n_past if the device copy is stale (after a prefill, a rewind, or steps that did not run the graph)
     void sync_n_past(int n_past, cudaStream_t st);
     // one decode step at position n_kv - 1 (its last kernel increments *d_n_past): enqueue(bucket, st, &nodes) enqueues the schedule for up to
     // `bucket` positions.  Runs it eagerly on the first step or when replay is false, else replays (capturing on first use) the bucket's graph.

@@ -728,6 +728,9 @@ static void attn_fused_reserve(size_t bytes) {
 size_t attn_fused_smem(int nlay, int hd) {
     return (((size_t)nlay * 6 + (size_t)hd * 2 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 32) * 2;
 }
+}  // namespace
+bool attn_fused_fits(int nlay, int hd) { return attn_fused_smem(nlay, hd) <= 227 * 1024; }
+namespace {
 // one cluster of hd/32 CTAs per head; a programmatic dependent of its predecessor unless B200_PDL clears bit 1
 template <bool TP>
 void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const __half *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
@@ -795,12 +798,13 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     // attn_fused_kernel reads n_past and the older KV cache ahead of its griddepcontrol.wait on that guarantee
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     if (tp) { launch_k(tp_spread_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.x, e); n++; }
-    // attention: one cluster launch per layer (default) or the two-kernel variant (B200_ATTN_FUSED=0, or head sizes a cluster cannot cover)
+    // attention: one cluster launch per layer (default) or the two-kernel variant (B200_ATTN_FUSED=0, head sizes a cluster cannot cover, or
+    // buckets whose scores and V rows do not fit one CTA's shared memory)
     static const bool fused_env = !(getenv("B200_ATTN_FUSED") && getenv("B200_ATTN_FUSED")[0] == '0');
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
     const size_t fa_smem = attn_fused_smem(nlay, P.hd);
-    const bool fused_attn = (fused_env || tp) && P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && fa_smem <= 227 * 1024;
-    B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue
+    const bool fused_attn = (fused_env || tp) && P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd);
+    B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue (start_session_tp checks the size)
     const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
     static size_t sv_set = 48 * 1024;
     if (sv_smem > sv_set) { B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem)); sv_set = sv_smem; }
@@ -950,7 +954,7 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
     const size_t fa_smem = attn_fused_smem(nlay, P.hd);
-    B200_ASSERT(P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && fa_smem <= 227 * 1024 && e <= 8192);
+    B200_ASSERT(P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd) && e <= 8192);   // neox.cu::forward checks both
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
@@ -1037,32 +1041,38 @@ void DecodeGraphCache::sync_n_past(int n_past, cudaStream_t st) {
     dev_n_past = n_past;
 }
 
+int DecodeGraphCache::bucket(int n_kv, int n_ctx) { return std::min((n_kv + 255) / 256 * 256, n_ctx); }
+
 int DecodeGraphCache::run(int n_kv, int n_ctx, bool replay, const std::function<void(int, cudaStream_t, int *)> &enqueue, cudaStream_t st) {
     sync_n_past(n_kv - 1, st);
-    const int bucket = std::min((n_kv + 255) / 256 * 256, n_ctx);
+    const int bucket = DecodeGraphCache::bucket(n_kv, n_ctx);
+    int nodes = 0;
     if (!warm || !replay) {
         enqueue(bucket, st, &nodes);
         warm = true;
     } else {
-        cudaGraphExec_t exec = nullptr;
-        for (auto &g : graphs) if (g.first == bucket) exec = g.second;
-        if (!exec) {
+        const Graph *g = nullptr;
+        for (const Graph &x : graphs) if (x.bucket == bucket) g = &x;
+        if (!g) {
             cudaGraph_t graph;
+            cudaGraphExec_t exec;
             B200_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
             enqueue(bucket, st, &nodes);
             B200_CHECK(cudaStreamEndCapture(st, &graph));
             B200_CHECK(cudaGraphInstantiate(&exec, graph, 0));
             B200_CHECK(cudaGraphDestroy(graph));
-            graphs.emplace_back(bucket, exec);
+            graphs.push_back(Graph{bucket, exec, nodes});
+            g = &graphs.back();
         }
-        B200_CHECK(cudaGraphLaunch(exec, st));
+        B200_CHECK(cudaGraphLaunch(g->exec, st));
+        nodes = g->nodes;
     }
     dev_n_past = n_kv;
     return nodes;
 }
 
 void DecodeGraphCache::drop() {
-    for (auto &g : graphs) cudaGraphExecDestroy(g.second);
+    for (const Graph &g : graphs) cudaGraphExecDestroy(g.exec);
     graphs.clear();
 }
 

@@ -97,7 +97,9 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     cudaStream_t st = rt().stream;
     const int e = hp.n_embd, hd = m->hd, n_head = hp.n_head, n_ctx = hp.context_size, n_past = s->n_past, n_kv = n_past + n;
     int L = 0;
-    if (n == 1 && s->decode_ok) {
+    // the graph schedule's attention keeps the whole bucket in shared memory: steps in buckets past 3264 positions run per op below, and the
+    // graph cache re-uploads the device n_past when graph steps resume (after a rewind)
+    if (n == 1 && s->decode_ok && attn_fused_fits((DecodeGraphCache::bucket(n_kv, n_ctx) + 63) / 64 * 64, hd)) {
         s->last_launches = s->decode.run(n_kv, n_ctx, true, [s, &hp](int bucket, cudaStream_t st, int *nodes) {
             neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
         }, st);
@@ -259,6 +261,14 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
 
 int32_t b200_neox_n_past(const b200_neox_session *s) { return s ? s->n_past : -1; }
 int b200_neox_set_n_past(b200_neox_session *s, int32_t n_past) { return s ? s->set_n_past(n_past) : B200_ERR_BAD_ARG; }
+int b200_neox_read_kv(b200_neox_session *s, int32_t which, void *host_out, size_t nbytes) {
+    if (!s || !host_out) return B200_ERR_BAD_ARG;
+    const size_t kv_bytes = (size_t)s->m->hp.n_layer * s->m->hp.context_size * s->m->hp.n_embd * 2;
+    if (nbytes != kv_bytes) return B200_ERR_TENSOR_SHAPE;
+    B200_CHECK(cudaStreamSynchronize(rt().stream));
+    B200_CHECK(cudaMemcpy(host_out, which ? s->memory_v.get() : s->memory_k.get(), kv_bytes, cudaMemcpyDeviceToHost));
+    return B200_OK;
+}
 int32_t b200_neox_last_launches(const b200_neox_session *s) { return s ? s->last_launches : 0; }
 int b200_neox_sync(b200_neox_session *s) { if (!s) return B200_ERR_BAD_ARG; B200_CHECK(cudaStreamSynchronize(rt().stream)); return B200_OK; }
 

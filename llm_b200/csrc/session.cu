@@ -425,6 +425,12 @@ static b200_session *start_session_tp(b200_session *s) {
     const b200_llama_hparams &hp = m->hp;
     const int G = m->tp_world, r = m->tp_rank;
     const size_t e = hp.n_embd, f = hp.n_ff, n_ctx = hp.context_size, V = hp.n_vocab;
+    // the exchange lives in the fused attention kernel, whose shared memory holds the whole context bucket
+    if (!attn_fused_fits((hp.context_size + 63) / 64 * 64, m->hd)) {
+        fprintf(stderr, "llm_b200: tensor-parallel session: context_size %d is more than the fused attention kernel holds (3264 positions)\n", hp.context_size);
+        b200_session_free(s);
+        return nullptr;
+    }
     start_common(s);
     // the exchange slab: arrays of 8-byte {word, tag} units (tp.cuh) -- x | ff | attention records | ffn records | logits, 256-byte aligned pieces
     TpCtx &T = s->dp.tp;

@@ -34,6 +34,7 @@ def _bind(L):
     L.b200_neox_evaluate_device.argtypes = [vp, i32]
     L.b200_neox_n_past.argtypes = [vp]
     L.b200_neox_set_n_past.argtypes = [vp, i32]
+    L.b200_neox_read_kv.argtypes = [vp, i32, vp, C.c_size_t]
     L.b200_neox_last_launches.argtypes = [vp]
     L.b200_neox_sync.argtypes = [vp]
     L.b200_neox_session_free.argtypes = [vp]
@@ -51,9 +52,10 @@ class GptNeoX(_Native):
         self.L = _bind(_lib.lib())
         _check(self.L.b200_init(device), "b200_init")
         self.hyperparameters = dict(hyperparameters)
+        self.context_size = context_size or hyperparameters["n_ctx"]
         hp = NeoxHparams(n_vocab=hyperparameters["n_vocab"], n_embd=hyperparameters["n_embd"], n_head=hyperparameters["n_head"], n_layer=hyperparameters["n_layer"],
                          n_rot=int(hyperparameters.get("n_rot", 0)), use_parallel_residual=int(hyperparameters.get("use_parallel_residual", 1)), wtype=hyperparameters["wtype"],
-                         context_size=context_size or hyperparameters["n_ctx"], arch=self.ARCH, has_lm_head=int(bool(tensors) and "model/lm_head" in tensors))
+                         context_size=self.context_size, arch=self.ARCH, has_lm_head=int(bool(tensors) and "model/lm_head" in tensors))
         self._m = self.L.b200_neox_new(C.byref(hp))
         if not self._m:
             raise ValueError(f"b200_neox_new rejected {hyperparameters}")
@@ -106,6 +108,13 @@ class NeoxSession(_Native):
 
     def rewind(self, n_past: int):
         _check(self.L.b200_neox_set_n_past(self._s, n_past), "rewind")
+
+    def kv(self, which: int) -> np.ndarray:
+        """the f16 cache as raw bits: K [n_layer][n_ctx][n_embd] (which = 0), V [n_layer][n_embd][n_ctx] (which = 1)"""
+        hp = self.model.hyperparameters
+        out = np.empty(hp["n_layer"] * self.model.context_size * hp["n_embd"], np.uint16)
+        _check(self.L.b200_neox_read_kv(self._s, which, out.ctypes.data_as(C.c_void_p), out.nbytes), "read_kv")
+        return out
 
     def sync(self):
         self.L.b200_neox_sync(self._s)

@@ -87,6 +87,10 @@ class RefLib:
             L.rh_gpt2_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
             L.rh_neox_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
             L.rh_gpt2_free.argtypes = [C.c_void_p]
+        L.ggml_get_data.restype = C.c_void_p
+        L.ggml_get_data.argtypes = [C.c_void_p]
+        L.ggml_nbytes.restype = C.c_size_t
+        L.ggml_nbytes.argtypes = [C.c_void_p]
         L.rh_op.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
                             C.c_void_p, C.c_void_p, C.c_int]
 
@@ -149,6 +153,12 @@ class RgParams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "wtype", "use_gpu", "n_threads", "n_batch", "has_lm_head", "arch", "n_rot", "use_parallel_residual")]
 
 
+class _RgHead(C.Structure):
+    """rg_model (oracle/ref_gpt2.c) from its start up to the KV cache tensors"""
+    _fields_ = [("hp", RgParams), ("ctx", C.c_void_p * 3), ("wte", C.c_void_p), ("tops", C.c_void_p * 4),
+                ("layers", C.c_void_p * (12 * 64)), ("memory_k", C.c_void_p), ("memory_v", C.c_void_p)]   # rg_layer[RG_MAX_LAYERS]
+
+
 class RefGpt2:
     """The reference's GPT-2 (crates/models/gpt2) on the reference ggml: CPU build = the oracle for GPT-2, seam build = the same graph over our backend."""
 
@@ -173,6 +183,20 @@ class RefGpt2:
         rc = (self.ref.lib.rh_neox_eval if self.arch else self.ref.lib.rh_gpt2_eval)(self.m, _p(tokens), tokens.size, _p(logits))
         assert rc == 0, rc
         return logits
+
+    def reset(self):
+        self.ref.lib.rh_gpt2_reset(self.m)
+
+    def kv(self, which):
+        """f16 bits of memory_k (0) / memory_v (1): GPT-2 keeps V by position, GPT-NeoX by channel.  The harness exports no accessor for
+        the cache (so a prebuilt oracle/_ref of an earlier recipe serves too), so the two tensors are found through the leading members
+        of rg_model, checked against a tensor the harness does export."""
+        L = self.ref.lib
+        head = _RgHead.from_address(self.m)
+        wte = b"gpt_neox.embed_in.weight" if self.arch else b"model/wte"
+        assert head.hp.n_ctx == self.hp["n_ctx"] and L.ggml_get_data(head.wte) == L.rh_gpt2_tensor(self.m, wte, None), "rg_model layout (oracle/ref_gpt2.c) changed"
+        t = head.memory_v if which else head.memory_k
+        return np.ctypeslib.as_array(C.cast(L.ggml_get_data(t), C.POINTER(C.c_uint16)), (L.ggml_nbytes(t) // 2,)).copy()
 
     def close(self):
         if self.m:

@@ -20,6 +20,10 @@ CHAOS = 8e-2      # what ANY order-free implementation (incl. the reference's ow
 FAST = 4          # B200_SESSION_FAST
 
 
+# "small" with n_ff 1536 (48 blocks of 32, a multiple of 8): the geometry the decode graph takes; "small" itself (n_ff 1408) decodes per op
+GRAPH_SMALL = dict(synth.CONFIGS["small"], n_ff=1536)
+
+
 def rel(g, c):
     c = c.astype(np.float64)
     return float(np.abs(g - c).max() / np.abs(c).max()), float(np.sqrt(((g - c) ** 2).sum() / (c ** 2).sum()))
@@ -212,7 +216,7 @@ def test_7b_geometry_two_layers(orc):
 def test_last_row_only_lm_head_and_top_k(orc):
     """OutputRequest without all_logits: only the last row goes through the lm_head (same bits as the all-rows pass); the sampler hand-off
     returns the k largest logits of that row, selected on the device (descending, ties by ascending token id)."""
-    hp, tens = synth.make_llama(synth.CONFIGS["small"], B.Q4_0, orc.quantize)
+    hp, tens = synth.make_llama(GRAPH_SMALL, B.Q4_0, orc.quantize)
     toks = synth.make_tokens(hp, 40)
     mo = orc.llama(hp, tens)
     want = np.asarray(mo.eval(toks[:37]), np.float32).reshape(37, -1)
@@ -225,6 +229,7 @@ def test_last_row_only_lm_head_and_top_k(orc):
         assert np.array_equal(ids, order.astype(np.int32)), k
         assert np.array_equal(vals.view(np.uint32), want[-1][order].view(np.uint32)), k
     one = np.asarray(s.evaluate(toks[37:38]), np.float32).ravel()                     # decode (CUDA graph) then top-k of that row
+    assert s.last_launches == 7 * hp["n_layer"] + 3, ("fused decode graph not used", s.last_launches)
     ref1 = np.asarray(mo.eval(toks[37:38]), np.float32).ravel()
     assert np.array_equal(one.view(np.uint32), ref1.view(np.uint32))
     ids, vals = s.top_k(8)
@@ -287,16 +292,18 @@ def test_decode_graph_bucket_edges(orc, name):
     """the decode CUDA graph is captured per context bucket (256 / 768 / ...): every step across the bucket edges
     n_past = 254..258 and 510..514 is bit-exact, and so is a prefill chunk that straddles an edge"""
     t = B.QUANT_TYPES[name]
-    hp, tens = synth.make_llama(dict(synth.CONFIGS["small"], n_ctx=1024), t, orc.quantize)
+    hp, tens = synth.make_llama(dict(GRAPH_SMALL, n_ctx=1024), t, orc.quantize)
     toks = synth.make_tokens(hp, 530)
     mo = _cpu_model(orc, hp, tens, n_threads=8)
     m, s = native(hp, tens, 1024, 256)
     check(s.evaluate(toks[:254], all_logits=True), mo.eval(toks[:254]), "prefill 254")
     for i in range(254, 259):
         check(s.evaluate(toks[i:i + 1], all_logits=True), mo.eval(toks[i:i + 1]), f"decode {i}")
+        assert s.last_launches == 7 * hp["n_layer"] + 3, ("fused decode graph not used", i, s.last_launches)
     check(s.evaluate(toks[259:510], all_logits=True), mo.eval(toks[259:510]), "prefill 259..509 (straddles 256)")
     for i in range(510, 515):
         check(s.evaluate(toks[i:i + 1], all_logits=True), mo.eval(toks[i:i + 1]), f"decode {i}")
+        assert s.last_launches == 7 * hp["n_layer"] + 3, ("fused decode graph not used", i, s.last_launches)
     check(s.evaluate(toks[515:530], all_logits=True), mo.eval(toks[515:530]), "batch 15 past 512")
     for which in (0, 1):
         a = s.kv(which)
@@ -307,7 +314,7 @@ def test_decode_graph_bucket_edges(orc, name):
 def test_rope_overrides(orc):
     """ModelParameters::rope_overrides (frequency_base / frequency_scale) reach every RoPE of prefill and of the decode graph"""
     import llm_b200
-    hp, tens = synth.make_llama(synth.CONFIGS["small"], B.Q4_0, orc.quantize)
+    hp, tens = synth.make_llama(GRAPH_SMALL, B.Q4_0, orc.quantize)
     toks = synth.make_tokens(hp, 48)
     mo = orc.llama(hp, tens)
     mo.set_rope(26000.0, 0.5)
@@ -316,6 +323,7 @@ def test_rope_overrides(orc):
     check(s.evaluate(toks[:40], all_logits=True), mo.eval(toks[:40]), "prefill, rope overrides")
     for i in range(40, 44):
         check(s.evaluate(toks[i:i + 1], all_logits=True), mo.eval(toks[i:i + 1]), f"decode {i}, rope overrides")
+        assert s.last_launches == 7 * hp["n_layer"] + 3, ("fused decode graph not used", s.last_launches)
     s.close(); m.close()
 
 

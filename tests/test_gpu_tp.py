@@ -26,6 +26,20 @@ WORKER = textwrap.dedent('''
     orc = B.Oracle()
     base = dict(synth.CONFIGS[cfg_name]) if cfg_name in synth.CONFIGS else json.loads(cfg_name)
     hp, tens = synth.make_llama(base, B.QUANT_TYPES[qname], orc.quantize)
+    if os.environ.get("TP_START_CTX"):            # session start only: which context sizes a tensor-parallel session accepts
+        started = {}
+        for n_ctx in json.loads(os.environ["TP_START_CTX"]):
+            m = tp.TpLlama(hp, llm_b200.ModelParameters(context_size=n_ctx), tens, rank=rank, world=world, device=local_rank)
+            try:
+                m.start_session(llm_b200.InferenceSessionConfig(n_batch=8), dist).close()
+                started[n_ctx] = True
+            except RuntimeError:
+                started[n_ctx] = False
+            m.close()
+        open(os.path.join(os.environ["RESULT_DIR"], "rank%%d.json" %% rank), "w").write(json.dumps({"rank": rank, "started": started}))
+        dist.barrier()
+        dist.destroy_process_group()
+        sys.exit(0)
     toks = synth.make_tokens(hp, n_steps + 4)
     m = tp.TpLlama(hp, llm_b200.ModelParameters(context_size=hp["n_ctx"]), tens, rank=rank, world=world, device=local_rank)
     s = m.start_session(llm_b200.InferenceSessionConfig(n_batch=8), dist)
@@ -65,10 +79,12 @@ def n_gpus():
         return torch.cuda.device_count()
 
 
-def run_tp(tmp_path, world, cfg, quant, steps, port):
+def run_tp(tmp_path, world, cfg, quant, steps, port, start_ctx=None):
     script = tmp_path / "tp_worker.py"
     script.write_text(WORKER)
     env = dict(os.environ, OMP_NUM_THREADS="4", RESULT_DIR=str(tmp_path), TP_CFG=cfg, TP_QUANT=quant, TP_STEPS=str(steps))
+    if start_ctx:
+        env["TP_START_CTX"] = json.dumps(start_ctx)
     out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
                           "--master-port", str(port), str(script)], capture_output=True, text=True, timeout=900, env=env)
     if out.returncode != 0:                                        # keep the workers' own words (pytest truncates long assertion payloads)
@@ -91,6 +107,16 @@ def test_tensor_parallel_decode_bit_exact(tmp_path, world, cfg, quant):
     res = run_tp(tmp_path, world, json.dumps(TP_CFGS[cfg]), quant, 40, 29530 + world)
     for r in res:
         assert r["bad"] == [] and r["kv_ok"] and r["timeouts"] == 0, r
+
+
+def test_tensor_parallel_context_limit(tmp_path):
+    """the exchange lives in the fused attention kernel, which holds a whole context bucket in shared memory (at most 3264 positions): a
+    longer context_size is refused when the session starts instead of aborting the first decode step past n_past 3072"""
+    if n_gpus() < 2:
+        pytest.skip("needs 2 GPUs")
+    res = run_tp(tmp_path, 2, json.dumps(TP_CFGS["mha"]), "q4_0", 0, 29539, start_ctx=[4096, 3264])
+    for r in res:
+        assert r["started"] == {"4096": False, "3264": True}, r
 
 
 @pytest.mark.slow
