@@ -102,11 +102,13 @@ typedef struct {
     uint64_t offset, nbytes;      /* TensorLoadInfo::start_offset, calc_size() */
 } b200_ggml_tensor_info;
 
-enum { B200_ARCH_LLAMA = 0, B200_ARCH_GPT2 = 1, B200_ARCH_GPTNEOX = 2 };         /* whose Hyperparameters::read_ggml lays out the header */
+enum { B200_ARCH_LLAMA = 0, B200_ARCH_GPT2 = 1, B200_ARCH_GPTNEOX = 2, B200_ARCH_MPT = 3, B200_ARCH_BLOOM = 4 };   /* whose Hyperparameters::read_ggml lays out the header */
 b200_ggml_file *b200_ggml_open(const char *path, int *err);                     /* LLaMA header; NULL + *err on LoadError */
 b200_ggml_file *b200_ggml_open_arch(const char *path, int32_t arch, int *err);
 /* the header words in file order: llama n_vocab n_embd n_mult n_head n_layer n_rot file_type | gpt2 n_vocab n_ctx n_embd n_head n_layer file_type n_vocab |
- * gptneox n_vocab n_ctx n_embd n_head n_layer n_rot use_parallel_residual file_type */
+ * gptneox n_vocab n_ctx n_embd n_head n_layer n_rot use_parallel_residual file_type |
+ * mpt n_embd max_seq_len n_head n_layer n_vocab alibi_bias_max(f32 bits) clip_kqv(f32 bits) file_type (mpt lib.rs:317-330; the vocabulary count is word 4) |
+ * bloom n_vocab n_embd n_mult n_head n_layer file_type */
 int     b200_ggml_hparams(const b200_ggml_file *f, int32_t *arch, int32_t *words8, int32_t *n_words);
 void    b200_ggml_close(b200_ggml_file *f);
 int     b200_ggml_container(const b200_ggml_file *f, uint32_t *magic, uint32_t *version);      /* ContainerType */
@@ -195,6 +197,16 @@ typedef struct b200_neox_hparams {
 typedef struct b200_neox_model b200_neox_model;
 typedef struct b200_neox_session b200_neox_session;
 b200_neox_model *b200_neox_new(const b200_neox_hparams *hp);
+/* MPT (crates/models/mpt) and BLOOM (crates/models/bloom) on the same runtime: the GPT-2 block (qkv rows in thirds, no RoPE, sequential residual,
+ * gelu FFN of width 4 n_embd) with ALiBi on the scaled scores (ggml_alibi: + key position x per-head slope, before the causal mask).
+ *   arch 2 = MPT: "transformer.wte.weight" (also the output projection), "transformer.norm_f.weight", "transformer.blocks.N.{norm_1.weight,
+ *            attn.Wqkv.weight, attn.out_proj.weight, norm_2.weight, ffn.up_proj.weight, ffn.down_proj.weight}"; no biases; alibi_bias_max from the header
+ *   arch 3 = BLOOM: "tok_embeddings.weight", "norm.{weight,bias}" (LayerNorm of the embedding row), "output_norm.{weight,bias}", "output.weight",
+ *            "layers.N.{attention_norm,ffn_norm}.{weight,bias}", "layers.N.attention.{query_key_value,wo}.{weight,bias}",
+ *            "layers.N.feed_forward.{w1,w2}.{weight,bias}"; alibi_bias_max 8 (bloom lib.rs:240)
+ * n_rot, use_parallel_residual and has_lm_head are ignored.  NULL for any other arch (and b200_neox_new returns NULL for 2 and 3).  Every other
+ * b200_neox_* entry point serves these models unchanged. */
+b200_neox_model *b200_neox_new_alibi(const b200_neox_hparams *hp, float alibi_bias_max);
 int  b200_neox_load_tensor(b200_neox_model *m, const char *name, int32_t type, const void *host_data, size_t nbytes);
 int  b200_neox_synthesize(b200_neox_model *m, uint64_t seed);          /* seeded weights generated in HBM (bench) */
 size_t b200_neox_weight_bytes(b200_neox_model *m);                     /* bytes streamed per decoded token */

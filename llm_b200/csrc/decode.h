@@ -52,6 +52,7 @@ struct NeoxLayer {
 struct NeoxParams {
     int n_layer, e, hd, n_head, n_ctx, n_vocab, n_rot, parallel_residual;
     int gpt2;                                   // GPT-2 (crates/models/gpt2/src/lib.rs:138-329): c_attn rows are [q | k | v] thirds, no RoPE, learned positions wpe, sequential residual
+                                                // (also set for MPT and BLOOM, which share the row layout and have no wpe)
     const float *wpe;                           // [n_ctx][e] f32 (GPT-2), else nullptr
     QWeight wte, lm_head;
     const float *lnf_g, *lnf_b;
@@ -61,7 +62,12 @@ struct NeoxParams {
     const int32_t *token; int *n_past;
     float *x, *qkv, *q, *attn_out, *logits;     // residual stream [e], raw qkv [3e], roped q [e], attention branch output [e]
     int4 *xpack_a, *xpack_d, *xpack_f;          // records: layer-norm output (K = e), attention rows (K = e), gelu output (K = 4e)
+    // MPT / BLOOM (crates/models/{mpt,bloom}): the GPT-2 row layout (gpt2 = 1, wpe = nullptr) plus ALiBi; MPT leaves every bias pointer null
+    const float *alibi = nullptr;               // per-head ALiBi slopes [n_head] (alibi_slopes), else nullptr
+    const float *emb_g = nullptr, *emb_b = nullptr;   // BLOOM: LayerNorm of the embedding row before layer 0, else nullptr
 };
+// ggml_alibi's per-head slopes (LC/ggml.c:11570-11588), computed with the host's libm powf exactly as the reference computes them
+std::vector<float> alibi_slopes(int n_head, float max_bias);
 void decode_set_tp(const TpCtx &T, cudaStream_t st);   // uploads the tensor-parallel context the decode kernels read (constant memory)
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches);
 

@@ -151,7 +151,8 @@ __global__ void __launch_bounds__(256) norm_pack_tp_kernel(const float *__restri
 }
 
 // ---- mat-vec with fused epilogues --------------------------------------------------------------------------------------------------
-enum { EPI_RES = 0, EPI_QKV = 1, EPI_SILU = 2, EPI_LOGITS = 3, EPI_BIAS = 4, EPI_GELU = 5 };   // BIAS / GELU: GPT-NeoX (bias adds, gelu table)
+// BIAS / GELU: GPT-NeoX (bias adds, gelu table); GELU_NB: gelu without a bias node (MPT)
+enum { EPI_RES = 0, EPI_QKV = 1, EPI_SILU = 2, EPI_LOGITS = 3, EPI_BIAS = 4, EPI_GELU = 5, EPI_GELU_NB = 6 };
 
 struct MmvArgs {
     const int4 *xpack;            // input records
@@ -256,9 +257,9 @@ __global__ void __launch_bounds__(STHREADS) mmv_fused_kernel(const QWeight w, co
             A.dst[row] = out;
         }, 1, A.prof);
         if (A.n_past_inc && blockIdx.x == 0 && tid == 0) *A.n_past_inc = *A.n_past_inc + 1;
-    } else if (EPI == EPI_GELU) {   // one 32-row tile = one quant block of the next mat-vec's input (rows past N: zero activations)
+    } else if (EPI == EPI_GELU || EPI == EPI_GELU_NB) {   // one 32-row tile = one quant block of the next mat-vec's input (rows past N: zero activations)
         consume_matvec<TYPE>(w, sx, R, blockIdx.x, gridDim.x, tid, [&](int64_t row, float v) {
-            if ((tid & 3) == 0) stash[row & 31] = row < w.N ? __fadd_rn(v, __ldg(A.bias + row)) : 0.f;
+            if ((tid & 3) == 0) stash[row & 31] = row < w.N ? (EPI == EPI_GELU ? __fadd_rn(v, __ldg(A.bias + row)) : v) : 0.f;
             compute_sync();
             if (warp == 0) {
                 const float4 a = ((const float4 *)stash)[lane & 7];
@@ -448,12 +449,15 @@ __device__ __forceinline__ void fma8(float (&acc)[8], const int4 &a, const int4 
     }
 }
 
+//
+// ALIBI (MPT, BLOOM): the score of key position j in head h is fma(j, slope[h], kq * kq_scale) -- ggml_alibi (LC/ggml.c:11534-11597) on the
+// scaled scores, one fused multiply-add as the reference's x86 build compiles it; the slopes come from alibi_slopes() on the host.
 constexpr int ATH = 256;
-template <bool TP>
-__global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
-                                                         int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
-                                                         float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                                                         unsigned long long *prof, const TpSync S, int head0) {
+template <bool TP, bool ALIBI>
+__device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
+                                                int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
+                                                float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                                                unsigned long long *prof, const TpSync &S, int head0, const float *__restrict__ alibi) {
     const TpCtx &T = c_tp;
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
@@ -519,6 +523,7 @@ __global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict
 
     // ---- KQ for this CTA's share of the positions ----
     {
+        const float slope = ALIBI ? __ldg(alibi + h) : 0.f;
         for (int jb = j0; jb < j1; jb += PU * (ATH / 4)) {
             if (jb != j0) {                                      // later passes (contexts beyond 4 * ATH / 4 positions per CTA)
 #pragma unroll
@@ -538,7 +543,8 @@ __global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict
 #pragma unroll
                 for (int i = 0; i < 4; i++) if (i < nvec) fma8(acc, kv[pu][i], *(const int4 *)(q16 + 32 * i + 8 * u));
                 const float s = quad_tree(acc);
-                if (j < j1 && u < per_head) cluster.map_shared_rank(sc, u)[j] = __fmul_rn(s, kq_scale);   // thread u of the quad feeds CTA u
+                if (j < j1 && u < per_head)                      // thread u of the quad feeds CTA u
+                    cluster.map_shared_rank(sc, u)[j] = ALIBI ? __fmaf_rn((float)j, slope, __fmul_rn(s, kq_scale)) : __fmul_rn(s, kq_scale);
             }
         }
     }
@@ -595,6 +601,20 @@ __global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict
         }
     }
     prof_end(prof);
+}
+template <bool TP>
+__global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
+                                                         int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
+                                                         float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                                                         unsigned long long *prof, const TpSync S, int head0) {
+    attn_fused_body<TP, false>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, nullptr);
+}
+// the ALiBi form (single GPU): alibi = the per-head slopes [n_head]
+__global__ void __launch_bounds__(ATH) attn_fused_alibi_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
+                                                               int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
+                                                               float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                                                               unsigned long long *prof, const TpSync S, int head0, const float *__restrict__ alibi) {
+    attn_fused_body<false, true>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, alibi);
 }
 
 // ---- ring and grid plan of the decode mat-vecs ------------------------------------------------------------------------------------------------
@@ -722,6 +742,7 @@ static void attn_fused_reserve(size_t bytes) {
     if (bytes <= set) return;
     B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_fused_alibi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
 // dynamic shared memory of attn_fused_kernel for nlay positions and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
@@ -731,11 +752,12 @@ size_t attn_fused_smem(int nlay, int hd) {
 }  // namespace
 bool attn_fused_fits(int nlay, int hd) { return attn_fused_smem(nlay, hd) <= 227 * 1024; }
 namespace {
-// one cluster of hd/32 CTAs per head; a programmatic dependent of its predecessor unless B200_PDL clears bit 1
+// one cluster of hd/32 CTAs per head; a programmatic dependent of its predecessor unless B200_PDL clears bit 1.  alibi: per-head slopes (the
+// ALiBi form, single GPU only) or nullptr
 template <bool TP>
 void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const __half *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
                        float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                       unsigned long long *prof, const TpSync &S, int head0) {
+                       unsigned long long *prof, const TpSync &S, int head0, const float *alibi = nullptr) {
     const size_t smem = attn_fused_smem(nlay, hd);
     attn_fused_reserve(smem);
     cudaLaunchConfig_t cfg{};
@@ -746,6 +768,12 @@ void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const 
     at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = (pdl_mask() & 2) ? 2 : 1;
+    if (alibi) {
+        B200_ASSERT(!TP);
+        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_alibi_kernel, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+                                      q81, off, scale16, prof, S, head0, alibi));
+        return;
+    }
     B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
                                   q81, off, scale16, prof, S, head0));
 }
@@ -863,8 +891,10 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
 // ---- GPT-NeoX --------------------------------------------------------------------------------------------------------------------------------
 // LayerNorm (ggml_compute_forward_norm_f32, LC/ggml.c:10063-10111) * gain + bias -> Q8 records.  Same shape as norm_pack_kernel: every CTA reduces
 // the whole row from registers (two passes: mean, then the variance of the centred values) and packs its own 32 blocks.
-__global__ void __launch_bounds__(256) ln_pack_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
-                                                      int e, int q81, int off, int scale16) {
+// BIAS false (MPT): norm * gain only -- no add node, so a -0 stays -0.
+template <bool BIAS>
+__device__ __forceinline__ void ln_pack_body(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
+                                             int e, int q81, int off, int scale16) {
     __shared__ double shd[8];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     pdl_trigger();
@@ -876,7 +906,7 @@ __global__ void __launch_bounds__(256) ln_pack_kernel(const float *__restrict__ 
     for (int k = 0; k < MAXV; k++) { const int i = tid + k * 256; v[k] = i < nv ? __ldcg((const float4 *)x + i) : make_float4(0.f, 0.f, 0.f, 0.f); }
     const bool active = mine < nv;
     const float4 gv = active ? __ldg((const float4 *)gain + mine) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float4 bv = active ? __ldg((const float4 *)bias + mine) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 bv = BIAS && active ? __ldg((const float4 *)bias + mine) : make_float4(0.f, 0.f, 0.f, 0.f);
     auto total = [&](double s) {
         s = warp_sum(s);
         __syncthreads();
@@ -900,9 +930,22 @@ __global__ void __launch_bounds__(256) ln_pack_kernel(const float *__restrict__ 
     const float variance = (float)(total(s2) / (double)e);
     const float scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(variance, 1e-5f)));
     float4 y;
-    y.x = __fadd_rn(__fmul_rn(__fmul_rn(xv.x, scale), gv.x), bv.x); y.y = __fadd_rn(__fmul_rn(__fmul_rn(xv.y, scale), gv.y), bv.y);
-    y.z = __fadd_rn(__fmul_rn(__fmul_rn(xv.z, scale), gv.z), bv.z); y.w = __fadd_rn(__fmul_rn(__fmul_rn(xv.w, scale), gv.w), bv.w);
+    if (BIAS) {
+        y.x = __fadd_rn(__fmul_rn(__fmul_rn(xv.x, scale), gv.x), bv.x); y.y = __fadd_rn(__fmul_rn(__fmul_rn(xv.y, scale), gv.y), bv.y);
+        y.z = __fadd_rn(__fmul_rn(__fmul_rn(xv.z, scale), gv.z), bv.z); y.w = __fadd_rn(__fmul_rn(__fmul_rn(xv.w, scale), gv.w), bv.w);
+    } else {
+        y.x = __fmul_rn(__fmul_rn(xv.x, scale), gv.x); y.y = __fmul_rn(__fmul_rn(xv.y, scale), gv.y);
+        y.z = __fmul_rn(__fmul_rn(xv.z, scale), gv.z); y.w = __fmul_rn(__fmul_rn(xv.w, scale), gv.w);
+    }
     pack_quad(y, pack + (active ? mine >> 3 : 0) * 4, lane, active, q81, off, scale16);
+}
+__global__ void __launch_bounds__(256) ln_pack_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
+                                                      int e, int q81, int off, int scale16) {
+    ln_pack_body<true>(x, gain, bias, pack, e, q81, off, scale16);
+}
+__global__ void __launch_bounds__(256) ln_pack_nobias_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
+                                                             int e, int q81, int off, int scale16) {
+    ln_pack_body<false>(x, gain, bias, pack, e, q81, off, scale16);
 }
 
 // qkv [3e] (bias added) -> q [e], k -> f16 cache row n_past, v -> f16 cache column n_past.  GPT-NeoX (gptneox lib.rs:205-247): rows per head are q | k | v
@@ -950,40 +993,50 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     int n = 0;
     // the token boundary: a plain launch (no programmatic attribute), so nothing of this token starts before the previous token has completed --
     // attn_fused_kernel reads n_past and the older KV cache ahead of its griddepcontrol.wait on that guarantee
-    get_rows_q(P.wte, P.token, P.x, 1, st); n++;
+    if (P.emb_g) {                                                // BLOOM (bloom lib.rs:139-144): the row, then LayerNorm -> the residual stream
+        get_rows_q(P.wte, P.token, P.qkv, 1, st); n++;
+        layer_norm(P.qkv, P.x, P.emb_g, P.emb_b, e, 1, st); n++;
+    } else {
+        get_rows_q(P.wte, P.token, P.x, 1, st); n++;
+    }
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
     const size_t fa_smem = attn_fused_smem(nlay, P.hd);
     B200_ASSERT(P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd) && e <= 8192);   // neox.cu::forward checks both
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
-    const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
-    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wqkv, footprint_of(neox_rope_store_kernel, 256, 0) + footprint_of(attn_fused_kernel<false>, ATH, fa_smem));
+    // MPT has no biases: its norms take ln_pack_nobias_kernel and its up-projection the gelu epilogue without a bias node
+    const bool biased = layers[0].ln1_b != nullptr, fc_bias = layers[0].bfc != nullptr;
+    auto ln_kernel = biased ? ln_pack_kernel : ln_pack_nobias_kernel;
+    const CtaFootprint f_ln = footprint_of(ln_kernel, 256, 0);
+    const CtaFootprint f_attn = P.alibi ? footprint_of(attn_fused_alibi_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
+    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wqkv, footprint_of(neox_rope_store_kernel, 256, 0) + f_attn);
     const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
-    const MmvPlan &p_fc = mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta);
+    const MmvPlan &p_fc = fc_bias ? mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta) : mmv_plan<TYPE, EPI_GELU_NB, false>(layers[0].wfc, p_proj.cta);
     const MmvPlan &p_dense = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wdense, f_ln + p_fc.cta);
     const MmvPlan &p_head = mmv_plan<TYPE, EPI_BIAS, false>(P.lm_head, CtaFootprint{});
     for (int il = 0; il < P.n_layer; il++) {
         const NeoxLayer &L = layers[il];
-        launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;          // :192-196
+        launch_k(ln_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;               // :192-196
         MmvArgs A{}; A.xpack = P.xpack_a; A.dst = P.qkv; A.bias = L.bqkv;
         launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, p_qkv, st); n++;                                                                                      // :199-200
         launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, L.K, L.V, (const int *)P.n_past, P.rope_cs, P.rope_half,
                  P.gpt2 ? 0 : P.n_rot, P.hd, e, P.n_ctx, P.gpt2 ? P.hd : 3 * P.hd, P.gpt2 ? e : P.hd, P.gpt2 ? 2 * e : 2 * P.hd); n++;               // :205-247
         launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, nlay, q81, off, s16,
-                                 nullptr, S, 0); n++;                                                                                     // :250-298
+                                 nullptr, S, 0, P.alibi); n++;                                                                            // :250-298
         // attention.dense (+bias); sequential residual: ff_in = that + inpL                                                                    :301-312
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out; Bo.bias = L.bdense; Bo.add1 = P.parallel_residual ? nullptr : P.x;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;
         // mlp: LayerNorm of inpL (parallel residual) or of ff_in                                                                                :313-316 / ffn
-        launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)(P.parallel_residual ? P.x : P.attn_out), L.ln2_g, L.ln2_b, P.xpack_a, e, q81, off, s16); n++;
+        launch_k(ln_kernel, ln_grid, dim3(256), 0, st, (const float *)(P.parallel_residual ? P.x : P.attn_out), L.ln2_g, L.ln2_b, P.xpack_a, e, q81, off, s16); n++;
         MmvArgs C{}; C.xpack = P.xpack_a; C.xpack_out = P.xpack_f; C.bias = L.bfc; C.lut_gelu = P.lut_gelu; C.q81 = q81; C.off = off; C.scale16 = s16;
-        launch_mmv<TYPE, EPI_GELU>(L.wfc, C, p_fc, st); n++;
+        if (fc_bias) launch_mmv<TYPE, EPI_GELU>(L.wfc, C, p_fc, st); else launch_mmv<TYPE, EPI_GELU_NB>(L.wfc, C, p_fc, st);
+        n++;
         // parallel: inpL = ((proj + bias) + attn) + inpL; sequential: inpL = (proj + bias) + ff_in                                              :317-325
         MmvArgs D{}; D.xpack = P.xpack_f; D.dst = P.x; D.bias = L.bproj; D.add1 = P.attn_out; D.add2 = P.parallel_residual ? P.x : nullptr;
         launch_mmv<TYPE, EPI_BIAS>(L.wproj, D, p_proj, st); n++;
     }
-    launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16); n++;                     // :332-334
+    launch_k(ln_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16); n++;                          // :332-334
     MmvArgs Z{}; Z.xpack = P.xpack_a; Z.dst = P.logits; Z.n_past_inc = P.n_past;
     launch_mmv<TYPE, EPI_BIAS>(P.lm_head, Z, p_head, st); n++;                                                                                        // :342
     B200_CHECK(cudaGetLastError());

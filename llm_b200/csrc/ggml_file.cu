@@ -9,6 +9,8 @@
 //   llama Hyperparameters        crates/models/llama/src/lib.rs:425-447     7 x i32: n_vocab n_embd n_mult n_head n_layer n_rot file_type
 //   gpt2 Hyperparameters         crates/models/gpt2/src/lib.rs:394-416      6 x i32: n_vocab n_ctx n_embd n_head n_layer file_type, then n_vocab AGAIN (must match)
 //   gptneox Hyperparameters      crates/models/gptneox/src/lib.rs:431-442   8 x i32: n_vocab n_ctx n_embd n_head n_layer n_rot use_parallel_residual(0|1) file_type
+//   mpt Hyperparameters          crates/models/mpt/src/lib.rs:317-330       n_embd max_seq_len n_head n_layer n_vocab (i32), alibi_bias_max clip_kqv (f32), file_type
+//   bloom Hyperparameters        crates/models/bloom/src/lib.rs             6 x i32: n_vocab n_embd n_mult n_head n_layer file_type
 //   FileType                     crates/llm-base/src/loader.rs:32-50        file_type = quantization_version * 1000 + llama_ftype
 //   quantization version rule    crates/llm-base/src/loader.rs:459-484      0 is read as 1 (GGJT v2) / 2 (GGJT v3); quantized tensors require 2
 //   ggml::format::save           crates/ggml/src/format/saver.rs:86-160     the writer (GGJT v3)
@@ -81,10 +83,10 @@ void b200_ggml_close(b200_ggml_file *f) {
 
 static b200_ggml_file *open_arch_impl(const char *path, int32_t arch, int *err) {
     int dummy; if (!err) err = &dummy;
-    if (arch < 0 || arch > 2) { *err = B200_ERR_BAD_ARG; return nullptr; }
+    if (arch < 0 || arch > B200_ARCH_BLOOM) { *err = B200_ERR_BAD_ARG; return nullptr; }
     *err = B200_OK;
     b200_ggml_file *f = new b200_ggml_file();
-    f->arch = arch; f->n_hp = arch == B200_ARCH_LLAMA ? 7 : arch == B200_ARCH_GPT2 ? 7 : 8;
+    f->arch = arch; f->n_hp = arch == B200_ARCH_LLAMA ? 7 : arch == B200_ARCH_GPT2 ? 7 : arch == B200_ARCH_BLOOM ? 6 : 8;
     auto fail = [&](int code) -> b200_ggml_file * { *err = code; b200_ggml_close(f); return nullptr; };
     f->fd = open(path, O_RDONLY);
     struct stat sb;
@@ -109,14 +111,16 @@ static b200_ggml_file *open_arch_impl(const char *path, int32_t arch, int *err) 
 
     for (int i = 0; i < f->n_hp; i++) f->hp[i] = (int32_t)rd32();
     if (eof) return fail(B200_ERR_IO);
-    for (int i = 0; i < f->n_hp; i++) if (f->hp[i] < 0) return fail(B200_ERR_INVARIANT_BROKEN);      // usize::try_from in the reference
+    for (int i = 0; i < f->n_hp; i++)                                                                 // usize::try_from in the reference; MPT's words 5 and 6
+        if (f->hp[i] < 0 && !(arch == B200_ARCH_MPT && (i == 5 || i == 6))) return fail(B200_ERR_INVARIANT_BROKEN);   // are f32 (read_f32 takes any value)
     if (arch == B200_ARCH_GPT2 && f->hp[6] != f->hp[0]) return fail(B200_ERR_INVARIANT_BROKEN);     // "GPT2 model expected n_vocab {} found {}"
     if (arch == B200_ARCH_GPTNEOX && f->hp[6] > 1) return fail(B200_ERR_IO);                        // read_bool: InvalidData
 
     const bool scored = f->magic == MAGIC_GGMF || f->magic == MAGIC_GGJT;
-    if ((uint64_t)f->hp[0] > (f->size - pos) / 4) return fail(B200_ERR_IO);       // every token record takes at least 4 bytes: a corrupt count cannot ask for gigabytes
-    f->tokens.reserve((size_t)f->hp[0]);
-    for (int32_t i = 0; i < f->hp[0]; i++) {
+    const int32_t n_vocab = f->hp[arch == B200_ARCH_MPT ? 4 : 0];                // MPT: n_embd max_seq_len n_head n_layer n_vocab ...
+    if ((uint64_t)n_vocab > (f->size - pos) / 4) return fail(B200_ERR_IO);       // every token record takes at least 4 bytes: a corrupt count cannot ask for gigabytes
+    f->tokens.reserve((size_t)n_vocab);
+    for (int32_t i = 0; i < n_vocab; i++) {
         const uint32_t len = rd32();
         if (eof || pos + len > f->size) return fail(B200_ERR_IO);
         f->tokens.emplace_back(pos, len);

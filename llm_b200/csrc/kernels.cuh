@@ -92,6 +92,8 @@ void top_k_rows(const float *x, int64_t n, int k, int32_t *ids, float *vals, cud
 void layer_norm(const float *x, float *y, const float *gain, const float *bias, int64_t n, int64_t rows, cudaStream_t st);
 // rows of nc: optional scale, optional causal mask (col > n_past + (row % nr) -> -inf), softmax through the fp16 exp table
 void soft_max(const float *x, float *y, int64_t nc, int64_t rows, int64_t nr, float scale, bool do_scale, int n_past, bool do_mask, bool do_softmax, cudaStream_t st);
+// scale, ALiBi (column i of a row of head row / nr: fma(i, alibi[head], v)), causal mask, softmax -- the MPT / BLOOM attention (alibi: device slopes)
+void soft_max_alibi(const float *x, float *y, int64_t nc, int64_t rows, int64_t nr, float scale, int n_past, const float *alibi, cudaStream_t st);
 enum { UNARY_SILU = 0, UNARY_GELU = 1 };
 void unary_lut(int which, const float *x, float *y, int64_t n, cudaStream_t st);
 // y = silu(a) * b  (silu node then mul node, llama lib.rs:328-330)

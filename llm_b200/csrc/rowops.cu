@@ -185,8 +185,11 @@ void layer_norm(const float *x, float *y, const float *gain, const float *bias, 
 
 // ---- scale -> diag_mask_inf -> soft_max (LC/ggml.c:10733, 11268-11316, 11352-11421), any subset, one pass over the row ---
 // Row values live in shared memory between the passes (rows are <= n_ctx floats).
-__global__ void soft_max_kernel(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int do_scale,
-                                int n_past, int do_mask, int do_softmax, const uint16_t *__restrict__ t_exp) {
+// ALIBI: between scale and mask, column i of a row of head r / nr gets fma(i, alibi[head], v) (ggml_alibi, LC/ggml.c:11534-11597, one fused
+// multiply-add as the reference's x86 build compiles it)
+template <bool ALIBI>
+__device__ __forceinline__ void soft_max_body(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int do_scale,
+                                              int n_past, int do_mask, int do_softmax, const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi) {
     extern __shared__ float row[];
     __shared__ double shd[32];
     __shared__ float shf[32];
@@ -195,9 +198,11 @@ __global__ void soft_max_kernel(const float *__restrict__ x, float *__restrict__
     const float *xr = x + r * nc;
     float *yr = y + r * nc;
     float mx = -INFINITY;
+    const float slope = ALIBI ? alibi[r / nr] : 0.f;
     for (int64_t i = threadIdx.x; i < nc; i += blockDim.x) {
         float v = xr[i];
         if (do_scale) v = __fmul_rn(v, scale);
+        if (ALIBI) v = __fmaf_rn((float)i, slope, v);
         if (do_mask && i > n_past + j) v = -INFINITY;
         row[i] = v;
         mx = fmaxf(mx, v);
@@ -218,6 +223,26 @@ __global__ void soft_max_kernel(const float *__restrict__ x, float *__restrict__
     const double sum = block_sum(s, shd);
     const float inv = (float)(1.0 / sum);
     for (int64_t i = threadIdx.x; i < nc; i += blockDim.x) yr[i] = __fmul_rn(row[i], inv);
+}
+__global__ void soft_max_kernel(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int do_scale,
+                                int n_past, int do_mask, int do_softmax, const uint16_t *__restrict__ t_exp) {
+    soft_max_body<false>(x, y, nc, nr, scale, do_scale, n_past, do_mask, do_softmax, t_exp, nullptr);
+}
+__global__ void soft_max_alibi_kernel(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int n_past,
+                                      const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi) {
+    soft_max_body<true>(x, y, nc, nr, scale, 1, n_past, 1, 1, t_exp, alibi);
+}
+void soft_max_alibi(const float *x, float *y, int64_t nc, int64_t rows, int64_t nr, float scale, int n_past, const float *alibi, cudaStream_t st) {
+    if (rows == 0 || nc == 0) return;
+    const size_t smem = (size_t)nc * sizeof(float);
+    static size_t smem_set = 48 * 1024;
+    if (smem > smem_set) {
+        B200_ASSERT(smem <= 200 * 1024);
+        B200_CHECK(cudaFuncSetAttribute(soft_max_alibi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        smem_set = smem;
+    }
+    soft_max_alibi_kernel<<<(unsigned)rows, nc >= 1024 ? 256 : 128, smem, st>>>(x, y, nc, nr, scale, n_past, luts().exp, alibi);
+    B200_CHECK(cudaGetLastError());
 }
 void soft_max(const float *x, float *y, int64_t nc, int64_t rows, int64_t nr, float scale, bool do_scale, int n_past, bool do_mask, bool do_softmax, cudaStream_t st) {
     if (rows == 0 || nc == 0) return;

@@ -26,12 +26,19 @@ class LoadError(Exception):
         super().__init__(f"{what}: {self.kind}")
 
 
-ARCH = {"llama": 0, "gpt2": 1, "gptneox": 2}
+ARCH = {"llama": 0, "gpt2": 1, "gptneox": 2, "mpt": 3, "bloom": 4}
 HPARAM_NAMES = {
     "llama": ("n_vocab", "n_embd", "n_mult", "n_head", "n_layer", "n_rot", "file_type"),                                   # llama lib.rs:425-447
     "gpt2": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "file_type", "n_vocab_again"),                              # gpt2 lib.rs:394-416
     "gptneox": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "n_rot", "use_parallel_residual", "file_type"),          # gptneox lib.rs:431-442
+    "mpt": ("n_embd", "max_seq_len", "n_head", "n_layer", "n_vocab", "alibi_bias_max", "clip_kqv", "file_type"),          # mpt lib.rs:317-330
+    "bloom": ("n_vocab", "n_embd", "n_mult", "n_head", "n_layer", "file_type"),                                           # bloom lib.rs
 }
+FLOAT_WORDS = {"alibi_bias_max", "clip_kqv"}                                                                             # f32 in the header (read_f32)
+
+
+def _f32_bits(x) -> int:
+    return int(np.array([x], np.float32).view(np.int32)[0])
 
 
 class GgmlFile:
@@ -50,7 +57,10 @@ class GgmlFile:
         """The header words of the file, named after the architecture's Hyperparameters struct."""
         arch, words, n = C.c_int32(), (C.c_int32 * 8)(), C.c_int32()
         self.L.b200_ggml_hparams(self._f, C.byref(arch), C.byref(words), C.byref(n))
-        return dict(zip(HPARAM_NAMES[self.arch], list(words)[:n.value]))
+        out = dict(zip(HPARAM_NAMES[self.arch], list(words)[:n.value]))
+        for k in FLOAT_WORDS & out.keys():
+            out[k] = float(np.array([out[k]], np.int32).view(np.float32)[0])
+        return out
 
     @property
     def container(self) -> Tuple[str, int]:
@@ -139,9 +149,9 @@ def write_llama(path: str, hyperparameters: Dict[str, int], tensors: Dict[str, n
 
 def write_model(path: str, arch: str, header: Dict[str, int], tensors: Dict[str, np.ndarray], shapes: Dict[str, Tuple[int, ...]], wtype: int,
                 vocabulary: Optional[Sequence[Tuple[bytes, float]]] = None):
-    """ggml::format::save for any of the three architectures: `header` holds the words of HPARAM_NAMES[arch]."""
+    """ggml::format::save for any of the architectures: `header` holds the words of HPARAM_NAMES[arch] (FLOAT_WORDS as floats)."""
     L = _lib.lib()
-    words = [int(header[k]) if k != "n_vocab_again" else int(header["n_vocab"]) for k in HPARAM_NAMES[arch]]
+    words = [_f32_bits(header[k]) if k in FLOAT_WORDS else int(header["n_vocab"]) if k == "n_vocab_again" else int(header[k]) for k in HPARAM_NAMES[arch]]
     infos = (_lib.GgmlTensorInfo * len(tensors))()
     datas = (C.c_void_p * len(tensors))()
     keep = []

@@ -2,6 +2,7 @@
 
   GptNeoX(KnownModel)     crates/models/gptneox/src/lib.rs:36-140     new / start_session / evaluate
   Hyperparameters         crates/models/gptneox/src/lib.rs (n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, file_type)
+  Gpt2 / Mpt / Bloom      crates/models/{gpt2,mpt,bloom} on the same runtime (Mpt, Bloom: ALiBi attention, b200_neox_new_alibi)
   InferenceSession        crates/llm-base/src/inference_session.rs     evaluate / n_past / rewind
 No arithmetic happens in Python."""
 import ctypes as C
@@ -23,6 +24,8 @@ def _bind(L):
     vp, i32 = C.c_void_p, C.c_int32
     L.b200_neox_new.restype = vp
     L.b200_neox_new.argtypes = [C.POINTER(NeoxHparams)]
+    L.b200_neox_new_alibi.restype = vp
+    L.b200_neox_new_alibi.argtypes = [C.POINTER(NeoxHparams), C.c_float]
     L.b200_neox_load_tensor.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
     L.b200_neox_synthesize.argtypes = [vp, C.c_uint64]
     L.b200_neox_weight_bytes.restype = C.c_size_t
@@ -56,13 +59,16 @@ class GptNeoX(_Native):
         hp = NeoxHparams(n_vocab=hyperparameters["n_vocab"], n_embd=hyperparameters["n_embd"], n_head=hyperparameters["n_head"], n_layer=hyperparameters["n_layer"],
                          n_rot=int(hyperparameters.get("n_rot", 0)), use_parallel_residual=int(hyperparameters.get("use_parallel_residual", 1)), wtype=hyperparameters["wtype"],
                          context_size=self.context_size, arch=self.ARCH, has_lm_head=int(bool(tensors) and "model/lm_head" in tensors))
-        self._m = self.L.b200_neox_new(C.byref(hp))
+        self._m = self._new(hp)
         if not self._m:
             raise ValueError(f"b200_neox_new rejected {hyperparameters}")
         for name, arr in (tensors or {}).items():
             arr = np.ascontiguousarray(arr)
             typ = 0 if arr.dtype == np.float32 else int(hyperparameters["wtype"])
             _check(self.L.b200_neox_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes), f"load_tensor({name})")
+
+    def _new(self, hp):
+        return self.L.b200_neox_new(C.byref(hp))
 
     def synthesize(self, seed: int = 0x4E580000):
         _check(self.L.b200_neox_synthesize(self._m, seed), "synthesize")
@@ -80,6 +86,29 @@ class Gpt2(GptNeoX):
     "model/wpe" (f32), "model/ln_f/g|b", optional "model/lm_head", "model/hN/{ln_1,ln_2}/{g,b}", "model/hN/attn/{c_attn,c_proj}/{w,b}",
     "model/hN/mlp/{c_fc,c_proj}/{w,b}".  context_size is the model's n_ctx (the rows of wpe)."""
     ARCH = 1
+
+
+class Mpt(GptNeoX):
+    """KnownModel for MPT (crates/models/mpt): hyperparameters n_vocab, n_ctx, n_embd, n_head, n_layer, wtype, alibi_bias_max (the header's float;
+    clip_kqv is read by the reference but never applied); tensors "transformer.wte.weight" (also the output projection), "transformer.norm_f.weight",
+    "transformer.blocks.N.{norm_1,norm_2}.weight", "transformer.blocks.N.attn.{Wqkv,out_proj}.weight", "transformer.blocks.N.ffn.{up_proj,down_proj}.weight"."""
+    ARCH = 2
+
+    def _alibi_bias_max(self):
+        return float(self.hyperparameters["alibi_bias_max"])
+
+    def _new(self, hp):
+        return self.L.b200_neox_new_alibi(C.byref(hp), self._alibi_bias_max())
+
+
+class Bloom(Mpt):
+    """KnownModel for BLOOM (crates/models/bloom): hyperparameters n_vocab, n_ctx, n_embd, n_head, n_layer, wtype; ALiBi bias 8 (bloom lib.rs:240);
+    tensors "tok_embeddings.weight", "norm.{weight,bias}", "output_norm.{weight,bias}", "output.weight", "layers.N.{attention_norm,ffn_norm}.{weight,bias}",
+    "layers.N.attention.{query_key_value,wo}.{weight,bias}", "layers.N.feed_forward.{w1,w2}.{weight,bias}"."""
+    ARCH = 3
+
+    def _alibi_bias_max(self):
+        return 8.0
 
 
 class NeoxSession(_Native):
