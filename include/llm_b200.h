@@ -49,7 +49,6 @@ typedef struct {
 enum {
     B200_SESSION_NO_GRAPH = 1,     /* launch the decode kernels one by one instead of replaying the captured CUDA graph (debug) */
     B200_SESSION_UNFUSED  = 2,     /* decode with the prefill schedule (one kernel per reference graph node, the seam's kernels) */
-    B200_SESSION_MEGA     = 8,     /* experimental: one persistent cooperative kernel per decoded token (decode.cu) instead of the graph */
     B200_SESSION_FAST     = 4,     /* order-free kernels: integer-exact block dots but a different f32 summation order than the
                                       reference's AVX2 build.  NOT conformant: the reference graph amplifies 1e-7 differences to ~1e-2
                                       in the logits (DESIGN.md "chaos").  Default (flag clear) = bit-exact kernels. */
@@ -150,9 +149,6 @@ int  b200_session_set_n_past(b200_session *s, int32_t n_past);   /* rewind (supp
 /* raw f16 KV cache bytes (get_snapshot, inference_session.rs:599-646): which = 0 memory_k, 1 memory_v */
 int  b200_session_read_kv(b200_session *s, int32_t which, void *host_out, size_t nbytes);
 int  b200_session_sync(b200_session *s);
-/* with B200_DECODE_PROF=1 in the environment the decode kernel stamps %globaltimer (ns) at its phase boundaries (CTA 0);
- * slot 0 = start, then pairs (before / after grid barrier) per phase in graph order, slot 127 = end of token */
-int  b200_session_decode_profile(b200_session *s, unsigned long long *out128);
 /* tuning aid (B200_DECODE_PROF=1): per-launch %globaltimer stamps of the graph decode schedule; out = 8*n values, see session.cu */
 int  b200_session_decode_timeline(b200_session *s, unsigned long long *out, int n, int reset);
 /* debug taps for parity work: keep a copy of one intermediate buffer of (layer, stage) during the next evaluate.

@@ -70,7 +70,6 @@ def lib():
     L.b200_session_set_n_past.argtypes = [vp, i32]
     L.b200_session_read_kv.argtypes = [vp, i32, vp, sz]
     L.b200_session_sync.argtypes = [vp]
-    L.b200_session_decode_profile.argtypes = [vp, vp]
     L.b200_session_decode_timeline.argtypes = [vp, vp, C.c_int, C.c_int]
     L.b200_session_set_tap.argtypes = [vp, i32, i32]
     L.b200_session_read_tap.restype = i64

@@ -1,4 +1,4 @@
-// llm_b200/csrc/decode.h -- parameters of the decode schedules (decode.cu, decode_ops.cu) and the sessions' cache of decode graphs
+// llm_b200/csrc/decode.h -- parameters of the decode schedules (decode_ops.cu) and the sessions' cache of decode graphs
 #pragma once
 #include <functional>
 #include <utility>
@@ -20,7 +20,6 @@ struct DecodeLayer {
 };
 
 struct DecodeParams {
-    const DecodeLayer *layers;
     int n_layer;
     QWeight wte, output;
     const float *norm;
@@ -29,18 +28,16 @@ struct DecodeParams {
     const float2 *rope_cs; int rope_half;
     const uint16_t *lut_silu, *lut_exp;
     const int32_t *token;
-    int *n_past;                        // device copy of InferenceSession::n_past; incremented at the end of the kernel
-    float *x, *q, *kq, *attn, *ff, *h13, *logits;
-    int scratch_bytes;                  // decode_scratch_bytes(): per-CTA shared memory behind the weight ring
-    int4 *xpack_d, *xpack_f;            // activation records produced by phase C (for wo) and phase E (for w2)
+    int *n_past;                        // device copy of InferenceSession::n_past; the step's last kernel increments it
+    float *x, *q, *kq, *ff, *logits;
+    int4 *xpack_d, *xpack_f;            // activation records of wo's input (written by the attention kernel) and of w2's input (the w13 epilogue)
     // tensor-parallel decode (tp.cuh): dims above are THIS RANK's (n_head, n_head_kv, gqa = local heads / cache width; f = local n_ff / G;
     // n_vocab = local rows of the lm_head) except e = the full n_embd; e_loc = n_embd / G (q rows, rows of wo / w2 owned here)
     TpCtx tp;
     int e_loc = 0, head0 = 0;           // first global head of this rank
     int n_vocab_full = 0;               // rows of the whole lm_head (the gathered logits)
     int64_t row0_e = 0, row0_w13 = 0, row0_v = 0;   // first row of this rank in the full wo / w2 output, the interleaved [w1|w3] rows, the lm_head
-    unsigned int *bar;                  // [0] arrival count, [1] generation
-    unsigned long long *prof;   /* graph schedule: 3 x B200_PROF_SLOTS timeline slots (begin | end | prologue done) */           // optional: %globaltimer stamps of CTA 0 at phase boundaries (debug / tuning), 128 slots
+    unsigned long long *prof;           // optional (B200_DECODE_PROF): 8 x B200_PROF_SLOTS per-launch %globaltimer slots, see b200_session_decode_timeline
 };
 
 // ---- GPT-NeoX (crates/models/gptneox/src/lib.rs:156-350) fused decode schedule: 8 kernels per layer, same mat-vec core -------------------------
@@ -71,11 +68,6 @@ std::vector<float> alibi_slopes(int n_head, float max_bias);
 void decode_set_tp(const TpCtx &T, cudaStream_t st);   // uploads the tensor-parallel context the decode kernels read (constant memory)
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches);
 
-int decode_scratch_bytes(int e, int f, int hd, int n_ctx);
-bool decode_supported(const DecodeParams &P, int wtype);
-// cooperative launch on `st`; returns false if the kernel cannot be made resident (caller falls back to the per-op schedule)
-bool launch_decode(const DecodeParams &P, int wtype, cudaStream_t st, int *grid_out);
-
 // whether attn_fused_kernel's shared memory for a bucket of nlay positions (a multiple of 64) and head size hd fits the 227 KB opt-in limit:
 // true up to nlay = 3264 for every hd <= 128.  Past it LLaMA decodes with the two-kernel attention and GPT-NeoX / GPT-2 per op.
 bool attn_fused_fits(int nlay, int hd);
@@ -98,10 +90,9 @@ struct DecodeGraphCache {
 
     // the context bucket a step at position n_kv - 1 runs in: n_kv rounded up to 256 positions, at most n_ctx
     static int bucket(int n_kv, int n_ctx);
-    // uploads n_past if the device copy is stale (after a prefill, a rewind, or steps that did not run the graph)
-    void sync_n_past(int n_past, cudaStream_t st);
     // one decode step at position n_kv - 1 (its last kernel increments *d_n_past): enqueue(bucket, st, &nodes) enqueues the schedule for up to
-    // `bucket` positions.  Runs it eagerly on the first step or when replay is false, else replays (capturing on first use) the bucket's graph.
+    // `bucket` positions.  Uploads n_past first if the device copy is stale (after a prefill, a rewind, or steps that did not run the schedule).
+    // Runs it eagerly on the first step or when replay is false, else replays (capturing on first use) the bucket's graph.
     // Returns the step's launch count.
     int run(int n_kv, int n_ctx, bool replay, const std::function<void(int, cudaStream_t, int *)> &enqueue, cudaStream_t st);
     // destroys every graph (they hold kernel arguments that changed)

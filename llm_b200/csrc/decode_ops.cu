@@ -4,16 +4,15 @@
 //   2 mmv<QKV>         [wq|wk|wv] x, epilogue: RoPE on Q/K rows, K/V rows -> f16 cache at n_past (:190-244)
 //   3 attn_fused       KQ = K . f16(Q), scale + soft_max, V^T . f16(P), epilogue: quantize the merged row -- one cluster of hd/32 CTAs per
 //                      head, scores exchanged through distributed shared memory                (:246-307)
-//                      (B200_ATTN_FUSED=0: the two-kernel variant attn_kq + attn_sv)
+//                      (buckets past 3264 positions: the two-kernel variant attn_kq + attn_sv)
 //   4 mmv<RES>         wo x + inpSA                                                           (:310-314)
 //   5 norm_pack        rms_norm(inpFF) * ffn_norm                                             (:318-321)
 //   6 mmv<SILU>        [w1|w3] x (rows interleaved in 32-row pieces), epilogue: silu(w1 x) * (w3 x) quantized (:323-330)
 //   7 mmv<RES>         w2 h + inpFF                                                           (:332-334)
 // Everything that depends on the position reads n_past from DEVICE memory, so the captured graph is valid for every token; the
-// last node increments it.  All arithmetic is the bit-exact arithmetic of exact.cu / rowops.cu (same device functions as decode.cu).
+// last node increments it.  All arithmetic is the bit-exact arithmetic of exact.cu / rowops.cu.
 // Variants that were tried on top of this and not kept: norm fusion, tiled weights + TMA, L2 prefetch.
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 #include <algorithm>
 #include <array>
@@ -37,7 +36,7 @@ namespace {
 // Programmatic dependent launch.  Every kernel of the chain touches nothing a predecessor writes (and writes nothing at all) before
 // `pdl_wait`; what runs ahead of the wait only reads the constant weights (the producer warp of the next mat-vec fills its ring).
 // WHERE the dependents are released matters: triggered at kernel entry, the successors sit on SM resources the running kernel's tail needs;
-// the default triggers from the producer warp as soon as every byte of the CTA is requested (B200_PDL_EARLY=0: after the last tile is consumed).
+// a mat-vec triggers from its producer warp as soon as every byte of the CTA is requested.
 // tuning aid: per-launch timeline (DecodeParams::prof), see b200_session_decode_timeline
 __device__ __forceinline__ unsigned long long gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ void prof_begin(unsigned long long *p) { if (p && threadIdx.x == 0) { const unsigned long long t = gtime(); atomicMin(p, t); atomicMax(p + 3 * B200_PROF_SLOTS, t); } }
@@ -47,21 +46,15 @@ __device__ __forceinline__ void prof_end(unsigned long long *p) { if (p && threa
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// B200_PDL: bit 0 = the weight mat-vecs are launched as programmatic dependents, bit 1 = the small kernels between them too (default 3)
-int pdl_mask() {
-    static int mask = -1;
-    if (mask < 0) { const char *e = getenv("B200_PDL"); mask = e ? atoi(e) : 3; }
-    return mask;
-}
-
-template <int CLASS = 2, typename... KArgs, typename... Args>
+// a launch as a programmatic dependent of its predecessor on `st`
+template <typename... KArgs, typename... Args>
 void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args &&...args) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = (pdl_mask() & CLASS) ? 1 : 0;
+    cfg.attrs = at; cfg.numAttrs = 1;
     B200_CHECK(cudaLaunchKernelEx(&cfg, kern, KArgs(args)...));
 }
 
@@ -170,7 +163,6 @@ struct MmvArgs {
     int q81, off, scale16;
     int *n_past_inc;              // EPI_LOGITS: the last node of the token increments InferenceSession::n_past on the device
     int nst;                      // ring depth chosen by mmv_plan
-    int pdl_early;                // trigger the dependents from the producer warp once every byte is requested (B200_PDL_EARLY, default 1)
     unsigned long long *prof;
     // tensor-parallel decode (tp.cuh): this rank owns rows [row0, row0 + w.N) of the full matrix; results go to buffer dst_buf of every rank
     TpSync ts; int64_t row0;
@@ -179,7 +171,6 @@ static_assert(sizeof(QWeight) + sizeof(MmvArgs) <= 256, "mat-vec argument block:
 
 template <int TYPE, int EPI, bool TP>
 __global__ void __launch_bounds__(STHREADS) mmv_fused_kernel(const QWeight w, const MmvArgs A) {
-    const bool pdl_early = A.pdl_early != 0;
     using T = St<TYPE>;
     extern __shared__ __align__(128) uint8_t smem[];
     Ring R{(uint64_t *)smem, (uint64_t *)smem + SST_MAX, smem + 256, 0u, (uint32_t)A.nst};
@@ -191,7 +182,7 @@ __global__ void __launch_bounds__(STHREADS) mmv_fused_kernel(const QWeight w, co
     __syncthreads();
     if (tid >= SCOMPUTE) {                                      // weights only: runs ahead of the predecessors
         produce_matvec<TYPE>(w, R, blockIdx.x, gridDim.x, tid & 31, G);
-        if (pdl_early) pdl_trigger();                           // every byte of this CTA is requested: let the successor's CTAs take the free slots
+        pdl_trigger();                                          // every byte of this CTA is requested: let the successor's CTAs take the free slots
         return;
     }
     if (!(TP && (c_tp.relax & 2) && A.ts.in_buf >= 0)) pdl_wait();    // records and addend arrive as tagged units: no dependence on the predecessor's completion (tp.cuh)
@@ -682,12 +673,11 @@ const MmvPlan &mmv_plan(const QWeight &w, const CtaFootprint &succ) {
     using T = St<TYPE>;
     auto kern = mmv_fused_kernel<TYPE, EPI, TP>;
     static std::map<std::array<int64_t, 5>, MmvPlan> plans;
-    static int smem_set = 0, depth_cap = -1;
+    static int smem_set = 0;
     const std::array<int64_t, 5> key{w.N, w.nb, succ.smem, succ.regs, succ.threads};
     auto it = plans.find(key);
     if (it != plans.end()) return it->second;
     const SmLimits &L = sm_limits();
-    if (depth_cap < 0) { const char *e = getenv("B200_RING_DEPTH"); depth_cap = e ? atoi(e) : SST_MAX; if (depth_cap < 2) depth_cap = 2; if (depth_cap > SST_MAX) depth_cap = SST_MAX; }
     auto smem_of = [&](int nst) { return 256 + T::ring_bytes(nst) + (int)w.nb * 64 + 256; };
     if (smem_of(SST_MAX) > smem_set) {
         const int want = smem_of(SST_MAX) < 227 * 1024 ? smem_of(SST_MAX) : 227 * 1024;
@@ -709,7 +699,7 @@ const MmvPlan &mmv_plan(const QWeight &w, const CtaFootprint &succ) {
             if (max_groups_per_sm(groups, grid, L.sms) > fair) continue;
             const int per_cta = (int)((groups + grid - 1) / grid) * chunks;
             int nst = 0;
-            for (int c = 2; c <= depth_cap && c <= (per_cta > 2 ? per_cta : 2); c++) {
+            for (int c = 2; c <= SST_MAX && c <= (per_cta > 2 ? per_cta : 2); c++) {
                 if (smem_of(c) > 227 * 1024) break;
                 int occ = 0;
                 B200_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, STHREADS, smem_of(c)));
@@ -719,7 +709,7 @@ const MmvPlan &mmv_plan(const QWeight &w, const CtaFootprint &succ) {
                 if (occ < k || all.smem > L.smem || all.regs > L.regs || all.threads > L.threads || all.ctas > L.ctas) break;
                 nst = c;
             }
-            const int need = pass == 2 ? 2 : std::min({min_stages, per_cta, depth_cap});
+            const int need = pass == 2 ? 2 : std::min({min_stages, per_cta, SST_MAX});
             if (nst < need || nst < 2) continue;
             best.nst = nst; best.grid = (int)grid; best.smem = smem_of(nst);
             best.cta = base; best.cta.smem += best.smem;
@@ -732,8 +722,7 @@ const MmvPlan &mmv_plan(const QWeight &w, const CtaFootprint &succ) {
 template <int TYPE, int EPI, bool TP = false>
 void launch_mmv(const QWeight &w, MmvArgs A, const MmvPlan &plan, cudaStream_t st) {
     A.nst = plan.nst;
-    { static int pe = -1; if (pe < 0) { const char *e = getenv("B200_PDL_EARLY"); pe = e ? atoi(e) : 1; } A.pdl_early = pe; }
-    launch_k<1>(mmv_fused_kernel<TYPE, EPI, TP>, dim3((unsigned)plan.grid), dim3(STHREADS), (size_t)plan.smem, st, w, A);
+    launch_k(mmv_fused_kernel<TYPE, EPI, TP>, dim3((unsigned)plan.grid), dim3(STHREADS), (size_t)plan.smem, st, w, A);
 }
 
 // dynamic shared memory opt-in of the cluster attention kernel: one high-water mark for both instantiations (the attribute is per function, not per caller)
@@ -752,8 +741,8 @@ size_t attn_fused_smem(int nlay, int hd) {
 }  // namespace
 bool attn_fused_fits(int nlay, int hd) { return attn_fused_smem(nlay, hd) <= 227 * 1024; }
 namespace {
-// one cluster of hd/32 CTAs per head; a programmatic dependent of its predecessor unless B200_PDL clears bit 1.  alibi: per-head slopes (the
-// ALiBi form, single GPU only) or nullptr
+// one cluster of hd/32 CTAs per head, a programmatic dependent of its predecessor.  alibi: per-head slopes (the ALiBi form, single GPU only)
+// or nullptr
 template <bool TP>
 void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const __half *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
                        float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
@@ -767,7 +756,7 @@ void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const 
     at[0].val.clusterDim.x = hd / 32; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = (pdl_mask() & 2) ? 2 : 1;
+    cfg.attrs = at; cfg.numAttrs = 2;
     if (alibi) {
         B200_ASSERT(!TP);
         B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_alibi_kernel, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
@@ -826,12 +815,11 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     // attn_fused_kernel reads n_past and the older KV cache ahead of its griddepcontrol.wait on that guarantee
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     if (tp) { launch_k(tp_spread_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.x, e); n++; }
-    // attention: one cluster launch per layer (default) or the two-kernel variant (B200_ATTN_FUSED=0, head sizes a cluster cannot cover, or
-    // buckets whose scores and V rows do not fit one CTA's shared memory)
-    static const bool fused_env = !(getenv("B200_ATTN_FUSED") && getenv("B200_ATTN_FUSED")[0] == '0');
+    // attention: one cluster launch per layer, or the two-kernel variant for head sizes a cluster cannot cover and for buckets whose scores
+    // and V rows do not fit one CTA's shared memory
     const int nlay = (n_kv_bucket + 63) / 64 * 64;
     const size_t fa_smem = attn_fused_smem(nlay, P.hd);
-    const bool fused_attn = (fused_env || tp) && P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd);
+    const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd);
     B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue (start_session_tp checks the size)
     const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
     static size_t sv_set = 48 * 1024;
@@ -1086,18 +1074,14 @@ DecodeGraphCache::~DecodeGraphCache() {
     B200_CHECK(cudaFreeHost(h_n_past));
 }
 
-void DecodeGraphCache::sync_n_past(int n_past, cudaStream_t st) {
-    if (dev_n_past == n_past) return;
-    B200_CHECK(cudaStreamSynchronize(st));      // the pinned staging word may still be in flight
-    *h_n_past = n_past;
-    B200_CHECK(cudaMemcpyAsync(d_n_past, h_n_past, sizeof(int), cudaMemcpyHostToDevice, st));
-    dev_n_past = n_past;
-}
-
 int DecodeGraphCache::bucket(int n_kv, int n_ctx) { return std::min((n_kv + 255) / 256 * 256, n_ctx); }
 
 int DecodeGraphCache::run(int n_kv, int n_ctx, bool replay, const std::function<void(int, cudaStream_t, int *)> &enqueue, cudaStream_t st) {
-    sync_n_past(n_kv - 1, st);
+    if (dev_n_past != n_kv - 1) {
+        B200_CHECK(cudaStreamSynchronize(st));      // the pinned staging word may still be in flight
+        *h_n_past = n_kv - 1;
+        B200_CHECK(cudaMemcpyAsync(d_n_past, h_n_past, sizeof(int), cudaMemcpyHostToDevice, st));
+    }
     const int bucket = DecodeGraphCache::bucket(n_kv, n_ctx);
     int nodes = 0;
     if (!warm || !replay) {

@@ -357,8 +357,7 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     P.x = s->x.get(); P.qkv = s->qkv.get(); P.q = s->qdec.get(); P.attn_out = s->attn.get(); P.logits = s->logits.get();
     P.xpack_a = s->xpack_a.get(); P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
     QWeight p1; p1.nb = (int64_t)e / QK; QWeight p2; p2.nb = 4 * (int64_t)e / QK;
-    s->decode_ok = m->hd % 32 == 0 && m->hd <= 128 && e % 128 == 0 && e <= 8192 && n_ctx % 8 == 0 && mmv_exact_stream_supported(p1) && mmv_exact_stream_supported(p2) &&
-                   !getenv("B200_NEOX_UNFUSED");
+    s->decode_ok = m->hd % 32 == 0 && m->hd <= 128 && e % 128 == 0 && e <= 8192 && n_ctx % 8 == 0 && mmv_exact_stream_supported(p1) && mmv_exact_stream_supported(p2);
     B200_CHECK(cudaDeviceSynchronize());
     return s;
 }

@@ -49,12 +49,11 @@ struct b200_session : SessionCore {     // memory_k [n_layer][n_ctx][gqa], memor
     DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh;
     PinnedBuf<int32_t> h_topk;
     int last_n = 0;
-    // one-launch-per-token decode kernel (decode.cu)
+    // the graph decode schedule (decode_ops.cu)
     DeviceBuf<unsigned long long> d_prof;
-    DeviceBuf<DecodeLayer> d_layers; DeviceBuf<unsigned int> d_bar;
-    DeviceBuf<float> qbuf, attn; DeviceBuf<int4> xpack_d, xpack_f;
-    bool mega_ok = false; int mega_grid = 0;
-    std::vector<DecodeLayer> h_layers;                 // host copy of the layer table (kernel arguments of the decode graph)
+    DeviceBuf<float> qbuf; DeviceBuf<int4> xpack_d, xpack_f;
+    bool graph_ok = false;                             // the session's geometry decodes through the graph schedule
+    std::vector<DecodeLayer> h_layers;                 // the layer table (kernel arguments of the decode graph)
     DeviceBuf<int4> xpack_a;
     DecodeParams dp;
     // debug taps (tests): copy one intermediate buffer of (layer, stage) aside during forward()
@@ -126,26 +125,13 @@ void forward(b200_session *s, int n, bool all_rows = true) {
     const bool tp = m->tp_world > 1;
     const bool fast = !tp && (s->cfg.flags & B200_SESSION_FAST) != 0;
     if (tp && (n != 1 || !s->tp_connected)) { fprintf(stderr, "llm_b200: tensor-parallel sessions decode one token per step, after b200_session_tp_connect\n"); exit(1); }
-    // On one GPU mega_ok is decode_supported(), the one-kernel decode's predicate, and it gates the graph schedule too: a geometry with
-    // n_embd > 6144 or context_size % 128 != 0 decodes on the per-op schedule below even without B200_SESSION_MEGA.
-    if (n == 1 && s->mega_ok && !fast && (tp || (!(s->cfg.flags & B200_SESSION_UNFUSED) && s->tap_layer == -2))) {
-        if (!tp && (s->cfg.flags & B200_SESSION_MEGA)) {
-            // experimental: the whole token in one persistent cooperative kernel (decode.cu)
-            s->decode.sync_n_past(n_past, st);
-            if (launch_decode(s->dp, hp.wtype, st, &s->mega_grid)) {
-                s->decode.dev_n_past = n_past + 1;      // the kernel increments it
-                s->last_launches = 1; s->last_n = 1; s->n_past += 1;
-                return;
-            }
-            s->mega_ok = false;
-        } else {
-            // default: 7 fused kernels per layer, replayed from one CUDA graph per token (decode_ops.cu)
-            s->last_launches = s->decode.run(n_kv, n_ctx, !(s->cfg.flags & B200_SESSION_NO_GRAPH), [s, &hp](int bucket, cudaStream_t st, int *nodes) {
-                decode_ops_enqueue(s->dp, s->h_layers, hp.wtype, bucket, s->xpack_a.get(), st, nodes);
-            }, st);
-            s->last_n = 1; s->n_past += 1;
-            return;
-        }
+    if (n == 1 && s->graph_ok && !fast && (tp || (!(s->cfg.flags & B200_SESSION_UNFUSED) && s->tap_layer == -2))) {
+        // 7 fused kernels per layer, replayed from one CUDA graph per token (decode_ops.cu)
+        s->last_launches = s->decode.run(n_kv, n_ctx, !(s->cfg.flags & B200_SESSION_NO_GRAPH), [s, &hp](int bucket, cudaStream_t st, int *nodes) {
+            decode_ops_enqueue(s->dp, s->h_layers, hp.wtype, bucket, s->xpack_a.get(), st, nodes);
+        }, st);
+        s->last_n = 1; s->n_past += 1;
+        return;
     }
     int il = -1;
     auto TAP = [&](int stage, const float *buf, size_t count) {
@@ -451,23 +437,23 @@ static b200_session *start_session_tp(b200_session *s) {
     const RopeTable &rt_ = rope_table(hp.n_rot, 0, hp.rope_freq_base, hp.rope_freq_scale, m->hd, (int)n_ctx);
     s->h_layers = decode_layers(s);
     DecodeParams &P = s->dp;
-    P.layers = nullptr; P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
+    P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
     P.e = (int)e; P.f = m->f_loc; P.hd = m->hd; P.gqa = m->gqa_loc; P.n_head = hp.n_head / G; P.n_head_kv = hp.n_head_kv / G; P.n_ctx = (int)n_ctx; P.n_vocab = m->v_loc;
     P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f;
     P.rope_cs = rt_.cs; P.rope_half = rt_.half;
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
-    P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = nullptr; P.attn = nullptr; P.ff = nullptr; P.h13 = nullptr; P.logits = s->logits.get();
-    P.xpack_d = nullptr; P.xpack_f = nullptr; P.bar = nullptr; P.scratch_bytes = 0;
+    P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = nullptr; P.ff = nullptr; P.logits = s->logits.get();
+    P.xpack_d = nullptr; P.xpack_f = nullptr;
     P.e_loc = m->e_loc; P.head0 = r * (hp.n_head / G); P.n_vocab_full = hp.n_vocab;
     P.row0_e = (int64_t)r * m->e_loc; P.row0_w13 = (int64_t)r * 2 * m->f_loc; P.row0_v = (int64_t)r * m->v_loc;
     P.prof = nullptr;
     QWeight probe; probe.nb = (int64_t)e / QK;
     QWeight probe2; probe2.nb = (int64_t)f / QK;
-    s->mega_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && mmv_exact_stream_supported(probe) && mmv_exact_stream_supported(probe2) &&
-                 m->gqa_loc % 32 == 0 && m->e_loc % 32 == 0 && hp.context_size % 8 == 0;
+    s->graph_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && mmv_exact_stream_supported(probe) && mmv_exact_stream_supported(probe2) &&
+                  m->gqa_loc % 32 == 0 && m->e_loc % 32 == 0 && hp.context_size % 8 == 0;
     B200_CHECK(cudaDeviceSynchronize());
-    if (!s->mega_ok) { fprintf(stderr, "llm_b200: tensor-parallel session: geometry not supported by the fused decode schedule\n"); b200_session_free(s); return nullptr; }
+    if (!s->graph_ok) { fprintf(stderr, "llm_b200: tensor-parallel session: geometry not supported by the fused decode schedule\n"); b200_session_free(s); return nullptr; }
     return s;
 }
 
@@ -495,26 +481,26 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     s->xh = device_alloc<__half>(xh_bytes(kmax, B));
     const RopeTable &rt_ = rope_table(hp.n_rot, 0, hp.rope_freq_base, hp.rope_freq_scale, m->hd, (int)n_ctx);
     // decode kernel parameters
-    s->attn = device_alloc<float>(e * 4);
-    s->d_bar = device_zeros<unsigned int>(2 * sizeof(unsigned int));
     s->h_layers = decode_layers(s);
-    s->d_layers = device_alloc<DecodeLayer>(s->h_layers.size() * sizeof(DecodeLayer));
-    B200_CHECK(cudaMemcpy(s->d_layers.get(), s->h_layers.data(), s->h_layers.size() * sizeof(DecodeLayer), cudaMemcpyHostToDevice));
     DecodeParams &P = s->dp;
-    P.layers = s->d_layers.get(); P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
+    P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
     P.e = (int)e; P.f = (int)f; P.hd = m->hd; P.gqa = m->gqa; P.n_head = hp.n_head; P.n_head_kv = hp.n_head_kv; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab;
     P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f;
     P.rope_cs = rt_.cs; P.rope_half = rt_.half;
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
-    P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = s->kq.get(); P.attn = s->attn.get(); P.ff = s->ff.get(); P.h13 = s->h13.get(); P.logits = s->logits.get();
-    P.bar = s->d_bar.get();
+    P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = s->kq.get(); P.ff = s->ff.get(); P.logits = s->logits.get();
     s->xpack_d = device_alloc<int4>((e / QK) * 64);
     s->xpack_f = device_alloc<int4>((f / QK) * 64);
     P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
-    P.scratch_bytes = decode_scratch_bytes((int)e, (int)f, m->hd, (int)n_ctx);
     P.prof = getenv("B200_DECODE_PROF") ? s->d_prof.get() : nullptr;
-    s->mega_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && decode_supported(P, hp.wtype);
+    // The graph schedule takes RoPE over whole heads of 64 or 128 channels and mat-vecs whose K (n_embd, n_ff) the streaming core takes, a multiple
+    // of 256.  With what llama_new_impl checks, that covers the rest: a classic weight type, a K/V width n_head_kv * hd of whole 32-row tiles.
+    // n_embd <= 6144 and context_size % 128 == 0 are limits of the removed one-kernel decode, kept so that the same geometries decode through the graph.
+    QWeight probe; probe.nb = (int64_t)e / QK;
+    QWeight probe2; probe2.nb = (int64_t)f / QK;
+    s->graph_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && mmv_exact_stream_supported(probe) && mmv_exact_stream_supported(probe2) &&
+                  e <= 6144 && n_ctx % 128 == 0;
     B200_CHECK(cudaDeviceSynchronize());   // the memsets / copies above ran on the legacy stream: order them before anything on the backend's non-blocking stream
     return s;
 }
@@ -600,13 +586,6 @@ int64_t b200_session_read_tap(b200_session *s, float *host_out, int64_t max_coun
     const size_t c = s->tap_count < (size_t)max_count ? s->tap_count : (size_t)max_count;
     if (c) B200_CHECK(cudaMemcpy(host_out, s->tap.get(), c * 4, cudaMemcpyDeviceToHost));
     return (int64_t)c;
-}
-
-int b200_session_decode_profile(b200_session *s, unsigned long long *out128) {
-    if (!s || !out128) return B200_ERR_BAD_ARG;
-    B200_CHECK(cudaStreamSynchronize(rt().stream));
-    B200_CHECK(cudaMemcpy(out128, s->d_prof.get(), 128 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    return B200_OK;
 }
 
 // Per-kernel timeline of the graph decode schedule (B200_DECODE_PROF=1): slot i = the i-th launch of the token;

@@ -1,5 +1,5 @@
 // llm_b200/csrc/stream_core.cuh -- building blocks of the bit-exact streaming mat-vec, shared by the stand-alone kernel
-// (exact_stream.cu) and the one-launch-per-token decode kernel (decode.cu).  See exact_stream.cu for the design notes.
+// (exact_stream.cu) and the fused mat-vecs of the decode schedules (decode_ops.cu).  See exact_stream.cu for the design notes.
 #pragma once
 #include "kernels.cuh"
 

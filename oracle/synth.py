@@ -12,7 +12,7 @@ from . import bindings as B
 CONFIGS = {
     # tiny shapes the CPU oracle finishes in milliseconds; K multiples of 64 (Q4 row rule, crates/ggml/src/lib.rs:112-118)
     "tiny":   dict(n_vocab=320, n_embd=256, n_head=4, n_head_kv=4, n_layer=2, n_ff=704, n_rot=64, n_ctx=128),
-    # shapes the one-launch decode kernel accepts (K % 256 == 0), incl. grouped-query attention
+    # shapes the decode graph accepts (K % 256 == 0), incl. grouped-query attention
     "tiny8":  dict(n_vocab=320, n_embd=256, n_head=4, n_head_kv=4, n_layer=2, n_ff=768, n_rot=64, n_ctx=128),
     "gqa8":   dict(n_vocab=352, n_embd=512, n_head=8, n_head_kv=2, n_layer=3, n_ff=1024, n_rot=64, n_ctx=256),
     "small":  dict(n_vocab=1024, n_embd=512, n_head=8, n_head_kv=8, n_layer=3, n_ff=1408, n_rot=64, n_ctx=256),

@@ -80,17 +80,16 @@ def test_native_vs_oracle(orc, cfg, name, n_prompt):
     s.close(); m.close()
 
 
-@pytest.mark.parametrize("mode", ["graph", "mega"])
 @pytest.mark.parametrize("cfg,name", [("tiny8", "q4_0"), ("tiny8", "q4_1"), ("tiny8", "q5_0"), ("tiny8", "q5_1"), ("tiny8", "q8_0"), ("gqa8", "q4_0"), ("gqa8", "q5_1")])
-def test_decode_kernel_bit_exact(orc, cfg, name, mode):
-    """decode schedules: 'graph' = 8 fused kernels per layer replayed from a CUDA graph (decode_ops.cu, the default), 'mega' = one
-    persistent cooperative kernel per token (decode.cu, experimental).  Prefill, then 40 decode steps, each side on its own KV cache."""
+def test_decode_kernel_bit_exact(orc, cfg, name):
+    """the decode schedule: 7 fused kernels per layer replayed from a CUDA graph (decode_ops.cu).  Prefill, then 40 decode steps, each side
+    on its own KV cache."""
     t = B.QUANT_TYPES[name]
     hp, tens = synth.make_llama(synth.CONFIGS[cfg], t, orc.quantize)
     toks = synth.make_tokens(hp, 70)
     mo = orc.llama(hp, tens)
-    m, s = native(hp, tens, hp["n_ctx"], 64, flags=8 if mode == "mega" else 0)
-    want_launches = 1 if mode == "mega" else 7 * hp["n_layer"] + 3      # 7 fused kernels per layer (attention = one cluster launch)
+    m, s = native(hp, tens, hp["n_ctx"], 64)
+    want_launches = 7 * hp["n_layer"] + 3      # 7 fused kernels per layer (attention = one cluster launch)
     check(s.evaluate(toks[:21], all_logits=True), mo.eval(toks[:21]), "prefill")
     for i in range(21, 61):
         g = s.evaluate(toks[i:i + 1], all_logits=True)

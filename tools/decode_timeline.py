@@ -16,7 +16,7 @@ toks = np.random.default_rng(0).integers(0, 32000, 520, dtype=np.int32)
 s.evaluate(toks[:512])
 for i in range(5):
     s.evaluate(toks[512 + i:513 + i])
-per_layer = ["norm", "qkv", "attn", "wo", "norm2", "w13", "w2"] if os.environ.get("B200_ATTN_FUSED", "1") != "0" else ["norm", "qkv", "kq", "sv", "wo", "norm2", "w13", "w2"]
+per_layer = ["norm", "qkv", "attn", "wo", "norm2", "w13", "w2"]      # the 2048-position context decodes with the cluster attention
 n = len(per_layer) * nl + 3
 L.b200_session_decode_timeline(s._s, None, 0, 1)
 s.evaluate(toks[517:518])
