@@ -101,13 +101,14 @@ typedef struct {
     uint64_t offset, nbytes;      /* TensorLoadInfo::start_offset, calc_size() */
 } b200_ggml_tensor_info;
 
-enum { B200_ARCH_LLAMA = 0, B200_ARCH_GPT2 = 1, B200_ARCH_GPTNEOX = 2, B200_ARCH_MPT = 3, B200_ARCH_BLOOM = 4 };   /* whose Hyperparameters::read_ggml lays out the header */
+enum { B200_ARCH_LLAMA = 0, B200_ARCH_GPT2 = 1, B200_ARCH_GPTNEOX = 2, B200_ARCH_MPT = 3, B200_ARCH_BLOOM = 4, B200_ARCH_GPTJ = 5 };   /* whose Hyperparameters::read_ggml lays out the header */
 b200_ggml_file *b200_ggml_open(const char *path, int *err);                     /* LLaMA header; NULL + *err on LoadError */
 b200_ggml_file *b200_ggml_open_arch(const char *path, int32_t arch, int *err);
 /* the header words in file order: llama n_vocab n_embd n_mult n_head n_layer n_rot file_type | gpt2 n_vocab n_ctx n_embd n_head n_layer file_type n_vocab |
  * gptneox n_vocab n_ctx n_embd n_head n_layer n_rot use_parallel_residual file_type |
  * mpt n_embd max_seq_len n_head n_layer n_vocab alibi_bias_max(f32 bits) clip_kqv(f32 bits) file_type (mpt lib.rs:317-330; the vocabulary count is word 4) |
- * bloom n_vocab n_embd n_mult n_head n_layer file_type */
+ * bloom n_vocab n_embd n_mult n_head n_layer file_type |
+ * gptj n_vocab n_ctx n_embd n_head n_layer n_rot file_type n_vocab (gptj lib.rs:366-401; the repeated n_vocab must match the first: InvariantBroken) */
 int     b200_ggml_hparams(const b200_ggml_file *f, int32_t *arch, int32_t *words8, int32_t *n_words);
 void    b200_ggml_close(b200_ggml_file *f);
 int     b200_ggml_container(const b200_ggml_file *f, uint32_t *magic, uint32_t *version);      /* ContainerType */
@@ -187,7 +188,11 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
 typedef struct b200_neox_hparams {
     int32_t n_vocab, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype, context_size;
     int32_t arch;          /* 0 = GPT-NeoX; 1 = GPT-2 (crates/models/gpt2): tensor names "model/wte", "model/wpe" (f32 [n_ctx][n_embd]), "model/hN/attn/c_attn/w" ...,
-                              c_attn rows in thirds, no RoPE (n_rot ignored), sequential residual; context_size = the model's n_ctx (rows of wpe) */
+                              c_attn rows in thirds, no RoPE (n_rot ignored), sequential residual; context_size = the model's n_ctx (rows of wpe);
+                              4 = GPT-J (crates/models/gptj): "transformer.wte.weight", "transformer.ln_f.{weight,bias}", "lm_head.{weight,bias}",
+                              "transformer.h.N.{ln_1.{weight,bias}, attn.{q_proj,k_proj,v_proj,out_proj}.weight, mlp.{fc_in,fc_out}.{weight,bias}}"; one LayerNorm
+                              per layer feeds attention and MLP, RoPE mode 0 over the whole head (n_rot sets the angle step; even, 0 < n_rot <= head size),
+                              out = x + ((fc_out gelu(fc_in ln_1(x) + b) + b) + out_proj attn), logits = lm_head x + lm_head.bias; heads up to 256 wide */
     int32_t has_lm_head;   /* GPT-2: "model/lm_head" present; 0 = output projection tied to model/wte (gpt2 lib.rs:319-320) */
 } b200_neox_hparams;
 typedef struct b200_neox_model b200_neox_model;

@@ -62,6 +62,10 @@ struct NeoxParams {
     // MPT / BLOOM (crates/models/{mpt,bloom}): the GPT-2 row layout (gpt2 = 1, wpe = nullptr) plus ALiBi; MPT leaves every bias pointer null
     const float *alibi = nullptr;               // per-head ALiBi slopes [n_head] (alibi_slopes), else nullptr
     const float *emb_g = nullptr, *emb_b = nullptr;   // BLOOM: LayerNorm of the embedding row before layer 0, else nullptr
+    // GPT-J (crates/models/gptj): q | k | v thirds with RoPE mode 0 over the whole head (rope_cs: rope_table(n_rot, 0, .., hd, ..)), one LayerNorm per
+    // layer feeding attention and MLP (ln2_*, bqkv, bdense null), the 6-kernel schedule of decode_ops.cu::gptj_ops_t
+    int gptj = 0;
+    const float *lm_head_b = nullptr;           // GPT-J: lm_head.bias [n_vocab], added after the lm_head; else nullptr
 };
 // ggml_alibi's per-head slopes (LC/ggml.c:11570-11588), computed with the host's libm powf exactly as the reference computes them
 std::vector<float> alibi_slopes(int n_head, float max_bias);
@@ -69,7 +73,7 @@ void decode_set_tp(const TpCtx &T, cudaStream_t st);   // uploads the tensor-par
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches);
 
 // whether attn_fused_kernel's shared memory for a bucket of nlay positions (a multiple of 64) and head size hd fits the 227 KB opt-in limit:
-// true up to nlay = 3264 for every hd <= 128.  Past it LLaMA decodes with the two-kernel attention and GPT-NeoX / GPT-2 per op.
+// true up to nlay = 3264 for every hd <= 256.  Past it LLaMA decodes with the two-kernel attention and GPT-NeoX / GPT-2 / GPT-J per op.
 bool attn_fused_fits(int nlay, int hd);
 
 // default decode schedule: 8 fused kernels per layer on `st` (decode_ops.cu); position read from *P.n_past on the device

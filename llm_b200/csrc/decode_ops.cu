@@ -443,8 +443,11 @@ __device__ __forceinline__ void fma8(float (&acc)[8], const int4 &a, const int4 
 //
 // ALIBI (MPT, BLOOM): the score of key position j in head h is fma(j, slope[h], kq * kq_scale) -- ggml_alibi (LC/ggml.c:11534-11597) on the
 // scaled scores, one fused multiply-add as the reference's x86 build compiles it; the slopes come from alibi_slopes() on the host.
+//
+// NV: the most 16-byte chunks per position and quad thread (hd / 32).  4 serves hd <= 128 (clusters of up to 4 CTAs); 8 serves hd <= 256 (GPT-J's
+// 256-wide heads, clusters of up to 8 CTAs, the portable limit) and halves the positions per pass, so kv[PU][NV] stays 16 int4 per thread.
 constexpr int ATH = 256;
-template <bool TP, bool ALIBI>
+template <bool TP, bool ALIBI, int NV = 4>
 __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
                                                 int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
                                                 float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
@@ -483,15 +486,15 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
     }
     const int per = (n_kv + per_head - 1) / per_head, j0 = part * per, j1 = n_kv < j0 + per ? n_kv : j0 + per;   // this CTA's KQ positions
     const int nvec = hd / 32;                                    // 16-byte loads per thread per position (chunks i = 0..nvec-1)
-    constexpr int PU = 4;                                        // positions per quad per pass: up to 4 * nvec 16-byte loads in flight per thread
-    int4 kv[PU][4];
+    constexpr int PU = 16 / NV;                                  // positions per quad per pass: up to PU * nvec 16-byte loads in flight per thread
+    int4 kv[PU][NV];
     auto krow_of = [&](int j) { return Kl + (int64_t)(j < j1 ? j : j0) * gqa + hk * hd + 8 * u; };
 #pragma unroll
     for (int pu = 0; pu < PU; pu++) {                            // the first pass's K rows below p
         const int j = j0 + pu * (ATH / 4) + (tid >> 2);
         const __half *krow = krow_of(j);
 #pragma unroll
-        for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = j < j1 && j < p ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+        for (int i = 0; i < NV; i++) if (i < nvec) kv[pu][i] = j < j1 && j < p ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
     }
     pdl_wait();
     float qv = 0.f;
@@ -503,7 +506,7 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
         if (j == p && j < j1) {
             const __half *krow = krow_of(j);
 #pragma unroll
-            for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = __ldcg((const int4 *)(krow + 32 * i));
+            for (int i = 0; i < NV; i++) if (i < nvec) kv[pu][i] = __ldcg((const int4 *)(krow + 32 * i));
         }
     }
     if (tid < hd) q16[tid] = __float2half_rn(qv);
@@ -516,13 +519,13 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
     {
         const float slope = ALIBI ? __ldg(alibi + h) : 0.f;
         for (int jb = j0; jb < j1; jb += PU * (ATH / 4)) {
-            if (jb != j0) {                                      // later passes (contexts beyond 4 * ATH / 4 positions per CTA)
+            if (jb != j0) {                                      // later passes (contexts beyond PU * ATH / 4 positions per CTA)
 #pragma unroll
                 for (int pu = 0; pu < PU; pu++) {
                     const int j = jb + pu * (ATH / 4) + (tid >> 2);
                     const __half *krow = krow_of(j);
 #pragma unroll
-                    for (int i = 0; i < 4; i++) if (i < nvec) kv[pu][i] = j < j1 ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+                    for (int i = 0; i < NV; i++) if (i < nvec) kv[pu][i] = j < j1 ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
                 }
             }
 #pragma unroll
@@ -532,10 +535,12 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
 #pragma unroll
                 for (int e = 0; e < 8; e++) acc[e] = 0.f;
 #pragma unroll
-                for (int i = 0; i < 4; i++) if (i < nvec) fma8(acc, kv[pu][i], *(const int4 *)(q16 + 32 * i + 8 * u));
+                for (int i = 0; i < NV; i++) if (i < nvec) fma8(acc, kv[pu][i], *(const int4 *)(q16 + 32 * i + 8 * u));
                 const float s = quad_tree(acc);
-                if (j < j1 && u < per_head)                      // thread u of the quad feeds CTA u
+                if (j < j1 && u < per_head)                      // thread u of the quad feeds CTA u (and CTA u + 4 of a cluster of more than 4)
                     cluster.map_shared_rank(sc, u)[j] = ALIBI ? __fmaf_rn((float)j, slope, __fmul_rn(s, kq_scale)) : __fmul_rn(s, kq_scale);
+                if (NV > 4 && j < j1 && u + 4 < per_head)
+                    cluster.map_shared_rank(sc, u + 4)[j] = ALIBI ? __fmaf_rn((float)j, slope, __fmul_rn(s, kq_scale)) : __fmul_rn(s, kq_scale);
             }
         }
     }
@@ -606,6 +611,13 @@ __global__ void __launch_bounds__(ATH) attn_fused_alibi_kernel(const float *__re
                                                                float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
                                                                unsigned long long *prof, const TpSync S, int head0, const float *__restrict__ alibi) {
     attn_fused_body<false, true>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, alibi);
+}
+// the wide form (single GPU, no ALiBi): head sizes 128 < hd <= 256, hd % 32 == 0 -- one cluster of hd/32 = 5..8 CTAs per head (GPT-J)
+__global__ void __launch_bounds__(ATH) attn_fused_wide_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
+                                                              int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
+                                                              float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                                                              unsigned long long *prof, const TpSync S, int head0) {
+    attn_fused_body<false, false, 8>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, nullptr);
 }
 
 // ---- ring and grid plan of the decode mat-vecs ------------------------------------------------------------------------------------------------
@@ -725,13 +737,14 @@ void launch_mmv(const QWeight &w, MmvArgs A, const MmvPlan &plan, cudaStream_t s
     launch_k(mmv_fused_kernel<TYPE, EPI, TP>, dim3((unsigned)plan.grid), dim3(STHREADS), (size_t)plan.smem, st, w, A);
 }
 
-// dynamic shared memory opt-in of the cluster attention kernel: one high-water mark for both instantiations (the attribute is per function, not per caller)
+// dynamic shared memory opt-in of the cluster attention kernels: one high-water mark for all of them (the attribute is per function, not per caller)
 static void attn_fused_reserve(size_t bytes) {
     static size_t set = 48 * 1024;
     if (bytes <= set) return;
     B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     B200_CHECK(cudaFuncSetAttribute(attn_fused_alibi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_fused_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
 // dynamic shared memory of attn_fused_kernel for nlay positions and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
@@ -758,9 +771,15 @@ void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const 
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 2;
     if (alibi) {
-        B200_ASSERT(!TP);
+        B200_ASSERT(!TP && hd <= 128);
         B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_alibi_kernel, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
                                       q81, off, scale16, prof, S, head0, alibi));
+        return;
+    }
+    if (hd > 128) {                                              // 5..8 CTAs per head
+        B200_ASSERT(!TP && hd <= 256 && hd % 32 == 0);
+        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_wide_kernel, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+                                      q81, off, scale16, prof, S, head0));
         return;
     }
     B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
@@ -1031,15 +1050,61 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     if (launches) *launches = n;
 }
 
+// ---- GPT-J (crates/models/gptj/src/lib.rs:153-305): 6 kernels per layer + 3 ------------------------------------------------------------------
+//   ln_pack(ln_1) -> xpack_a;  qkv [q|k|v thirds] with the LLaMA epilogue (RoPE mode 0 over the whole head on q, k; K by row, V by column);
+//   cluster attention -> xpack_d;  out_proj (no bias) -> attn_out;  fc_in + bias, gelu, quantized, reading the SAME xpack_a records (one LayerNorm feeds
+//   attention and MLP, :174, :270);  fc_out: ((W h + b_out) + attn_out) + x -> x (:276-282).  Then ln_f and the lm_head + lm_head.bias (:286-296).
+template <int TYPE>
+void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n_kv_bucket, cudaStream_t st, int *launches) {
+    const int q81 = has_min(TYPE) ? 1 : 0, off = TYPE == T_Q5_0 ? 16 : 0, s16 = TYPE == T_Q4_0 ? 1 : 0;
+    const int e = P.e;
+    int n = 0;
+    // the token boundary: a plain launch (no programmatic attribute), see neox_ops_t
+    get_rows_q(P.wte, P.token, P.x, 1, st); n++;                                                                                                     // :161
+    const int nlay = (n_kv_bucket + 63) / 64 * 64;
+    const size_t fa_smem = attn_fused_smem(nlay, P.hd);
+    B200_ASSERT(P.hd % 32 == 0 && P.hd <= 256 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd) && e <= 8192 && !P.alibi);   // neox.cu::forward checks these
+    const dim3 ln_grid((e / 4 + 255) / 256);
+    const TpSync S{};
+    const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
+    const CtaFootprint f_attn = P.hd > 128 ? footprint_of(attn_fused_wide_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
+    // each ring planned against the node launched after it: qkv -> attention, out_proj -> fc_in, fc_in -> fc_out, fc_out -> next layer's ln_1 + qkv
+    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_QKV, false>(layers[0].wqkv, f_attn);
+    const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
+    const MmvPlan &p_fc = mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta);
+    const MmvPlan &p_dense = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wdense, p_fc.cta);
+    const MmvPlan &p_head = mmv_plan<TYPE, EPI_BIAS, false>(P.lm_head, CtaFootprint{});
+    for (int il = 0; il < P.n_layer; il++) {
+        const NeoxLayer &L = layers[il];
+        launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;                 // :168-174
+        MmvArgs A{}; A.xpack = P.xpack_a; A.q = P.q; A.K = L.K; A.V = L.V; A.rope_cs = P.rope_cs; A.rope_half = P.rope_half; A.hd = P.hd; A.e = e; A.gqa = e;
+        A.n_ctx = P.n_ctx; A.n_past = P.n_past;
+        launch_mmv<TYPE, EPI_QKV>(L.wqkv, A, p_qkv, st); n++;                                                                                          // :178-220
+        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, nlay, q81, off, s16,
+                                 nullptr, S, 0); n++;                                                                                                   // :222-262
+        MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out;
+        launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;                                                                                    // :265
+        MmvArgs C{}; C.xpack = P.xpack_a; C.xpack_out = P.xpack_f; C.bias = L.bfc; C.lut_gelu = P.lut_gelu; C.q81 = q81; C.off = off; C.scale16 = s16;
+        launch_mmv<TYPE, EPI_GELU>(L.wfc, C, p_fc, st); n++;                                                                                           // :270-273
+        MmvArgs D{}; D.xpack = P.xpack_f; D.dst = P.x; D.bias = L.bproj; D.add1 = P.attn_out; D.add2 = P.x;
+        launch_mmv<TYPE, EPI_BIAS>(L.wproj, D, p_proj, st); n++;                                                                                       // :276-282
+    }
+    launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16); n++;                          // :286-287
+    MmvArgs Z{}; Z.xpack = P.xpack_a; Z.dst = P.logits; Z.bias = P.lm_head_b; Z.n_past_inc = P.n_past;
+    launch_mmv<TYPE, EPI_BIAS>(P.lm_head, Z, p_head, st); n++;                                                                                        // :292-296
+    B200_CHECK(cudaGetLastError());
+    if (launches) *launches = n;
+}
+
 }  // namespace
 
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches) {
     switch (wtype) {
-        case T_Q4_0: neox_ops_t<T_Q4_0>(P, layers, n_kv_bucket, st, launches); break;
-        case T_Q4_1: neox_ops_t<T_Q4_1>(P, layers, n_kv_bucket, st, launches); break;
-        case T_Q5_0: neox_ops_t<T_Q5_0>(P, layers, n_kv_bucket, st, launches); break;
-        case T_Q5_1: neox_ops_t<T_Q5_1>(P, layers, n_kv_bucket, st, launches); break;
-        case T_Q8_0: neox_ops_t<T_Q8_0>(P, layers, n_kv_bucket, st, launches); break;
+        case T_Q4_0: if (P.gptj) gptj_ops_t<T_Q4_0>(P, layers, n_kv_bucket, st, launches); else neox_ops_t<T_Q4_0>(P, layers, n_kv_bucket, st, launches); break;
+        case T_Q4_1: if (P.gptj) gptj_ops_t<T_Q4_1>(P, layers, n_kv_bucket, st, launches); else neox_ops_t<T_Q4_1>(P, layers, n_kv_bucket, st, launches); break;
+        case T_Q5_0: if (P.gptj) gptj_ops_t<T_Q5_0>(P, layers, n_kv_bucket, st, launches); else neox_ops_t<T_Q5_0>(P, layers, n_kv_bucket, st, launches); break;
+        case T_Q5_1: if (P.gptj) gptj_ops_t<T_Q5_1>(P, layers, n_kv_bucket, st, launches); else neox_ops_t<T_Q5_1>(P, layers, n_kv_bucket, st, launches); break;
+        case T_Q8_0: if (P.gptj) gptj_ops_t<T_Q8_0>(P, layers, n_kv_bucket, st, launches); else neox_ops_t<T_Q8_0>(P, layers, n_kv_bucket, st, launches); break;
         default: B200_ASSERT(!"neox_decode_enqueue: unsupported weight type");
     }
 }

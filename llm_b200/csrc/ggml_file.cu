@@ -83,7 +83,7 @@ void b200_ggml_close(b200_ggml_file *f) {
 
 static b200_ggml_file *open_arch_impl(const char *path, int32_t arch, int *err) {
     int dummy; if (!err) err = &dummy;
-    if (arch < 0 || arch > B200_ARCH_BLOOM) { *err = B200_ERR_BAD_ARG; return nullptr; }
+    if (arch < 0 || arch > B200_ARCH_GPTJ) { *err = B200_ERR_BAD_ARG; return nullptr; }
     *err = B200_OK;
     b200_ggml_file *f = new b200_ggml_file();
     f->arch = arch; f->n_hp = arch == B200_ARCH_LLAMA ? 7 : arch == B200_ARCH_GPT2 ? 7 : arch == B200_ARCH_BLOOM ? 6 : 8;
@@ -114,6 +114,7 @@ static b200_ggml_file *open_arch_impl(const char *path, int32_t arch, int *err) 
     for (int i = 0; i < f->n_hp; i++)                                                                 // usize::try_from in the reference; MPT's words 5 and 6
         if (f->hp[i] < 0 && !(arch == B200_ARCH_MPT && (i == 5 || i == 6))) return fail(B200_ERR_INVARIANT_BROKEN);   // are f32 (read_f32 takes any value)
     if (arch == B200_ARCH_GPT2 && f->hp[6] != f->hp[0]) return fail(B200_ERR_INVARIANT_BROKEN);     // "GPT2 model expected n_vocab {} found {}"
+    if (arch == B200_ARCH_GPTJ && f->hp[7] != f->hp[0]) return fail(B200_ERR_INVARIANT_BROKEN);     // "GPTJ model expected n_vocab {} found {}" (gptj lib.rs:377-386)
     if (arch == B200_ARCH_GPTNEOX && f->hp[6] > 1) return fail(B200_ERR_IO);                        // read_bool: InvalidData
 
     const bool scored = f->magic == MAGIC_GGMF || f->magic == MAGIC_GGJT;

@@ -4,6 +4,9 @@
 //           GptNeoX::evaluate (the graph)       crates/models/gptneox/src/lib.rs:156-350   (feed-forward: :487-515)
 //           Gpt2::new / Gpt2::evaluate          crates/models/gpt2/src/lib.rs:43-136, 138-329   (hp.arch == 1: c_attn rows in thirds, no RoPE, learned positions,
 //                                                                                               sequential residual, lm_head optional -> tied to wte)
+//           GptJ::new / GptJ::evaluate          crates/models/gptj/src/lib.rs:47-122, 134-311   (hp.arch == 4: q_proj | k_proj | v_proj as thirds of one wqkv,
+//                                                                                               RoPE mode 0 over the whole head, one LayerNorm feeding attention and
+//                                                                                               MLP, lm_head + lm_head.bias; decode: decode_ops.cu::gptj_ops_t)
 //           InferenceSession::compute           crates/llm-base/src/inference_session.rs:114-295
 // Batches (prefill) run node by node on the bit-exact kernels of this directory (LayerNorm, bias adds, RoPE mode 2 on n_rot of the head size, gelu table,
 // exact quantized mat-muls incl. the wgmma GEMM, exact f16 attention mat-muls); single tokens run the fused 8-kernels-per-layer schedule of
@@ -26,19 +29,24 @@ struct b200_neox_model : Weights {
     float *lnf_g = nullptr, *lnf_b = nullptr, *wpe = nullptr;     // wpe: GPT-2 learned positions [n_ctx][e] f32
     float *emb_g = nullptr, *emb_b = nullptr;                     // BLOOM: LayerNorm of the embedding row
     DeviceBuf<float> alibi;                                       // MPT / BLOOM: ALiBi slopes [n_head] (alibi_slopes)
+    float *lm_head_b = nullptr;                                   // GPT-J: lm_head.bias [n_vocab]
     bool gpt2() const { return hp.arch == 1; }
     bool mpt() const { return hp.arch == 2; }
     bool bloom() const { return hp.arch == 3; }
-    bool thirds() const { return hp.arch >= 1; }                  // GPT-2, MPT, BLOOM: q | k | v are the thirds of the fused row, no RoPE
-    struct Layer { QWeight wqkv, wdense, wfc, wproj; float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj; };   // MPT: every bias null
+    bool gptj() const { return hp.arch == 4; }
+    bool thirds() const { return hp.arch >= 1; }                  // GPT-2, MPT, BLOOM, GPT-J: q | k | v are the thirds of the fused row (GPT-J: RoPE mode 0, the others none)
+    // MPT: every bias null; GPT-J: ln2_*, bqkv and bdense null (one LayerNorm per layer, no attention biases)
+    struct Layer { QWeight wqkv, wdense, wfc, wproj; float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj; };
     std::vector<Layer> layers;
     int n_slots() const {
         if (mpt()) return 2 + 6 * hp.n_layer;                                 // wte, norm_f, 6 per block
         if (bloom()) return 6 + 12 * hp.n_layer;                              // wte, norm.{weight,bias}, output_norm.{weight,bias}, output, 12 per layer
+        if (gptj()) return 5 + 10 * hp.n_layer;                               // wte, ln_f.{weight,bias}, lm_head.{weight,bias}, 10 per layer
         return 4 + 12 * hp.n_layer + (gpt2() && hp.has_lm_head ? 1 : 0);       // GPT-2: slot 3 = wpe, lm_head (if present) last
     }
     bool lookup(const char *name, Slot &s, int &id);
     bool lookup_alibi(const char *name, Slot &s, int &id);
+    bool lookup_gptj(const char *name, Slot &s, int &id);
 };
 
 struct b200_neox_session : SessionCore {   // memory_k [n_layer][n_ctx][e], memory_v [n_layer][e][n_ctx]
@@ -98,10 +106,38 @@ bool b200_neox_model::lookup_alibi(const char *name, Slot &s, int &id) {
     return false;
 }
 
+// GPT-J: crates/models/gptj/src/lib.rs:59-103.  q_proj / k_proj / v_proj are rows [0, e), [e, 2e), [2e, 3e) of one wqkv.
+bool b200_neox_model::lookup_gptj(const char *name, Slot &s, int &id) {
+    const int e = hp.n_embd;
+    if (!strcmp(name, "transformer.wte.weight")) { s.q = wte; s.is_q = true; id = 0; return true; }
+    if (!strcmp(name, "transformer.ln_f.weight")) { s.f = lnf_g; s.n = e; id = 1; return true; }
+    if (!strcmp(name, "transformer.ln_f.bias")) { s.f = lnf_b; s.n = e; id = 2; return true; }
+    if (!strcmp(name, "lm_head.weight")) { s.q = lm_head; s.is_q = true; id = 3; return true; }
+    if (!strcmp(name, "lm_head.bias")) { s.f = lm_head_b; s.n = hp.n_vocab; id = 4; return true; }
+    int il = -1; char sub[96];
+    if (sscanf(name, "transformer.h.%d.%95s", &il, sub) != 2 || il < 0 || il >= hp.n_layer) return false;
+    Layer &L = layers[il];
+    const QWeight wq = row_view(L.wqkv, 0, e), wk = row_view(L.wqkv, e, e), wv = row_view(L.wqkv, 2 * (int64_t)e, e);
+    struct { const char *n; const QWeight *q; float *f; int64_t len; } tab[] = {
+        {"ln_1.weight", nullptr, L.ln1_g, e}, {"ln_1.bias", nullptr, L.ln1_b, e},
+        {"attn.q_proj.weight", &wq, nullptr, 0}, {"attn.k_proj.weight", &wk, nullptr, 0}, {"attn.v_proj.weight", &wv, nullptr, 0},
+        {"attn.out_proj.weight", &L.wdense, nullptr, 0},
+        {"mlp.fc_in.weight", &L.wfc, nullptr, 0}, {"mlp.fc_in.bias", nullptr, L.bfc, 4 * (int64_t)e},
+        {"mlp.fc_out.weight", &L.wproj, nullptr, 0}, {"mlp.fc_out.bias", nullptr, L.bproj, e}};
+    for (int k = 0; k < 10; k++)
+        if (!strcmp(sub, tab[k].n)) {
+            if (tab[k].q) { s.q = *tab[k].q; s.is_q = true; } else { s.f = tab[k].f; s.n = tab[k].len; }
+            id = 5 + 10 * il + k;
+            return true;
+        }
+    return false;
+}
+
 bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
     const int e = hp.n_embd;
     s = Slot();
-    if (hp.arch >= 2) return lookup_alibi(name, s, id);
+    if (gptj()) return lookup_gptj(name, s, id);
+    if (mpt() || bloom()) return lookup_alibi(name, s, id);
     if (gpt2()) {                                                         // tensor names of crates/models/gpt2/src/lib.rs:59-107
         if (!strcmp(name, "model/wte")) { s.q = wte; s.is_q = true; id = 0; return true; }
         if (!strcmp(name, "model/ln_f/g")) { s.f = lnf_g; s.n = e; id = 1; return true; }
@@ -166,8 +202,10 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     }
     const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()};
     const float kq_scale = 1.0f / sqrtf((float)e / (float)n_head);                                                  // :270-273
-    const bool g2 = m->thirds(), parallel = !g2 && hp.use_parallel_residual;
-    const RopeTable *rope = g2 ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, hd, n_ctx);
+    const bool g2 = m->thirds(), gptj = m->gptj(), parallel = !g2 && hp.use_parallel_residual;
+    // GPT-NeoX: mode 2 on n_rot of every head; GPT-J: mode 0 over ALL hd elements of the head with theta_scale base^(-2/n_rot) (gptj lib.rs:178-201,
+    // LC/ggml.c:11859-11874 walks ne0, not n_dims)
+    const RopeTable *rope = gptj ? &rope_table(hp.n_rot, 0, 10000.0f, 1.0f, hd, n_ctx) : g2 ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, hd, n_ctx);
     const int64_t ld3 = 3 * (int64_t)e;
     // where q / k / v of head h live inside a row of the fused projection: NeoX per head [q | k | v], GPT-2 / MPT / BLOOM the three thirds of the row
     const int64_t hs = g2 ? hd : 3 * hd, koff = g2 ? e : hd, voff = g2 ? 2 * (int64_t)e : 2 * hd;
@@ -184,7 +222,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         layer_norm(s->x.get(), s->cur.get(), ly.ln1_g, ly.ln1_b, e, n, st); L++;                                                  // :192-196
         L += mul_mat_exact_auto(ly.wqkv, s->cur.get(), e, n, s->qkv.get(), ld3, nullptr, 0, acts, st);                                // :199
         if (ly.bqkv) { add_f32(s->qkv.get(), ly.bqkv, s->qkv.get(), (int64_t)n * ld3, ld3, st); L++; }                            // :200 (MPT: no bias)
-        if (!g2) {   // RoPE mode 2 in place on q and k                                                                       :205-228
+        if (rope) {   // RoPE in place on q and k: mode 2 (GPT-NeoX :205-228), mode 0 (GPT-J :178-201)
             rope_f32(s->qkv.get(), s->qkv.get(), hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
             rope_f32(s->qkv.get() + koff, s->qkv.get() + koff, hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
         }
@@ -199,9 +237,21 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         if (m->alibi) soft_max_alibi(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, kq_scale, n_past, m->alibi.get(), st);   // MPT / BLOOM: + ALiBi
         else soft_max(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, kq_scale, true, n_past, true, true, st);                // :270-279
         L++;
+        // GPT-J: cur (ln_1's output, input_sa) still feeds fc_in, so the merged KQV goes to t
+        float *kqv = gptj ? s->t.get() : s->cur.get();
         mul_mat_f16_exact(Vl, n_kv, hd, n_head, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2, s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
-                          s->cur.get(), (int64_t)e * 4, (int64_t)hd * 4, -1, st); L++;                                      // :282-298
-        L += mul_mat_exact_auto(ly.wdense, s->cur.get(), e, n, s->attn.get(), e, nullptr, 0, acts, st);                               // :301
+                          kqv, (int64_t)e * 4, (int64_t)hd * 4, -1, st); L++;                                               // :282-298
+        L += mul_mat_exact_auto(ly.wdense, kqv, e, n, s->attn.get(), e, nullptr, 0, acts, st);                                        // :301
+        if (gptj) {   // gptj lib.rs:265-282: t = (fc_out gelu(fc_in input_sa + b_in) + b_out) + attn; inpL = t + inpL
+            L += mul_mat_exact_auto(ly.wfc, s->cur.get(), e, n, s->h4.get(), 4 * (int64_t)e, nullptr, 0, acts, st);
+            add_f32(s->h4.get(), ly.bfc, s->h4.get(), (int64_t)n * 4 * e, 4 * (int64_t)e, st); L++;
+            unary_lut(UNARY_GELU, s->h4.get(), s->hact.get(), (int64_t)n * 4 * e, st); L++;
+            L += mul_mat_exact_auto(ly.wproj, s->hact.get(), 4 * (int64_t)e, n, s->t.get(), e, nullptr, 0, acts, st);
+            add_f32(s->t.get(), ly.bproj, s->t.get(), (int64_t)n * e, e, st); L++;
+            add_f32(s->t.get(), s->attn.get(), s->t.get(), (int64_t)n * e, (int64_t)n * e, st); L++;
+            add_f32(s->t.get(), s->x.get(), s->x.get(), (int64_t)n * e, (int64_t)n * e, st); L++;
+            continue;
+        }
         if (ly.bdense) { add_f32(s->attn.get(), ly.bdense, s->attn.get(), (int64_t)n * e, e, st); L++; }                          // :302
         const float *ff_in = s->x.get();
         if (!parallel) { add_f32(s->attn.get(), s->x.get(), s->attn.get(), (int64_t)n * e, (int64_t)n * e, st); L++; ff_in = s->attn.get(); }   // :308-309 / gpt2 :279
@@ -218,19 +268,23 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     if (all_rows || n == 1) {
         layer_norm(s->x.get(), s->cur.get(), m->lnf_g, m->lnf_b, e, n, st); L++;                                                   // :332-334
         L += mul_mat_exact_auto(m->lm_head, s->cur.get(), e, n, s->logits.get(), hp.n_vocab, nullptr, 0, acts, st);                   // :342
+        if (m->lm_head_b) { add_f32(s->logits.get(), m->lm_head_b, s->logits.get(), (int64_t)n * hp.n_vocab, hp.n_vocab, st); L++; }  // gptj lib.rs:296
     } else {
         const size_t last = (size_t)(n - 1);
+        float *row = s->logits.get() + last * hp.n_vocab;
         layer_norm(s->x.get() + last * e, s->cur.get() + last * e, m->lnf_g, m->lnf_b, e, 1, st); L++;
-        L += mul_mat_exact_auto(m->lm_head, s->cur.get() + last * e, e, 1, s->logits.get() + last * hp.n_vocab, hp.n_vocab, nullptr, 0, acts, st);
+        L += mul_mat_exact_auto(m->lm_head, s->cur.get() + last * e, e, 1, row, hp.n_vocab, nullptr, 0, acts, st);
+        if (m->lm_head_b) { add_f32(row, m->lm_head_b, row, hp.n_vocab, hp.n_vocab, st); L++; }
     }
     s->last_launches = L;
     s->n_past += n;
 }
 
-// hp->arch 0 / 1 (b200_neox_new) or 2 / 3 (b200_neox_new_alibi, alibi_bias_max: the ALiBi bias of MPT's header, 8 for BLOOM)
+// hp->arch 0 / 1 / 4 (b200_neox_new) or 2 / 3 (b200_neox_new_alibi, alibi_bias_max: the ALiBi bias of MPT's header, 8 for BLOOM).
+// GPT-NeoX and GPT-J rotate: n_rot even, positive and at most the head size (the asserts of ggml_rope, LC/ggml.c:11807-11808)
 b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
     if (!hp || !is_quant(hp->wtype) || hp->n_embd % 64 || hp->n_head <= 0 || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0 ||
-        (hp->arch == 0 && (hp->n_rot <= 0 || hp->n_rot % 2 || hp->n_rot > hp->n_embd / hp->n_head))) return nullptr;
+        ((hp->arch == 0 || hp->arch == 4) && (hp->n_rot <= 0 || hp->n_rot % 2 || hp->n_rot > hp->n_embd / hp->n_head))) return nullptr;
     rt().ensure_init();
     b200_neox_model *m = new b200_neox_model();
     m->hp = *hp;
@@ -241,6 +295,15 @@ b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
         m->carve(t, m->n_slots(), [m, e, v](SlabCarver &c) {
             c.q(m->wte, e, v); c.f(m->lnf_g, e);
             for (auto &L : m->layers) { c.f(L.ln1_g, e); c.f(L.ln2_g, e); c.q(L.wqkv, e, 3 * e); c.q(L.wdense, e, e); c.q(L.wfc, e, 4 * e); c.q(L.wproj, 4 * e, e); }
+        });
+    } else if (m->gptj()) {                                               // gptj lib.rs:59-103: no attention biases, one LayerNorm per layer
+        m->carve(t, m->n_slots(), [m, e, v](SlabCarver &c) {
+            c.q(m->wte, e, v); c.q(m->lm_head, e, v);
+            c.f(m->lnf_g, e); c.f(m->lnf_b, e); c.f(m->lm_head_b, v);
+            for (auto &L : m->layers) {
+                c.f(L.ln1_g, e); c.f(L.ln1_b, e); c.f(L.bfc, 4 * e); c.f(L.bproj, e);
+                c.q(L.wqkv, e, 3 * e); c.q(L.wdense, e, e); c.q(L.wfc, e, 4 * e); c.q(L.wproj, 4 * e, e);
+            }
         });
     } else {
         m->carve(t, m->n_slots(), [m, hp, e, v](SlabCarver &c) {
@@ -258,7 +321,7 @@ b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
     // tied output projection (gpt2 lib.rs:319-320, MPT always): wte is streamed as the lm_head
     if ((m->gpt2() && !hp->has_lm_head) || m->mpt()) m->lm_head = m->wte;
     else m->weight_bytes -= (size_t)v * (e / QK) * ggml_block_bytes(t);  // the embedding table is gathered from, not streamed
-    if (hp->arch >= 2) {
+    if (m->mpt() || m->bloom()) {
         const std::vector<float> slopes = alibi_slopes(hp->n_head, alibi_bias_max);
         m->alibi = device_alloc<float>(slopes.size() * 4);
         B200_CHECK(cudaMemcpy(m->alibi.get(), slopes.data(), slopes.size() * 4, cudaMemcpyHostToDevice));
@@ -281,7 +344,7 @@ std::vector<float> b200::alibi_slopes(int n_head, float max_bias) {
 
 extern "C" {
 
-b200_neox_model *b200_neox_new(const b200_neox_hparams *hp) { return hp && (hp->arch == 0 || hp->arch == 1) ? neox_new(hp, 0.0f) : nullptr; }
+b200_neox_model *b200_neox_new(const b200_neox_hparams *hp) { return hp && (hp->arch == 0 || hp->arch == 1 || hp->arch == 4) ? neox_new(hp, 0.0f) : nullptr; }
 
 b200_neox_model *b200_neox_new_alibi(const b200_neox_hparams *hp, float alibi_bias_max) {
     return hp && (hp->arch == 2 || hp->arch == 3) ? neox_new(hp, alibi_bias_max) : nullptr;   // MPT, BLOOM
@@ -306,6 +369,14 @@ int b200_neox_synthesize(b200_neox_model *m, uint64_t seed) {
         if (m->mpt()) {
             r.q(m->wte); r.gain(m->lnf_g, e);
             for (auto &L : m->layers) { r.gain(L.ln1_g, e); r.gain(L.ln2_g, e); r.q(L.wqkv); r.q(L.wdense); r.q(L.wfc); r.q(L.wproj); }
+            return;
+        }
+        if (m->gptj()) {
+            r.q(m->wte); r.q(m->lm_head); r.gain(m->lnf_g, e); r.bias(m->lnf_b, e); r.bias(m->lm_head_b, m->hp.n_vocab);
+            for (auto &L : m->layers) {
+                r.gain(L.ln1_g, e); r.bias(L.ln1_b, e); r.bias(L.bfc, 4 * e); r.bias(L.bproj, e);
+                r.q(L.wqkv); r.q(L.wdense); r.q(L.wfc); r.q(L.wproj);
+            }
             return;
         }
         r.q(m->wte); if (!m->gpt2() || m->hp.has_lm_head) r.q(m->lm_head); r.gain(m->lnf_g, e); r.bias(m->lnf_b, e);
@@ -341,7 +412,8 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     s->xpack = device_alloc<int4>((4 * e / QK) * 64); s->xh = device_alloc<__half>(xh_bytes(4 * e, B));
     s->qdec = device_alloc<float>(e * 4);
     s->xpack_a = device_alloc<int4>((e / QK) * 64); s->xpack_d = device_alloc<int4>((e / QK) * 64); s->xpack_f = device_alloc<int4>((4 * e / QK) * 64);
-    const RopeTable *rt_ = m->thirds() ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, m->hd, (int)n_ctx);
+    const RopeTable *rt_ = m->gptj() ? &rope_table(hp.n_rot, 0, 10000.0f, 1.0f, m->hd, (int)n_ctx)
+                         : m->thirds() ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, m->hd, (int)n_ctx);
     s->dl.resize(hp.n_layer);
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &L = m->layers[il];
@@ -352,12 +424,15 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     P.n_layer = hp.n_layer; P.e = (int)e; P.hd = m->hd; P.n_head = hp.n_head; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab; P.n_rot = hp.n_rot;
     P.parallel_residual = !m->thirds() && hp.use_parallel_residual; P.gpt2 = m->thirds() ? 1 : 0; P.wpe = m->wpe;
     P.alibi = m->alibi.get(); P.emb_g = m->emb_g; P.emb_b = m->emb_b; P.wte = m->wte; P.lm_head = m->lm_head; P.lnf_g = m->lnf_g; P.lnf_b = m->lnf_b;
+    P.gptj = m->gptj() ? 1 : 0; P.lm_head_b = m->lm_head_b;
     P.kq_scale = 1.0f / sqrtf((float)e / (float)hp.n_head); P.rope_cs = rt_ ? rt_->cs : nullptr; P.rope_half = rt_ ? rt_->half : 0;
     P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
     P.x = s->x.get(); P.qkv = s->qkv.get(); P.q = s->qdec.get(); P.attn_out = s->attn.get(); P.logits = s->logits.get();
     P.xpack_a = s->xpack_a.get(); P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
     QWeight p1; p1.nb = (int64_t)e / QK; QWeight p2; p2.nb = 4 * (int64_t)e / QK;
-    s->decode_ok = m->hd % 32 == 0 && m->hd <= 128 && e % 128 == 0 && e <= 8192 && n_ctx % 8 == 0 && mmv_exact_stream_supported(p1) && mmv_exact_stream_supported(p2);
+    // GPT-J's schedule also takes heads of 128 < hd <= 256 (the wide cluster attention, up to 8 CTAs per head)
+    s->decode_ok = m->hd % 32 == 0 && (m->hd <= 128 || (m->gptj() && m->hd <= 256)) && e % 128 == 0 && e <= 8192 && n_ctx % 8 == 0 &&
+                   mmv_exact_stream_supported(p1) && mmv_exact_stream_supported(p2);
     B200_CHECK(cudaDeviceSynchronize());
     return s;
 }

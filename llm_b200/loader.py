@@ -26,13 +26,14 @@ class LoadError(Exception):
         super().__init__(f"{what}: {self.kind}")
 
 
-ARCH = {"llama": 0, "gpt2": 1, "gptneox": 2, "mpt": 3, "bloom": 4}
+ARCH = {"llama": 0, "gpt2": 1, "gptneox": 2, "mpt": 3, "bloom": 4, "gptj": 5}
 HPARAM_NAMES = {
     "llama": ("n_vocab", "n_embd", "n_mult", "n_head", "n_layer", "n_rot", "file_type"),                                   # llama lib.rs:425-447
     "gpt2": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "file_type", "n_vocab_again"),                              # gpt2 lib.rs:394-416
     "gptneox": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "n_rot", "use_parallel_residual", "file_type"),          # gptneox lib.rs:431-442
     "mpt": ("n_embd", "max_seq_len", "n_head", "n_layer", "n_vocab", "alibi_bias_max", "clip_kqv", "file_type"),          # mpt lib.rs:317-330
     "bloom": ("n_vocab", "n_embd", "n_mult", "n_head", "n_layer", "file_type"),                                           # bloom lib.rs
+    "gptj": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "n_rot", "file_type", "n_vocab_again"),                    # gptj lib.rs:366-401
 }
 FLOAT_WORDS = {"alibi_bias_max", "clip_kqv"}                                                                             # f32 in the header (read_f32)
 

@@ -3,6 +3,7 @@
   GptNeoX(KnownModel)     crates/models/gptneox/src/lib.rs:36-140     new / start_session / evaluate
   Hyperparameters         crates/models/gptneox/src/lib.rs (n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, file_type)
   Gpt2 / Mpt / Bloom      crates/models/{gpt2,mpt,bloom} on the same runtime (Mpt, Bloom: ALiBi attention, b200_neox_new_alibi)
+  GptJ                    crates/models/gptj on the same runtime (RoPE mode 0 over the whole head, heads up to 256 wide)
   InferenceSession        crates/llm-base/src/inference_session.rs     evaluate / n_past / rewind
 No arithmetic happens in Python."""
 import ctypes as C
@@ -109,6 +110,13 @@ class Bloom(Mpt):
 
     def _alibi_bias_max(self):
         return 8.0
+
+
+class GptJ(GptNeoX):
+    """KnownModel for GPT-J (crates/models/gptj): hyperparameters n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, wtype; tensors "transformer.wte.weight",
+    "transformer.ln_f.{weight,bias}", "lm_head.{weight,bias}", "transformer.h.N.ln_1.{weight,bias}", "transformer.h.N.attn.{q_proj,k_proj,v_proj,out_proj}.weight",
+    "transformer.h.N.mlp.{fc_in,fc_out}.{weight,bias}".  n_rot is the angle step of RoPE mode 0, which rotates every pair of the head."""
+    ARCH = 4
 
 
 class NeoxSession(_Native):
