@@ -46,11 +46,14 @@ struct NeoxLayer {
     const float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj;
     __half *K, *V;                      // [n_ctx][e] by position / [e][n_ctx] transposed, as the reference lays out memory_k / memory_v (:233-247)
 };
+// where q / k / v of head h start inside a row of the fused qkv projection: h * head_stride, + k_off, + v_off.  GPT-NeoX: per head [q | k | v]
+// (3 hd, hd, 2 hd); GPT-2, MPT, BLOOM, GPT-J: the three thirds of the row (hd, e, 2 e)
+struct QkvLayout { int head_stride, k_off, v_off; };
 struct NeoxParams {
-    int n_layer, e, hd, n_head, n_ctx, n_vocab, n_rot, parallel_residual;
-    int gpt2;                                   // GPT-2 (crates/models/gpt2/src/lib.rs:138-329): c_attn rows are [q | k | v] thirds, no RoPE, learned positions wpe, sequential residual
-                                                // (also set for MPT and BLOOM, which share the row layout and have no wpe)
-    const float *wpe;                           // [n_ctx][e] f32 (GPT-2), else nullptr
+    int n_layer, e, hd, n_head, n_ctx, n_vocab, parallel_residual;
+    int n_rot;                                  // RoPE mode 2 (GPT-NeoX) on n_rot of every head; 0: no mode-2 rotation
+    QkvLayout qkv_layout;
+    const float *wpe;                           // GPT-2 (crates/models/gpt2/src/lib.rs:138-329): learned positions [n_ctx][e] f32, else nullptr
     QWeight wte, lm_head;
     const float *lnf_g, *lnf_b;
     float kq_scale;
@@ -59,7 +62,7 @@ struct NeoxParams {
     const int32_t *token; int *n_past;
     float *x, *qkv, *q, *attn_out, *logits;     // residual stream [e], raw qkv [3e], roped q [e], attention branch output [e]
     int4 *xpack_a, *xpack_d, *xpack_f;          // records: layer-norm output (K = e), attention rows (K = e), gelu output (K = 4e)
-    // MPT / BLOOM (crates/models/{mpt,bloom}): the GPT-2 row layout (gpt2 = 1, wpe = nullptr) plus ALiBi; MPT leaves every bias pointer null
+    // MPT / BLOOM (crates/models/{mpt,bloom}): the GPT-2 row layout (no wpe) plus ALiBi; MPT leaves every bias pointer null
     const float *alibi = nullptr;               // per-head ALiBi slopes [n_head] (alibi_slopes), else nullptr
     const float *emb_g = nullptr, *emb_b = nullptr;   // BLOOM: LayerNorm of the embedding row before layer 0, else nullptr
     // GPT-J (crates/models/gptj): q | k | v thirds with RoPE mode 0 over the whole head (rope_cs: rope_table(n_rot, 0, .., hd, ..)), one LayerNorm per
@@ -71,10 +74,12 @@ struct NeoxParams {
 std::vector<float> alibi_slopes(int n_head, float max_bias);
 void decode_set_tp(const TpCtx &T, cudaStream_t st);   // uploads the tensor-parallel context the decode kernels read (constant memory)
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches);
+// whether neox_decode_enqueue takes a session of P's geometry and a step in the context bucket n_kv_bucket; otherwise the step runs per op
+bool neox_decode_fits(const NeoxParams &P, int n_kv_bucket);
 
-// whether attn_fused_kernel's shared memory for a bucket of nlay positions (a multiple of 64) and head size hd fits the 227 KB opt-in limit:
-// true up to nlay = 3264 for every hd <= 256.  Past it LLaMA decodes with the two-kernel attention and GPT-NeoX / GPT-2 / GPT-J per op.
-bool attn_fused_fits(int nlay, int hd);
+// whether attn_fused_kernel's shared memory for a context bucket of n_kv_bucket positions (rounded up to 64) and head size hd fits the 227 KB
+// opt-in limit: true up to 3264 positions for every hd <= 256.  Past it LLaMA decodes with the two-kernel attention and the GPT-NeoX family per op.
+bool attn_fused_fits(int n_kv_bucket, int hd);
 
 // default decode schedule: 8 fused kernels per layer on `st` (decode_ops.cu); position read from *P.n_past on the device
 void decode_ops_enqueue(const DecodeParams &P, const std::vector<DecodeLayer> &layers, int wtype, int n_kv_bucket, int4 *xpack_a, cudaStream_t st, int *launches);

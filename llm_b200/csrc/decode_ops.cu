@@ -747,20 +747,24 @@ static void attn_fused_reserve(size_t bytes) {
     B200_CHECK(cudaFuncSetAttribute(attn_fused_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
-// dynamic shared memory of attn_fused_kernel for nlay positions and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
-size_t attn_fused_smem(int nlay, int hd) {
+// the positions attn_fused_kernel holds for a context bucket: the bucket rounded up to whole 64-position tiles
+int attn_fused_rows(int n_kv_bucket) { return (n_kv_bucket + 63) / 64 * 64; }
+// dynamic shared memory of attn_fused_kernel for a context bucket and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
+size_t attn_fused_smem(int n_kv_bucket, int hd) {
+    const int nlay = attn_fused_rows(n_kv_bucket);
     return (((size_t)nlay * 6 + (size_t)hd * 2 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 32) * 2;
 }
 }  // namespace
-bool attn_fused_fits(int nlay, int hd) { return attn_fused_smem(nlay, hd) <= 227 * 1024; }
+bool attn_fused_fits(int n_kv_bucket, int hd) { return attn_fused_smem(n_kv_bucket, hd) <= 227 * 1024; }
 namespace {
 // one cluster of hd/32 CTAs per head, a programmatic dependent of its predecessor.  alibi: per-head slopes (the ALiBi form, single GPU only)
 // or nullptr
 template <bool TP>
 void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const __half *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
-                       float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                       float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int n_kv_bucket, int q81, int off, int scale16,
                        unsigned long long *prof, const TpSync &S, int head0, const float *alibi = nullptr) {
-    const size_t smem = attn_fused_smem(nlay, hd);
+    const int nlay = attn_fused_rows(n_kv_bucket);
+    const size_t smem = attn_fused_smem(n_kv_bucket, hd);
     attn_fused_reserve(smem);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(n_head * (hd / 32)); cfg.blockDim = dim3(ATH); cfg.dynamicSmemBytes = smem; cfg.stream = st;
@@ -836,9 +840,8 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     if (tp) { launch_k(tp_spread_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.x, e); n++; }
     // attention: one cluster launch per layer, or the two-kernel variant for head sizes a cluster cannot cover and for buckets whose scores
     // and V rows do not fit one CTA's shared memory
-    const int nlay = (n_kv_bucket + 63) / 64 * 64;
-    const size_t fa_smem = attn_fused_smem(nlay, P.hd);
-    const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd);
+    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd);
+    const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(n_kv_bucket, P.hd);
     B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue (start_session_tp checks the size)
     const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
     static size_t sv_set = 48 * 1024;
@@ -861,7 +864,7 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
         A.prof = pr(); launch_mmv<TYPE, EPI_QKV, TP>(L.wqkv, A, p_qkv, st); n++;
         if (fused_attn) {
-            launch_attn_fused<TP>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, nlay, q81, off, s16, pr(),
+            launch_attn_fused<TP>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, n_kv_bucket, q81, off, s16, pr(),
                                   ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0);
             n++;
         } else {
@@ -1007,9 +1010,8 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     }
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
-    const int nlay = (n_kv_bucket + 63) / 64 * 64;
-    const size_t fa_smem = attn_fused_smem(nlay, P.hd);
-    B200_ASSERT(P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd) && e <= 8192);   // neox.cu::forward checks both
+    B200_ASSERT(neox_decode_fits(P, n_kv_bucket));
+    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     // MPT has no biases: its norms take ln_pack_nobias_kernel and its up-projection the gelu epilogue without a bias node
@@ -1028,8 +1030,8 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         MmvArgs A{}; A.xpack = P.xpack_a; A.dst = P.qkv; A.bias = L.bqkv;
         launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, p_qkv, st); n++;                                                                                      // :199-200
         launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, L.K, L.V, (const int *)P.n_past, P.rope_cs, P.rope_half,
-                 P.gpt2 ? 0 : P.n_rot, P.hd, e, P.n_ctx, P.gpt2 ? P.hd : 3 * P.hd, P.gpt2 ? e : P.hd, P.gpt2 ? 2 * e : 2 * P.hd); n++;               // :205-247
-        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, nlay, q81, off, s16,
+                 P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off); n++;                               // :205-247
+        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
                                  nullptr, S, 0, P.alibi); n++;                                                                            // :250-298
         // attention.dense (+bias); sequential residual: ff_in = that + inpL                                                                    :301-312
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out; Bo.bias = L.bdense; Bo.add1 = P.parallel_residual ? nullptr : P.x;
@@ -1061,9 +1063,8 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     int n = 0;
     // the token boundary: a plain launch (no programmatic attribute), see neox_ops_t
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;                                                                                                     // :161
-    const int nlay = (n_kv_bucket + 63) / 64 * 64;
-    const size_t fa_smem = attn_fused_smem(nlay, P.hd);
-    B200_ASSERT(P.hd % 32 == 0 && P.hd <= 256 && P.n_ctx % 8 == 0 && attn_fused_fits(nlay, P.hd) && e <= 8192 && !P.alibi);   // neox.cu::forward checks these
+    B200_ASSERT(neox_decode_fits(P, n_kv_bucket));
+    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
@@ -1080,7 +1081,7 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         MmvArgs A{}; A.xpack = P.xpack_a; A.q = P.q; A.K = L.K; A.V = L.V; A.rope_cs = P.rope_cs; A.rope_half = P.rope_half; A.hd = P.hd; A.e = e; A.gqa = e;
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
         launch_mmv<TYPE, EPI_QKV>(L.wqkv, A, p_qkv, st); n++;                                                                                          // :178-220
-        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, nlay, q81, off, s16,
+        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
                                  nullptr, S, 0); n++;                                                                                                   // :222-262
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;                                                                                    // :265
@@ -1097,6 +1098,15 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
 }
 
 }  // namespace
+
+// The cluster attention takes heads of up to 128 (GPT-J's wide form: up to 256) in 32-wide slices and the bucket's scores and V rows in shared
+// memory; ln_pack_body holds rows of up to 8192; the mat-vecs stream rows of n_embd and 4 n_embd.
+bool neox_decode_fits(const NeoxParams &P, int n_kv_bucket) {
+    QWeight k_e, k_4e;
+    k_e.nb = P.e / QK; k_4e.nb = 4 * P.e / QK;
+    return P.hd % 32 == 0 && P.hd <= (P.gptj ? 256 : 128) && P.e % 128 == 0 && P.e <= 8192 && P.n_ctx % 8 == 0 &&
+           mmv_exact_stream_supported(k_e) && mmv_exact_stream_supported(k_4e) && attn_fused_fits(n_kv_bucket, P.hd);
+}
 
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches) {
     switch (wtype) {

@@ -22,6 +22,35 @@
 
 using namespace b200;
 
+namespace {
+
+// One tensor of an architecture.  Sizes: E = n_embd, E3 / E4 = 3 / 4 n_embd, VOCAB = n_vocab, CTX_E = context_size x n_embd.
+enum Dim : uint8_t { E, E3, E4, VOCAB, CTX_E };
+enum Kind : uint8_t {
+    MAT,        // quantized K x N matrix
+    GAIN,       // f32 vector of K floats, synthesized as 1 + 0.1 N(0,1)
+    BIAS,       // f32 vector of K floats, synthesized as 0.01 N(0,1)
+    ROWS,       // rows [at n_embd, (at + 1) n_embd) of the matrix q, which another entry carves and draws
+};
+template <class O> using QRef = QWeight O::*;
+template <class O> using FRef = float *O::*;
+template <class Owner> struct TensorDef {
+    const char *name;           // the model's name, or a layer's suffix under the layer prefix; nullptr: carved and drawn, never loaded by name
+    Kind kind;
+    QRef<Owner> q;
+    FRef<Owner> f;
+    Dim K, N = E;
+    uint8_t at = 0;
+    bool if_lm_head = false;    // present only when hparams.has_lm_head (GPT-2's model/lm_head)
+};
+template <class O> constexpr TensorDef<O> mat(const char *n, QRef<O> q, Dim K, Dim N) { return {n, MAT, q, nullptr, K, N}; }
+template <class O> constexpr TensorDef<O> gain(const char *n, FRef<O> f, Dim K = E) { return {n, GAIN, nullptr, f, K}; }
+template <class O> constexpr TensorDef<O> bias(const char *n, FRef<O> f, Dim K = E) { return {n, BIAS, nullptr, f, K}; }
+template <class O> constexpr TensorDef<O> rows(const char *n, QRef<O> q, uint8_t at) { return {n, ROWS, q, nullptr, E, E, at}; }
+template <class O> constexpr TensorDef<O> if_lm_head(TensorDef<O> d) { d.if_lm_head = true; return d; }
+
+}  // namespace
+
 struct b200_neox_model : Weights {
     b200_neox_hparams hp;
     int hd = 0;
@@ -30,23 +59,20 @@ struct b200_neox_model : Weights {
     float *emb_g = nullptr, *emb_b = nullptr;                     // BLOOM: LayerNorm of the embedding row
     DeviceBuf<float> alibi;                                       // MPT / BLOOM: ALiBi slopes [n_head] (alibi_slopes)
     float *lm_head_b = nullptr;                                   // GPT-J: lm_head.bias [n_vocab]
-    bool gpt2() const { return hp.arch == 1; }
+    const RopeTable *rope = nullptr;                              // GPT-NeoX: mode 2 on n_rot of every head; GPT-J: mode 0 over the whole head; else none
+    QkvLayout qkv_layout;
+    bool parallel = false;                                        // GPT-NeoX with use_parallel_residual: attention and MLP both read inpL
+    float kq_scale = 0.0f;
+    bool neox() const { return hp.arch == 0; }
     bool mpt() const { return hp.arch == 2; }
     bool bloom() const { return hp.arch == 3; }
     bool gptj() const { return hp.arch == 4; }
-    bool thirds() const { return hp.arch >= 1; }                  // GPT-2, MPT, BLOOM, GPT-J: q | k | v are the thirds of the fused row (GPT-J: RoPE mode 0, the others none)
     // MPT: every bias null; GPT-J: ln2_*, bqkv and bdense null (one LayerNorm per layer, no attention biases)
     struct Layer { QWeight wqkv, wdense, wfc, wproj; float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj; };
     std::vector<Layer> layers;
-    int n_slots() const {
-        if (mpt()) return 2 + 6 * hp.n_layer;                                 // wte, norm_f, 6 per block
-        if (bloom()) return 6 + 12 * hp.n_layer;                              // wte, norm.{weight,bias}, output_norm.{weight,bias}, output, 12 per layer
-        if (gptj()) return 5 + 10 * hp.n_layer;                               // wte, ln_f.{weight,bias}, lm_head.{weight,bias}, 10 per layer
-        return 4 + 12 * hp.n_layer + (gpt2() && hp.has_lm_head ? 1 : 0);       // GPT-2: slot 3 = wpe, lm_head (if present) last
-    }
+    template <class F> void each_tensor(F &&f);
+    int64_t dim(Dim d) const;
     bool lookup(const char *name, Slot &s, int &id);
-    bool lookup_alibi(const char *name, Slot &s, int &id);
-    bool lookup_gptj(const char *name, Slot &s, int &id);
 };
 
 struct b200_neox_session : SessionCore {   // memory_k [n_layer][n_ctx][e], memory_v [n_layer][e][n_ctx]
@@ -55,132 +81,110 @@ struct b200_neox_session : SessionCore {   // memory_k [n_layer][n_ctx][e], memo
     DeviceBuf<float> qdec;
     DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh;
     DeviceBuf<int4> xpack_a, xpack_d, xpack_f;
-    bool decode_ok = false;
     std::vector<NeoxLayer> dl;
     NeoxParams dp;
 };
 
-// MPT: crates/models/mpt/src/lib.rs:49-65; BLOOM: crates/models/bloom/src/lib.rs:56-83
-bool b200_neox_model::lookup_alibi(const char *name, Slot &s, int &id) {
-    const int e = hp.n_embd;
-    int il = -1; char sub[96];
-    struct Entry { const char *n; QWeight *q; float *f; int64_t len; };
-    if (mpt()) {
-        if (!strcmp(name, "transformer.wte.weight")) { s.q = wte; s.is_q = true; id = 0; return true; }
-        if (!strcmp(name, "transformer.norm_f.weight")) { s.f = lnf_g; s.n = e; id = 1; return true; }
-        if (sscanf(name, "transformer.blocks.%d.%95s", &il, sub) != 2 || il < 0 || il >= hp.n_layer) return false;
-        Layer &L = layers[il];
-        const Entry tab[] = {{"norm_1.weight", nullptr, L.ln1_g, e}, {"attn.Wqkv.weight", &L.wqkv, nullptr, 0}, {"attn.out_proj.weight", &L.wdense, nullptr, 0},
-                             {"norm_2.weight", nullptr, L.ln2_g, e}, {"ffn.up_proj.weight", &L.wfc, nullptr, 0}, {"ffn.down_proj.weight", &L.wproj, nullptr, 0}};
-        for (int k = 0; k < 6; k++)
-            if (!strcmp(sub, tab[k].n)) {
-                if (tab[k].q) { s.q = *tab[k].q; s.is_q = true; } else { s.f = tab[k].f; s.n = tab[k].len; }
-                id = 2 + 6 * il + k;
-                return true;
-            }
-        return false;
-    }
-    const Entry glob[] = {{"tok_embeddings.weight", &wte, nullptr, 0}, {"norm.weight", nullptr, emb_g, e}, {"norm.bias", nullptr, emb_b, e},
-                          {"output_norm.weight", nullptr, lnf_g, e}, {"output_norm.bias", nullptr, lnf_b, e}, {"output.weight", &lm_head, nullptr, 0}};
-    for (int k = 0; k < 6; k++)
-        if (!strcmp(name, glob[k].n)) {
-            if (glob[k].q) { s.q = *glob[k].q; s.is_q = true; } else { s.f = glob[k].f; s.n = glob[k].len; }
-            id = k;
-            return true;
-        }
-    if (sscanf(name, "layers.%d.%95s", &il, sub) != 2 || il < 0 || il >= hp.n_layer) return false;
-    Layer &L = layers[il];
-    const Entry tab[] = {
-        {"attention_norm.weight", nullptr, L.ln1_g, e}, {"attention_norm.bias", nullptr, L.ln1_b, e},
-        {"attention.query_key_value.weight", &L.wqkv, nullptr, 0}, {"attention.query_key_value.bias", nullptr, L.bqkv, 3 * (int64_t)e},
-        {"attention.wo.weight", &L.wdense, nullptr, 0}, {"attention.wo.bias", nullptr, L.bdense, e},
-        {"ffn_norm.weight", nullptr, L.ln2_g, e}, {"ffn_norm.bias", nullptr, L.ln2_b, e},
-        {"feed_forward.w1.weight", &L.wfc, nullptr, 0}, {"feed_forward.w1.bias", nullptr, L.bfc, 4 * (int64_t)e},
-        {"feed_forward.w2.weight", &L.wproj, nullptr, 0}, {"feed_forward.w2.bias", nullptr, L.bproj, e}};
-    for (int k = 0; k < 12; k++)
-        if (!strcmp(sub, tab[k].n)) {
-            if (tab[k].q) { s.q = *tab[k].q; s.is_q = true; } else { s.f = tab[k].f; s.n = tab[k].len; }
-            id = 6 + 12 * il + k;
-            return true;
-        }
-    return false;
+namespace {
+
+using Model = b200_neox_model;
+using Layer = b200_neox_model::Layer;
+
+// The tensors of each architecture in slab order: the slab is carved and b200_neox_synthesize draws in this order, so it fixes both the slab
+// layout and the synthetic weights.  A tensor's slot (the loaded bitmap) is its place among the named entries.
+struct ArchTensors {
+    std::vector<TensorDef<Model>> globals;
+    const char *layer_fmt;      // a per-layer name: the layer prefix, then the suffix
+    std::vector<TensorDef<Layer>> layer;
+};
+const ArchTensors &arch_tensors(int arch) {      // by b200_neox_hparams.arch
+    static const ArchTensors tab[] = {
+        {   // GPT-NeoX: crates/models/gptneox/src/lib.rs:59-127
+            {mat("gpt_neox.embed_in.weight", &Model::wte, E, VOCAB), mat("embed_out.weight", &Model::lm_head, E, VOCAB),
+             gain("gpt_neox.final_layer_norm.weight", &Model::lnf_g), bias("gpt_neox.final_layer_norm.bias", &Model::lnf_b)},
+            "gpt_neox.layers.%d.%95s",
+            {gain("input_layernorm.weight", &Layer::ln1_g), bias("input_layernorm.bias", &Layer::ln1_b),
+             gain("post_attention_layernorm.weight", &Layer::ln2_g), bias("post_attention_layernorm.bias", &Layer::ln2_b),
+             bias("attention.query_key_value.bias", &Layer::bqkv, E3), bias("attention.dense.bias", &Layer::bdense),
+             bias("mlp.dense_h_to_4h.bias", &Layer::bfc, E4), bias("mlp.dense_4h_to_h.bias", &Layer::bproj),
+             mat("attention.query_key_value.weight", &Layer::wqkv, E, E3), mat("attention.dense.weight", &Layer::wdense, E, E),
+             mat("mlp.dense_h_to_4h.weight", &Layer::wfc, E, E4), mat("mlp.dense_4h_to_h.weight", &Layer::wproj, E4, E)}},
+        {   // GPT-2: crates/models/gpt2/src/lib.rs:59-107
+            {mat("model/wte", &Model::wte, E, VOCAB), if_lm_head(mat("model/lm_head", &Model::lm_head, E, VOCAB)),
+             gain("model/ln_f/g", &Model::lnf_g), bias("model/ln_f/b", &Model::lnf_b), bias("model/wpe", &Model::wpe, CTX_E)},
+            "model/h%d/%95s",
+            {gain("ln_1/g", &Layer::ln1_g), bias("ln_1/b", &Layer::ln1_b), gain("ln_2/g", &Layer::ln2_g), bias("ln_2/b", &Layer::ln2_b),
+             bias("attn/c_attn/b", &Layer::bqkv, E3), bias("attn/c_proj/b", &Layer::bdense), bias("mlp/c_fc/b", &Layer::bfc, E4), bias("mlp/c_proj/b", &Layer::bproj),
+             mat("attn/c_attn/w", &Layer::wqkv, E, E3), mat("attn/c_proj/w", &Layer::wdense, E, E),
+             mat("mlp/c_fc/w", &Layer::wfc, E, E4), mat("mlp/c_proj/w", &Layer::wproj, E4, E)}},
+        {   // MPT: crates/models/mpt/src/lib.rs:49-65, no biases
+            {mat("transformer.wte.weight", &Model::wte, E, VOCAB), gain("transformer.norm_f.weight", &Model::lnf_g)},
+            "transformer.blocks.%d.%95s",
+            {gain("norm_1.weight", &Layer::ln1_g), gain("norm_2.weight", &Layer::ln2_g),
+             mat("attn.Wqkv.weight", &Layer::wqkv, E, E3), mat("attn.out_proj.weight", &Layer::wdense, E, E),
+             mat("ffn.up_proj.weight", &Layer::wfc, E, E4), mat("ffn.down_proj.weight", &Layer::wproj, E4, E)}},
+        {   // BLOOM: crates/models/bloom/src/lib.rs:56-83
+            {mat("tok_embeddings.weight", &Model::wte, E, VOCAB), mat("output.weight", &Model::lm_head, E, VOCAB),
+             gain("output_norm.weight", &Model::lnf_g), bias("output_norm.bias", &Model::lnf_b), gain("norm.weight", &Model::emb_g), bias("norm.bias", &Model::emb_b)},
+            "layers.%d.%95s",
+            {gain("attention_norm.weight", &Layer::ln1_g), bias("attention_norm.bias", &Layer::ln1_b),
+             gain("ffn_norm.weight", &Layer::ln2_g), bias("ffn_norm.bias", &Layer::ln2_b),
+             bias("attention.query_key_value.bias", &Layer::bqkv, E3), bias("attention.wo.bias", &Layer::bdense),
+             bias("feed_forward.w1.bias", &Layer::bfc, E4), bias("feed_forward.w2.bias", &Layer::bproj),
+             mat("attention.query_key_value.weight", &Layer::wqkv, E, E3), mat("attention.wo.weight", &Layer::wdense, E, E),
+             mat("feed_forward.w1.weight", &Layer::wfc, E, E4), mat("feed_forward.w2.weight", &Layer::wproj, E4, E)}},
+        {   // GPT-J: crates/models/gptj/src/lib.rs:59-103, no attention biases, one LayerNorm per layer; q_proj / k_proj / v_proj are the thirds of wqkv
+            {mat("transformer.wte.weight", &Model::wte, E, VOCAB), mat("lm_head.weight", &Model::lm_head, E, VOCAB),
+             gain("transformer.ln_f.weight", &Model::lnf_g), bias("transformer.ln_f.bias", &Model::lnf_b), bias("lm_head.bias", &Model::lm_head_b, VOCAB)},
+            "transformer.h.%d.%95s",
+            {gain("ln_1.weight", &Layer::ln1_g), bias("ln_1.bias", &Layer::ln1_b), bias("mlp.fc_in.bias", &Layer::bfc, E4), bias("mlp.fc_out.bias", &Layer::bproj),
+             mat(nullptr, &Layer::wqkv, E, E3), rows("attn.q_proj.weight", &Layer::wqkv, 0), rows("attn.k_proj.weight", &Layer::wqkv, 1),
+             rows("attn.v_proj.weight", &Layer::wqkv, 2), mat("attn.out_proj.weight", &Layer::wdense, E, E),
+             mat("mlp.fc_in.weight", &Layer::wfc, E, E4), mat("mlp.fc_out.weight", &Layer::wproj, E4, E)}},
+    };
+    return tab[arch];
 }
 
-// GPT-J: crates/models/gptj/src/lib.rs:59-103.  q_proj / k_proj / v_proj are rows [0, e), [e, 2e), [2e, 3e) of one wqkv.
-bool b200_neox_model::lookup_gptj(const char *name, Slot &s, int &id) {
-    const int e = hp.n_embd;
-    if (!strcmp(name, "transformer.wte.weight")) { s.q = wte; s.is_q = true; id = 0; return true; }
-    if (!strcmp(name, "transformer.ln_f.weight")) { s.f = lnf_g; s.n = e; id = 1; return true; }
-    if (!strcmp(name, "transformer.ln_f.bias")) { s.f = lnf_b; s.n = e; id = 2; return true; }
-    if (!strcmp(name, "lm_head.weight")) { s.q = lm_head; s.is_q = true; id = 3; return true; }
-    if (!strcmp(name, "lm_head.bias")) { s.f = lm_head_b; s.n = hp.n_vocab; id = 4; return true; }
-    int il = -1; char sub[96];
-    if (sscanf(name, "transformer.h.%d.%95s", &il, sub) != 2 || il < 0 || il >= hp.n_layer) return false;
-    Layer &L = layers[il];
-    const QWeight wq = row_view(L.wqkv, 0, e), wk = row_view(L.wqkv, e, e), wv = row_view(L.wqkv, 2 * (int64_t)e, e);
-    struct { const char *n; const QWeight *q; float *f; int64_t len; } tab[] = {
-        {"ln_1.weight", nullptr, L.ln1_g, e}, {"ln_1.bias", nullptr, L.ln1_b, e},
-        {"attn.q_proj.weight", &wq, nullptr, 0}, {"attn.k_proj.weight", &wk, nullptr, 0}, {"attn.v_proj.weight", &wv, nullptr, 0},
-        {"attn.out_proj.weight", &L.wdense, nullptr, 0},
-        {"mlp.fc_in.weight", &L.wfc, nullptr, 0}, {"mlp.fc_in.bias", nullptr, L.bfc, 4 * (int64_t)e},
-        {"mlp.fc_out.weight", &L.wproj, nullptr, 0}, {"mlp.fc_out.bias", nullptr, L.bproj, e}};
-    for (int k = 0; k < 10; k++)
-        if (!strcmp(sub, tab[k].n)) {
-            if (tab[k].q) { s.q = *tab[k].q; s.is_q = true; } else { s.f = tab[k].f; s.n = tab[k].len; }
-            id = 5 + 10 * il + k;
-            return true;
-        }
-    return false;
+}  // namespace
+
+// f(def, owner, il) for every tensor of the model in slab order: the model's own (il = -1, owner = the model), then layer by layer
+template <class F> void b200_neox_model::each_tensor(F &&f) {
+    const ArchTensors &a = arch_tensors(hp.arch);
+    for (const TensorDef<Model> &d : a.globals)
+        if (!d.if_lm_head || hp.has_lm_head) f(d, *this, -1);
+    for (int il = 0; il < hp.n_layer; il++)
+        for (const TensorDef<Layer> &d : a.layer) f(d, layers[il], il);
+}
+
+int64_t b200_neox_model::dim(Dim d) const {
+    const int64_t e = hp.n_embd;
+    switch (d) {
+        case E3: return 3 * e;
+        case E4: return 4 * e;
+        case VOCAB: return hp.n_vocab;
+        case CTX_E: return hp.context_size * e;
+        default: return e;
+    }
 }
 
 bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
-    const int e = hp.n_embd;
-    s = Slot();
-    if (gptj()) return lookup_gptj(name, s, id);
-    if (mpt() || bloom()) return lookup_alibi(name, s, id);
-    if (gpt2()) {                                                         // tensor names of crates/models/gpt2/src/lib.rs:59-107
-        if (!strcmp(name, "model/wte")) { s.q = wte; s.is_q = true; id = 0; return true; }
-        if (!strcmp(name, "model/ln_f/g")) { s.f = lnf_g; s.n = e; id = 1; return true; }
-        if (!strcmp(name, "model/ln_f/b")) { s.f = lnf_b; s.n = e; id = 2; return true; }
-        if (!strcmp(name, "model/wpe")) { s.f = wpe; s.n = (int64_t)hp.context_size * e; id = 3; return true; }
-        if (!strcmp(name, "model/lm_head")) { if (!hp.has_lm_head) return false; s.q = lm_head; s.is_q = true; id = 4 + 12 * hp.n_layer; return true; }
-        int il = -1; char sub[96];
-        if (sscanf(name, "model/h%d/%95s", &il, sub) != 2 || il < 0 || il >= hp.n_layer) return false;
-        Layer &L = layers[il];
-        struct { const char *n; QWeight *q; float *f; int64_t len; } tab[] = {
-            {"ln_1/g", nullptr, L.ln1_g, e}, {"ln_1/b", nullptr, L.ln1_b, e}, {"ln_2/g", nullptr, L.ln2_g, e}, {"ln_2/b", nullptr, L.ln2_b, e},
-            {"attn/c_attn/w", &L.wqkv, nullptr, 0}, {"attn/c_attn/b", nullptr, L.bqkv, 3 * (int64_t)e}, {"attn/c_proj/w", &L.wdense, nullptr, 0}, {"attn/c_proj/b", nullptr, L.bdense, e},
-            {"mlp/c_fc/w", &L.wfc, nullptr, 0}, {"mlp/c_fc/b", nullptr, L.bfc, 4 * (int64_t)e}, {"mlp/c_proj/w", &L.wproj, nullptr, 0}, {"mlp/c_proj/b", nullptr, L.bproj, e}};
-        for (int k = 0; k < 12; k++)
-            if (!strcmp(sub, tab[k].n)) {
-                if (tab[k].q) { s.q = *tab[k].q; s.is_q = true; } else { s.f = tab[k].f; s.n = tab[k].len; }
-                id = 4 + 12 * il + k;
-                return true;
-            }
-        return false;
-    }
-    if (!strcmp(name, "gpt_neox.embed_in.weight")) { s.q = wte; s.is_q = true; id = 0; return true; }
-    if (!strcmp(name, "gpt_neox.final_layer_norm.weight")) { s.f = lnf_g; s.n = e; id = 1; return true; }
-    if (!strcmp(name, "gpt_neox.final_layer_norm.bias")) { s.f = lnf_b; s.n = e; id = 2; return true; }
-    if (!strcmp(name, "embed_out.weight")) { s.q = lm_head; s.is_q = true; id = 3; return true; }
     int il = -1; char sub[96];
-    if (sscanf(name, "gpt_neox.layers.%d.%95s", &il, sub) != 2 || il < 0 || il >= hp.n_layer) return false;
-    Layer &L = layers[il];
-    const int base = 4 + 12 * il;
-    struct { const char *n; QWeight *q; float *f; int64_t len; } tab[] = {
-        {"input_layernorm.weight", nullptr, L.ln1_g, e}, {"input_layernorm.bias", nullptr, L.ln1_b, e},
-        {"post_attention_layernorm.weight", nullptr, L.ln2_g, e}, {"post_attention_layernorm.bias", nullptr, L.ln2_b, e},
-        {"attention.query_key_value.weight", &L.wqkv, nullptr, 0}, {"attention.query_key_value.bias", nullptr, L.bqkv, 3 * (int64_t)e},
-        {"attention.dense.weight", &L.wdense, nullptr, 0}, {"attention.dense.bias", nullptr, L.bdense, e},
-        {"mlp.dense_h_to_4h.weight", &L.wfc, nullptr, 0}, {"mlp.dense_h_to_4h.bias", nullptr, L.bfc, 4 * (int64_t)e},
-        {"mlp.dense_4h_to_h.weight", &L.wproj, nullptr, 0}, {"mlp.dense_4h_to_h.bias", nullptr, L.bproj, e}};
-    for (int k = 0; k < 12; k++)
-        if (!strcmp(sub, tab[k].n)) {
-            if (tab[k].q) { s.q = *tab[k].q; s.is_q = true; } else { s.f = tab[k].f; s.n = tab[k].len; }
-            id = base + k;
-            return true;
+    if (sscanf(name, arch_tensors(hp.arch).layer_fmt, &il, sub) != 2) il = -1;
+    int slot = 0;
+    bool found = false;
+    each_tensor([&](const auto &d, auto &o, int l) {
+        if (found || !d.name) return;
+        if (l < 0 ? !strcmp(name, d.name) : l == il && !strcmp(sub, d.name)) {
+            s = Slot();
+            if (d.kind == MAT) { s.q = o.*d.q; s.is_q = true; }
+            else if (d.kind == ROWS) { s.q = row_view(o.*d.q, d.at * (int64_t)hp.n_embd, hp.n_embd); s.is_q = true; }
+            else { s.f = o.*d.f; s.n = dim(d.K); }
+            id = slot;
+            found = true;
         }
-    return false;
+        slot++;
+    });
+    return found;
 }
 
 namespace {
@@ -193,7 +197,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     int L = 0;
     // the graph schedule's attention keeps the whole bucket in shared memory: steps in buckets past 3264 positions run per op below, and the
     // graph cache re-uploads the device n_past when graph steps resume (after a rewind)
-    if (n == 1 && s->decode_ok && attn_fused_fits((DecodeGraphCache::bucket(n_kv, n_ctx) + 63) / 64 * 64, hd)) {
+    if (n == 1 && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {
         s->last_launches = s->decode.run(n_kv, n_ctx, true, [s, &hp](int bucket, cudaStream_t st, int *nodes) {
             neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
         }, st);
@@ -201,21 +205,17 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         return;
     }
     const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()};
-    const float kq_scale = 1.0f / sqrtf((float)e / (float)n_head);                                                  // :270-273
-    const bool g2 = m->thirds(), gptj = m->gptj(), parallel = !g2 && hp.use_parallel_residual;
-    // GPT-NeoX: mode 2 on n_rot of every head; GPT-J: mode 0 over ALL hd elements of the head with theta_scale base^(-2/n_rot) (gptj lib.rs:178-201,
-    // LC/ggml.c:11859-11874 walks ne0, not n_dims)
-    const RopeTable *rope = gptj ? &rope_table(hp.n_rot, 0, 10000.0f, 1.0f, hd, n_ctx) : g2 ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, hd, n_ctx);
+    const bool gptj = m->gptj(), parallel = m->parallel;
+    const RopeTable *rope = m->rope;
     const int64_t ld3 = 3 * (int64_t)e;
-    // where q / k / v of head h live inside a row of the fused projection: NeoX per head [q | k | v], GPT-2 / MPT / BLOOM the three thirds of the row
-    const int64_t hs = g2 ? hd : 3 * hd, koff = g2 ? e : hd, voff = g2 ? 2 * (int64_t)e : 2 * hd;
-    if (m->bloom()) {                                                                                                             // bloom lib.rs:139-144
+    const int64_t hs = m->qkv_layout.head_stride, koff = m->qkv_layout.k_off, voff = m->qkv_layout.v_off;
+    if (m->emb_g) {                                                                                                               // bloom lib.rs:139-144
         get_rows_q(m->wte, s->d_tokens.get(), s->t.get(), n, st); L++;
         layer_norm(s->t.get(), s->x.get(), m->emb_g, m->emb_b, e, n, st); L++;
     } else {
         get_rows_q(m->wte, s->d_tokens.get(), s->x.get(), n, st); L++;                                                           // :178
     }
-    if (m->gpt2()) { add_f32(s->x.get(), m->wpe + (size_t)n_past * e, s->x.get(), (int64_t)n * e, (int64_t)n * e, st); L++; }             // gpt2 lib.rs:164-172: + wpe[n_past + i]
+    if (m->wpe) { add_f32(s->x.get(), m->wpe + (size_t)n_past * e, s->x.get(), (int64_t)n * e, (int64_t)n * e, st); L++; }               // gpt2 lib.rs:164-172: + wpe[n_past + i]
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &ly = m->layers[il];
         __half *Kl = s->memory_k.get() + (size_t)il * n_ctx * e, *Vl = s->memory_v.get() + (size_t)il * n_ctx * e;
@@ -234,8 +234,8 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         }
         mul_mat_f16_exact(Kl, hd, n_kv, n_head, (int64_t)e * 2, (int64_t)hd * 2, s->qkv.get(), n, n_head, ld3 * 4, hs * 4,
                           s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st); L++;                          // :250-267
-        if (m->alibi) soft_max_alibi(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, kq_scale, n_past, m->alibi.get(), st);   // MPT / BLOOM: + ALiBi
-        else soft_max(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, kq_scale, true, n_past, true, true, st);                // :270-279
+        if (m->alibi) soft_max_alibi(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, m->kq_scale, n_past, m->alibi.get(), st);   // MPT / BLOOM: + ALiBi
+        else soft_max(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, m->kq_scale, true, n_past, true, true, st);                // :270-279
         L++;
         // GPT-J: cur (ln_1's output, input_sa) still feeds fc_in, so the merged KQV goes to t
         float *kqv = gptj ? s->t.get() : s->cur.get();
@@ -288,44 +288,32 @@ b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
     rt().ensure_init();
     b200_neox_model *m = new b200_neox_model();
     m->hp = *hp;
-    const int e = hp->n_embd, v = hp->n_vocab, t = hp->wtype;
-    m->hd = e / hp->n_head;
+    const int e = hp->n_embd, v = hp->n_vocab, t = hp->wtype, hd = e / hp->n_head;
+    m->hd = hd;
     m->layers.resize(hp->n_layer);
-    if (m->mpt()) {                                                       // no biases (mpt lib.rs:49-65)
-        m->carve(t, m->n_slots(), [m, e, v](SlabCarver &c) {
-            c.q(m->wte, e, v); c.f(m->lnf_g, e);
-            for (auto &L : m->layers) { c.f(L.ln1_g, e); c.f(L.ln2_g, e); c.q(L.wqkv, e, 3 * e); c.q(L.wdense, e, e); c.q(L.wfc, e, 4 * e); c.q(L.wproj, 4 * e, e); }
+    int n_slots = 0;
+    m->each_tensor([&n_slots](const auto &d, auto &, int) { n_slots += d.name != nullptr; });
+    m->carve(t, n_slots, [m](SlabCarver &c) {
+        m->each_tensor([&](const auto &d, auto &o, int) {
+            if (d.kind == MAT) c.q(o.*d.q, m->dim(d.K), m->dim(d.N));
+            else if (d.kind != ROWS) c.f(o.*d.f, m->dim(d.K));
         });
-    } else if (m->gptj()) {                                               // gptj lib.rs:59-103: no attention biases, one LayerNorm per layer
-        m->carve(t, m->n_slots(), [m, e, v](SlabCarver &c) {
-            c.q(m->wte, e, v); c.q(m->lm_head, e, v);
-            c.f(m->lnf_g, e); c.f(m->lnf_b, e); c.f(m->lm_head_b, v);
-            for (auto &L : m->layers) {
-                c.f(L.ln1_g, e); c.f(L.ln1_b, e); c.f(L.bfc, 4 * e); c.f(L.bproj, e);
-                c.q(L.wqkv, e, 3 * e); c.q(L.wdense, e, e); c.q(L.wfc, e, 4 * e); c.q(L.wproj, 4 * e, e);
-            }
-        });
-    } else {
-        m->carve(t, m->n_slots(), [m, hp, e, v](SlabCarver &c) {
-            c.q(m->wte, e, v);
-            if (!m->gpt2() || hp->has_lm_head) c.q(m->lm_head, e, v);
-            c.f(m->lnf_g, e); c.f(m->lnf_b, e);
-            if (m->gpt2()) c.f(m->wpe, (int64_t)hp->context_size * e);
-            if (m->bloom()) { c.f(m->emb_g, e); c.f(m->emb_b, e); }
-            for (auto &L : m->layers) {
-                c.f(L.ln1_g, e); c.f(L.ln1_b, e); c.f(L.ln2_g, e); c.f(L.ln2_b, e); c.f(L.bqkv, 3 * e); c.f(L.bdense, e); c.f(L.bfc, 4 * e); c.f(L.bproj, e);
-                c.q(L.wqkv, e, 3 * e); c.q(L.wdense, e, e); c.q(L.wfc, e, 4 * e); c.q(L.wproj, 4 * e, e);
-            }
-        });
-    }
-    // tied output projection (gpt2 lib.rs:319-320, MPT always): wte is streamed as the lm_head
-    if ((m->gpt2() && !hp->has_lm_head) || m->mpt()) m->lm_head = m->wte;
+    });
+    // no output matrix (GPT-2 without model/lm_head, gpt2 lib.rs:319-320; MPT): the output projection is tied to wte, which is streamed as the lm_head
+    if (!m->lm_head.qs) m->lm_head = m->wte;
     else m->weight_bytes -= (size_t)v * (e / QK) * ggml_block_bytes(t);  // the embedding table is gathered from, not streamed
     if (m->mpt() || m->bloom()) {
         const std::vector<float> slopes = alibi_slopes(hp->n_head, alibi_bias_max);
         m->alibi = device_alloc<float>(slopes.size() * 4);
         B200_CHECK(cudaMemcpy(m->alibi.get(), slopes.data(), slopes.size() * 4, cudaMemcpyHostToDevice));
     }
+    // GPT-NeoX: mode 2 on n_rot of every head; GPT-J: mode 0 over ALL hd elements of the head with theta_scale base^(-2/n_rot) (gptj lib.rs:178-201,
+    // LC/ggml.c:11859-11874 walks ne0, not n_dims)
+    if (m->neox() || m->gptj()) m->rope = &rope_table(hp->n_rot, m->neox() ? 2 : 0, 10000.0f, 1.0f, hd, hp->context_size);
+    // where q / k / v of head h live inside a row of the fused projection: GPT-NeoX per head [q | k | v], the others the three thirds of the row
+    m->qkv_layout = m->neox() ? QkvLayout{3 * hd, hd, 2 * hd} : QkvLayout{hd, e, 2 * e};
+    m->parallel = m->neox() && hp->use_parallel_residual;
+    m->kq_scale = 1.0f / sqrtf((float)e / (float)hp->n_head);                                                                   // gptneox lib.rs:270-273
     return m;
 }
 
@@ -364,28 +352,12 @@ int b200_neox_load_tensor(b200_neox_model *m, const char *name, int32_t type, co
 // seeded synthetic weights generated in HBM (bench): LayerNorm gains 1 + 0.1 N(0,1), biases = gains - 1 (small)
 int b200_neox_synthesize(b200_neox_model *m, uint64_t seed) {
     if (!m) return B200_ERR_BAD_ARG;
-    const int64_t e = m->hp.n_embd;
-    m->synthesize(seed, [m, e](SeedSeq &r) {
-        if (m->mpt()) {
-            r.q(m->wte); r.gain(m->lnf_g, e);
-            for (auto &L : m->layers) { r.gain(L.ln1_g, e); r.gain(L.ln2_g, e); r.q(L.wqkv); r.q(L.wdense); r.q(L.wfc); r.q(L.wproj); }
-            return;
-        }
-        if (m->gptj()) {
-            r.q(m->wte); r.q(m->lm_head); r.gain(m->lnf_g, e); r.bias(m->lnf_b, e); r.bias(m->lm_head_b, m->hp.n_vocab);
-            for (auto &L : m->layers) {
-                r.gain(L.ln1_g, e); r.bias(L.ln1_b, e); r.bias(L.bfc, 4 * e); r.bias(L.bproj, e);
-                r.q(L.wqkv); r.q(L.wdense); r.q(L.wfc); r.q(L.wproj);
-            }
-            return;
-        }
-        r.q(m->wte); if (!m->gpt2() || m->hp.has_lm_head) r.q(m->lm_head); r.gain(m->lnf_g, e); r.bias(m->lnf_b, e);
-        if (m->gpt2()) r.bias(m->wpe, (int64_t)m->hp.context_size * e);
-        if (m->bloom()) { r.gain(m->emb_g, e); r.bias(m->emb_b, e); }
-        for (auto &L : m->layers) {
-            r.gain(L.ln1_g, e); r.bias(L.ln1_b, e); r.gain(L.ln2_g, e); r.bias(L.ln2_b, e); r.bias(L.bqkv, 3 * e); r.bias(L.bdense, e); r.bias(L.bfc, 4 * e); r.bias(L.bproj, e);
-            r.q(L.wqkv); r.q(L.wdense); r.q(L.wfc); r.q(L.wproj);
-        }
+    m->synthesize(seed, [m](SeedSeq &r) {
+        m->each_tensor([&](const auto &d, auto &o, int) {
+            if (d.kind == MAT) r.q(o.*d.q);
+            else if (d.kind == GAIN) r.gain(o.*d.f, m->dim(d.K));
+            else if (d.kind == BIAS) r.bias(o.*d.f, m->dim(d.K));
+        });
     });
     return B200_OK;
 }
@@ -398,7 +370,7 @@ void b200_neox_free(b200_neox_model *m) {
 
 b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) {
     if (!m || n_batch < 1) return nullptr;
-    if (!m->all_loaded()) { fprintf(stderr, "llm_b200: neox start_session: %d of %d tensors loaded\n", m->n_loaded, m->n_slots()); return nullptr; }
+    if (!m->all_loaded()) { fprintf(stderr, "llm_b200: neox start_session: %d of %d tensors loaded\n", m->n_loaded, (int)m->loaded.size()); return nullptr; }
     b200_neox_session *s = new b200_neox_session();
     s->m = m;
     const b200_neox_hparams &hp = m->hp;
@@ -412,8 +384,6 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     s->xpack = device_alloc<int4>((4 * e / QK) * 64); s->xh = device_alloc<__half>(xh_bytes(4 * e, B));
     s->qdec = device_alloc<float>(e * 4);
     s->xpack_a = device_alloc<int4>((e / QK) * 64); s->xpack_d = device_alloc<int4>((e / QK) * 64); s->xpack_f = device_alloc<int4>((4 * e / QK) * 64);
-    const RopeTable *rt_ = m->gptj() ? &rope_table(hp.n_rot, 0, 10000.0f, 1.0f, m->hd, (int)n_ctx)
-                         : m->thirds() ? nullptr : &rope_table(hp.n_rot, 2, 10000.0f, 1.0f, m->hd, (int)n_ctx);
     s->dl.resize(hp.n_layer);
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &L = m->layers[il];
@@ -421,18 +391,14 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
                               s->memory_k.get() + (size_t)il * n_ctx * e, s->memory_v.get() + (size_t)il * n_ctx * e};
     }
     NeoxParams &P = s->dp;
-    P.n_layer = hp.n_layer; P.e = (int)e; P.hd = m->hd; P.n_head = hp.n_head; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab; P.n_rot = hp.n_rot;
-    P.parallel_residual = !m->thirds() && hp.use_parallel_residual; P.gpt2 = m->thirds() ? 1 : 0; P.wpe = m->wpe;
+    P.n_layer = hp.n_layer; P.e = (int)e; P.hd = m->hd; P.n_head = hp.n_head; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab;
+    P.parallel_residual = m->parallel; P.qkv_layout = m->qkv_layout; P.n_rot = m->rope && m->rope->mode ? m->rope->n_dims : 0; P.wpe = m->wpe;
     P.alibi = m->alibi.get(); P.emb_g = m->emb_g; P.emb_b = m->emb_b; P.wte = m->wte; P.lm_head = m->lm_head; P.lnf_g = m->lnf_g; P.lnf_b = m->lnf_b;
     P.gptj = m->gptj() ? 1 : 0; P.lm_head_b = m->lm_head_b;
-    P.kq_scale = 1.0f / sqrtf((float)e / (float)hp.n_head); P.rope_cs = rt_ ? rt_->cs : nullptr; P.rope_half = rt_ ? rt_->half : 0;
+    P.kq_scale = m->kq_scale; P.rope_cs = m->rope ? m->rope->cs : nullptr; P.rope_half = m->rope ? m->rope->half : 0;
     P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
     P.x = s->x.get(); P.qkv = s->qkv.get(); P.q = s->qdec.get(); P.attn_out = s->attn.get(); P.logits = s->logits.get();
     P.xpack_a = s->xpack_a.get(); P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
-    QWeight p1; p1.nb = (int64_t)e / QK; QWeight p2; p2.nb = 4 * (int64_t)e / QK;
-    // GPT-J's schedule also takes heads of 128 < hd <= 256 (the wide cluster attention, up to 8 CTAs per head)
-    s->decode_ok = m->hd % 32 == 0 && (m->hd <= 128 || (m->gptj() && m->hd <= 256)) && e % 128 == 0 && e <= 8192 && n_ctx % 8 == 0 &&
-                   mmv_exact_stream_supported(p1) && mmv_exact_stream_supported(p2);
     B200_CHECK(cudaDeviceSynchronize());
     return s;
 }

@@ -412,7 +412,7 @@ static b200_session *start_session_tp(b200_session *s) {
     const int G = m->tp_world, r = m->tp_rank;
     const size_t e = hp.n_embd, f = hp.n_ff, n_ctx = hp.context_size, V = hp.n_vocab;
     // the exchange lives in the fused attention kernel, whose shared memory holds the whole context bucket
-    if (!attn_fused_fits((hp.context_size + 63) / 64 * 64, m->hd)) {
+    if (!attn_fused_fits(hp.context_size, m->hd)) {
         fprintf(stderr, "llm_b200: tensor-parallel session: context_size %d is more than the fused attention kernel holds (3264 positions)\n", hp.context_size);
         b200_session_free(s);
         return nullptr;
