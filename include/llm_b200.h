@@ -232,7 +232,7 @@ int  b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);
 /* quantize_row_q8_K (LC/k_quants.c:1133-1183) of B rows of K floats -> B * K/256 block_q8_K {f32 d; i8 qs[256]; i16 bsums[16]} (292 bytes each), bit-exact */
 int  b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_out);
-enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = EXACT; TC5 = the tensor-core prefill GEMMs (the name predates the sm_90a port): wgmma/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->wgmma GEMM (mmq_tc5.cu, non-conformant) */
+enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = the exact kernel the sessions pick for B rows (the streaming mat-vec at B == 1 where K allows it, EXACT below 16, EXACT_MMA below 96, EXACT_TC5 from 96; K-quants: EXACT); TC5 = the tensor-core prefill GEMMs (the name predates the sm_90a port): wgmma/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->wgmma GEMM (mmq_tc5.cu, non-conformant) */
 
 #ifdef __cplusplus
 }

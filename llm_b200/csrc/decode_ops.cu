@@ -747,6 +747,14 @@ static void attn_fused_reserve(size_t bytes) {
     B200_CHECK(cudaFuncSetAttribute(attn_fused_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
+// the same for attn_sv_kernel: one record per process.  Every decode_ops_t<TYPE, TP> launches this one kernel, so a record per instantiation
+// would let a session of another weight type with a shorter context LOWER the attribute under a session that already relies on more.
+static void attn_sv_reserve(size_t bytes) {
+    static size_t set = 48 * 1024;
+    if (bytes <= set) return;
+    B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    set = bytes;
+}
 // the positions attn_fused_kernel holds for a context bucket: the bucket rounded up to whole 64-position tiles
 int attn_fused_rows(int n_kv_bucket) { return (n_kv_bucket + 63) / 64 * 64; }
 // dynamic shared memory of attn_fused_kernel for a context bucket and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
@@ -844,8 +852,7 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(n_kv_bucket, P.hd);
     B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue (start_session_tp checks the size)
     const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
-    static size_t sv_set = 48 * 1024;
-    if (sv_smem > sv_set) { B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem)); sv_set = sv_smem; }
+    attn_sv_reserve(sv_smem);
     // mat-vec plans, each leaving room for what follows it (planned from the successor backwards; every layer has the same shapes): the norm
     // kernels release their dependents at entry, so beside wo and w2 there has to be room for the norm AND the next mat-vec
     const CtaFootprint f_norm = TP ? footprint_of(norm_pack_tp_kernel, 256, 0) : footprint_of(norm_pack_kernel, 256, 0);

@@ -99,7 +99,6 @@ int b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, con
     const size_t pb = qweight_layout(w, wtype, K, N, nullptr);
     qweight_layout(w, wtype, K, N, R.op_arena.get(pb, st));
     repack_weights(w, raw, st);
-    if (impl == B200_MM_AUTO) impl = B200_MM_EXACT;
     float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
     float *dd = (float *)R.op_arena.get((size_t)B * N * 4, st);
     Acts a{};
@@ -107,9 +106,15 @@ int b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, con
     a.xds = (float2 *)R.op_arena.get((size_t)B * (K / QK) * sizeof(float2), st);
     if (impl == B200_MM_EXACT_MMA) a.xh = (__half *)R.op_arena.get(xh_bytes(K, B), st);
     else if (impl == B200_MM_EXACT_TC5 || impl == B200_MM_FAST_TC5) a.xh = (__half *)R.op_arena.get((size_t)B * K * 2 + 16, st);
+    else if (impl == B200_MM_AUTO) a.xh = (__half *)R.op_arena.get(xh_bytes(K, B) + 16, st);       // the larger of the two above
     B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
-    prepare(impl, wtype, dx, K, B, a, st);
-    if (impl == B200_MM_EXACT_STREAM) {
+    if (impl != B200_MM_AUTO) prepare(impl, wtype, dx, K, B, a, st);
+    if (impl == B200_MM_AUTO) {                          // the exact dispatch of the sessions and the seam (mul_mat.cu): the kernel follows from B and K
+        int4 *pack = (int4 *)R.op_arena.get((size_t)(K / QK) * 64, st);
+        mul_mat_exact_auto(w, dx, K, B, dd, N, nullptr, 0, {a.xq, a.xds, pack, a.xh}, st);
+        B200_CHECK(cudaStreamSynchronize(st));
+        if (const int rc = check_timeout(B200_MM_EXACT_TC5)) return rc;
+    } else if (impl == B200_MM_EXACT_STREAM) {
         if (!mmv_exact_stream_supported(w)) return B200_ERR_BAD_ARG;
         int4 *pack = (int4 *)R.op_arena.get((size_t)(K / QK) * 64, st);
         for (int64_t b = 0; b < B; b++) { quantize_act_pack(wtype, dx + b * K, pack, K, st); mul_mat_vec_q_exact_stream(w, pack, dd + b * N, nullptr, st); }
