@@ -101,14 +101,16 @@ typedef struct {
     uint64_t offset, nbytes;      /* TensorLoadInfo::start_offset, calc_size() */
 } b200_ggml_tensor_info;
 
-enum { B200_ARCH_LLAMA = 0, B200_ARCH_GPT2 = 1, B200_ARCH_GPTNEOX = 2, B200_ARCH_MPT = 3, B200_ARCH_BLOOM = 4, B200_ARCH_GPTJ = 5 };   /* whose Hyperparameters::read_ggml lays out the header */
+enum { B200_ARCH_LLAMA = 0, B200_ARCH_GPT2 = 1, B200_ARCH_GPTNEOX = 2, B200_ARCH_MPT = 3, B200_ARCH_BLOOM = 4, B200_ARCH_GPTJ = 5,
+       B200_ARCH_LORA = 6 };   /* whose Hyperparameters::read_ggml lays out the header; LORA: a LoRA adapter (LoraParameters, crates/llm-base/src/lora.rs) */
 b200_ggml_file *b200_ggml_open(const char *path, int *err);                     /* LLaMA header; NULL + *err on LoadError */
 b200_ggml_file *b200_ggml_open_arch(const char *path, int32_t arch, int *err);
 /* the header words in file order: llama n_vocab n_embd n_mult n_head n_layer n_rot file_type | gpt2 n_vocab n_ctx n_embd n_head n_layer file_type n_vocab |
  * gptneox n_vocab n_ctx n_embd n_head n_layer n_rot use_parallel_residual file_type |
  * mpt n_embd max_seq_len n_head n_layer n_vocab alibi_bias_max(f32 bits) clip_kqv(f32 bits) file_type (mpt lib.rs:317-330; the vocabulary count is word 4) |
  * bloom n_vocab n_embd n_mult n_head n_layer file_type |
- * gptj n_vocab n_ctx n_embd n_head n_layer n_rot file_type n_vocab (gptj lib.rs:366-401; the repeated n_vocab must match the first: InvariantBroken) */
+ * gptj n_vocab n_ctx n_embd n_head n_layer n_rot file_type n_vocab (gptj lib.rs:366-401; the repeated n_vocab must match the first: InvariantBroken) |
+ * lora r alpha (no vocabulary; r <= 0 is InvariantBroken, where the reference would divide by it) */
 int     b200_ggml_hparams(const b200_ggml_file *f, int32_t *arch, int32_t *words8, int32_t *n_words);
 void    b200_ggml_close(b200_ggml_file *f);
 int     b200_ggml_container(const b200_ggml_file *f, uint32_t *magic, uint32_t *version);      /* ContainerType */
@@ -131,6 +133,16 @@ b200_model *b200_llama_load_file(const char *path, int32_t context_size, float r
 b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa, int *err);
 /* b200_model_load_tensor + the loader's dims check (LoadError::TensorWrongSize on a dims mismatch even when the byte count matches) */
 int  b200_model_load_tensor_shaped(b200_model *m, const char *name, int32_t type, int32_t n_dims, int64_t ne0, int64_t ne1, const void *host_data, size_t nbytes);
+/* ---- LoRA adapters (ModelParameters::lora_adapters, crates/llm-base/src/model/mod.rs:205-206): each adapter is a file opened with B200_ARCH_LORA.
+ * For a tensor named in an adapter's patch set (its tensor names without the last "."-component), every adapter in the order given applies
+ * W = W + (alpha / r) * (loraA x loraB) on the GPU before the tensor is placed -- LoraAdapter::patch (crates/llm-base/src/lora.rs:71-140), bit-exact
+ * with the reference's CPU graph.  loraA [r, ne0] F32 or F16, loraB [r, ne1] F32 (else UnsupportedElementType); a missing .loraA / .loraB is
+ * UnknownTensor, shapes that do not fit are TensorWrongSize.  n_adapters == 0 is the shaped load; tensor-parallel models take no adapters (BadArgument). */
+int  b200_model_load_tensor_lora(b200_model *m, const char *name, int32_t type, int32_t n_dims, int64_t ne0, int64_t ne1, const void *host_data, size_t nbytes,
+                                 const b200_ggml_file *const *adapters, int32_t n_adapters);
+/* b200_llama_load_file_gqa with the adapter files lora_paths[0..n_lora), opened and closed here */
+b200_model *b200_llama_load_file_lora(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa,
+                                      const char *const *lora_paths, int32_t n_lora, int *err);
 
 b200_session *b200_model_start_session(b200_model *m, const b200_session_config *cfg);
 /* One forward pass over `n` tokens appended at n_past (InferenceSession::compute + Llama::evaluate).  tokens: HOST int32.
@@ -209,6 +221,9 @@ b200_neox_model *b200_neox_new(const b200_neox_hparams *hp);
  * b200_neox_* entry point serves these models unchanged. */
 b200_neox_model *b200_neox_new_alibi(const b200_neox_hparams *hp, float alibi_bias_max);
 int  b200_neox_load_tensor(b200_neox_model *m, const char *name, int32_t type, const void *host_data, size_t nbytes);
+/* shaped load (2-D: ne0 = row length, ne1 = rows; 1-D: ne1 = 1) with the LoRA adapters of b200_model_load_tensor_lora */
+int  b200_neox_load_tensor_lora(b200_neox_model *m, const char *name, int32_t type, int32_t n_dims, int64_t ne0, int64_t ne1, const void *host_data, size_t nbytes,
+                                const b200_ggml_file *const *adapters, int32_t n_adapters);
 int  b200_neox_synthesize(b200_neox_model *m, uint64_t seed);          /* seeded weights generated in HBM (bench) */
 size_t b200_neox_weight_bytes(b200_neox_model *m);                     /* bytes streamed per decoded token */
 void b200_neox_free(b200_neox_model *m);
@@ -232,6 +247,9 @@ int  b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);
 /* quantize_row_q8_K (LC/k_quants.c:1133-1183) of B rows of K floats -> B * K/256 block_q8_K {f32 d; i8 qs[256]; i16 bsums[16]} (292 bytes each), bit-exact */
 int  b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_out);
+/* LoraAdapter::patch of one adapter on host buffers: w (N rows of K, F32 or Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 GGML blocks) += scaling * ba, ba[n][k] = dot(a row k,
+ * b row n), a: K rows of r (a_type 0 F32 / 1 F16), b: N rows of r f32 -- bit-exact with the reference's ggml_mul_mat / ggml_scale / ggml_add on the CPU */
+int  b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, int32_t a_type, const void *a, const float *b, int64_t r, float scaling);
 enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = the exact kernel the sessions pick for B rows (the streaming mat-vec at B == 1 where K allows it, EXACT below 16, EXACT_MMA below 96, EXACT_TC5 from 96; K-quants: EXACT); TC5 = the tensor-core prefill GEMMs (the name predates the sm_90a port): wgmma/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->wgmma GEMM (mmq_tc5.cu, non-conformant) */
 
 #ifdef __cplusplus

@@ -105,5 +105,9 @@ def lib():
     L.b200_op_quantize_weights.argtypes = [i32, vp, i64, i64, vp]
     L.b200_op_mul_mat.argtypes = [i32, vp, i64, i64, vp, i64, vp, i32]
     L.b200_op_quantize_q8_K.argtypes = [vp, i64, i64, vp]
+    L.b200_op_lora_patch.argtypes = [i32, vp, i64, i64, i32, vp, vp, i64, C.c_float]
+    L.b200_model_load_tensor_lora.argtypes = [vp, C.c_char_p, i32, i32, i64, i64, vp, sz, C.POINTER(vp), i32]
+    L.b200_llama_load_file_lora.restype = vp
+    L.b200_llama_load_file_lora.argtypes = [C.c_char_p, i32, C.c_float, C.c_float, i32, C.POINTER(C.c_char_p), i32, C.POINTER(C.c_int)]
     _lib = L
     return L

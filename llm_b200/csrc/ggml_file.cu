@@ -11,6 +11,7 @@
 //   gptneox Hyperparameters      crates/models/gptneox/src/lib.rs:431-442   8 x i32: n_vocab n_ctx n_embd n_head n_layer n_rot use_parallel_residual(0|1) file_type
 //   mpt Hyperparameters          crates/models/mpt/src/lib.rs:317-330       n_embd max_seq_len n_head n_layer n_vocab (i32), alibi_bias_max clip_kqv (f32), file_type
 //   bloom Hyperparameters        crates/models/bloom/src/lib.rs             6 x i32: n_vocab n_embd n_mult n_head n_layer file_type
+//   lora LoraParameters          crates/llm-base/src/lora.rs:27-35          2 x i32: r alpha, no vocabulary (r <= 0: InvariantBroken, a deliberate deviation)
 //   FileType                     crates/llm-base/src/loader.rs:32-50        file_type = quantization_version * 1000 + llama_ftype
 //   quantization version rule    crates/llm-base/src/loader.rs:459-484      0 is read as 1 (GGJT v2) / 2 (GGJT v3); quantized tensors require 2
 //   ggml::format::save           crates/ggml/src/format/saver.rs:86-160     the writer (GGJT v3)
@@ -28,6 +29,7 @@
 
 #include "../../include/llm_b200.h"
 #include "common.cuh"
+#include "host.h"
 
 namespace {
 
@@ -72,6 +74,19 @@ struct b200_ggml_file {
     std::vector<TensorInfo> tensors;
 };
 
+// ---- the LoRA hook's view of an adapter file (host.h) ----
+int64_t b200::ggml_find_tensor(const b200_ggml_file *f, const char *name) {
+    for (size_t i = 0; i < f->tensors.size(); i++) if (f->tensors[i].name == name) return (int64_t)i;
+    return -1;
+}
+bool b200::lora_in_patch_set(const b200_ggml_file *f, const char *name) {     // rsplit_once('.') of some tensor name gives `name`
+    const size_t n = strlen(name);
+    for (const TensorInfo &t : f->tensors)
+        if (t.name.size() > n && t.name.compare(0, n, name) == 0 && t.name[n] == '.' && t.name.find('.', n + 1) == std::string::npos) return true;
+    return false;
+}
+float b200::lora_scaling(const b200_ggml_file *f) { return (float)f->hp[1] / (float)f->hp[0]; }    // LoraParameters::calculate_scaling
+
 extern "C" {
 
 void b200_ggml_close(b200_ggml_file *f) {
@@ -83,10 +98,10 @@ void b200_ggml_close(b200_ggml_file *f) {
 
 static b200_ggml_file *open_arch_impl(const char *path, int32_t arch, int *err) {
     int dummy; if (!err) err = &dummy;
-    if (arch < 0 || arch > B200_ARCH_GPTJ) { *err = B200_ERR_BAD_ARG; return nullptr; }
+    if (arch < 0 || arch > B200_ARCH_LORA) { *err = B200_ERR_BAD_ARG; return nullptr; }
     *err = B200_OK;
     b200_ggml_file *f = new b200_ggml_file();
-    f->arch = arch; f->n_hp = arch == B200_ARCH_LLAMA ? 7 : arch == B200_ARCH_GPT2 ? 7 : arch == B200_ARCH_BLOOM ? 6 : 8;
+    f->arch = arch; f->n_hp = arch == B200_ARCH_LLAMA ? 7 : arch == B200_ARCH_GPT2 ? 7 : arch == B200_ARCH_BLOOM ? 6 : arch == B200_ARCH_LORA ? 2 : 8;
     auto fail = [&](int code) -> b200_ggml_file * { *err = code; b200_ggml_close(f); return nullptr; };
     f->fd = open(path, O_RDONLY);
     struct stat sb;
@@ -112,13 +127,14 @@ static b200_ggml_file *open_arch_impl(const char *path, int32_t arch, int *err) 
     for (int i = 0; i < f->n_hp; i++) f->hp[i] = (int32_t)rd32();
     if (eof) return fail(B200_ERR_IO);
     for (int i = 0; i < f->n_hp; i++)                                                                 // usize::try_from in the reference; MPT's words 5 and 6
-        if (f->hp[i] < 0 && !(arch == B200_ARCH_MPT && (i == 5 || i == 6))) return fail(B200_ERR_INVARIANT_BROKEN);   // are f32 (read_f32 takes any value)
+        if (f->hp[i] < 0 && !(arch == B200_ARCH_MPT && (i == 5 || i == 6)) && arch != B200_ARCH_LORA) return fail(B200_ERR_INVARIANT_BROKEN);   // are f32 (read_f32 takes any value)
+    if (arch == B200_ARCH_LORA && f->hp[0] <= 0) return fail(B200_ERR_INVARIANT_BROKEN);             // r and alpha are i32; the scaling alpha / r needs r > 0
     if (arch == B200_ARCH_GPT2 && f->hp[6] != f->hp[0]) return fail(B200_ERR_INVARIANT_BROKEN);     // "GPT2 model expected n_vocab {} found {}"
     if (arch == B200_ARCH_GPTJ && f->hp[7] != f->hp[0]) return fail(B200_ERR_INVARIANT_BROKEN);     // "GPTJ model expected n_vocab {} found {}" (gptj lib.rs:377-386)
     if (arch == B200_ARCH_GPTNEOX && f->hp[6] > 1) return fail(B200_ERR_IO);                        // read_bool: InvalidData
 
     const bool scored = f->magic == MAGIC_GGMF || f->magic == MAGIC_GGJT;
-    const int32_t n_vocab = f->hp[arch == B200_ARCH_MPT ? 4 : 0];                // MPT: n_embd max_seq_len n_head n_layer n_vocab ...
+    const int32_t n_vocab = arch == B200_ARCH_LORA ? 0 : f->hp[arch == B200_ARCH_MPT ? 4 : 0];   // MPT: n_embd max_seq_len n_head n_layer n_vocab ...; LoRA: none
     if ((uint64_t)n_vocab > (f->size - pos) / 4) return fail(B200_ERR_IO);       // every token record takes at least 4 bytes: a corrupt count cannot ask for gigabytes
     f->tokens.reserve((size_t)n_vocab);
     for (int32_t i = 0; i < n_vocab; i++) {
@@ -272,8 +288,9 @@ int b200_ggml_write_llama(const char *path, const b200_llama_hparams *hp, int32_
 
 // llm::load::<Llama>(path, params): parse, build the model for the file's geometry, upload every tensor from the mapping.
 // n_gqa > 1: ModelParameters::n_gqa (grouped-query attention, e.g. 8 for LLaMA-2 70B): n_head_kv = n_head / n_gqa (llama lib.rs:403-447).
-b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa, int *err) {
-    int dummy; if (!err) err = &dummy;
+// With adapters, each tensor goes through b200_model_load_tensor_lora (MmapCompatibleLoader::load, crates/llm-base/src/loader.rs:661-669).
+static b200_model *load_file_impl(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa,
+                                  const b200_ggml_file *const *adapters, int32_t n_adapters, int *err) {
     b200_ggml_file *f = b200_ggml_open(path, err);
     if (!f) return nullptr;
     b200_llama_hparams hp;
@@ -297,12 +314,33 @@ b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, flo
                     type_name(t.type), type_name(hp.wtype));
             *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; b200_model_free(m); b200_ggml_close(f); return nullptr;
         }
-        const int rc = b200_model_load_tensor_shaped(m, t.name.c_str(), t.type, t.n_dims, t.ne[0], t.ne[1], f->map + t.offset, (size_t)t.nbytes);
+        const int rc = b200_model_load_tensor_lora(m, t.name.c_str(), t.type, t.n_dims, t.ne[0], t.ne[1], f->map + t.offset, (size_t)t.nbytes, adapters, n_adapters);
         if (rc != B200_OK) { *err = rc; b200_model_free(m); b200_ggml_close(f); return nullptr; }
     }
     if (!b200_model_is_loaded(m)) { *err = B200_ERR_NOT_LOADED; b200_model_free(m); b200_ggml_close(f); return nullptr; }
     b200_ggml_close(f);
     *err = B200_OK;
+    return m;
+}
+b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa, int *err) {
+    int dummy; if (!err) err = &dummy;
+    return load_file_impl(path, context_size, rope_freq_base, rope_freq_scale, n_gqa, nullptr, 0, err);
+}
+
+// ModelParameters::lora_adapters: every adapter is opened (ggml::format::load with LoraParameters) and stays open while the model's tensors load
+b200_model *b200_llama_load_file_lora(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa,
+                                      const char *const *lora_paths, int32_t n_lora, int *err) {
+    int dummy; if (!err) err = &dummy;
+    if (n_lora < 0 || (n_lora > 0 && !lora_paths)) { *err = B200_ERR_BAD_ARG; return nullptr; }
+    std::vector<b200_ggml_file *> ad;
+    auto close_all = [&]() { for (b200_ggml_file *a : ad) b200_ggml_close(a); };
+    for (int32_t i = 0; i < n_lora; i++) {
+        b200_ggml_file *a = b200_ggml_open_arch(lora_paths[i], B200_ARCH_LORA, err);
+        if (!a) { close_all(); return nullptr; }
+        ad.push_back(a);
+    }
+    b200_model *m = load_file_impl(path, context_size, rope_freq_base, rope_freq_scale, n_gqa, ad.data(), n_lora, err);
+    close_all();
     return m;
 }
 b200_model *b200_llama_load_file(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int *err) {

@@ -1,10 +1,43 @@
 // llm_b200/csrc/host.cu -- tensor slots and session state shared by the LLaMA and GPT-NeoX / GPT-2 runtimes (host.h)
 #include <string.h>
 
+#include <string>
+
 #include "../../include/llm_b200.h"
 #include "host.h"
 
 namespace b200 {
+
+// loraA / loraB of `name` in one adapter (UnknownTensor if either is missing), checked against the target [K, N] of wtype
+static int lora_factors(const b200_ggml_file *f, const char *name, int wtype, int64_t K, int64_t N, int64_t idx[2], b200_ggml_tensor_info info[2]) {
+    const std::string base(name);
+    idx[0] = ggml_find_tensor(f, (base + ".loraA").c_str());
+    idx[1] = ggml_find_tensor(f, (base + ".loraB").c_str());
+    if (idx[0] < 0 || idx[1] < 0) return B200_ERR_UNKNOWN_TENSOR;
+    b200_ggml_tensor(f, idx[0], &info[0]);
+    b200_ggml_tensor(f, idx[1], &info[1]);
+    return lora_check(wtype, K, N, info[0].type, info[0].ne[0], info[0].ne[1], info[1].type, info[1].ne[0], info[1].ne[1]);
+}
+
+// LoraAdapter::patch of every adapter in order on w (device, file layout); check = true only validates, so that a bad adapter changes nothing
+static int lora_apply(const LoraTarget &t, int wtype, int64_t K, int64_t N, void *w, bool check) {
+    Runtime &R = rt();
+    for (int i = 0; i < t.n; i++) {
+        const b200_ggml_file *f = t.adapters[i];
+        if (!f) return B200_ERR_BAD_ARG;
+        if (!lora_in_patch_set(f, t.name)) continue;
+        int64_t idx[2]; b200_ggml_tensor_info info[2];
+        const int rc = lora_factors(f, t.name, wtype, K, N, idx, info);
+        if (rc != B200_OK) return rc;
+        if (check) continue;
+        void *a = R.op_arena.get(info[0].nbytes ? info[0].nbytes : 1, R.stream);
+        float *b = (float *)R.op_arena.get(info[1].nbytes ? info[1].nbytes : 4, R.stream);
+        B200_CHECK(cudaMemcpyAsync(a, b200_ggml_tensor_data(f, idx[0]), info[0].nbytes, cudaMemcpyHostToDevice, R.stream));
+        B200_CHECK(cudaMemcpyAsync(b, b200_ggml_tensor_data(f, idx[1]), info[1].nbytes, cudaMemcpyHostToDevice, R.stream));
+        lora_patch(wtype, w, K, N, info[0].type, a, b, info[0].ne[0], info[1].ne[1], lora_scaling(f), R.stream);
+    }
+    return B200_OK;
+}
 
 QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows) {
     QWeight v = w;
@@ -16,13 +49,23 @@ QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows) {
     return v;
 }
 
-int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes) {
+int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes, const LoraTarget *lora) {
     Runtime &R = rt();
+    // the target as the adapters see it: the tensor in file row order (a vector is one row)
+    const int64_t K = s.is_q ? s.q.K : lora ? lora->ne0 : 0, N = s.is_q ? s.q_rows() : lora ? lora->ne1 : 0;
+    if (lora) {
+        if (!s.is_q && K * N != s.n) return B200_ERR_TENSOR_SHAPE;
+        if (type == (s.is_q ? s.q.type : T_F32) && nbytes == s.bytes()) {
+            const int rc = lora_apply(*lora, type, K, N, nullptr, true);
+            if (rc != B200_OK) return rc;
+        }
+    }
     if (s.is_q) {
         if (type != s.q.type || nbytes != s.bytes()) return B200_ERR_TENSOR_SHAPE;
         R.op_arena.reset();
         void *raw = R.op_arena.get(nbytes, R.stream);
         B200_CHECK(cudaMemcpyAsync(raw, host, nbytes, cudaMemcpyHostToDevice, R.stream));
+        if (lora) lora_apply(*lora, type, K, N, raw, false);
         if (!s.chunk) repack_weights(s.q, raw, R.stream);
         else {
             const size_t piece = (size_t)s.chunk * s.q.nb * ggml_block_bytes(type);
@@ -34,6 +77,11 @@ int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes) {
         if (type != T_F32 || nbytes != s.bytes()) return B200_ERR_TENSOR_SHAPE;
         B200_CHECK(cudaMemcpy(s.f, host, nbytes, cudaMemcpyHostToDevice));
         B200_CHECK(cudaDeviceSynchronize());   // legacy-stream copy/memset: not ordered with our non-blocking stream, and a pageable H2D cudaMemcpy may return before its DMA lands
+        if (lora) {
+            R.op_arena.reset();
+            lora_apply(*lora, type, K, N, s.f, false);
+            B200_CHECK(cudaStreamSynchronize(R.stream));
+        }
     }
     return B200_OK;
 }

@@ -9,6 +9,8 @@
 #include "kernels.cuh"
 #include "runtime.h"
 
+struct b200_ggml_file;
+
 namespace b200 {
 
 // ---- owned allocations: one cudaMalloc / cudaMallocHost / event each, released with the struct that holds the handle ---------------
@@ -86,8 +88,17 @@ struct Slot {
     int64_t q_rows() const { return chunk ? rows : q.N; }
     size_t bytes() const { return is_q ? (size_t)q_rows() * q.nb * ggml_block_bytes(q.type) : (size_t)n * 4; }
 };
-int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes);   // GGML blocks (repacked on the GPU) or f32; B200_OK / B200_ERR_TENSOR_SHAPE
+// The LoRA adapters of one tensor load: the tensor's name and shape [ne0, ne1] (ne1 = 1 for a vector) and the adapter files, applied in order
+struct LoraTarget { const char *name; int64_t ne0, ne1; const b200_ggml_file *const *adapters; int n; };
+// GGML blocks (repacked on the GPU) or f32; B200_OK / B200_ERR_TENSOR_SHAPE, or the adapters' LoadError.  With `lora`, every adapter whose patch set
+// names the tensor patches its bytes in file layout after the upload and before they are placed (lora.cu).
+int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes, const LoraTarget *lora = nullptr);
 int read_slot(const Slot &s, void *host, size_t nbytes);                       // the inverse: GGML blocks or f32 back to the host
+
+// ---- adapter files (ggml_file.cu) ----
+int64_t ggml_find_tensor(const b200_ggml_file *f, const char *name);        // index in the tensor table, -1 if absent
+bool lora_in_patch_set(const b200_ggml_file *f, const char *name);          // some tensor of the adapter is `name` + "." + a last component
+float lora_scaling(const b200_ggml_file *f);                                // (f32)alpha / (f32)r
 
 // ---- what every session keeps: the f16 KV cache, the position, token and logits staging, the decode graphs -------------------------
 struct SessionCore {

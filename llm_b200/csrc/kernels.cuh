@@ -81,6 +81,13 @@ void synth_gain(float *g, int64_t n, uint64_t seed, cudaStream_t st);           
 void quantize_weights(const QWeight &w, const float *src, cudaStream_t st);                  // ggml_quantize_q* on the GPU: f32 [N][K] -> planes, bit-exact
 void scale_shift_f32(float *p, int64_t n, float a, float b, cudaStream_t st);                // p = p * a + b
 
+// ---- lora.cu : LoRA adapters patched into a weight at load time, bit-exact with the reference's CPU graph (LoraAdapter::patch) ----------------------
+// B200_OK, or the LoadError (TensorWrongSize / UnsupportedElementType) for factors A [a_ne0 = r, a_ne1] and B [b_ne0, b_ne1] on a target [K, N] of wtype
+int lora_check(int wtype, int64_t K, int64_t N, int a_type, int64_t a_ne0, int64_t a_ne1, int b_type, int64_t b_ne0, int64_t b_ne1);
+// in place, on device memory: w (N rows of K in GGML layout, F32 or a 32-element block type) += scaling * (A x B); a: K rows of r (F32 / F16),
+// b: nb_rows rows of r f32 (row n of W takes row n % nb_rows).  Arguments checked by lora_check.
+void lora_patch(int wtype, void *w, int64_t K, int64_t N, int a_type, const void *a, const float *b, int64_t r, int64_t nb_rows, float scaling, cudaStream_t st);
+
 // ---- rowops.cu : warp/block-reduce kernels ------------------------------------------------------------------------
 struct Luts { const uint16_t *silu, *gelu, *exp; };   // 3 x 64 Ki fp16 tables built on the host with libm (LC/ggml.c:4313-4326)
 const Luts &luts();                                   // uploaded on first use

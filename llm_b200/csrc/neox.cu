@@ -349,6 +349,20 @@ int b200_neox_load_tensor(b200_neox_model *m, const char *name, int32_t type, co
     return rc;
 }
 
+// the loader's dims check (2-D: ne0 = row length, ne1 = rows; an f32 matrix such as GPT-2's wpe is one slot of ne0 * ne1 floats) and the adapters
+int b200_neox_load_tensor_lora(b200_neox_model *m, const char *name, int32_t type, int32_t n_dims, int64_t ne0, int64_t ne1, const void *host_data, size_t nbytes,
+                               const b200_ggml_file *const *adapters, int32_t n_adapters) {
+    if (!m || !name || !host_data || n_adapters < 0 || (n_adapters > 0 && !adapters)) return B200_ERR_BAD_ARG;
+    Slot s; int id;
+    if (!m->lookup(name, s, id)) return B200_ERR_UNKNOWN_TENSOR;
+    if (n_dims == 1) ne1 = 1;
+    if (n_dims < 1 || n_dims > 2 || (s.is_q ? n_dims != 2 || ne0 != s.q.K || ne1 != s.q_rows() : ne0 * ne1 != s.n)) return B200_ERR_TENSOR_SHAPE;
+    const LoraTarget t{name, ne0, ne1, adapters, n_adapters};
+    const int rc = load_slot(s, type, host_data, nbytes, n_adapters ? &t : nullptr);
+    if (rc == B200_OK) m->mark(id);
+    return rc;
+}
+
 // seeded synthetic weights generated in HBM (bench): LayerNorm gains 1 + 0.1 N(0,1), biases = gains - 1 (small)
 int b200_neox_synthesize(b200_neox_model *m, uint64_t seed) {
     if (!m) return B200_ERR_BAD_ARG;

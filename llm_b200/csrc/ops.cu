@@ -150,6 +150,26 @@ int b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int6
     return B200_OK;
 }
 
+// LoraAdapter::patch of one adapter on host buffers: w (N rows of K, GGML layout) += scaling * (A [r, K] x B [r, N])
+int b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, int32_t a_type, const void *a, const float *b, int64_t r, float scaling) {
+    if (!w_ggml_inout || !a || !b || K < 1 || N < 1 || r < 0) return B200_ERR_BAD_ARG;
+    const int rc = lora_check(wtype, K, N, a_type, r, K, T_F32, r, N);
+    if (rc != B200_OK) return rc;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    const size_t wb = (size_t)N * (wtype == T_F32 ? (size_t)K * 4 : (size_t)(K / QK) * ggml_block_bytes(wtype));
+    const size_t ab = (size_t)K * r * (a_type == T_F16 ? 2 : 4), bb = (size_t)N * r * 4;
+    void *dw = R.op_arena.get(wb, st), *da = R.op_arena.get(ab ? ab : 1, st);
+    float *db = (float *)R.op_arena.get(bb ? bb : 4, st);
+    B200_CHECK(cudaMemcpyAsync(dw, w_ggml_inout, wb, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(da, a, ab, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(db, b, bb, cudaMemcpyHostToDevice, st));
+    lora_patch(wtype, dw, K, N, a_type, da, db, r, N, scaling, st);
+    B200_CHECK(cudaMemcpyAsync(w_ggml_inout, dw, wb, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
 // Kernel-only timing of one weight mat-mul on device-resident synthetic operands (seeded random weights and activations): used by
 // tools/prefill_gemm_bench.py and bench.py's prefill roofline; impl = B200_MM_EXACT_MMA / B200_MM_EXACT_TC5 / B200_MM_TENSOR
 int b200_op_bench_mul_mat(int32_t wtype, int64_t K, int64_t N, int64_t B, int32_t impl, int32_t iters, float *ms_out) {

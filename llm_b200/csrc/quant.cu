@@ -1,5 +1,6 @@
 // llm_b200/csrc/quant.cu -- weight re-layout at upload, the bit-faithful activation quantizer, get_rows.
 #include "kernels.cuh"
+#include "quant_rules.cuh"
 
 namespace b200 {
 
@@ -59,9 +60,7 @@ void unpack_weights(const QWeight &w, void *raw, cudaStream_t st) {
 }
 
 // ---- activation quantizer ----------------------------------------------------------------------------------------
-// One warp per 32-element block, lane j <-> element j.  Reference (AVX2) arithmetic, LC/ggml.c:1239-1254 / 1449-1474:
-//   d = amax / 127 ; id = amax != 0 ? 127 / amax : 0 ; q = round-half-even(x * id)      (NOT 1/d, NOT roundf)
-// IEEE division and a separately rounded multiply are forced with __fdiv_rn / __fmul_rn.
+// One warp per 32-element block, lane j <-> element j: the AVX2 rule of quantize_q8_avx2 (quant_rules.cuh).
 template <bool Q81>
 __global__ void __launch_bounds__(256) quantize_act_kernel(const float *__restrict__ x, int64_t ldx, int8_t *__restrict__ qs,
                                                            float2 *__restrict__ ds, int64_t nbk, int64_t total_blocks) {
@@ -70,10 +69,8 @@ __global__ void __launch_bounds__(256) quantize_act_kernel(const float *__restri
     const int lane = threadIdx.x & 31;
     const int64_t row = blk / nbk, b = blk - row * nbk;
     const float v = x[row * ldx + b * QK + lane];
-    const float amax = warp_max(fabsf(v));
-    const float d = __fdiv_rn(amax, 127.f);
-    const float id = (amax != 0.0f) ? __fdiv_rn(127.f, amax) : 0.0f;
-    const int q = __float2int_rn(__fmul_rn(v, id));
+    float d;
+    const int q = quantize_q8_avx2(v, d);
     const int isum = warp_sum(q);
     qs[blk * QK + lane] = (int8_t)q;
     if (lane == 0) {
@@ -92,20 +89,7 @@ void quantize_act(int vdt, const float *x, int64_t ldx, int8_t *qs, float2 *ds, 
     B200_CHECK(cudaGetLastError());
 }
 
-// ---- get_rows: dequantize_row_* (LC/ggml.c:1525-1635).  `x*d + m` is a fused multiply-add in the reference build. -----
-__device__ __forceinline__ void dequant_block(int type, const uint8_t *qs, uint32_t qh, float d, float m, int lane16, float &lo, float &hi) {
-    // element lane16 (lo half) and lane16 + 16 (hi half) of the block
-    if (type == T_Q8_0) { lo = (float)((const int8_t *)qs)[lane16] * d; hi = (float)((const int8_t *)qs)[lane16 + 16] * d; return; }
-    const int q = qs[lane16];
-    int q0 = q & 0xF, q1 = q >> 4;
-    if (has_qh(type)) { q0 |= ((qh >> lane16) & 1) << 4; q1 |= ((qh >> (lane16 + 16)) & 1) << 4; }
-    switch (type) {
-        case T_Q4_0: lo = (float)(q0 - 8) * d;  hi = (float)(q1 - 8) * d; break;
-        case T_Q5_0: lo = (float)(q0 - 16) * d; hi = (float)(q1 - 16) * d; break;
-        default:     lo = __fmaf_rn((float)q0, d, m); hi = __fmaf_rn((float)q1, d, m); break;   // Q4_1, Q5_1
-    }
-}
-
+// ---- get_rows: dequantize_row_* (dequant_block, quant_rules.cuh) -----------------------------------------------------
 // 16 threads per block; planes layout
 __global__ void get_rows_q_kernel(QWeight w, const int32_t *__restrict__ ids, float *__restrict__ dst, int64_t n) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -137,16 +121,10 @@ __global__ void get_rows_raw_kernel(int type, const uint8_t *__restrict__ raw, i
     const int64_t blk = t >> 4; const int j = (int)(t & 15);
     if (blk >= n * nb) return;
     const int64_t i = blk / nb, b = blk - i * nb;
-    const uint8_t *p = raw + ((int64_t)ids[i] * nb + b) * ggml_block_bytes(type);
-    const uint16_t *p16 = (const uint16_t *)p;
-    int o = 0;
-    const float d = f16_bits_to_f32(p16[o++]);
-    float m = 0.f;
-    if (has_min(type)) m = f16_bits_to_f32(p16[o++]);
-    uint32_t qh = 0;
-    if (has_qh(type)) { qh = (uint32_t)p16[o] | ((uint32_t)p16[o + 1] << 16); o += 2; }
-    float lo, hi;
-    dequant_block(type, p + 2 * o, qh, d, m, j, lo, hi);
+    float d, m, lo, hi;
+    uint32_t qh;
+    const uint8_t *qs = raw_block_header(type, raw + ((int64_t)ids[i] * nb + b) * ggml_block_bytes(type), d, m, qh);
+    dequant_block(type, qs, qh, d, m, j, lo, hi);
     const int64_t K = nb * QK;
     dst[i * K + b * QK + j] = lo;
     dst[i * K + b * QK + j + 16] = hi;

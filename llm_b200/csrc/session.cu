@@ -355,6 +355,20 @@ int b200_model_load_tensor_shaped(b200_model *m, const char *name, int32_t type,
     return b200_model_load_tensor(m, name, type, host_data, nbytes);
 }
 
+int b200_model_load_tensor_lora(b200_model *m, const char *name, int32_t type, int32_t n_dims, int64_t ne0, int64_t ne1, const void *host_data, size_t nbytes,
+                                const b200_ggml_file *const *adapters, int32_t n_adapters) {
+    if (n_adapters == 0) return b200_model_load_tensor_shaped(m, name, type, n_dims, ne0, ne1, host_data, nbytes);
+    if (!m || !name || !host_data || !adapters || n_adapters < 0 || m->tp_world > 1) return B200_ERR_BAD_ARG;   // shards: out of scope
+    Slot s; int id;
+    if (!m->lookup(name, s, id)) return B200_ERR_UNKNOWN_TENSOR;
+    if (s.is_q) { if (n_dims != 2 || ne0 != s.q.K || ne1 != s.q_rows()) return B200_ERR_TENSOR_SHAPE; }
+    else if (n_dims != 1 || ne0 != s.n) return B200_ERR_TENSOR_SHAPE;
+    const LoraTarget t{name, ne0, s.is_q ? ne1 : 1, adapters, n_adapters};
+    const int rc = load_slot(s, type, host_data, nbytes, &t);
+    if (rc == B200_OK) m->mark(id);
+    return rc;
+}
+
 int b200_model_read_tensor(b200_model *m, const char *name, void *host_out, size_t nbytes) {
     if (!m || !name || !host_out) return B200_ERR_BAD_ARG;
     Slot s; int id;

@@ -3,6 +3,7 @@
 // (quantize_row_q{4_0,4_1,5_0,5_1,8_0}_reference, LC/ggml.c:943-1145) straight into the planes layout; 1-D norm gains are
 // 1 + 0.1 N(0,1).  The generator is a counter-based hash, so a tensor's content depends only on (seed, tensor id, element).
 #include "kernels.cuh"
+#include "quant_rules.cuh"
 
 namespace b200 {
 
@@ -26,32 +27,8 @@ __global__ void __launch_bounds__(256) synth_q_kernel(QWeight w, uint64_t seed, 
     if (blk >= w.N * w.nb) return;
     const int lane = threadIdx.x & 31;
     const float v = src ? src[blk * 32 + lane] : gauss(seed, (uint64_t)blk * 32 + lane) * sigma;
-    int q = 0;
-    float d = 0.f, mn = 0.f;
-    if (w.type == T_Q4_0 || w.type == T_Q5_0) {
-        const float amax = warp_max(fabsf(v));
-        const unsigned who = __ballot_sync(0xffffffffu, fabsf(v) == amax);
-        const float mx = __shfl_sync(0xffffffffu, v, __ffs(who) - 1);           // first element attaining amax (strict `<` scan)
-        const float div = w.type == T_Q4_0 ? -8.f : -16.f;
-        d = __fdiv_rn(mx, div);
-        const float id = d != 0.f ? __fdiv_rn(1.0f, d) : 0.f;
-        const float off = w.type == T_Q4_0 ? 8.5f : 16.5f;
-        q = min(w.type == T_Q4_0 ? 15 : 31, (int)(int8_t)__float2int_rz(__fadd_rn(__fmul_rn(v, id), off)));
-    } else if (w.type == T_Q4_1 || w.type == T_Q5_1) {
-        mn = -warp_max(-v);
-        const float mx = warp_max(v);
-        const int levels = w.type == T_Q4_1 ? 15 : 31;
-        d = __fdiv_rn(__fsub_rn(mx, mn), (float)levels);
-        const float id = d != 0.f ? __fdiv_rn(1.0f, d) : 0.f;
-        q = __float2int_rz(__fadd_rn(__fmul_rn(__fsub_rn(v, mn), id), 0.5f));
-        if (w.type == T_Q4_1) q = min(15, q);
-        q &= 0xff;
-    } else {   // Q8_0
-        const float amax = warp_max(fabsf(v));
-        d = __fdiv_rn(amax, 127.f);
-        const float id = d != 0.f ? __fdiv_rn(1.0f, d) : 0.f;
-        q = (int)roundf(__fmul_rn(v, id));
-    }
+    float d, mn;
+    const int q = quantize_block_ref(w.type, v, d, mn);
     if (w.type == T_Q8_0) {
         ((int8_t *)w.qs)[blk * 32 + lane] = (int8_t)q;
     } else {

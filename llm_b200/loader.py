@@ -26,7 +26,7 @@ class LoadError(Exception):
         super().__init__(f"{what}: {self.kind}")
 
 
-ARCH = {"llama": 0, "gpt2": 1, "gptneox": 2, "mpt": 3, "bloom": 4, "gptj": 5}
+ARCH = {"llama": 0, "gpt2": 1, "gptneox": 2, "mpt": 3, "bloom": 4, "gptj": 5, "lora": 6}
 HPARAM_NAMES = {
     "llama": ("n_vocab", "n_embd", "n_mult", "n_head", "n_layer", "n_rot", "file_type"),                                   # llama lib.rs:425-447
     "gpt2": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "file_type", "n_vocab_again"),                              # gpt2 lib.rs:394-416
@@ -34,6 +34,7 @@ HPARAM_NAMES = {
     "mpt": ("n_embd", "max_seq_len", "n_head", "n_layer", "n_vocab", "alibi_bias_max", "clip_kqv", "file_type"),          # mpt lib.rs:317-330
     "bloom": ("n_vocab", "n_embd", "n_mult", "n_head", "n_layer", "file_type"),                                           # bloom lib.rs
     "gptj": ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "n_rot", "file_type", "n_vocab_again"),                    # gptj lib.rs:366-401
+    "lora": ("r", "alpha"),                                                                                                 # LoraParameters, lora.rs:27-35
 }
 FLOAT_WORDS = {"alibi_bias_max", "clip_kqv"}                                                                             # f32 in the header (read_f32)
 
@@ -182,7 +183,8 @@ def write_model(path: str, arch: str, header: Dict[str, int], tensors: Dict[str,
 
 
 def load(path: str, params: ModelParameters = None, device: int = 0) -> Llama:
-    """llm::load::<Llama>: parse the file, create the model for its geometry, upload every tensor from the mapping to HBM."""
+    """llm::load::<Llama>: parse the file, create the model for its geometry, upload every tensor from the mapping to HBM, patched by
+    params.lora_adapters (in order) where they name it."""
     params = params or ModelParameters()
     if not params.use_gpu:
         raise ValueError("llm_b200 has no CPU path: ModelParameters.use_gpu must be True")
@@ -194,7 +196,12 @@ def load(path: str, params: ModelParameters = None, device: int = 0) -> Llama:
     hp = with_hp.llama_hyperparameters()
     with_hp.close()
     err = C.c_int(0)
-    m = L.b200_llama_load_file(path.encode(), params.context_size, params.rope_freq_base, params.rope_freq_scale, C.byref(err))
+    if params.lora_adapters:
+        paths = (C.c_char_p * len(params.lora_adapters))(*[p.encode() for p in params.lora_adapters])
+        m = L.b200_llama_load_file_lora(path.encode(), params.context_size, params.rope_freq_base, params.rope_freq_scale, 1, paths,
+                                        len(params.lora_adapters), C.byref(err))
+    else:
+        m = L.b200_llama_load_file(path.encode(), params.context_size, params.rope_freq_base, params.rope_freq_scale, C.byref(err))
     if not m:
         raise LoadError(err.value, f"load {path}")
     model = Llama.__new__(Llama)

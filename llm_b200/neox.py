@@ -7,12 +7,12 @@
   InferenceSession        crates/llm-base/src/inference_session.rs     evaluate / n_past / rewind
 No arithmetic happens in Python."""
 import ctypes as C
-from typing import Dict
+from typing import Dict, List, Optional
 
 import numpy as np
 
 from . import _lib
-from .session import _check, _Native
+from .session import LoraAdapters, _check, _Native, ggml_dims
 
 
 class NeoxHparams(C.Structure):
@@ -28,6 +28,7 @@ def _bind(L):
     L.b200_neox_new_alibi.restype = vp
     L.b200_neox_new_alibi.argtypes = [C.POINTER(NeoxHparams), C.c_float]
     L.b200_neox_load_tensor.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
+    L.b200_neox_load_tensor_lora.argtypes = [vp, C.c_char_p, i32, i32, C.c_int64, C.c_int64, vp, C.c_size_t, C.POINTER(vp), i32]
     L.b200_neox_synthesize.argtypes = [vp, C.c_uint64]
     L.b200_neox_weight_bytes.restype = C.c_size_t
     L.b200_neox_weight_bytes.argtypes = [vp]
@@ -47,12 +48,14 @@ def _bind(L):
 
 
 class GptNeoX(_Native):
-    """hyperparameters: n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype"""
+    """hyperparameters: n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype.  lora_adapters: LoRA adapter files applied in
+    order to every tensor they name (ModelParameters::lora_adapters)."""
 
     ARCH = 0
     _HANDLE, _FREE = "_m", "b200_neox_free"
 
-    def __init__(self, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray] = None, context_size: int = None, device: int = 0):
+    def __init__(self, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray] = None, context_size: int = None, device: int = 0,
+                 lora_adapters: Optional[List[str]] = None):
         self.L = _bind(_lib.lib())
         _check(self.L.b200_init(device), "b200_init")
         self.hyperparameters = dict(hyperparameters)
@@ -63,10 +66,23 @@ class GptNeoX(_Native):
         self._m = self._new(hp)
         if not self._m:
             raise ValueError(f"b200_neox_new rejected {hyperparameters}")
+        if lora_adapters:
+            with LoraAdapters(self.L, lora_adapters) as ad:
+                for name, arr in (tensors or {}).items():
+                    self._load_lora(name, np.ascontiguousarray(arr), ad)
+            return
         for name, arr in (tensors or {}).items():
             arr = np.ascontiguousarray(arr)
             typ = 0 if arr.dtype == np.float32 else int(hyperparameters["wtype"])
             _check(self.L.b200_neox_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes), f"load_tensor({name})")
+
+    def _load_lora(self, name, arr, ad):
+        typ = 0 if arr.dtype == np.float32 else int(self.hyperparameters["wtype"])
+        nd, ne0, ne1 = ggml_dims(arr, typ)
+        rc = self.L.b200_neox_load_tensor_lora(self._m, name.encode(), typ, nd, ne0, ne1, arr.ctypes.data_as(C.c_void_p), arr.nbytes, ad.handles, ad.n)
+        if rc != 0:
+            from .loader import LoadError
+            raise LoadError(rc, f"load_tensor({name})")
 
     def _new(self, hp):
         return self.L.b200_neox_new(C.byref(hp))

@@ -10,7 +10,7 @@ Names follow the reference so that the parity tests read like its own integratio
 """
 import ctypes as C
 from dataclasses import dataclass, field
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import numpy as np
 
@@ -27,6 +27,7 @@ class ModelParameters:
     use_gpu: bool = True              # this backend IS the GPU path; False is rejected (no CPU fallback)
     rope_freq_base: float = 10000.0   # RoPEOverrides
     rope_freq_scale: float = 1.0
+    lora_adapters: Optional[List[str]] = None   # model/mod.rs:205-206: LoRA adapter files, applied in this order to every tensor they name
 
 
 @dataclass
@@ -83,6 +84,44 @@ class _Native:
             pass
 
 
+class LoraAdapters:
+    """The adapter files of ModelParameters::lora_adapters, opened as LoRA containers (r, alpha, no vocabulary) for the span of a load:
+    `handles` is the array the b200_*_load_tensor_lora entry points take."""
+    LORA_ARCH = 6                                 # B200_ARCH_LORA
+
+    def __init__(self, L, paths: Optional[List[str]]):
+        self.L, self._open = L, []
+        for p in paths or []:
+            err = C.c_int(0)
+            f = L.b200_ggml_open_arch(p.encode(), self.LORA_ARCH, C.byref(err))
+            if not f:
+                self.close()
+                from .loader import LoadError
+                raise LoadError(err.value, f"open LoRA adapter {p}")
+            self._open.append(f)
+        self.handles = (C.c_void_p * max(1, len(self._open)))(*self._open)
+        self.n = len(self._open)
+
+    def close(self):
+        for f in self._open:
+            self.L.b200_ggml_close(f)
+        self._open = []
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def ggml_dims(arr: np.ndarray, wtype: int):
+    """(n_dims, ne0, ne1) of a tensor given as GGML-layout block rows (uint8 [rows][row bytes]) or f32 ([n] or [rows][cols])"""
+    if arr.dtype == np.float32:
+        return (1, arr.shape[0], 1) if arr.ndim == 1 else (2, arr.shape[-1], arr.size // arr.shape[-1])
+    block = {2: 18, 3: 20, 6: 22, 7: 24, 8: 34}[wtype]
+    return 2, arr.shape[-1] // block * 32, arr.size // arr.shape[-1]
+
+
 class Llama(_Native):
     """KnownModel for LLaMA.  `hyperparameters` is a dict with n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff, wtype."""
     _HANDLE, _FREE = "_m", "b200_model_free"
@@ -102,16 +141,30 @@ class Llama(_Native):
         self._m = self.L.b200_llama_new(C.byref(hp))
         if not self._m:
             raise ValueError(f"b200_llama_new rejected hyperparameters {hyperparameters}")
-        if tensors is not None:
+        if tensors is not None and params.lora_adapters:
+            shapes = llama_tensor_shapes(self.hyperparameters)
+            with LoraAdapters(self.L, params.lora_adapters) as ad:
+                for name, arr in tensors.items():
+                    self.load_tensor(name, arr, ad, shapes.get(name))
+        elif tensors is not None:
             for name, arr in tensors.items():
                 self.load_tensor(name, arr)
 
     # TensorLoader::load + transfer_to(Backend::Gpu)
-    def load_tensor(self, name: str, arr: np.ndarray):
+    def load_tensor(self, name: str, arr: np.ndarray, adapters: "LoraAdapters" = None, shape: tuple = None):
+        """`adapters`: patch the tensor with them (LoraAdapter::patch); `shape` is then its (rows, cols) / (n,) as in llama_tensor_shapes"""
         arr = np.ascontiguousarray(arr)
         typ = 0 if arr.dtype == np.float32 else int(self.hyperparameters["wtype"])
-        _check(self.L.b200_model_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes),
-               f"load_tensor({name})")
+        if adapters is None:
+            _check(self.L.b200_model_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes),
+                   f"load_tensor({name})")
+            return
+        nd, ne0, ne1 = (len(shape), shape[-1], shape[0] if len(shape) == 2 else 1) if shape else ggml_dims(arr, typ)
+        rc = self.L.b200_model_load_tensor_lora(self._m, name.encode(), typ, nd, ne0, ne1, arr.ctypes.data_as(C.c_void_p), arr.nbytes,
+                                                adapters.handles, adapters.n)
+        if rc != 0:
+            from .loader import LoadError
+            raise LoadError(rc, f"load_tensor({name})")
 
     def synthesize(self, seed: int = 0x5EED0000):
         _check(self.L.b200_model_synthesize(self._m, seed), "synthesize")
