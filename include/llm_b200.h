@@ -35,7 +35,7 @@ typedef struct b200_session b200_session;
 
 typedef struct {
     int32_t n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff;
-    int32_t wtype;            /* enum ggml_type of the 2-D weights: 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0 */
+    int32_t wtype;            /* enum ggml_type of the 2-D weights: 1 F16, 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0 */
     int32_t context_size;     /* ModelParameters::context_size (default 2048) */
     float   rope_freq_base;   /* RoPEOverrides::frequency_base (10000) */
     float   rope_freq_scale;  /* RoPEOverrides::frequency_scale (1) */
@@ -196,7 +196,8 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
 
 /* ---- GPT-NeoX (crates/models/gptneox): KnownModel + InferenceSession, same conventions as the LLaMA entry points above --------------------------
  * Hyperparameters (gptneox lib.rs:403-447 region): tensor names are the loader's ("gpt_neox.embed_in.weight", "gpt_neox.layers.N.attention.
- * query_key_value.weight" [3e x e, rows per head: q | k | v], ..., "embed_out.weight"); every 2-D ".weight" is quantized to wtype, biases / LayerNorm f32. */
+ * query_key_value.weight" [3e x e, rows per head: q | k | v], ..., "embed_out.weight"); every 2-D ".weight" is of wtype (1 = F16 or a block format), biases / LayerNorm f32;
+ * GPT-2's "model/wpe" may also be F16. */
 typedef struct b200_neox_hparams {
     int32_t n_vocab, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype, context_size;
     int32_t arch;          /* 0 = GPT-NeoX; 1 = GPT-2 (crates/models/gpt2): tensor names "model/wte", "model/wpe" (f32 [n_ctx][n_embd]), "model/hN/attn/c_attn/w" ...,
@@ -242,7 +243,7 @@ void b200_neox_session_free(b200_neox_session *s);
 int  b200_op_quantize_act(int32_t vec_dot_type, const float *x, int64_t K, int64_t B, int8_t *qs_out, float *d_out, float *aux_out);
 /* ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} (LC/ggml.c:18083-18230) on the GPU: w_host f32 [N][K] -> N rows of GGML blocks, bit-exact with the reference */
 int  b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int64_t N, void *ggml_blocks_out);
-/* wtype: GGML_TYPE_Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 (2,3,6,7,8; K % 64 == 0), or the K-quants Q2_K..Q6_K (10..14; K % 256 == 0, impl AUTO or EXACT:
+/* wtype: GGML_TYPE_F16 (1; K % 64 == 0, impl AUTO or EXACT = mul_mat_f16_exact), GGML_TYPE_Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 (2,3,6,7,8; K % 64 == 0), or the K-quants Q2_K..Q6_K (10..14; K % 256 == 0, impl AUTO or EXACT:
  * ggml_vec_dot_q{2,3,4,5,6}_K_q8_K of LC/k_quants.c:1240,1763,2492,3023,3592 on quantize_row_q8_K activations, bit-exact with the reference's AVX2 build) */
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);
 /* quantize_row_q8_K (LC/k_quants.c:1133-1183) of B rows of K floats -> B * K/256 block_q8_K {f32 d; i8 qs[256]; i16 bsums[16]} (292 bytes each), bit-exact */

@@ -53,13 +53,18 @@ __host__ __device__ inline int vec_dot_type(int t) { return (t == T_Q4_1 || t ==
 __host__ __device__ inline bool has_min(int t) { return t == T_Q4_1 || t == T_Q5_1; }
 __host__ __device__ inline bool has_qh(int t) { return t == T_Q5_0 || t == T_Q5_1; }
 __host__ __device__ inline int qs_bytes(int t) { return t == T_Q8_0 ? 32 : 16; }
+// types a QWeight holds: the five block formats and F16 (one plane of N rows x K halves, GGML's bytes)
+inline bool is_qweight_type(int t) { return is_quant(t) || t == T_F16; }
+// GGML bytes per 32 elements of a QWeight row: an F16 row counts as blocks of 32 halves
+inline int qweight_block_bytes(int t) { return t == T_F16 ? 64 : ggml_block_bytes(t); }
 
 // A quantized weight matrix resident in HBM, repacked at upload from GGML's array-of-blocks (2-byte aligned, 18..34 B
 // blocks) into 16-byte aligned planes so that every access is a full 128-bit transaction and TMA boxes are legal:
 //   qs : [N][nb][16] packed nibbles (Q4_x, Q5_x) or [N][nb][32] int8 (Q8_0)   -- bit-identical to GGML's qs bytes
 //   qh : [N][nb] uint32 fifth bits (Q5_x)
 //   dm : [N][nb] fp16 d  (Q4_0, Q5_0, Q8_0)  or  [N][nb] half2 {d, m} (Q4_1, Q5_1)
-// Bytes per weight are exactly GGML's (18/20/22/24/34 per 32).
+// Bytes per weight are exactly GGML's (18/20/22/24/34 per 32).  An F16 weight keeps GGML's bytes in `qs` alone ([N][K] halves, row pitch 2K,
+// 16-byte aligned since K % 64 == 0); nb = K/32 then counts 64-byte groups of 32 halves, so row views and chunked loads work unchanged.
 struct QWeight {
     int type = 0;
     int64_t K = 0, N = 0, nb = 0;

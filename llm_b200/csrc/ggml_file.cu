@@ -296,8 +296,8 @@ static b200_model *load_file_impl(const char *path, int32_t context_size, float 
     b200_llama_hparams hp;
     *err = b200_ggml_llama_hparams(f, &hp, nullptr, nullptr, nullptr);
     if (*err != B200_OK) { b200_ggml_close(f); return nullptr; }
-    if (!b200::is_quant(hp.wtype)) {            // F16 / F32 / K-quant files parse, but this backend streams the five 32-element block formats only
-        fprintf(stderr, "llm_b200: %s: layers.0.attention.wq.weight is %s; this backend loads Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 weights\n", path, type_name(hp.wtype));
+    if (!b200::is_qweight_type(hp.wtype)) {     // F32 / K-quant files parse, but this backend streams F16 and the five 32-element block formats only
+        fprintf(stderr, "llm_b200: %s: layers.0.attention.wq.weight is %s; this backend loads F16/Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 weights\n", path, type_name(hp.wtype));
         *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; b200_ggml_close(f); return nullptr;
     }
     if (context_size > 0) hp.context_size = context_size;

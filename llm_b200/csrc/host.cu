@@ -42,9 +42,9 @@ static int lora_apply(const LoraTarget &t, int wtype, int64_t K, int64_t N, void
 QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows) {
     QWeight v = w;
     v.N = nrows;
-    v.qs = w.qs + (size_t)row0 * w.nb * qs_bytes(w.type);
+    v.qs = w.qs + (size_t)row0 * w.nb * (w.type == T_F16 ? 64 : qs_bytes(w.type));
     if (w.qh) v.qh = w.qh + (size_t)row0 * w.nb;
-    v.dm = (const uint8_t *)w.dm + (size_t)row0 * w.nb * (has_min(w.type) ? 4 : 2);
+    if (w.dm) v.dm = (const uint8_t *)w.dm + (size_t)row0 * w.nb * (has_min(w.type) ? 4 : 2);
     v.base = nullptr;
     return v;
 }
@@ -68,10 +68,18 @@ int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes, cons
         if (lora) lora_apply(*lora, type, K, N, raw, false);
         if (!s.chunk) repack_weights(s.q, raw, R.stream);
         else {
-            const size_t piece = (size_t)s.chunk * s.q.nb * ggml_block_bytes(type);
+            const size_t piece = (size_t)s.chunk * s.q.nb * qweight_block_bytes(type);
             for (int64_t c = 0; c * s.chunk < s.rows; c++)
                 repack_weights(row_view(s.q, c * s.stride + s.row0, s.chunk), (const char *)raw + c * piece, R.stream);
         }
+        B200_CHECK(cudaStreamSynchronize(R.stream));
+    } else if (type == T_F16 && s.f16_src && nbytes == (size_t)s.n * 2) {
+        if (lora)                                    // the reference would patch the F16 tensor before it is widened
+            for (int i = 0; i < lora->n; i++) if (lora->adapters[i] && lora_in_patch_set(lora->adapters[i], lora->name)) return B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+        R.op_arena.reset();
+        void *raw = R.op_arena.get(nbytes, R.stream);
+        B200_CHECK(cudaMemcpyAsync(raw, host, nbytes, cudaMemcpyHostToDevice, R.stream));
+        f16_to_f32(raw, s.f, s.n, R.stream);
         B200_CHECK(cudaStreamSynchronize(R.stream));
     } else {
         if (type != T_F32 || nbytes != s.bytes()) return B200_ERR_TENSOR_SHAPE;
@@ -94,7 +102,7 @@ int read_slot(const Slot &s, void *host, size_t nbytes) {
         void *raw = R.op_arena.get(nbytes, R.stream);
         if (!s.chunk) unpack_weights(s.q, raw, R.stream);
         else {
-            const size_t piece = (size_t)s.chunk * s.q.nb * ggml_block_bytes(s.q.type);
+            const size_t piece = (size_t)s.chunk * s.q.nb * qweight_block_bytes(s.q.type);
             for (int64_t c = 0; c * s.chunk < s.rows; c++)
                 unpack_weights(row_view(s.q, c * s.stride + s.row0, s.chunk), (char *)raw + c * piece, R.stream);
         }

@@ -36,7 +36,7 @@ struct SlabCarver {
     size_t off = 0, streamed = 0;       // streamed: GGML bytes of every matrix carved
     void q(QWeight &w, int64_t K, int64_t N) {
         off += qweight_layout(w, wtype, K, N, base ? base + off : nullptr);
-        streamed += (size_t)N * (K / QK) * ggml_block_bytes(wtype);
+        streamed += (size_t)N * (K / QK) * qweight_block_bytes(wtype);
     }
     void f(float *&p, int64_t n) { if (base) p = (float *)(base + off); off += ((size_t)n * 4 + 255) & ~(size_t)255; }
 };
@@ -85,8 +85,9 @@ struct Weights {
 // (LLaMA's w1 / w3 are interleaved in 32-row pieces inside w13 so that 64 consecutive rows hold both factors of 32 silu*mul outputs)
 struct Slot {
     QWeight q; float *f = nullptr; int64_t n = 0; bool is_q = false; int chunk = 0; int64_t row0 = 0, stride = 0, rows = 0;
+    bool f16_src = false;     // f32 slot that also takes F16 bytes, widened (exactly) to f32 on upload
     int64_t q_rows() const { return chunk ? rows : q.N; }
-    size_t bytes() const { return is_q ? (size_t)q_rows() * q.nb * ggml_block_bytes(q.type) : (size_t)n * 4; }
+    size_t bytes() const { return is_q ? (size_t)q_rows() * q.nb * qweight_block_bytes(q.type) : (size_t)n * 4; }
 };
 // The LoRA adapters of one tensor load: the tensor's name and shape [ne0, ne1] (ne1 = 1 for a vector) and the adapter files, applied in order
 struct LoraTarget { const char *name; int64_t ne0, ne1; const b200_ggml_file *const *adapters; int n; };

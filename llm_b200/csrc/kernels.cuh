@@ -60,12 +60,20 @@ bool mmv_exact_stream_supported(const QWeight &w);
 void quantize_act_pack(int wtype, const float *x, int4 *pack, int64_t K, cudaStream_t st);
 void mul_mat_vec_q_exact_stream(const QWeight &w, const int4 *xpack, float *dst, const float *addend, cudaStream_t st);
 
+// ---- exact_f16.cu : F16 weights (QWeight type T_F16), ggml_vec_dot_f16 order on fp16-rounded activations (xh: cvt_act_f16 rows) ----------
+bool mmv_f16_supported(const QWeight &w);      // the streaming mat-vec's shared memory holds the activation row
+void mul_mat_vec_f16(const QWeight &w, const __half *xh, float *dst, const float *addend, cudaStream_t st);                    // one row
+void mul_mat_f16_gemm(const QWeight &w, const __half *xh, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda, cudaStream_t st);
+void get_rows_f16(const QWeight &w, const int32_t *ids, float *dst, int64_t n, cudaStream_t st);
+void f16_to_f32(const void *src, float *dst, int64_t n, cudaStream_t st);          // exact widening (F16 tensors kept as f32)
+
 // ---- mul_mat.cu : the bit-exact ggml_mul_mat of every front end -------------------------------------------------------------------------
 bool prefill_gemm_tc5();         // B200_PREFILL_GEMM != "mma" (the default)
 // activation buffers for B rows of K: xq [B][K] int8, xds [B][K/32], xpack (K/32) * 64 bytes, xh xh_bytes(K, B)
 struct ExactActs { int8_t *xq; float2 *xds; int4 *xpack; __half *xh; };
 // dst[b*ldd + n] (+ addend[b*lda + n]) for B rows of x (row stride ldx): quantizes x and runs the exact kernel for B -- the streaming mat-vec
-// (B == 1), the wgmma GEMM (B >= 96, prefill_gemm_tc5()), the mma.sync GEMM (B >= 16) or exact.cu.  Returns the number of launches (2).
+// (B == 1), the wgmma GEMM (B >= 96, prefill_gemm_tc5()), the mma.sync GEMM (B >= 16) or exact.cu.  An F16 weight rounds x to fp16 and runs
+// exact_f16.cu's mat-vec (B == 1) or GEMM.  Returns the number of launches (2).
 int mul_mat_exact_auto(const QWeight &w, const float *x, int64_t ldx, int64_t B, float *dst, int64_t ldd, const float *addend, int64_t lda,
                        const ExactActs &a, cudaStream_t st);
 

@@ -115,6 +115,11 @@ __global__ void __launch_bounds__(LP_THREADS) lora_patch_kernel(uint8_t *__restr
             if (k < K) { float *p = (float *)w + n * K + k; *p = __fadd_rn(*p, v); }
             continue;
         }
+        if (WT == T_F16) {                                            // add_f16_f32 (LC/ggml.c:8165-8215): fp16(f32(w) + ba)
+            const int64_t k = kb * 32 + lane;
+            if (k < K) { __half *p = (__half *)w + n * K + k; *p = __float2half_rn(__fadd_rn(__half2float(*p), v)); }
+            continue;
+        }
         uint8_t *blk = w + (n * (K / QK) + kb) * ggml_block_bytes(WT);
         float d, m, lo, hi;
         uint32_t qh;
@@ -155,7 +160,7 @@ static void launch_lora(uint8_t *w, int64_t K, int64_t N, int a_type, const void
 
 int lora_check(int wtype, int64_t K, int64_t N, int a_type, int64_t a_ne0, int64_t a_ne1, int b_type, int64_t b_ne0, int64_t b_ne1) {
     if ((a_type != T_F32 && a_type != T_F16) || b_type != T_F32) return B200_ERR_UNSUPPORTED_ELEMENT_TYPE;   // nb10 == sizeof(float), LC/ggml.c:10424-10427
-    if (wtype != T_F32 && !is_quant(wtype)) return B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+    if (wtype != T_F32 && wtype != T_F16 && !is_quant(wtype)) return B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
     if (a_ne0 != b_ne0 || a_ne1 != K || b_ne1 < 1) return B200_ERR_TENSOR_SHAPE;                         // ggml_can_mul_mat; ba has K rows
     if (wtype == T_F32 ? N % b_ne1 != 0 : b_ne1 != N) return B200_ERR_TENSOR_SHAPE;                      // ggml_can_repeat_rows / add_q_f32's same shape
     if (is_quant(wtype) && K % QK) return B200_ERR_TENSOR_SHAPE;
@@ -168,6 +173,7 @@ void lora_patch(int wtype, void *w, int64_t K, int64_t N, int a_type, const void
     uint8_t *p = (uint8_t *)w;
     switch (wtype) {
         case T_F32:  launch_lora<T_F32>(p, K, N, a_type, a, b, r, nb_rows, scaling, st); break;
+        case T_F16:  launch_lora<T_F16>(p, K, N, a_type, a, b, r, nb_rows, scaling, st); break;
         case T_Q4_0: launch_lora<T_Q4_0>(p, K, N, a_type, a, b, r, nb_rows, scaling, st); break;
         case T_Q4_1: launch_lora<T_Q4_1>(p, K, N, a_type, a, b, r, nb_rows, scaling, st); break;
         case T_Q5_0: launch_lora<T_Q5_0>(p, K, N, a_type, a, b, r, nb_rows, scaling, st); break;

@@ -16,6 +16,12 @@ bool prefill_gemm_tc5() {
 
 int mul_mat_exact_auto(const QWeight &w, const float *x, int64_t ldx, int64_t B, float *dst, int64_t ldd, const float *addend, int64_t lda,
                        const ExactActs &a, cudaStream_t st) {
+    if (w.type == T_F16) {                                   // ggml_fp32_to_fp16_row, then ggml_vec_dot_f16 per output (exact_f16.cu)
+        cvt_act_f16(x, ldx, a.xh, w.K, B, st);
+        if (B == 1 && mmv_f16_supported(w)) mul_mat_vec_f16(w, a.xh, dst, addend, st);
+        else mul_mat_f16_gemm(w, a.xh, dst, ldd, B, addend, lda, st);
+        return 2;
+    }
     const int vdt = vec_dot_type(w.type);
     if (B == 1 && mmv_exact_stream_supported(w)) {          // decode: TMA bulk-copy ring at HBM speed (exact_stream.cu)
         quantize_act_pack(w.type, x, a.xpack, w.K, st);

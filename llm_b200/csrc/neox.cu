@@ -184,6 +184,7 @@ bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
         }
         slot++;
     });
+    if (found && wpe && s.f == wpe) s.f16_src = true;      // gpt2 lib.rs:59 loads wpe in the file's type; get_rows of F16 rows is exact in f32
     return found;
 }
 
@@ -197,7 +198,8 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     int L = 0;
     // the graph schedule's attention keeps the whole bucket in shared memory: steps in buckets past 3264 positions run per op below, and the
     // graph cache re-uploads the device n_past when graph steps resume (after a rewind)
-    if (n == 1 && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {
+    // F16 weights decode per op (exact_f16.cu's mat-vec): the graph schedule is built on Q8 activation records
+    if (n == 1 && hp.wtype != T_F16 && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {
         s->last_launches = s->decode.run(n_kv, n_ctx, true, [s, &hp](int bucket, cudaStream_t st, int *nodes) {
             neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
         }, st);
@@ -283,7 +285,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
 // hp->arch 0 / 1 / 4 (b200_neox_new) or 2 / 3 (b200_neox_new_alibi, alibi_bias_max: the ALiBi bias of MPT's header, 8 for BLOOM).
 // GPT-NeoX and GPT-J rotate: n_rot even, positive and at most the head size (the asserts of ggml_rope, LC/ggml.c:11807-11808)
 b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
-    if (!hp || !is_quant(hp->wtype) || hp->n_embd % 64 || hp->n_head <= 0 || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0 ||
+    if (!hp || !is_qweight_type(hp->wtype) || hp->n_embd % 64 || hp->n_head <= 0 || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0 ||
         ((hp->arch == 0 || hp->arch == 4) && (hp->n_rot <= 0 || hp->n_rot % 2 || hp->n_rot > hp->n_embd / hp->n_head))) return nullptr;
     rt().ensure_init();
     b200_neox_model *m = new b200_neox_model();
@@ -301,7 +303,7 @@ b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
     });
     // no output matrix (GPT-2 without model/lm_head, gpt2 lib.rs:319-320; MPT): the output projection is tied to wte, which is streamed as the lm_head
     if (!m->lm_head.qs) m->lm_head = m->wte;
-    else m->weight_bytes -= (size_t)v * (e / QK) * ggml_block_bytes(t);  // the embedding table is gathered from, not streamed
+    else m->weight_bytes -= (size_t)v * (e / QK) * qweight_block_bytes(t);  // the embedding table is gathered from, not streamed
     if (m->mpt() || m->bloom()) {
         const std::vector<float> slopes = alibi_slopes(hp->n_head, alibi_bias_max);
         m->alibi = device_alloc<float>(slopes.size() * 4);

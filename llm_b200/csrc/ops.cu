@@ -29,6 +29,12 @@ void run(int32_t impl, const QWeight &w, const Acts &a, float *dd, int64_t N, in
     else mul_mat_q(w, a.xq, a.xds, dd, N, B, nullptr, 0, st);
 }
 
+// F16 weight rows: AUTO = the sessions' dispatch (exact_f16.cu), EXACT = exact.cu's mul_mat_f16_exact (the attention mat-mul kernel) on the same rows
+void run_f16(int32_t impl, const QWeight &w, const float *dx, __half *xh, float *dd, int64_t B, cudaStream_t st) {
+    if (impl == B200_MM_AUTO) mul_mat_exact_auto(w, dx, w.K, B, dd, w.N, nullptr, 0, {nullptr, nullptr, nullptr, xh}, st);
+    else mul_mat_f16_exact((const __half *)w.qs, w.K, w.N, 1, w.K * 2, w.N * w.K * 2, dx, B, 1, w.K * 4, B * w.K * 4, dd, w.N * 4, B * w.N * 4, -1, st);
+}
+
 // B200_ERR_IO if a pipeline barrier of the wgmma kernel `impl` ever timed out (call after the stream is synchronized)
 int check_timeout(int32_t impl) {
     if (impl == B200_MM_EXACT_TC5 && exact_tc5_check_timeout() != 0) return B200_ERR_IO;
@@ -85,6 +91,22 @@ int b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, con
         B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
         quantize_act_q8k(dx, K, xq, K, B, st);
         mul_mat_kq_exact(wtype, raw, xq, dd, N, K, N, B, nullptr, 0, st);
+        B200_CHECK(cudaMemcpyAsync(dst, dd, (size_t)B * N * 4, cudaMemcpyDeviceToHost, st));
+        B200_CHECK(cudaStreamSynchronize(st));
+        return B200_OK;
+    }
+    if (wtype == T_F16) {                                // ggml_vec_dot_f16 order; `impl` must be AUTO or EXACT
+        if (!w_ggml || !x || !dst || K % 64 || K < 64 || N < 1 || B < 1 || B > 65535 || (impl != B200_MM_AUTO && impl != B200_MM_EXACT)) return B200_ERR_BAD_ARG;
+        Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+        cudaStream_t st = R.stream;
+        QWeight w;
+        qweight_layout(w, T_F16, K, N, R.op_arena.get(qweight_layout(w, T_F16, K, N, nullptr), st));
+        float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
+        float *dd = (float *)R.op_arena.get((size_t)B * N * 4, st);
+        __half *xh = (__half *)R.op_arena.get((size_t)B * K * 2, st);
+        B200_CHECK(cudaMemcpyAsync((void *)w.qs, w_ggml, (size_t)N * K * 2, cudaMemcpyHostToDevice, st));
+        B200_CHECK(cudaMemcpyAsync(dx, x, (size_t)B * K * 4, cudaMemcpyHostToDevice, st));
+        run_f16(impl, w, dx, xh, dd, B, st);
         B200_CHECK(cudaMemcpyAsync(dst, dd, (size_t)B * N * 4, cudaMemcpyDeviceToHost, st));
         B200_CHECK(cudaStreamSynchronize(st));
         return B200_OK;
@@ -157,7 +179,7 @@ int b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, 
     if (rc != B200_OK) return rc;
     Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
     cudaStream_t st = R.stream;
-    const size_t wb = (size_t)N * (wtype == T_F32 ? (size_t)K * 4 : (size_t)(K / QK) * ggml_block_bytes(wtype));
+    const size_t wb = (size_t)N * (wtype == T_F32 ? (size_t)K * 4 : wtype == T_F16 ? (size_t)K * 2 : (size_t)(K / QK) * ggml_block_bytes(wtype));
     const size_t ab = (size_t)K * r * (a_type == T_F16 ? 2 : 4), bb = (size_t)N * r * 4;
     void *dw = R.op_arena.get(wb, st), *da = R.op_arena.get(ab ? ab : 1, st);
     float *db = (float *)R.op_arena.get(bb ? bb : 4, st);
@@ -173,7 +195,8 @@ int b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, 
 // Kernel-only timing of one weight mat-mul on device-resident synthetic operands (seeded random weights and activations): used by
 // tools/prefill_gemm_bench.py and bench.py's prefill roofline; impl = B200_MM_EXACT_MMA / B200_MM_EXACT_TC5 / B200_MM_TENSOR
 int b200_op_bench_mul_mat(int32_t wtype, int64_t K, int64_t N, int64_t B, int32_t impl, int32_t iters, float *ms_out) {
-    if (!is_quant(wtype) || K % 64 || !ms_out || iters < 1) return B200_ERR_BAD_ARG;
+    if (!is_qweight_type(wtype) || K % 64 || !ms_out || iters < 1) return B200_ERR_BAD_ARG;
+    if (wtype == T_F16 && ((impl != B200_MM_AUTO && impl != B200_MM_EXACT) || B < 1 || B > 65535)) return B200_ERR_BAD_ARG;
     Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
     cudaStream_t st = R.stream;
     QWeight w;
@@ -183,6 +206,22 @@ int b200_op_bench_mul_mat(int32_t wtype, int64_t K, int64_t N, int64_t B, int32_
     synth_qweight(w, 777u, st);
     float *dx = (float *)R.op_arena.get((size_t)B * K * 4, st);
     float *dd = (float *)R.op_arena.get((size_t)B * N * 4, st);
+    if (wtype == T_F16) {                                // the whole mat-mul as a session runs it: the activation rounding included
+        __half *xh = (__half *)R.op_arena.get((size_t)B * K * 2, st);
+        synth_gain(dx, B * K, 12345u, st);
+        for (int i = 0; i < 2; i++) run_f16(impl, w, dx, xh, dd, B, st);
+        cudaEvent_t e0, e1;
+        B200_CHECK(cudaEventCreate(&e0)); B200_CHECK(cudaEventCreate(&e1));
+        B200_CHECK(cudaEventRecord(e0, st));
+        for (int i = 0; i < iters; i++) run_f16(impl, w, dx, xh, dd, B, st);
+        B200_CHECK(cudaEventRecord(e1, st));
+        B200_CHECK(cudaEventSynchronize(e1));
+        float ms = 0.f;
+        B200_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+        *ms_out = ms / iters;
+        B200_CHECK(cudaEventDestroy(e0)); B200_CHECK(cudaEventDestroy(e1));
+        return B200_OK;
+    }
     Acts a;
     a.xds = (float2 *)R.op_arena.get((size_t)B * (K / QK) * sizeof(float2), st);
     a.xh = (__half *)R.op_arena.get(xh_bytes(K, B) + 16, st);

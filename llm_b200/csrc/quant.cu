@@ -7,8 +7,13 @@ namespace b200 {
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 size_t qweight_layout(QWeight &w, int type, int64_t K, int64_t N, void *base) {
-    B200_ASSERT(is_quant(type) && K % QK == 0);
+    B200_ASSERT(is_qweight_type(type) && K % QK == 0);
     w.type = type; w.K = K; w.N = N; w.nb = K / QK;
+    if (type == T_F16) {                                 // one plane: the file's [N][K] halves
+        w.bytes = align_up((size_t)N * K * 2, 256);
+        if (base) { w.base = base; w.qs = (const uint8_t *)base; w.qh = nullptr; w.dm = nullptr; }
+        return w.bytes;
+    }
     const size_t nblk = (size_t)N * (size_t)w.nb;
     size_t off = 0;
     const size_t qs_off = off; off = align_up(off + nblk * qs_bytes(type), 256);
@@ -49,12 +54,14 @@ __global__ void repack_kernel(int type, int64_t nblk, uint8_t *raw, uint8_t *qs,
 void repack_weights(const QWeight &w, const void *raw, cudaStream_t st) {
     const int64_t nblk = w.N * w.nb;
     if (nblk == 0) return;
+    if (w.type == T_F16) { B200_CHECK(cudaMemcpyAsync((void *)w.qs, raw, (size_t)w.N * w.K * 2, cudaMemcpyDeviceToDevice, st)); return; }
     repack_kernel<true><<<(unsigned)((nblk + 255) / 256), 256, 0, st>>>(w.type, nblk, (uint8_t *)raw, (uint8_t *)w.qs, (uint32_t *)w.qh, (uint8_t *)w.dm);
     B200_CHECK(cudaGetLastError());
 }
 void unpack_weights(const QWeight &w, void *raw, cudaStream_t st) {
     const int64_t nblk = w.N * w.nb;
     if (nblk == 0) return;
+    if (w.type == T_F16) { B200_CHECK(cudaMemcpyAsync(raw, w.qs, (size_t)w.N * w.K * 2, cudaMemcpyDeviceToDevice, st)); return; }
     repack_kernel<false><<<(unsigned)((nblk + 255) / 256), 256, 0, st>>>(w.type, nblk, (uint8_t *)raw, (uint8_t *)w.qs, (uint32_t *)w.qh, (uint8_t *)w.dm);
     B200_CHECK(cudaGetLastError());
 }
@@ -108,6 +115,7 @@ __global__ void get_rows_q_kernel(QWeight w, const int32_t *__restrict__ ids, fl
 }
 
 void get_rows_q(const QWeight &w, const int32_t *ids, float *dst, int64_t n, cudaStream_t st) {
+    if (w.type == T_F16) { get_rows_f16(w, ids, dst, n, st); return; }
     const int64_t threads = n * w.nb * 16;
     if (threads == 0) return;
     get_rows_q_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(w, ids, dst, n);

@@ -269,10 +269,15 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
     B200_CHECK(cudaMemsetAsync(s->hmul.get(), 0, (size_t)f * 4, st));
     quantize_act(vec_dot_type(m->hp.wtype), s->hmul.get(), f, s->xq.get(), s->xds.get(), f, 1, st);
     quantize_act_pack(m->hp.wtype, s->hmul.get(), s->xpack.get(), f, st);
+    cvt_act_f16(s->hmul.get(), f, s->xh.get(), f, 1, st);
     (void)e;
     int64_t n = 0;
     auto mv = [&](const QWeight &w, float *out) {
-        if (fast) mul_mat_vec_q(w, s->xq.get(), s->xds.get(), out, nullptr, st);
+        if (w.type == T_F16) {
+            if (mmv_f16_supported(w)) mul_mat_vec_f16(w, s->xh.get(), out, nullptr, st);
+            else mul_mat_f16_gemm(w, s->xh.get(), out, w.N, 1, nullptr, 0, st);
+        }
+        else if (fast) mul_mat_vec_q(w, s->xq.get(), s->xds.get(), out, nullptr, st);
         else if (mmv_exact_stream_supported(w)) mul_mat_vec_q_exact_stream(w, s->xpack.get(), out, nullptr, st);
         else mul_mat_q_exact(w, s->xq.get(), s->xds.get(), out, w.N, 1, nullptr, 0, st);
         n++;
@@ -292,10 +297,11 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
 }
 
 static b200_model *llama_new_impl(const b200_llama_hparams *hp, int tp_rank, int tp_world) {
-    if (!hp || !is_quant(hp->wtype) || hp->n_embd % 64 || hp->n_ff % 64 || hp->n_head <= 0 || hp->n_head_kv <= 0 ||
+    if (!hp || !is_qweight_type(hp->wtype) || hp->n_embd % 64 || hp->n_ff % 64 || hp->n_head <= 0 || hp->n_head_kv <= 0 ||
         hp->n_head % hp->n_head_kv || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0) return nullptr;
     const int G = tp_world;
     if (G < 1 || G > TP_MAX || tp_rank < 0 || tp_rank >= G) return nullptr;
+    if (G > 1 && hp->wtype == T_F16) return nullptr;      // shards decode through the fused schedule only, which is built on Q8 activation records
     const int gqa_full = hp->n_embd / (hp->n_head / hp->n_head_kv);
     // row split: whole heads per rank, 32-row pieces of w1|w3 and of the lm_head, 32-element blocks of wo / w2's output slices
     if (G > 1 && (hp->n_head % G || hp->n_head_kv % G || (hp->n_ff / G) % 32 || hp->n_ff % G || (hp->n_embd / G) % 32 || hp->n_vocab % G || (hp->n_vocab / G) % 32)) return nullptr;
@@ -317,7 +323,7 @@ static b200_model *llama_new_impl(const b200_llama_hparams *hp, int tp_rank, int
             c.q(L.wqkv, e, m->e_loc + 2 * m->gqa_loc); c.q(L.wo, e, m->e_loc); c.q(L.w13, e, 2 * m->f_loc); c.q(L.w2, hp->n_ff, m->e_loc);
         }
     });
-    m->weight_bytes -= (size_t)v * (e / QK) * ggml_block_bytes(t);   // tok_embeddings is only gathered from, never streamed
+    m->weight_bytes -= (size_t)v * (e / QK) * qweight_block_bytes(t);   // tok_embeddings is only gathered from, never streamed
     return m;
 }
 
@@ -478,6 +484,11 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     s->m = m; s->cfg = *cfg;
     if (m->tp_world > 1) return start_session_tp(s);
     const b200_llama_hparams &hp = m->hp;
+    if (hp.wtype == T_F16 && (cfg->flags & B200_SESSION_FAST)) {   // the order-free kernels take the five block formats only
+        fprintf(stderr, "llm_b200: start_session: B200_SESSION_FAST has no kernels for F16 weights\n");
+        b200_session_free(s);
+        return nullptr;
+    }
     const size_t e = hp.n_embd, f = hp.n_ff, B = cfg->n_batch, n_ctx = hp.context_size, gqa = m->gqa;
     start_common(s);
     const size_t kmax = e > f ? e : f;
@@ -513,8 +524,9 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     // n_embd <= 6144 and context_size % 128 == 0 are limits of the removed one-kernel decode, kept so that the same geometries decode through the graph.
     QWeight probe; probe.nb = (int64_t)e / QK;
     QWeight probe2; probe2.nb = (int64_t)f / QK;
+    // F16 weights decode through the per-op path (exact_f16.cu's mat-vec): the fused schedule is built on Q8 activation records.
     s->graph_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && mmv_exact_stream_supported(probe) && mmv_exact_stream_supported(probe2) &&
-                  e <= 6144 && n_ctx % 128 == 0;
+                  e <= 6144 && n_ctx % 128 == 0 && hp.wtype != T_F16;
     B200_CHECK(cudaDeviceSynchronize());   // the memsets / copies above ran on the legacy stream: order them before anything on the backend's non-blocking stream
     return s;
 }

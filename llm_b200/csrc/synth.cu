@@ -45,6 +45,12 @@ __global__ void __launch_bounds__(256) synth_q_kernel(QWeight w, uint64_t seed, 
     }
 }
 
+// F16 weights: N(0, 1/K) rounded to fp16 (RNE), element i of the matrix drawn as element i of a quantized one
+__global__ void synth_f16_kernel(__half *w, int64_t n, uint64_t seed, float sigma) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) w[i] = __float2half_rn(gauss(seed, (uint64_t)i) * sigma);
+}
+
 __global__ void synth_gain_kernel(float *g, int64_t n, uint64_t seed) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) g[i] = 1.0f + 0.1f * gauss(seed, (uint64_t)i);
@@ -53,6 +59,12 @@ __global__ void synth_gain_kernel(float *g, int64_t n, uint64_t seed) {
 void synth_qweight(const QWeight &w, uint64_t seed, cudaStream_t st) {
     const int64_t nblk = w.N * w.nb;
     if (nblk == 0) return;
+    if (w.type == T_F16) {
+        const int64_t n = w.N * w.K;
+        synth_f16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((__half *)w.qs, n, seed, 1.0f / sqrtf((float)w.K));
+        B200_CHECK(cudaGetLastError());
+        return;
+    }
     synth_q_kernel<<<(unsigned)((nblk + 7) / 8), 256, 0, st>>>(w, seed, 1.0f / sqrtf((float)w.K), nullptr);
     B200_CHECK(cudaGetLastError());
 }

@@ -73,11 +73,11 @@ class GptNeoX(_Native):
             return
         for name, arr in (tensors or {}).items():
             arr = np.ascontiguousarray(arr)
-            typ = 0 if arr.dtype == np.float32 else int(hyperparameters["wtype"])
+            typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(hyperparameters["wtype"])
             _check(self.L.b200_neox_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes), f"load_tensor({name})")
 
     def _load_lora(self, name, arr, ad):
-        typ = 0 if arr.dtype == np.float32 else int(self.hyperparameters["wtype"])
+        typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.hyperparameters["wtype"])
         nd, ne0, ne1 = ggml_dims(arr, typ)
         rc = self.L.b200_neox_load_tensor_lora(self._m, name.encode(), typ, nd, ne0, ne1, arr.ctypes.data_as(C.c_void_p), arr.nbytes, ad.handles, ad.n)
         if rc != 0:

@@ -118,6 +118,8 @@ def ggml_dims(arr: np.ndarray, wtype: int):
     """(n_dims, ne0, ne1) of a tensor given as GGML-layout block rows (uint8 [rows][row bytes]) or f32 ([n] or [rows][cols])"""
     if arr.dtype == np.float32:
         return (1, arr.shape[0], 1) if arr.ndim == 1 else (2, arr.shape[-1], arr.size // arr.shape[-1])
+    if arr.dtype == np.float16:                  # F16 weights: [rows][cols] halves
+        return 2, arr.shape[-1], arr.size // arr.shape[-1]
     block = {2: 18, 3: 20, 6: 22, 7: 24, 8: 34}[wtype]
     return 2, arr.shape[-1] // block * 32, arr.size // arr.shape[-1]
 
@@ -154,7 +156,7 @@ class Llama(_Native):
     def load_tensor(self, name: str, arr: np.ndarray, adapters: "LoraAdapters" = None, shape: tuple = None):
         """`adapters`: patch the tensor with them (LoraAdapter::patch); `shape` is then its (rows, cols) / (n,) as in llama_tensor_shapes"""
         arr = np.ascontiguousarray(arr)
-        typ = 0 if arr.dtype == np.float32 else int(self.hyperparameters["wtype"])
+        typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.hyperparameters["wtype"])
         if adapters is None:
             _check(self.L.b200_model_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes),
                    f"load_tensor({name})")
