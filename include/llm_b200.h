@@ -154,6 +154,15 @@ int  b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, fl
  * ties by ascending token id -- so that 8 k bytes cross PCIe instead of n_vocab floats */
 int  b200_session_top_k(b200_session *s, int32_t k, int32_t *ids_out, float *logits_out);
 int  b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out);
+/* InferenceSession::perplexity (crates/llm-base/src/inference_session.rs:514-589) over HOST token ids tokens[0, n), computed on the device.
+ * With C = context_size, chunk i covers [iC, (i+1)C) for i < n_chunk = n / C (n < C: zero chunks).  Each chunk is evaluated in batches of n_batch
+ * with all logits, its first token replaced by `bos` (the model's bot_token_id, else 1); rows j in [min(512, C/2), C - 1) are scored as
+ * -ln(softmax(row j)[t[iC + j + 1]]), the reference's f32 arithmetic with glibc's expf / logf, bit-exact.  The logits never leave HBM; nll (f32)
+ * runs over all chunks and ppl_out[i] = expf(nll / count) after chunk i.  terms_out (nullable): the n_chunk x (C - 1 - min(512, C/2)) terms.
+ * Deviation: every chunk starts at n_past 0 (the reference never rewinds, so its chunk 1 would run past the end of the KV cache); chunk 0 is exactly
+ * the reference's loop on a fresh session.  Afterwards n_past = C (unchanged when there are zero chunks) and the cache holds the last chunk.
+ * B200_ERR_BAD_ARG: null pointers, n < 0, bos or a token id outside [0, n_vocab), a tensor-parallel session.  B200_SESSION_FAST sessions run. */
+int  b200_session_perplexity(b200_session *s, const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out);
 /* Device-resident variant for measurements: tokens already in HBM, logits stay in HBM (no host copies, no sync) */
 int  b200_session_evaluate_device(b200_session *s, const int32_t *d_tokens, int32_t n);
 const float *b200_session_device_logits(b200_session *s);    /* [n][n_vocab] of the last evaluate */
@@ -237,6 +246,8 @@ int  b200_neox_set_n_past(b200_neox_session *s, int32_t n_past);
 int  b200_neox_read_kv(b200_neox_session *s, int32_t which, void *host_out, size_t nbytes);
 int32_t b200_neox_last_launches(const b200_neox_session *s);
 int  b200_neox_sync(b200_neox_session *s);
+/* b200_session_perplexity for every architecture of this runtime (bos: 1 for GPT-NeoX, GPT-2 and GPT-J; BLOOM's "<s>", MPT's "<|padding|>") */
+int  b200_neox_perplexity(b200_neox_session *s, const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out);
 void b200_neox_session_free(b200_neox_session *s);
 
 /* ---- single-op entry points on HOST buffers (unit tests, INTEGRATION examples).  Each uploads, runs the kernel, downloads. */
@@ -251,6 +262,8 @@ int  b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_ou
 /* LoraAdapter::patch of one adapter on host buffers: w (N rows of K, F32 or Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 GGML blocks) += scaling * ba, ba[n][k] = dot(a row k,
  * b row n), a: K rows of r (a_type 0 F32 / 1 F16), b: N rows of r f32 -- bit-exact with the reference's ggml_mul_mat / ggml_scale / ggml_add on the CPU */
 int  b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, int32_t a_type, const void *a, const float *b, int64_t r, float scaling);
+/* the scoring step of b200_session_perplexity on host rows: terms_out[r] = -ln(softmax(logits row r)[targets[r]]), `rows` rows of n_vocab f32 */
+int  b200_op_nll_rows(const float *logits, int64_t rows, int64_t n_vocab, const int32_t *targets, float *terms_out);
 enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = the exact kernel the sessions pick for B rows (the streaming mat-vec at B == 1 where K allows it, EXACT below 16, EXACT_MMA below 96, EXACT_TC5 from 96; K-quants: EXACT); TC5 = the tensor-core prefill GEMMs (the name predates the sm_90a port): wgmma/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->wgmma GEMM (mmq_tc5.cu, non-conformant) */
 
 #ifdef __cplusplus

@@ -62,6 +62,8 @@ def lib():
     L.b200_model_start_session.argtypes = [vp, C.POINTER(SessionConfig)]
     L.b200_session_evaluate.argtypes = [vp, vp, i32, vp, i32]
     L.b200_session_feed_prompt.argtypes = [vp, vp, i32, vp]
+    L.b200_session_perplexity.argtypes = [vp, vp, i64, i32, vp, vp, C.POINTER(i32)]
+    L.b200_op_nll_rows.argtypes = [vp, i64, i64, vp, vp]
     L.b200_session_top_k.argtypes = [vp, i32, vp, vp]
     L.b200_session_evaluate_device.argtypes = [vp, vp, i32]
     L.b200_session_device_logits.restype = vp

@@ -2,6 +2,7 @@
 #include <string.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/llm_b200.h"
 #include "host.h"
@@ -156,6 +157,44 @@ void SessionCore::copy_logits(float *out, const float *logits, int n, bool all_r
 int SessionCore::set_n_past(int v) {
     if (v < 0 || v > n_past) return B200_ERR_BAD_ARG;
     n_past = v;
+    return B200_OK;
+}
+
+// inference_session.rs:514-589, except that every chunk starts at n_past 0 (the reference never rewinds, so its chunk 1 would run past the end of
+// the KV cache); chunk 0 is exactly the reference's loop on a fresh session
+int SessionCore::perplexity(const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out, const float *logits,
+                            const std::function<void(int)> &forward) {
+    if ((!tokens && n > 0) || n < 0 || !n_chunk_out || bos < 0 || bos >= n_vocab) return B200_ERR_BAD_ARG;
+    for (int64_t i = 0; i < n; i++) if (tokens[i] < 0 || tokens[i] >= n_vocab) return B200_ERR_BAD_ARG;
+    const int64_t C = n_ctx, n_chunk = n / C;
+    if (n_chunk > INT32_MAX || (n_chunk > 0 && !ppl_out)) return B200_ERR_BAD_ARG;
+    *n_chunk_out = (int32_t)n_chunk;
+    if (n_chunk == 0) return B200_OK;
+    const int64_t first = C / 2 < 512 ? C / 2 : 512, scored = C - 1 > first ? C - 1 - first : 0;
+    cudaStream_t st = rt().stream;
+    DeviceBuf<int32_t> d_tok = device_alloc<int32_t>((size_t)n_chunk * C * 4);                    // the targets t[iC + j + 1]
+    DeviceBuf<float> d_terms = device_alloc<float>(((size_t)n_chunk * scored + 1) * 4), d_ppl = device_alloc<float>((size_t)n_chunk * 4);
+    DeviceBuf<PplState> state = device_alloc<PplState>(sizeof(PplState));
+    B200_CHECK(cudaMemcpyAsync(d_tok.get(), tokens, (size_t)n_chunk * C * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemsetAsync(state.get(), 0, sizeof(PplState), st));                             // nll = 0.0f, count = 0
+    std::vector<int32_t> batch(n_batch);
+    for (int64_t i = 0; i < n_chunk; i++) {
+        const int64_t start = i * C;
+        n_past = 0;
+        for (int64_t b0 = 0; b0 < C; b0 += n_batch) {
+            const int nb = (int)(C - b0 < n_batch ? C - b0 : n_batch);
+            memcpy(batch.data(), tokens + start + b0, (size_t)nb * 4);
+            if (b0 == 0) batch[0] = bos;                                                          // the chunk's first token, not each batch's
+            stage_tokens(batch.data(), nb);                                                       // ids checked above
+            forward(nb);
+            const int64_t r0 = b0 > first ? b0 : first, r1 = b0 + nb < C - 1 ? b0 + nb : C - 1;   // scored rows of this batch
+            if (r1 > r0) nll_rows(logits + (size_t)(r0 - b0) * n_vocab, r1 - r0, n_vocab, d_tok.get() + start + r0 + 1, d_terms.get() + i * scored + (r0 - first), st);
+        }
+        nll_fold(d_terms.get() + i * scored, scored, state.get(), d_ppl.get() + i, st);
+    }
+    B200_CHECK(cudaMemcpyAsync(ppl_out, d_ppl.get(), (size_t)n_chunk * 4, cudaMemcpyDeviceToHost, st));
+    if (terms_out && scored) B200_CHECK(cudaMemcpyAsync(terms_out, d_terms.get(), (size_t)n_chunk * scored * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
     return B200_OK;
 }
 

@@ -1,6 +1,7 @@
 // llm_b200/csrc/host.h -- host plumbing shared by the LLaMA (session.cu) and GPT-NeoX / GPT-2 (neox.cu) runtimes: owned device and pinned
 // buffers, the weight slab and its named tensor slots, seeded synthesis, and the state every session keeps (KV cache, token / logits staging).
 #pragma once
+#include <functional>
 #include <memory>
 #include <type_traits>
 #include <vector>
@@ -116,6 +117,12 @@ struct SessionCore {
     int stage_tokens(const int32_t *tokens, int n);   // validates the ids and uploads them to d_tokens
     void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)
     int set_n_past(int v);
+    // InferenceSession::perplexity over tokens[0, n) with C = n_ctx: chunk i = [iC, (i+1)C) is evaluated from n_past 0 in batches of n_batch, its
+    // first token replaced by bos; rows [min(512, C/2), C - 1) are scored on the device (ppl.cu).  forward(rows) runs one batch of the staged
+    // tokens at n_past and leaves every row's logits in `logits`.  Each batch's terms are computed on the stream before the next batch overwrites
+    // them.  ppl_out: n_chunk values; terms_out (nullable): n_chunk x scored rows.  n_past ends at C (unchanged when n < C).
+    int perplexity(const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out, const float *logits,
+                   const std::function<void(int)> &forward);
 };
 
 }  // namespace b200

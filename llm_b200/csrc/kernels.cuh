@@ -96,6 +96,13 @@ int lora_check(int wtype, int64_t K, int64_t N, int a_type, int64_t a_ne0, int64
 // b: nb_rows rows of r f32 (row n of W takes row n % nb_rows).  Arguments checked by lora_check.
 void lora_patch(int wtype, void *w, int64_t K, int64_t N, int a_type, const void *a, const float *b, int64_t r, int64_t nb_rows, float scaling, cudaStream_t st);
 
+// ---- ppl.cu : the reference's perplexity arithmetic on logits in HBM, bit-exact (glibc expf / logf restated in libm_f32.h) ---------------------
+// terms[r] = -ln(softmax(row r)[targets[r]]) of `rows` rows of n_vocab logits: max, in-order f32 sum of expf(v - max), expf(l[t] - max) / sum
+void nll_rows(const float *logits, int64_t rows, int64_t n_vocab, const int32_t *targets, float *terms, cudaStream_t st);
+struct PplState { float nll; int64_t count; };        // the running f32 nll and row count of one perplexity call (device memory)
+// state += terms[0..n) in order; *ppl = expf(nll / (f32)count)
+void nll_fold(const float *terms, int64_t n, PplState *state, float *ppl, cudaStream_t st);
+
 // ---- rowops.cu : warp/block-reduce kernels ------------------------------------------------------------------------
 struct Luts { const uint16_t *silu, *gelu, *exp; };   // 3 x 64 Ki fp16 tables built on the host with libm (LC/ggml.c:4313-4326)
 const Luts &luts();                                   // uploaded on first use

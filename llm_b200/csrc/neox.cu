@@ -449,6 +449,11 @@ int b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, f
     return B200_OK;
 }
 
+int b200_neox_perplexity(b200_neox_session *s, const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out) {
+    if (!s) return B200_ERR_BAD_ARG;
+    return s->perplexity(tokens, n, bos, ppl_out, terms_out, n_chunk_out, s->logits.get(), [s](int rows) { forward(s, rows, true); });
+}
+
 void b200_neox_session_free(b200_neox_session *s) {
     if (!s) return;
     B200_CHECK(cudaStreamSynchronize(rt().stream));

@@ -192,6 +192,21 @@ int b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, 
     return B200_OK;
 }
 
+int b200_op_nll_rows(const float *logits, int64_t rows, int64_t n_vocab, const int32_t *targets, float *terms_out) {
+    if (!logits || !targets || !terms_out || rows < 1 || rows > INT32_MAX || n_vocab < 1) return B200_ERR_BAD_ARG;
+    for (int64_t r = 0; r < rows; r++) if (targets[r] < 0 || targets[r] >= n_vocab) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    float *dl = (float *)R.op_arena.get((size_t)rows * n_vocab * 4, st), *dt = (float *)R.op_arena.get((size_t)rows * 4, st);
+    int32_t *dtg = (int32_t *)R.op_arena.get((size_t)rows * 4, st);
+    B200_CHECK(cudaMemcpyAsync(dl, logits, (size_t)rows * n_vocab * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(dtg, targets, (size_t)rows * 4, cudaMemcpyHostToDevice, st));
+    nll_rows(dl, rows, n_vocab, dtg, dt, st);
+    B200_CHECK(cudaMemcpyAsync(terms_out, dt, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
 // Kernel-only timing of one weight mat-mul on device-resident synthetic operands (seeded random weights and activations): used by
 // tools/prefill_gemm_bench.py and bench.py's prefill roofline; impl = B200_MM_EXACT_MMA / B200_MM_EXACT_TC5 / B200_MM_TENSOR
 int b200_op_bench_mul_mat(int32_t wtype, int64_t K, int64_t N, int64_t B, int32_t impl, int32_t iters, float *ms_out) {

@@ -563,6 +563,12 @@ int b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, flo
     return B200_OK;
 }
 
+// InferenceSession::perplexity (SessionCore::perplexity): tensor-parallel sessions are refused, FAST sessions run (their logits are not the reference's)
+int b200_session_perplexity(b200_session *s, const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out) {
+    if (!s || s->m->tp_world > 1) return B200_ERR_BAD_ARG;
+    return s->perplexity(tokens, n, bos, ppl_out, terms_out, n_chunk_out, s->logits.get(), [s](int rows) { forward(s, rows); });
+}
+
 // Sampler hand-off (SURVEY.md §8f-3): the k largest logits of the last evaluated row, selected on the device; 8 k bytes cross PCIe instead of
 // n_vocab floats.  Order = descending logit, ties by ascending token id (what a stable descending sort of (id, logit) pairs yields: llm-samplers top-k).
 int b200_session_top_k(b200_session *s, int32_t k, int32_t *ids_out, float *logits_out) {

@@ -7,12 +7,12 @@
   InferenceSession        crates/llm-base/src/inference_session.rs     evaluate / n_past / rewind
 No arithmetic happens in Python."""
 import ctypes as C
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
-from .session import LoraAdapters, _check, _Native, ggml_dims
+from .session import LoraAdapters, _check, _Native, _perplexity, ggml_dims
 
 
 class NeoxHparams(C.Structure):
@@ -42,6 +42,7 @@ def _bind(L):
     L.b200_neox_read_kv.argtypes = [vp, i32, vp, C.c_size_t]
     L.b200_neox_last_launches.argtypes = [vp]
     L.b200_neox_sync.argtypes = [vp]
+    L.b200_neox_perplexity.argtypes = [vp, vp, C.c_int64, i32, vp, vp, C.POINTER(i32)]
     L.b200_neox_session_free.argtypes = [vp]
     L._neox_ready = True
     return L
@@ -54,11 +55,15 @@ class GptNeoX(_Native):
     ARCH = 0
     _HANDLE, _FREE = "_m", "b200_neox_free"
 
+    BOT_TOKEN: Optional[bytes] = None       # the vocabulary entry bot_token_id() names (MPT, BLOOM); None: the model has no BOS token
+
     def __init__(self, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray] = None, context_size: int = None, device: int = 0,
-                 lora_adapters: Optional[List[str]] = None):
+                 lora_adapters: Optional[List[str]] = None, vocabulary: Optional[Sequence] = None):
+        """vocabulary: the model file's tokens (GgmlFile.vocabulary(): (bytes, score) pairs, or bytes), consulted by bot_token_id()"""
         self.L = _bind(_lib.lib())
         _check(self.L.b200_init(device), "b200_init")
         self.hyperparameters = dict(hyperparameters)
+        self.vocabulary = [t[0] if isinstance(t, tuple) else bytes(t) for t in vocabulary] if vocabulary is not None else None
         self.context_size = context_size or hyperparameters["n_ctx"]
         hp = NeoxHparams(n_vocab=hyperparameters["n_vocab"], n_embd=hyperparameters["n_embd"], n_head=hyperparameters["n_head"], n_layer=hyperparameters["n_layer"],
                          n_rot=int(hyperparameters.get("n_rot", 0)), use_parallel_residual=int(hyperparameters.get("use_parallel_residual", 1)), wtype=hyperparameters["wtype"],
@@ -97,6 +102,16 @@ class GptNeoX(_Native):
     def start_session(self, n_batch: int = 8) -> "NeoxSession":
         return NeoxSession(self, n_batch)
 
+    def bot_token_id(self) -> Optional[int]:
+        """KnownModel::bot_token_id: GPT-NeoX, GPT-2 and GPT-J have none; MPT's is "<|padding|>" and BLOOM's "<s>" when the vocabulary has it
+        (mpt lib.rs:273-275, bloom lib.rs:356-358).  Without a vocabulary there is nothing to look up: None."""
+        if self.BOT_TOKEN is None or self.vocabulary is None:
+            return None
+        try:
+            return self.vocabulary.index(self.BOT_TOKEN)
+        except ValueError:
+            return None
+
 
 class Gpt2(GptNeoX):
     """KnownModel for GPT-2 (crates/models/gpt2/src/lib.rs): hyperparameters n_vocab, n_ctx, n_embd, n_head, n_layer, wtype; tensors "model/wte",
@@ -110,6 +125,7 @@ class Mpt(GptNeoX):
     clip_kqv is read by the reference but never applied); tensors "transformer.wte.weight" (also the output projection), "transformer.norm_f.weight",
     "transformer.blocks.N.{norm_1,norm_2}.weight", "transformer.blocks.N.attn.{Wqkv,out_proj}.weight", "transformer.blocks.N.ffn.{up_proj,down_proj}.weight"."""
     ARCH = 2
+    BOT_TOKEN = b"<|padding|>"
 
     def _alibi_bias_max(self):
         return float(self.hyperparameters["alibi_bias_max"])
@@ -123,6 +139,7 @@ class Bloom(Mpt):
     tensors "tok_embeddings.weight", "norm.{weight,bias}", "output_norm.{weight,bias}", "output.weight", "layers.N.{attention_norm,ffn_norm}.{weight,bias}",
     "layers.N.attention.{query_key_value,wo}.{weight,bias}", "layers.N.feed_forward.{w1,w2}.{weight,bias}"."""
     ARCH = 3
+    BOT_TOKEN = b"<s>"
 
     def _alibi_bias_max(self):
         return 8.0
@@ -158,6 +175,12 @@ class NeoxSession(_Native):
         out = np.empty((tokens.size if all_logits else 1, self.n_vocab), np.float32)
         _check(self.L.b200_neox_evaluate(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size, out.ctypes.data_as(C.c_void_p), 1 if all_logits else 0), "evaluate")
         return out if all_logits else out[0]
+
+    def perplexity(self, tokens, callback=None, bos: Optional[int] = None, return_terms: bool = False):
+        """InferenceSession::perplexity on the device (see InferenceSession.perplexity); bos defaults to bot_token_id() or 1"""
+        bot = self.model.bot_token_id()
+        bos = (1 if bot is None else bot) if bos is None else bos
+        return _perplexity(self.L.b200_neox_perplexity, self._s, tokens, bos, self.model.context_size, callback, return_terms)
 
     def rewind(self, n_past: int):
         _check(self.L.b200_neox_set_n_past(self._s, n_past), "rewind")

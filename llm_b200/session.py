@@ -66,6 +66,25 @@ def _check(rc, what):
         raise RuntimeError(f"{what} failed with code {rc}")
 
 
+def _perplexity(entry, handle, tokens, bos: int, context_size: int, callback, return_terms: bool):
+    """InferenceSession::perplexity through b200_session_perplexity / b200_neox_perplexity: the per-chunk perplexities (and, with return_terms,
+    the [n_chunk, scored rows] -ln p terms); callback(chunk, ppl) is called for each chunk in order, as the reference's perplexity_callback"""
+    tokens = np.ascontiguousarray(tokens, np.int32).ravel()
+    n_chunk_max = tokens.size // context_size
+    first = min(512, context_size // 2)
+    scored = max(context_size - 1 - first, 0)
+    ppl = np.empty(max(n_chunk_max, 1), np.float32)
+    terms = np.empty((max(n_chunk_max, 1), max(scored, 1)), np.float32)
+    n_chunk = C.c_int32(0)
+    _check(entry(handle, tokens.ctypes.data_as(C.c_void_p), tokens.size, int(bos), ppl.ctypes.data_as(C.c_void_p),
+                 terms.ctypes.data_as(C.c_void_p) if return_terms else None, C.byref(n_chunk)), "perplexity")
+    out = [float(p) for p in ppl[:n_chunk.value]]
+    if callback is not None:
+        for i, p in enumerate(out):
+            callback(i, p)
+    return (out, terms[:n_chunk.value, :scored]) if return_terms else out
+
+
 class _Native:
     """Owner of one native handle (attribute `_HANDLE`, released by the library function `_FREE`): close() frees it once, and so does
     garbage collection."""
@@ -190,6 +209,10 @@ class Llama(_Native):
     def context_size(self) -> int:
         return self.params.context_size
 
+    def bot_token_id(self) -> Optional[int]:
+        """KnownModel::bot_token_id: LLaMA has none (llama lib.rs:382-384)"""
+        return None
+
 
 class InferenceSession(_Native):
     _HANDLE, _FREE = "_s", "b200_session_free"
@@ -233,6 +256,14 @@ class InferenceSession(_Native):
                                                out.ctypes.data_as(C.c_void_p)), "feed_prompt")
         self.last_logits = out
         return out
+
+    def perplexity(self, tokens, callback=None, bos: Optional[int] = None, return_terms: bool = False):
+        """InferenceSession::perplexity on token ids (tokenization is the caller's), computed on the device: one perplexity per chunk of
+        context_size tokens, callback(chunk, ppl) after each.  bos replaces each chunk's first token (default: bot_token_id() or 1).  Every chunk
+        starts at n_past 0; afterwards n_past is context_size (unchanged when there are fewer tokens than that).  See include/llm_b200.h."""
+        bot = self.model.bot_token_id()
+        bos = (1 if bot is None else bot) if bos is None else bos
+        return _perplexity(self.L.b200_session_perplexity, self._s, tokens, bos, self.model.params.context_size, callback, return_terms)
 
     def rewind(self, n_past: int):
         _check(self.L.b200_session_set_n_past(self._s, n_past), "rewind")
