@@ -8,7 +8,8 @@
  *   ModelParameters                 crates/llm-base/src/model/mod.rs:197-229   (context_size, rope overrides)
  *   KnownModel::new / TensorLoader  crates/models/llama/src/lib.rs:43-140      (tensor names "layers.N.attention.wq.weight", ...)
  *   KnownModel::start_session       crates/models/llama/src/lib.rs:130-141  -> InferenceSession::new (inference_session.rs:114-217)
- *   InferenceSessionConfig          crates/llm-base/src/inference_session.rs:799-841 (n_batch; KV cache is f16)
+ *   InferenceSessionConfig          crates/llm-base/src/inference_session.rs:799-841 (n_batch; memory_k_type / memory_v_type: f16, or f32 with
+ *                                   B200_SESSION_KV_F32 -- the CLI's --no-float16)
  *   Model::evaluate + OutputRequest crates/models/llama/src/lib.rs:144-368, crates/llm-base/src/model/common.rs:6-39
  *   InferenceSession::feed_prompt   crates/llm-base/src/inference_session.rs:299-350 (chunks of n_batch, ContextFull)
  *
@@ -51,7 +52,12 @@ enum {
     B200_SESSION_UNFUSED  = 2,     /* decode with the prefill schedule (one kernel per reference graph node, the seam's kernels) */
     B200_SESSION_FAST     = 4,     /* order-free kernels: integer-exact block dots but a different f32 summation order than the
                                       reference's AVX2 build.  NOT conformant: the reference graph amplifies 1e-7 differences to ~1e-2
-                                      in the logits (DESIGN.md "chaos").  Default (flag clear) = bit-exact kernels. */
+                                      in the logits (DESIGN.md "chaos").  Default (flag clear) = bit-exact kernels.  The attention on an
+                                      f32 cache stays exact: only the weight mat-muls go order-free. */
+    B200_SESSION_KV_F32   = 8,     /* memory_k and memory_v are GGML_TYPE_F32 (InferenceSessionConfig::memory_k_type = memory_v_type = Float32,
+                                      the reference CLI's --no-float16): twice the bytes, no fp16 rounding of K, V, Q or the probabilities;
+                                      the attention is ggml_vec_dot_f32, bit-exact.  Clear (or a zero-initialised config): f16.
+                                      NULL from start_session on a tensor-parallel model. */
 };
 
 enum {                            /* return codes (0 = ok).  CUDA failures print and exit(1) like the reference backend. */
@@ -168,7 +174,8 @@ int  b200_session_evaluate_device(b200_session *s, const int32_t *d_tokens, int3
 const float *b200_session_device_logits(b200_session *s);    /* [n][n_vocab] of the last evaluate */
 int32_t b200_session_n_past(const b200_session *s);
 int  b200_session_set_n_past(b200_session *s, int32_t n_past);   /* rewind (supports_rewind, llama lib.rs:396-398) */
-/* raw f16 KV cache bytes (get_snapshot, inference_session.rs:599-646): which = 0 memory_k, 1 memory_v */
+/* raw KV cache bytes (get_snapshot, inference_session.rs:599-646): which = 0 memory_k, 1 memory_v; 2 bytes per element (f16), 4 with
+ * B200_SESSION_KV_F32 (f32), same layout */
 int  b200_session_read_kv(b200_session *s, int32_t which, void *host_out, size_t nbytes);
 int  b200_session_sync(b200_session *s);
 /* tuning aid (B200_DECODE_PROF=1): per-launch %globaltimer stamps of the graph decode schedule; out = 8*n values, see session.cu */
@@ -237,12 +244,15 @@ int  b200_neox_load_tensor_lora(b200_neox_model *m, const char *name, int32_t ty
 int  b200_neox_synthesize(b200_neox_model *m, uint64_t seed);          /* seeded weights generated in HBM (bench) */
 size_t b200_neox_weight_bytes(b200_neox_model *m);                     /* bytes streamed per decoded token */
 void b200_neox_free(b200_neox_model *m);
-b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch);
+b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch);                     /* the flags = 0 form of the next */
+/* flags: 0 (f16 KV cache) or B200_SESSION_KV_F32 (f32 cache, bit-exact with the reference's F32 memory_k / memory_v); NULL for any other flag */
+b200_neox_session *b200_neox_start_session_flags(b200_neox_model *m, int32_t n_batch, int32_t flags);
 int  b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits);
 int  b200_neox_evaluate_device(b200_neox_session *s, int32_t n);       /* tokens of the last evaluate stay in HBM, logits stay in HBM */
 int32_t b200_neox_n_past(const b200_neox_session *s);
 int  b200_neox_set_n_past(b200_neox_session *s, int32_t n_past);
-/* raw f16 KV cache bytes, which = 0 memory_k [n_layer][n_ctx][n_embd], 1 memory_v [n_layer][n_embd][n_ctx] (V by channel, also for GPT-2) */
+/* raw KV cache bytes (2 per element for f16, 4 for an f32 cache), which = 0 memory_k [n_layer][n_ctx][n_embd], 1 memory_v [n_layer][n_embd][n_ctx]
+ * (V by channel, also for GPT-2) */
 int  b200_neox_read_kv(b200_neox_session *s, int32_t which, void *host_out, size_t nbytes);
 int32_t b200_neox_last_launches(const b200_neox_session *s);
 int  b200_neox_sync(b200_neox_session *s);

@@ -6,7 +6,7 @@ The product is the C-ABI shared library llm_b200/libllm_b200.so (sources in llm_
 This Python package is only the host-side mirror of that interface over ctypes (tests, bench.py); it contains no
 arithmetic and no fallback path.
 """
-from .session import ContextFull, InferenceSession, InferenceSessionConfig, Llama, ModelParameters, OutputRequest  # noqa: F401
+from .session import ContextFull, InferenceSession, InferenceSessionConfig, Llama, ModelKVMemoryType, ModelParameters, OutputRequest  # noqa: F401
 from . import ggml  # noqa: F401
 
 # enum ggml_type values of the five block formats on the hot path (LC/ggml.h:262-285)

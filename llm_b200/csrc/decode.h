@@ -16,7 +16,7 @@ namespace b200 {
 struct DecodeLayer {
     QWeight wqkv, wo, w13, w2;
     const float *attn_norm, *ffn_norm;
-    __half *K, *V;                      // this layer's slice of memory_k ([n_ctx][gqa]) / memory_v ([gqa][n_ctx], transposed)
+    void *K, *V;                        // this layer's slice of memory_k ([n_ctx][gqa]) / memory_v ([gqa][n_ctx], transposed), of DecodeParams::kv_type
 };
 
 struct DecodeParams {
@@ -25,6 +25,7 @@ struct DecodeParams {
     const float *norm;
     int e, f, hd, gqa, n_head, n_head_kv, n_ctx, n_vocab;
     float kq_scale, eps;
+    int kv_type;                        // the KV cache's element type: T_F16 or T_F32 (single GPU only)
     const float2 *rope_cs; int rope_half;
     const uint16_t *lut_silu, *lut_exp;
     const int32_t *token;
@@ -44,13 +45,15 @@ struct DecodeParams {
 struct NeoxLayer {
     QWeight wqkv, wdense, wfc, wproj;   // query_key_value [3e x e] (rows per head: q | k | v), attention.dense, mlp.dense_h_to_4h, mlp.dense_4h_to_h
     const float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj;
-    __half *K, *V;                      // [n_ctx][e] by position / [e][n_ctx] transposed, as the reference lays out memory_k / memory_v (:233-247)
+    void *K, *V;                        // [n_ctx][e] by position / [e][n_ctx] transposed, as the reference lays out memory_k / memory_v (:233-247),
+                                        // of NeoxParams::kv_type
 };
 // where q / k / v of head h start inside a row of the fused qkv projection: h * head_stride, + k_off, + v_off.  GPT-NeoX: per head [q | k | v]
 // (3 hd, hd, 2 hd); GPT-2, MPT, BLOOM, GPT-J: the three thirds of the row (hd, e, 2 e)
 struct QkvLayout { int head_stride, k_off, v_off; };
 struct NeoxParams {
     int n_layer, e, hd, n_head, n_ctx, n_vocab, parallel_residual;
+    int kv_type;                                // the KV cache's element type: T_F16 or T_F32
     int n_rot;                                  // RoPE mode 2 (GPT-NeoX) on n_rot of every head; 0: no mode-2 rotation
     QkvLayout qkv_layout;
     const float *wpe;                           // GPT-2 (crates/models/gpt2/src/lib.rs:138-329): learned positions [n_ctx][e] f32, else nullptr
@@ -78,8 +81,13 @@ void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &laye
 bool neox_decode_fits(const NeoxParams &P, int n_kv_bucket);
 
 // whether attn_fused_kernel's shared memory for a context bucket of n_kv_bucket positions (rounded up to 64) and head size hd fits the 227 KB
-// opt-in limit: true up to 3264 positions for every hd <= 256.  Past it LLaMA decodes with the two-kernel attention and the GPT-NeoX family per op.
-bool attn_fused_fits(int n_kv_bucket, int hd);
+// opt-in limit: true up to 3264 positions for every hd <= 256 with an f16 cache (kv_type T_F16), up to 1664 with an f32 cache (T_F32: f32
+// probabilities and V rows, 136 bytes per position instead of 70), so 256-position buckets up to 1536.  Past it LLaMA decodes with the two-kernel
+// attention and the GPT-NeoX family per op.
+bool attn_fused_fits(int n_kv_bucket, int hd, int kv_type = T_F16);
+// the longest context (27520 positions) whose scores, f32 probabilities and V tiles the two-kernel attention of an f32 cache holds in one CTA's
+// shared memory; LLaMA sessions with an f32 cache and a longer context decode per op
+int attn_sv_f32_max_ctx();
 
 // default decode schedule: 8 fused kernels per layer on `st` (decode_ops.cu); position read from *P.n_past on the device
 void decode_ops_enqueue(const DecodeParams &P, const std::vector<DecodeLayer> &layers, int wtype, int n_kv_bucket, int4 *xpack_a, cudaStream_t st, int *launches);

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "decode.h"
+#include "f32dot.cuh"
 #include "stream_core.cuh"
 #include "tp.cuh"
 
@@ -144,8 +145,8 @@ __global__ void __launch_bounds__(256) norm_pack_tp_kernel(const float *__restri
 }
 
 // ---- mat-vec with fused epilogues --------------------------------------------------------------------------------------------------
-// BIAS / GELU: GPT-NeoX (bias adds, gelu table); GELU_NB: gelu without a bias node (MPT)
-enum { EPI_RES = 0, EPI_QKV = 1, EPI_SILU = 2, EPI_LOGITS = 3, EPI_BIAS = 4, EPI_GELU = 5, EPI_GELU_NB = 6 };
+// BIAS / GELU: GPT-NeoX (bias adds, gelu table); GELU_NB: gelu without a bias node (MPT); QKV_F32: EPI_QKV storing K / V into an f32 cache
+enum { EPI_RES = 0, EPI_QKV = 1, EPI_SILU = 2, EPI_LOGITS = 3, EPI_BIAS = 4, EPI_GELU = 5, EPI_GELU_NB = 6, EPI_QKV_F32 = 7 };
 
 struct MmvArgs {
     const int4 *xpack;            // input records
@@ -153,11 +154,11 @@ struct MmvArgs {
     // Two pointer groups that no launch uses together share their 32 bytes: the argument block (QWeight 72 B + this struct) then stays within four 64-byte
     // lines of the constant bank (248 B; 280 B with both groups, one more line read on every launch of the decode graph).
     union {
-        struct { float *q; __half *K, *V; const float2 *rope_cs; };                            // EPI_QKV (LLaMA: RoPE + KV store)
+        struct { float *q; void *K, *V; const float2 *rope_cs; };                              // EPI_QKV / EPI_QKV_F32 (LLaMA: RoPE + KV store)
         // EPI_BIAS: dst = ((W x + bias) [+ add1]) [+ add2] in that order (ggml_add nodes of gptneox lib.rs:200,302,308-325); EPI_GELU: gelu(W x + bias) quantized
         struct { const float *bias, *add1, *add2; const uint16_t *lut_gelu; };
     };
-    int rope_half, hd, e, gqa, n_ctx; const int *n_past;                                      // EPI_QKV
+    int rope_half, hd, e, gqa, n_ctx; const int *n_past;                                      // EPI_QKV / EPI_QKV_F32
     // EPI_SILU
     int4 *xpack_out; const uint16_t *lut_silu;
     int q81, off, scale16;
@@ -222,7 +223,7 @@ __global__ void __launch_bounds__(STHREADS) mmv_fused_kernel(const QWeight w, co
             } else A.dst[g] = A.addend ? __fadd_rn(v, __ldcg(A.addend + g)) : v;
         }, 1, A.prof);
         if (EPI == EPI_LOGITS && blockIdx.x == 0 && tid == 0) *A.n_past_inc = *A.n_past_inc + 1;
-    } else if (EPI == EPI_QKV) {
+    } else if (EPI == EPI_QKV || EPI == EPI_QKV_F32) {
         const int p = __ldcg(A.n_past);
         consume_matvec<TYPE>(w, sx, R, blockIdx.x, gridDim.x, tid, [&](int64_t row, float v) {
             const float other = __shfl_xor_sync(0xffffffffu, v, 4);              // rotation partner: rows 2i, 2i+1 sit in adjacent quads
@@ -234,9 +235,11 @@ __global__ void __launch_bounds__(STHREADS) mmv_fused_kernel(const QWeight w, co
                 const float x0 = even ? v : other, x1 = even ? other : v;
                 const float out = even ? __fmaf_rn(x0, cs.x, -__fmul_rn(x1, cs.y)) : __fmaf_rn(x0, cs.y, __fmul_rn(x1, cs.x));
                 if (row < A.e) A.q[row] = out;
-                else A.K[(int64_t)p * A.gqa + within] = __float2half_rn(out);
+                else if (EPI == EPI_QKV) ((__half *)A.K)[(int64_t)p * A.gqa + within] = __float2half_rn(out);
+                else ((float *)A.K)[(int64_t)p * A.gqa + within] = out;
             } else {
-                A.V[(int64_t)(row - A.e - A.gqa) * A.n_ctx + p] = __float2half_rn(v);
+                if (EPI == EPI_QKV) ((__half *)A.V)[(int64_t)(row - A.e - A.gqa) * A.n_ctx + p] = __float2half_rn(v);
+                else ((float *)A.V)[(int64_t)(row - A.e - A.gqa) * A.n_ctx + p] = v;
             }
         });
     } else if (EPI == EPI_BIAS) {
@@ -319,6 +322,44 @@ __global__ void __launch_bounds__(128) attn_kq_kernel(const float *__restrict__ 
         for (int k = 0; k < HD; k += 32) s = __fmaf_rn(__half2float(krow[k + lane]), __half2float(q16[k + lane]), s);
         s = f16dot_tree(s);
         if (lane == 0) kq[(int64_t)h * n_ctx + j0 + jj] = (float)(double)s;
+    }
+    prof_end(prof);
+}
+
+// the f32 cache's form: K rows and q as they are (ggml_vec_dot_f32: the chains and tree of the f16 dot; hd % 32 == 0 leaves no leftovers)
+template <int HD>
+__global__ void __launch_bounds__(128) attn_kq_f32_kernel(const float *__restrict__ q, const float *__restrict__ Kl, float *__restrict__ kq,
+                                                          const int *__restrict__ n_past, int gqa, int n_head, int n_head_kv, int n_ctx, unsigned long long *prof) {
+    __shared__ __align__(16) float qs[HD];
+    __shared__ __align__(16) float kt[64 * HD];
+    pdl_trigger();
+    pdl_wait();
+    prof_begin(prof);
+    const int n_kv = __ldcg(n_past) + 1;
+    const int j0 = blockIdx.x * 64, h = blockIdx.y;
+    if (j0 >= n_kv) return;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int hk = h / (n_head / n_head_kv);
+    const int rows = n_kv - j0 < 64 ? n_kv - j0 : 64;
+    constexpr int VPR = HD / 4;                       // 16-byte vectors per K row
+    constexpr int NV = 64 * VPR / 128;                // vectors per thread
+    int4 v[NV];
+#pragma unroll
+    for (int u = 0; u < NV; u++) {
+        const int i = tid + u * 128, rr = i / VPR, cc = i % VPR;
+        v[u] = rr < rows ? __ldcg((const int4 *)(Kl + (int64_t)(j0 + rr) * gqa + hk * HD) + cc) : make_int4(0, 0, 0, 0);
+    }
+    for (int i = tid; i < HD; i += 128) qs[i] = __ldcg(q + h * HD + i);
+#pragma unroll
+    for (int u = 0; u < NV; u++) ((int4 *)kt)[tid + u * 128] = v[u];
+    __syncthreads();
+    for (int jj = warp; jj < rows; jj += 4) {
+        const float *krow = kt + jj * HD;
+        float s = 0.f;
+#pragma unroll
+        for (int k = 0; k < HD; k += 32) s = __fmaf_rn(krow[k + lane], qs[k + lane], s);
+        s = f16dot_tree(s);                           // GGML_F32x8_REDUCE, the tree both dots share
+        if (lane == 0) kq[(int64_t)h * n_ctx + j0 + jj] = s;
     }
     prof_end(prof);
 }
@@ -415,6 +456,103 @@ __global__ void __launch_bounds__(128) attn_sv_kernel(const float *__restrict__ 
     prof_end(prof);
 }
 
+
+// the f32 cache's form: probabilities kept f32, V tiles of KC_F32 = 64 positions (the same 16 KB and 4 vectors per thread as the f16 kernel's
+// 128), leftovers added in float (f32dot.cuh).  Dynamic shared memory: scores and probabilities, a V tile, 32 leftover columns -- it holds the
+// context of n_ctx positions up to attn_sv_f32_max_ctx()
+constexpr int KC_F32 = KC / 2;
+constexpr size_t attn_sv_f32_smem(int n_ctx) { return (size_t)n_ctx * 8 + (size_t)(32 * KC_F32 + 32 * 32) * 4; }
+__global__ void __launch_bounds__(128) attn_sv_f32_kernel(const float *__restrict__ kq, const float *__restrict__ Vl, int4 *__restrict__ xpack_out,
+                                                          const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp, float kq_scale,
+                                                          int hd, int n_head, int n_head_kv, int n_ctx, int q81, int off, int scale16, unsigned long long *prof) {
+    constexpr int TC = KC_F32;
+    constexpr int VL = 8;                             // 16-byte vectors of 32 positions
+    extern __shared__ __align__(16) uint8_t sm[];
+    __shared__ double shd[8];
+    __shared__ float shf[4], stash[32];
+    pdl_trigger();
+    pdl_wait();
+    prof_begin(prof);
+    const int n_kv = __ldcg(n_past) + 1;
+    const int per_head = hd / 32, h = blockIdx.x / per_head, c0 = (blockIdx.x - h * per_head) * 32;
+    const int hk = h / (n_head / n_head_kv);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    float *sc = (float *)sm;
+    float *p = (float *)(sm + (size_t)n_ctx * 4);
+    float *vt = (float *)(sm + (size_t)n_ctx * 8);
+    float *vleft = vt + 32 * TC;
+    // leftover V columns and the first V tile are requested before anything else so that their latency hides behind the soft_max
+    const int np = n_kv & ~31;
+    if (np < n_kv) {
+#pragma unroll
+        for (int i = tid; i < 32 * VL; i += 128) ((int4 *)vleft)[i] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + i / VL) * n_ctx + np) + i % VL);
+    }
+    constexpr int TV = TC / 4;                        // 16-byte vectors per row of a tile
+    int4 pre[32 * TV / 128];
+    auto fetch = [&](int k0) {
+#pragma unroll
+        for (int u = 0; u < 32 * TV / 128; u++) {
+            const int i = tid + u * 128, rr = i / TV, cc = i - rr * TV;
+            pre[u] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + rr) * n_ctx + k0) + cc);
+        }
+    };
+    if (np > 0) fetch(0);
+    float mx = -INFINITY;
+    constexpr int SB = 8;                              // scores per thread per pass: 8 loads in flight
+    for (int jb = 0; jb < n_kv; jb += SB * 128) {
+        float sv[SB];
+#pragma unroll
+        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; sv[u] = j < n_kv ? __ldcg(kq + (int64_t)h * n_ctx + j) : 0.f; }
+#pragma unroll
+        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; if (j < n_kv) { const float v = __fmul_rn(sv[u], kq_scale); sc[j] = v; mx = fmaxf(mx, v); } }
+    }
+    mx = warp_max(mx);
+    if (lane == 0) shf[warp] = mx;
+    __syncthreads();
+    mx = fmaxf(fmaxf(shf[0], shf[1]), fmaxf(shf[2], shf[3]));
+    double s = 0.0;
+    for (int jb = 0; jb < n_kv; jb += SB * 128) {
+        uint16_t ev16[SB];
+#pragma unroll
+        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; ev16[u] = j < n_kv ? __ldg(lut_exp + f32_to_f16_bits(__fsub_rn(sc[j], mx))) : (uint16_t)0; }
+#pragma unroll
+        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; if (j < n_kv) { const float ev = f16_bits_to_f32(ev16[u]); sc[j] = ev; s += (double)ev; } }
+    }
+    s = warp_sum(s);
+    if (lane == 0) shd[warp] = s;
+    __syncthreads();
+    const float inv = (float)(1.0 / ((shd[0] + shd[1]) + (shd[2] + shd[3])));
+    for (int j = tid; j < n_kv; j += 128) p[j] = __fmul_rn(sc[j], inv);             // the probabilities stay f32
+    float acc[8];
+#pragma unroll
+    for (int cc = 0; cc < 8; cc++) acc[cc] = 0.f;
+    for (int k0 = 0; k0 < np; k0 += TC) {
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < 32 * TV / 128; u++) ((int4 *)vt)[tid + u * 128] = pre[u];
+        __syncthreads();
+        if (k0 + TC < np) fetch(k0 + TC);
+        const int kend = np - k0 < TC ? np - k0 : TC;
+#pragma unroll
+        for (int cc = 0; cc < 8; cc++) {
+            const float *vrow = vt + (warp * 8 + cc) * TC;
+            for (int k = lane; k < kend; k += 32) acc[cc] = __fmaf_rn(vrow[k], p[k0 + k], acc[cc]);
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int cc = 0; cc < 8; cc++) {
+        const float a = f16dot_tree(acc[cc]);
+        if (lane == 0) {
+            const float *vrow = vleft + (warp * 8 + cc) * 32;
+            stash[warp * 8 + cc] = f32_leftovers(a, n_kv - np, [&](int i) { return vrow[i]; }, [&](int i) { return p[np + i]; });
+        }
+    }
+    __syncthreads();
+    if (warp == 0) pack_quad(((const float4 *)stash)[lane & 7], xpack_out + (int64_t)((h * hd + c0) / QK) * 4, lane, lane < 8, q81, off, scale16);
+    prof_end(prof);
+}
+
 // ---- 3+4 fused: KQ, scale, soft_max, KQV and the quantize epilogue for one head, as ONE cluster of hd/32 CTAs ----------------------------
 // CTA `part` of the cluster owns 32 channels of the head (its V rows are staged by cp.async at kernel entry, long before they are needed)
 // and 1/(hd/32) of the cached positions for KQ; the scaled scores are written straight into every CTA's shared memory (DSMEM) and one
@@ -439,16 +577,25 @@ __device__ __forceinline__ void fma8(float (&acc)[8], const int4 &a, const int4 
         acc[2 * e] = __fmaf_rn(af.x, bf.x, acc[2 * e]); acc[2 * e + 1] = __fmaf_rn(af.y, bf.y, acc[2 * e + 1]);
     }
 }
+// the f32 cache's form: chains 8u..8u+7 of a 32-element step are two 16-byte vectors of each operand
+__device__ __forceinline__ void fma8(float (&acc)[8], const int4 &a0, const int4 &a1, const float4 &b0, const float4 &b1) {
+    const float4 x0 = *(const float4 *)&a0, x1 = *(const float4 *)&a1;
+    acc[0] = __fmaf_rn(x0.x, b0.x, acc[0]); acc[1] = __fmaf_rn(x0.y, b0.y, acc[1]); acc[2] = __fmaf_rn(x0.z, b0.z, acc[2]); acc[3] = __fmaf_rn(x0.w, b0.w, acc[3]);
+    acc[4] = __fmaf_rn(x1.x, b1.x, acc[4]); acc[5] = __fmaf_rn(x1.y, b1.y, acc[5]); acc[6] = __fmaf_rn(x1.z, b1.z, acc[6]); acc[7] = __fmaf_rn(x1.w, b1.w, acc[7]);
+}
 
 //
 // ALIBI (MPT, BLOOM): the score of key position j in head h is fma(j, slope[h], kq * kq_scale) -- ggml_alibi (LC/ggml.c:11534-11597) on the
 // scaled scores, one fused multiply-add as the reference's x86 build compiles it; the slopes come from alibi_slopes() on the host.
 //
-// NV: the most 16-byte chunks per position and quad thread (hd / 32).  4 serves hd <= 128 (clusters of up to 4 CTAs); 8 serves hd <= 256 (GPT-J's
-// 256-wide heads, clusters of up to 8 CTAs, the portable limit) and halves the positions per pass, so kv[PU][NV] stays 16 int4 per thread.
+// NV: the most 32-element steps per position and quad thread (hd / 32).  4 serves hd <= 128 (clusters of up to 4 CTAs); 8 serves hd <= 256 (GPT-J's
+// 256-wide heads, clusters of up to 8 CTAs, the portable limit) and halves the positions per pass, so kv[PU][NV * CW] stays 16 int4 per thread.
+//
+// KT = float (an f32 cache, ggml_vec_dot_f32): a step of a quad thread is two 16-byte K vectors (CW = 2, so half the positions per pass); q and
+// the probabilities stay f32 in shared memory, the V rows take twice the bytes, and the KQV leftovers are added in float (f32dot.cuh).
 constexpr int ATH = 256;
-template <bool TP, bool ALIBI, int NV = 4>
-__device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
+template <bool TP, bool ALIBI, int NV = 4, typename KT = __half>
+__device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, const KT *__restrict__ Kl, const KT *__restrict__ Vl,
                                                 int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
                                                 float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
                                                 unsigned long long *prof, const TpSync &S, int head0, const float *__restrict__ alibi) {
@@ -462,13 +609,17 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
     const int per_head = hd / 32, h = blockIdx.x / per_head, part = blockIdx.x - h * per_head, c0 = part * 32;
     const int hk = h / (n_head / n_head_kv);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, u = tid & 3;
+    constexpr bool F32 = sizeof(KT) == 4;
+    constexpr int CW = F32 ? 2 : 1;                              // 16-byte K vectors per 32-element step and quad thread
+    constexpr int PER16 = 16 / (int)sizeof(KT);                 // cache elements per 16-byte chunk
     // shared-memory layout for nlay >= n_kv positions (the context bucket the graph was captured for, a multiple of 64: small enough that the
     // next mat-vec's CTAs fit beside this kernel's and stream their weights while it runs)
-    const int vstride = nlay + 32;                              // halves; (nlay + 32) * 2 B = 64 B mod 128 B: the two columns of a quarter-warp hit different banks
+    // f16: (nlay + 32) * 2 B = 64 B mod 128 B; f32: (nlay + 4) * 4 B = 16 B mod 128 B -- either way the two columns of a quarter-warp hit different banks
+    const int vstride = F32 ? nlay + 4 : nlay + 32;             // elements
     float *sc = (float *)sm;
-    __half *p16 = (__half *)(sm + (size_t)nlay * 4);
-    __half *q16 = p16 + nlay;
-    __half *vs = (__half *)(sm + (((size_t)nlay * 6 + (size_t)hd * 2 + 127) & ~(size_t)127));
+    KT *p16 = (KT *)(sm + (size_t)nlay * 4);
+    KT *q16 = p16 + nlay;
+    KT *vs = (KT *)(sm + (((size_t)nlay * (4 + sizeof(KT)) + (size_t)hd * sizeof(KT) + 127) & ~(size_t)127));
     pdl_trigger();                                              // the successor (wo) only needs shared memory beside us: let it prefetch its tiles now
     // Ahead of the wait: n_past and the KV cache below it.  Of these, this token's kernels write only cache position n_past of each layer (the
     // qkv node).  The older positions were written by earlier tokens or the prefill, n_past by the previous token's last kernel or by a
@@ -479,37 +630,44 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
     const int p = __ldcg(n_past), n_kv = p + 1;
     const int np = n_kv & ~31;
     const int64_t vrow0 = (int64_t)(hk * hd + c0) * n_ctx;
-    const int cold = p / 8;                                      // 16-byte V chunks per row wholly before position p
+    const int cold = p / PER16;                                  // 16-byte V chunks per row wholly before position p
     for (int i = tid; i < 32 * cold; i += ATH) {                 // V rows of this CTA's 32 channels: consumed after the soft_max
         const int rr = i / cold, cc = i - rr * cold;
-        cp16(smem_u32(vs + rr * vstride + cc * 8), Vl + vrow0 + (int64_t)rr * n_ctx + cc * 8);
+        cp16(smem_u32(vs + rr * vstride + cc * PER16), Vl + vrow0 + (int64_t)rr * n_ctx + cc * PER16);
     }
     const int per = (n_kv + per_head - 1) / per_head, j0 = part * per, j1 = n_kv < j0 + per ? n_kv : j0 + per;   // this CTA's KQ positions
-    const int nvec = hd / 32;                                    // 16-byte loads per thread per position (chunks i = 0..nvec-1)
-    constexpr int PU = 16 / NV;                                  // positions per quad per pass: up to PU * nvec 16-byte loads in flight per thread
-    int4 kv[PU][NV];
+    const int nvec = hd / 32;                                    // 32-element steps per position (i = 0..nvec-1), CW 16-byte loads each
+    constexpr int PU = 16 / (NV * CW);                           // positions per quad per pass: up to PU * nvec * CW 16-byte loads in flight per thread
+    int4 kv[PU][NV * CW];
     auto krow_of = [&](int j) { return Kl + (int64_t)(j < j1 ? j : j0) * gqa + hk * hd + 8 * u; };
 #pragma unroll
     for (int pu = 0; pu < PU; pu++) {                            // the first pass's K rows below p
         const int j = j0 + pu * (ATH / 4) + (tid >> 2);
-        const __half *krow = krow_of(j);
+        const KT *krow = krow_of(j);
 #pragma unroll
-        for (int i = 0; i < NV; i++) if (i < nvec) kv[pu][i] = j < j1 && j < p ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+        for (int i = 0; i < NV; i++)
+#pragma unroll
+            for (int c = 0; c < CW; c++)
+                if (i < nvec) kv[pu][i * CW + c] = j < j1 && j < p ? __ldcg((const int4 *)(krow + 32 * i) + c) : make_int4(0, 0, 0, 0);
     }
     pdl_wait();
     float qv = 0.f;
     if (tid < hd) qv = __ldcg(q + h * hd + tid);               // hd <= 256 = ATH
-    if (tid < 32) cp16(smem_u32(vs + tid * vstride + cold * 8), Vl + vrow0 + (int64_t)tid * n_ctx + cold * 8);
+    if (tid < 32) cp16(smem_u32(vs + tid * vstride + cold * PER16), Vl + vrow0 + (int64_t)tid * n_ctx + cold * PER16);
 #pragma unroll
     for (int pu = 0; pu < PU; pu++) {
         const int j = j0 + pu * (ATH / 4) + (tid >> 2);
         if (j == p && j < j1) {
-            const __half *krow = krow_of(j);
+            const KT *krow = krow_of(j);
 #pragma unroll
-            for (int i = 0; i < NV; i++) if (i < nvec) kv[pu][i] = __ldcg((const int4 *)(krow + 32 * i));
+            for (int i = 0; i < NV; i++)
+#pragma unroll
+                for (int c = 0; c < CW; c++)
+                    if (i < nvec) kv[pu][i * CW + c] = __ldcg((const int4 *)(krow + 32 * i) + c);
         }
     }
-    if (tid < hd) q16[tid] = __float2half_rn(qv);
+    if constexpr (F32) { if (tid < hd) q16[tid] = qv; }         // ggml_vec_dot_f32: q as it is
+    else { if (tid < hd) q16[tid] = __float2half_rn(qv); }
     // q16 visible inside the CTA; every CTA of the cluster is running before its shared memory is written remotely (no data is exchanged
     // yet, so the cluster barrier can be the relaxed one: no fence)
     __syncthreads();
@@ -523,9 +681,12 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
 #pragma unroll
                 for (int pu = 0; pu < PU; pu++) {
                     const int j = jb + pu * (ATH / 4) + (tid >> 2);
-                    const __half *krow = krow_of(j);
+                    const KT *krow = krow_of(j);
 #pragma unroll
-                    for (int i = 0; i < NV; i++) if (i < nvec) kv[pu][i] = j < j1 ? __ldcg((const int4 *)(krow + 32 * i)) : make_int4(0, 0, 0, 0);
+                    for (int i = 0; i < NV; i++)
+#pragma unroll
+                        for (int c = 0; c < CW; c++)
+                            if (i < nvec) kv[pu][i * CW + c] = j < j1 ? __ldcg((const int4 *)(krow + 32 * i) + c) : make_int4(0, 0, 0, 0);
                 }
             }
 #pragma unroll
@@ -535,7 +696,10 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
 #pragma unroll
                 for (int e = 0; e < 8; e++) acc[e] = 0.f;
 #pragma unroll
-                for (int i = 0; i < NV; i++) if (i < nvec) fma8(acc, kv[pu][i], *(const int4 *)(q16 + 32 * i + 8 * u));
+                for (int i = 0; i < NV; i++) {
+                    if constexpr (F32) { if (i < nvec) fma8(acc, kv[pu][2 * i], kv[pu][2 * i + 1], *(const float4 *)(q16 + 32 * i + 8 * u), *(const float4 *)(q16 + 32 * i + 8 * u + 4)); }
+                    else { if (i < nvec) fma8(acc, kv[pu][i], *(const int4 *)(q16 + 32 * i + 8 * u)); }
+                }
                 const float s = quad_tree(acc);
                 if (j < j1 && u < per_head)                      // thread u of the quad feeds CTA u (and CTA u + 4 of a cluster of more than 4)
                     cluster.map_shared_rank(sc, u)[j] = ALIBI ? __fmaf_rn((float)j, slope, __fmul_rn(s, kq_scale)) : __fmul_rn(s, kq_scale);
@@ -568,24 +732,35 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
     if (lane == 0) shd[warp] = s;
     __syncthreads();
     const float inv = (float)(1.0 / (((shd[0] + shd[1]) + (shd[2] + shd[3])) + ((shd[4] + shd[5]) + (shd[6] + shd[7]))));
-    for (int j = tid; j < n_kv; j += ATH) p16[j] = __float2half_rn(__fmul_rn(sc[j], inv));
+    if constexpr (F32) { for (int j = tid; j < n_kv; j += ATH) p16[j] = __fmul_rn(sc[j], inv); }
+    else { for (int j = tid; j < n_kv; j += ATH) p16[j] = __float2half_rn(__fmul_rn(sc[j], inv)); }
     asm volatile("cp.async.wait_all;" ::: "memory");
     __syncthreads();
 
     // ---- KQV: 32 channels x 4 threads ----
     if (tid < 128) {
         const int col = tid >> 2;
-        const __half *vrow = vs + col * vstride;
+        const KT *vrow = vs + col * vstride;
         float acc[8];
 #pragma unroll
         for (int e = 0; e < 8; e++) acc[e] = 0.f;
+        if constexpr (F32) {
 #pragma unroll 4
-        for (int k = 0; k < np; k += 32) fma8(acc, *(const int4 *)(vrow + k + 8 * u), *(const int4 *)(p16 + k + 8 * u));
+            for (int k = 0; k < np; k += 32)
+                fma8(acc, *(const int4 *)(vrow + k + 8 * u), *(const int4 *)(vrow + k + 8 * u + 4), *(const float4 *)(p16 + k + 8 * u), *(const float4 *)(p16 + k + 8 * u + 4));
+        } else {
+#pragma unroll 4
+            for (int k = 0; k < np; k += 32) fma8(acc, *(const int4 *)(vrow + k + 8 * u), *(const int4 *)(p16 + k + 8 * u));
+        }
         const float a = quad_tree(acc);
         if (u == 0) {
-            double sumf = (double)a;
-            for (int k = np; k < n_kv; k++) sumf += (double)__fmul_rn(__half2float(vrow[k]), __half2float(p16[k]));
-            stash[col] = (float)sumf;
+            if constexpr (F32) {
+                stash[col] = f32_leftovers(a, n_kv - np, [&](int i) { return vrow[np + i]; }, [&](int i) { return p16[np + i]; });
+            } else {
+                double sumf = (double)a;
+                for (int k = np; k < n_kv; k++) sumf += (double)__fmul_rn(__half2float(vrow[k]), __half2float(p16[k]));
+                stash[col] = (float)sumf;
+            }
         }
     }
     __syncthreads();
@@ -618,6 +793,14 @@ __global__ void __launch_bounds__(ATH) attn_fused_wide_kernel(const float *__res
                                                               float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
                                                               unsigned long long *prof, const TpSync S, int head0) {
     attn_fused_body<false, false, 8>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, nullptr);
+}
+// the three single-GPU forms on an f32 cache (MHA / GQA, ALiBi, wide); alibi: nullptr except for the ALiBi form
+template <bool ALIBI, int NV>
+__global__ void __launch_bounds__(ATH) attn_fused_f32_kernel(const float *__restrict__ q, const float *__restrict__ Kl, const float *__restrict__ Vl,
+                                                             int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
+                                                             float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                                                             unsigned long long *prof, const TpSync S, int head0, const float *__restrict__ alibi) {
+    attn_fused_body<false, ALIBI, NV, float>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, alibi);
 }
 
 // ---- ring and grid plan of the decode mat-vecs ------------------------------------------------------------------------------------------------
@@ -745,34 +928,41 @@ static void attn_fused_reserve(size_t bytes) {
     B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     B200_CHECK(cudaFuncSetAttribute(attn_fused_alibi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     B200_CHECK(cudaFuncSetAttribute(attn_fused_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_fused_f32_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_fused_f32_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_fused_f32_kernel<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
-// the same for attn_sv_kernel: one record per process.  Every decode_ops_t<TYPE, TP> launches this one kernel, so a record per instantiation
-// would let a session of another weight type with a shorter context LOWER the attribute under a session that already relies on more.
+// the same for attn_sv_kernel (and its f32 form): one record per process.  Every decode_ops_t<TYPE, TP> launches this one kernel, so a record per
+// instantiation would let a session of another weight type with a shorter context LOWER the attribute under a session that already relies on more.
 static void attn_sv_reserve(size_t bytes) {
     static size_t set = 48 * 1024;
     if (bytes <= set) return;
     B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_sv_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
 // the positions attn_fused_kernel holds for a context bucket: the bucket rounded up to whole 64-position tiles
 int attn_fused_rows(int n_kv_bucket) { return (n_kv_bucket + 63) / 64 * 64; }
-// dynamic shared memory of attn_fused_kernel for a context bucket and head size hd: scores (f32), probabilities and q (f16), then 32 V rows
-size_t attn_fused_smem(int n_kv_bucket, int hd) {
+// dynamic shared memory of attn_fused_kernel for a context bucket and head size hd: scores (f32), probabilities and q (f16), then 32 V rows;
+// an f32 cache (kv_type T_F32): probabilities, q and the V rows in f32 (136 bytes per position)
+size_t attn_fused_smem(int n_kv_bucket, int hd, int kv_type = T_F16) {
     const int nlay = attn_fused_rows(n_kv_bucket);
+    if (kv_type == T_F32) return (((size_t)nlay * 8 + (size_t)hd * 4 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 4) * 4;
     return (((size_t)nlay * 6 + (size_t)hd * 2 + 127) & ~(size_t)127) + (size_t)32 * (nlay + 32) * 2;
 }
 }  // namespace
-bool attn_fused_fits(int n_kv_bucket, int hd) { return attn_fused_smem(n_kv_bucket, hd) <= 227 * 1024; }
+bool attn_fused_fits(int n_kv_bucket, int hd, int kv_type) { return attn_fused_smem(n_kv_bucket, hd, kv_type) <= 227 * 1024; }
+int attn_sv_f32_max_ctx() { return (int)((227 * 1024 - attn_sv_f32_smem(0)) / 8); }
 namespace {
 // one cluster of hd/32 CTAs per head, a programmatic dependent of its predecessor.  alibi: per-head slopes (the ALiBi form, single GPU only)
-// or nullptr
+// or nullptr.  kv_type T_F32: Kl / Vl are an f32 cache (single GPU only)
 template <bool TP>
-void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const __half *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
+void launch_attn_fused(cudaStream_t st, const float *q, const void *Kl, const void *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
                        float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int n_kv_bucket, int q81, int off, int scale16,
-                       unsigned long long *prof, const TpSync &S, int head0, const float *alibi = nullptr) {
+                       unsigned long long *prof, const TpSync &S, int head0, const float *alibi = nullptr, int kv_type = T_F16) {
     const int nlay = attn_fused_rows(n_kv_bucket);
-    const size_t smem = attn_fused_smem(n_kv_bucket, hd);
+    const size_t smem = attn_fused_smem(n_kv_bucket, hd, kv_type);
     attn_fused_reserve(smem);
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(n_head * (hd / 32)); cfg.blockDim = dim3(ATH); cfg.dynamicSmemBytes = smem; cfg.stream = st;
@@ -782,20 +972,36 @@ void launch_attn_fused(cudaStream_t st, const float *q, const __half *Kl, const 
     at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 2;
+    if (kv_type == T_F32) {
+        B200_ASSERT(!TP && hd <= 256 && hd % 32 == 0 && (!alibi || hd <= 128));
+        const float *K32 = (const float *)Kl, *V32 = (const float *)Vl;
+        auto kern = alibi ? attn_fused_f32_kernel<true, 4> : hd > 128 ? attn_fused_f32_kernel<false, 8> : attn_fused_f32_kernel<false, 4>;
+        B200_CHECK(cudaLaunchKernelEx(&cfg, kern, q, K32, V32, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+                                      q81, off, scale16, prof, S, head0, alibi));
+        return;
+    }
+    const __half *K16 = (const __half *)Kl, *V16 = (const __half *)Vl;
     if (alibi) {
         B200_ASSERT(!TP && hd <= 128);
-        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_alibi_kernel, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_alibi_kernel, q, K16, V16, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
                                       q81, off, scale16, prof, S, head0, alibi));
         return;
     }
     if (hd > 128) {                                              // 5..8 CTAs per head
         B200_ASSERT(!TP && hd <= 256 && hd % 32 == 0);
-        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_wide_kernel, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_wide_kernel, q, K16, V16, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
                                       q81, off, scale16, prof, S, head0));
         return;
     }
-    B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
+    B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, q, K16, V16, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
                                   q81, off, scale16, prof, S, head0));
+}
+// the footprint of the cluster attention launch_attn_fused picks for the geometry (the successor the qkv node's ring is planned against)
+CtaFootprint attn_fused_footprint(bool tp, int hd, bool alibi, int kv_type, size_t smem) {
+    if (kv_type == T_F32) return footprint_of(alibi ? attn_fused_f32_kernel<true, 4> : hd > 128 ? attn_fused_f32_kernel<false, 8> : attn_fused_f32_kernel<false, 4>, ATH, smem);
+    if (alibi) return footprint_of(attn_fused_alibi_kernel, ATH, smem);
+    if (hd > 128) return footprint_of(attn_fused_wide_kernel, ATH, smem);
+    return tp ? footprint_of(attn_fused_kernel<true>, ATH, smem) : footprint_of(attn_fused_kernel<false>, ATH, smem);
 }
 
 // tensor-parallel helpers (tp.cuh).  spread: the embedding row every rank computed for itself -> the X exchange buffer's unit form (stamp 0);
@@ -818,6 +1024,18 @@ __global__ void tp_bump_kernel() {
     const TpCtx &T = c_tp;
     pdl_wait();
     if (threadIdx.x == 0) *T.epoch = *(volatile unsigned *)T.epoch + 1;
+}
+
+// the qkv mat-vec with the RoPE + KV store epilogue for the session's cache (an f32 cache: single GPU only)
+template <int TYPE, bool TP>
+const MmvPlan &qkv_plan(bool kv32, const QWeight &w, const CtaFootprint &succ) {
+    if constexpr (!TP) if (kv32) return mmv_plan<TYPE, EPI_QKV_F32, false>(w, succ);
+    return mmv_plan<TYPE, EPI_QKV, TP>(w, succ);
+}
+template <int TYPE, bool TP>
+void launch_qkv(bool kv32, const QWeight &w, const MmvArgs &A, const MmvPlan &plan, cudaStream_t st) {
+    if constexpr (!TP) if (kv32) { launch_mmv<TYPE, EPI_QKV_F32>(w, A, plan, st); return; }
+    launch_mmv<TYPE, EPI_QKV, TP>(w, A, plan, st);
 }
 
 template <int TYPE, bool TP>
@@ -847,18 +1065,21 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;
     if (tp) { launch_k(tp_spread_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.x, e); n++; }
     // attention: one cluster launch per layer, or the two-kernel variant for head sizes a cluster cannot cover and for buckets whose scores
-    // and V rows do not fit one CTA's shared memory
-    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd);
-    const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(n_kv_bucket, P.hd);
+    // and V rows do not fit one CTA's shared memory (an f32 cache: past 1664 positions)
+    const bool kv32 = !TP && P.kv_type == T_F32;                // sessions of a tensor-parallel model keep an f16 cache
+    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd, P.kv_type);
+    const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(n_kv_bucket, P.hd, P.kv_type);
     B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue (start_session_tp checks the size)
-    const size_t sv_smem = (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
+    const size_t sv_smem = kv32 ? attn_sv_f32_smem(P.n_ctx) : (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
     attn_sv_reserve(sv_smem);
     // mat-vec plans, each leaving room for what follows it (planned from the successor backwards; every layer has the same shapes): the norm
     // kernels release their dependents at entry, so beside wo and w2 there has to be room for the norm AND the next mat-vec
     const CtaFootprint f_norm = TP ? footprint_of(norm_pack_tp_kernel, 256, 0) : footprint_of(norm_pack_kernel, 256, 0);
-    const CtaFootprint f_attn = fused_attn ? footprint_of(attn_fused_kernel<TP>, ATH, fa_smem)
+    const CtaFootprint f_attn = kv32 ? (fused_attn ? attn_fused_footprint(false, P.hd, false, T_F32, fa_smem)
+                                                   : footprint_of(P.hd == 128 ? attn_kq_f32_kernel<128> : attn_kq_f32_kernel<64>, 128, 0))
+                              : fused_attn ? footprint_of(attn_fused_kernel<TP>, ATH, fa_smem)
                                            : footprint_of(P.hd == 128 ? attn_kq_kernel<128> : attn_kq_kernel<64>, 128, 0);
-    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_QKV, TP>(layers[0].wqkv, f_attn);
+    const MmvPlan &p_qkv = qkv_plan<TYPE, TP>(kv32, layers[0].wqkv, f_attn);
     const MmvPlan &p_w2 = mmv_plan<TYPE, EPI_RES, TP>(layers[0].w2, f_norm + p_qkv.cta);
     const MmvPlan &p_w13 = mmv_plan<TYPE, EPI_SILU, TP>(layers[0].w13, p_w2.cta);
     const MmvPlan &p_wo = mmv_plan<TYPE, EPI_RES, TP>(layers[0].wo, f_norm + p_w13.cta);
@@ -869,16 +1090,22 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         launch_norm(P.x, L.attn_norm, ts(TPB_X, (unsigned)il, -1, 0, -1, 0));
         MmvArgs A{}; A.xpack = xpack_a; A.q = P.q; A.K = L.K; A.V = L.V; A.rope_cs = P.rope_cs; A.rope_half = P.rope_half; A.hd = P.hd; A.e = e_loc; A.gqa = P.gqa;
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
-        A.prof = pr(); launch_mmv<TYPE, EPI_QKV, TP>(L.wqkv, A, p_qkv, st); n++;
+        A.prof = pr(); launch_qkv<TYPE, TP>(kv32, L.wqkv, A, p_qkv, st); n++;
         if (fused_attn) {
             launch_attn_fused<TP>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, n_kv_bucket, q81, off, s16, pr(),
-                                  ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0);
+                                  ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0, nullptr, kv32 ? T_F32 : T_F16);
             n++;
+        } else if (kv32) {
+            launch_k(P.hd == 128 ? attn_kq_f32_kernel<128> : attn_kq_f32_kernel<64>, dim3((n_kv_bucket + 63) / 64, P.n_head), dim3(128), 0, st,
+                     P.q, (const float *)L.K, P.kq, P.n_past, P.gqa, P.n_head, P.n_head_kv, P.n_ctx, pr());
+            n++;
+            launch_k(attn_sv_f32_kernel, dim3(P.n_head * (P.hd / 32)), dim3(128), sv_smem, st, P.kq, (const float *)L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale,
+                     P.hd, P.n_head, P.n_head_kv, P.n_ctx, q81, off, s16, pr()); n++;
         } else {
             launch_k(P.hd == 128 ? attn_kq_kernel<128> : attn_kq_kernel<64>, dim3((n_kv_bucket + 63) / 64, P.n_head), dim3(128), 0, st,
-                     P.q, L.K, P.kq, P.n_past, P.gqa, P.n_head, P.n_head_kv, P.n_ctx, pr());
+                     P.q, (const __half *)L.K, P.kq, P.n_past, P.gqa, P.n_head, P.n_head_kv, P.n_ctx, pr());
             n++;
-            launch_k(attn_sv_kernel, dim3(P.n_head * (P.hd / 32)), dim3(128), sv_smem, st, P.kq, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head,
+            launch_k(attn_sv_kernel, dim3(P.n_head * (P.hd / 32)), dim3(128), sv_smem, st, P.kq, (const __half *)L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head,
                      P.n_head_kv, P.n_ctx, q81, off, s16, pr()); n++;
         }
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.ff; Bo.addend = P.x;
@@ -968,9 +1195,13 @@ __global__ void __launch_bounds__(256) ln_pack_nobias_kernel(const float *__rest
 // qkv [3e] (bias added) -> q [e], k -> f16 cache row n_past, v -> f16 cache column n_past.  GPT-NeoX (gptneox lib.rs:205-247): rows per head are q | k | v
 // (head stride 3 hd) and q, k get RoPE mode 2 -- the ggml neox branch (LC/ggml.c:11876-11897) rotates EVERY block of n_rot dims of the head, pairs
 // (c, c + n_rot/2).  GPT-2 (gpt2 lib.rs:190-210): the three thirds of the row, no rotation (n_rot = 0).  One thread per channel.
-__global__ void __launch_bounds__(256) neox_rope_store_kernel(const float *__restrict__ qkv, float *__restrict__ q, __half *__restrict__ Kl, __half *__restrict__ Vl,
-                                                              const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e, int n_ctx,
-                                                              int head_stride, int k_off, int v_off) {
+// KT: the cache's element type (float: K and V stored as they are)
+__device__ __forceinline__ void kv_store(__half *p, float v) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void kv_store(float *p, float v) { *p = v; }
+template <typename KT>
+__device__ __forceinline__ void neox_rope_store_body(const float *__restrict__ qkv, float *__restrict__ q, KT *__restrict__ Kl, KT *__restrict__ Vl,
+                                                     const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e, int n_ctx,
+                                                     int head_stride, int k_off, int v_off) {
     pdl_trigger();
     pdl_wait();
     const int i = blockIdx.x * 256 + threadIdx.x;
@@ -992,8 +1223,18 @@ __global__ void __launch_bounds__(256) neox_rope_store_kernel(const float *__res
         }
     }
     q[i] = qo;
-    Kl[(int64_t)p * e + i] = __float2half_rn(ko);
-    Vl[(int64_t)i * n_ctx + p] = __float2half_rn(__ldcg(base + v_off + c));
+    kv_store(Kl + (int64_t)p * e + i, ko);
+    kv_store(Vl + (int64_t)i * n_ctx + p, __ldcg(base + v_off + c));
+}
+__global__ void __launch_bounds__(256) neox_rope_store_kernel(const float *__restrict__ qkv, float *__restrict__ q, __half *__restrict__ Kl, __half *__restrict__ Vl,
+                                                              const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e, int n_ctx,
+                                                              int head_stride, int k_off, int v_off) {
+    neox_rope_store_body(qkv, q, Kl, Vl, n_past, rope_cs, rope_half, n_rot, hd, e, n_ctx, head_stride, k_off, v_off);
+}
+__global__ void __launch_bounds__(256) neox_rope_store_f32_kernel(const float *__restrict__ qkv, float *__restrict__ q, float *__restrict__ Kl, float *__restrict__ Vl,
+                                                                  const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e,
+                                                                  int n_ctx, int head_stride, int k_off, int v_off) {
+    neox_rope_store_body(qkv, q, Kl, Vl, n_past, rope_cs, rope_half, n_rot, hd, e, n_ctx, head_stride, k_off, v_off);
 }
 
 // GPT-2: inpL = wte[token] + wpe[n_past]  (gpt2 lib.rs:164-172), position read from device memory
@@ -1018,15 +1259,18 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     }
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
     B200_ASSERT(neox_decode_fits(P, n_kv_bucket));
-    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd);
+    const bool kv32 = P.kv_type == T_F32;
+    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd, P.kv_type);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     // MPT has no biases: its norms take ln_pack_nobias_kernel and its up-projection the gelu epilogue without a bias node
     const bool biased = layers[0].ln1_b != nullptr, fc_bias = layers[0].bfc != nullptr;
     auto ln_kernel = biased ? ln_pack_kernel : ln_pack_nobias_kernel;
     const CtaFootprint f_ln = footprint_of(ln_kernel, 256, 0);
-    const CtaFootprint f_attn = P.alibi ? footprint_of(attn_fused_alibi_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
-    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wqkv, footprint_of(neox_rope_store_kernel, 256, 0) + f_attn);
+    const CtaFootprint f_attn = kv32 ? attn_fused_footprint(false, P.hd, P.alibi != nullptr, T_F32, fa_smem)
+                              : P.alibi ? footprint_of(attn_fused_alibi_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
+    const CtaFootprint f_store = kv32 ? footprint_of(neox_rope_store_f32_kernel, 256, 0) : footprint_of(neox_rope_store_kernel, 256, 0);
+    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wqkv, f_store + f_attn);
     const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
     const MmvPlan &p_fc = fc_bias ? mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta) : mmv_plan<TYPE, EPI_GELU_NB, false>(layers[0].wfc, p_proj.cta);
     const MmvPlan &p_dense = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wdense, f_ln + p_fc.cta);
@@ -1036,10 +1280,13 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         launch_k(ln_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;               // :192-196
         MmvArgs A{}; A.xpack = P.xpack_a; A.dst = P.qkv; A.bias = L.bqkv;
         launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, p_qkv, st); n++;                                                                                      // :199-200
-        launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, L.K, L.V, (const int *)P.n_past, P.rope_cs, P.rope_half,
-                 P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off); n++;                               // :205-247
+        if (kv32) launch_k(neox_rope_store_f32_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, (float *)L.K, (float *)L.V, (const int *)P.n_past,
+                           P.rope_cs, P.rope_half, P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off);
+        else launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, (__half *)L.K, (__half *)L.V, (const int *)P.n_past,
+                      P.rope_cs, P.rope_half, P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off);
+        n++;                                                                                                                                  // :205-247
         launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
-                                 nullptr, S, 0, P.alibi); n++;                                                                            // :250-298
+                                 nullptr, S, 0, P.alibi, P.kv_type); n++;                                                                 // :250-298
         // attention.dense (+bias); sequential residual: ff_in = that + inpL                                                                    :301-312
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out; Bo.bias = L.bdense; Bo.add1 = P.parallel_residual ? nullptr : P.x;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;
@@ -1071,13 +1318,15 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     // the token boundary: a plain launch (no programmatic attribute), see neox_ops_t
     get_rows_q(P.wte, P.token, P.x, 1, st); n++;                                                                                                     // :161
     B200_ASSERT(neox_decode_fits(P, n_kv_bucket));
-    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd);
+    const bool kv32 = P.kv_type == T_F32;
+    const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd, P.kv_type);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
-    const CtaFootprint f_attn = P.hd > 128 ? footprint_of(attn_fused_wide_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
+    const CtaFootprint f_attn = kv32 ? attn_fused_footprint(false, P.hd, false, T_F32, fa_smem)
+                              : P.hd > 128 ? footprint_of(attn_fused_wide_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
     // each ring planned against the node launched after it: qkv -> attention, out_proj -> fc_in, fc_in -> fc_out, fc_out -> next layer's ln_1 + qkv
-    const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_QKV, false>(layers[0].wqkv, f_attn);
+    const MmvPlan &p_qkv = qkv_plan<TYPE, false>(kv32, layers[0].wqkv, f_attn);
     const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
     const MmvPlan &p_fc = mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta);
     const MmvPlan &p_dense = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wdense, p_fc.cta);
@@ -1087,9 +1336,9 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;                 // :168-174
         MmvArgs A{}; A.xpack = P.xpack_a; A.q = P.q; A.K = L.K; A.V = L.V; A.rope_cs = P.rope_cs; A.rope_half = P.rope_half; A.hd = P.hd; A.e = e; A.gqa = e;
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
-        launch_mmv<TYPE, EPI_QKV>(L.wqkv, A, p_qkv, st); n++;                                                                                          // :178-220
+        launch_qkv<TYPE, false>(kv32, L.wqkv, A, p_qkv, st); n++;                                                                                     // :178-220
         launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
-                                 nullptr, S, 0); n++;                                                                                                   // :222-262
+                                 nullptr, S, 0, nullptr, P.kv_type); n++;                                                                               // :222-262
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;                                                                                    // :265
         MmvArgs C{}; C.xpack = P.xpack_a; C.xpack_out = P.xpack_f; C.bias = L.bfc; C.lut_gelu = P.lut_gelu; C.q81 = q81; C.off = off; C.scale16 = s16;
@@ -1107,12 +1356,12 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
 }  // namespace
 
 // The cluster attention takes heads of up to 128 (GPT-J's wide form: up to 256) in 32-wide slices and the bucket's scores and V rows in shared
-// memory; ln_pack_body holds rows of up to 8192; the mat-vecs stream rows of n_embd and 4 n_embd.
+// memory (an f32 cache: up to 1664 positions); ln_pack_body holds rows of up to 8192; the mat-vecs stream rows of n_embd and 4 n_embd.
 bool neox_decode_fits(const NeoxParams &P, int n_kv_bucket) {
     QWeight k_e, k_4e;
     k_e.nb = P.e / QK; k_4e.nb = 4 * P.e / QK;
     return P.hd % 32 == 0 && P.hd <= (P.gptj ? 256 : 128) && P.e % 128 == 0 && P.e <= 8192 && P.n_ctx % 8 == 0 &&
-           mmv_exact_stream_supported(k_e) && mmv_exact_stream_supported(k_4e) && attn_fused_fits(n_kv_bucket, P.hd);
+           mmv_exact_stream_supported(k_e) && mmv_exact_stream_supported(k_4e) && attn_fused_fits(n_kv_bucket, P.hd, P.kv_type);
 }
 
 void neox_decode_enqueue(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int wtype, int n_kv_bucket, cudaStream_t st, int *launches) {

@@ -18,6 +18,9 @@
 //   ggml_vec_dot_f16 (AVX, LC/ggml.c:2325-2359, macros :1876-1975): 4 accumulators x 8 lanes, element k goes to lane k % 32,
 //       fma in order; GGML_F32x8_REDUCE: (s0+s2)+(s1+s3), then lanes (q + q+4), then hadd, hadd; leftovers (n % 32) are added
 //       in DOUBLE on top.  Here: one warp per dot product, lane l = element k % 32, shuffle tree with offsets 16, 8, 4, 1, 2.
+#include <type_traits>
+
+#include "f32dot.cuh"
 #include "kernels.cuh"
 
 namespace b200 {
@@ -123,49 +126,82 @@ void mul_mat_q_exact(const QWeight &w, const int8_t *xq, const float2 *xds, floa
     }
 }
 
-// ---- ggml_vec_dot_f16 order: one warp per output element ------------------------------------------------------------------------
-// dst[i2][i1][i0] = dot(src0[i2/(ne12/ne02)][i0][0..ne00), f16round(src1[i2][i1][0..ne00)).  `causal_past` >= 0 skips outputs with
+// ---- the attention mat-muls on the KV cache: one warp per output element ------------------------------------------------------------
+// dst[i2][i1][i0] = dot(src0[i2/(ne12/ne02)][i0][0..ne00), src1[i2][i1][0..ne00)).  `causal_past` >= 0 skips outputs with
 // i0 > causal_past + i1 (they are overwritten with -inf by diag_mask_inf before anyone reads them; llama lib.rs:274-276).
+// F32 = false: an f16 cache, ggml_vec_dot_f16 on src1 rounded to fp16 (leftovers in double); F32 = true: an f32 cache, ggml_vec_dot_f32 on src1
+// as it is (leftovers in float, f32dot.cuh).  Both share the 32 chains and the reduction tree.
+template <bool F32> struct AttnSrc0 { using T = __half; };
+template <> struct AttnSrc0<true> { using T = float; };
+template <bool F32> __device__ __forceinline__ float attn_a(const typename AttnSrc0<F32>::T *a, int64_t k) {
+    if constexpr (F32) return a[k]; else return __half2float(a[k]);
+}
+template <bool F32> __device__ __forceinline__ float attn_b(const float *b, int64_t k) {   // from_float of the vec_dot_type (F32: none)
+    if constexpr (F32) return b[k]; else return __half2float(__float2half_rn(b[k]));
+}
+
 constexpr int F16X_WARPS = 8;
-__global__ void __launch_bounds__(F16X_WARPS * 32) mul_mat_f16_exact_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
-                                                                            const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
-                                                                            char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+template <bool F32>
+__device__ __forceinline__ void mul_mat_attn_warp(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                                                  const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                                                  char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+    using T0 = typename AttnSrc0<F32>::T;
     const int lane = threadIdx.x & 31;
     const int64_t i0 = (int64_t)blockIdx.x * F16X_WARPS + (threadIdx.x >> 5);
     const int64_t i1 = blockIdx.y, i2 = blockIdx.z;
     if (i0 >= ne01) return;
     if (causal_past >= 0 && i0 > causal_past + i1) return;
     const int64_t i02 = i2 / (ne12 / ne02);
-    const __half *a = (const __half *)(src0 + i02 * nb02 + i0 * nb01);
+    const T0 *a = (const T0 *)(src0 + i02 * nb02 + i0 * nb01);
     const float *b = (const float *)(src1 + i2 * nb12 + i1 * nb11);
     const int64_t np = ne00 & ~(int64_t)31;
     float s = 0.f;
-    for (int64_t k = lane; k < np; k += 32)                       // sum[j][q] with l = j*8 + q: GGML_F16_VEC_FMA in order of i
-        s = __fmaf_rn(__half2float(a[k]), __half2float(__float2half_rn(b[k])), s);
+    for (int64_t k = lane; k < np; k += 32)                       // sum[j][q] with l = j*8 + q: GGML_F16_VEC_FMA / GGML_F32_VEC_FMA in order of i
+        s = __fmaf_rn(attn_a<F32>(a, k), attn_b<F32>(b, k), s);
     s = __fadd_rn(s, __shfl_down_sync(0xffffffffu, s, 16));        // x[0] += x[2]; x[1] += x[3]
     s = __fadd_rn(s, __shfl_down_sync(0xffffffffu, s, 8));         // x[0] += x[1]
     s = __fadd_rn(s, __shfl_down_sync(0xffffffffu, s, 4));         // t0 = lo128 + hi128
     s = __fadd_rn(s, __shfl_down_sync(0xffffffffu, s, 1));         // hadd
     s = __fadd_rn(s, __shfl_down_sync(0xffffffffu, s, 2));         // hadd
     if (lane == 0) {
-        double sumf = (double)s;
-        for (int64_t k = np; k < ne00; ++k)                        // leftovers: double += (double)(f32 product)
-            sumf += (double)__fmul_rn(__half2float(a[k]), __half2float(__float2half_rn(b[k])));
-        *(float *)(dst + i2 * nbd2 + i1 * nbd1 + i0 * 4) = (float)sumf;
+        float r;
+        if constexpr (F32) {
+            r = f32_leftovers(s, (int)(ne00 - np), [&](int i) { return a[np + i]; }, [&](int i) { return b[np + i]; });
+        } else {
+            double sumf = (double)s;
+            for (int64_t k = np; k < ne00; ++k)                    // leftovers: double += (double)(f32 product)
+                sumf += (double)__fmul_rn(__half2float(a[k]), __half2float(__float2half_rn(b[k])));
+            r = (float)sumf;
+        }
+        *(float *)(dst + i2 * nbd2 + i1 * nbd1 + i0 * 4) = r;
     }
+}
+__global__ void __launch_bounds__(F16X_WARPS * 32) mul_mat_f16_exact_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                                                                            const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                                                                            char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+    mul_mat_attn_warp<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+}
+__global__ void __launch_bounds__(F16X_WARPS * 32) mul_mat_f32_exact_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                                                                            const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                                                                            char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+    mul_mat_attn_warp<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
 }
 
 // ---- batched version: shared-memory tiles, 4 threads per dot, 8 dots per thread --------------------------------------------------------
-// CTA = 16 src0 rows x 32 src1 rows (512 dots), 64 elements of the reduction per stage, operands staged as f32 (src0: f16 -> f32,
-// src1: f32 -> f16 -> f32, the rounding ggml_compute_forward_mul_mat applies before the f16 dot).  The 32 chains of ggml_vec_dot_f16
-// (chain l over elements k = l mod 32, sequential in k) are split over the 4 threads of a quad as l in {4u..4u+3} u {16+4u..16+4u+3}: two
-// 16-byte shared loads per operand row and step, and the reduction tree (offsets 16, 8, 4, then the two hadds) is: in-thread, quad shuffle 2,
-// quad shuffle 1, in-thread -- the reference's association exactly.  Inner loop per thread and 32-element step: 12 LDS.128 + 64 FFMA.
+// CTA = 16 src0 rows x 32 src1 rows (512 dots), 64 elements of the reduction per stage, operands staged as f32 (src0: f16 -> f32 or f32,
+// src1: f32 -> f16 -> f32, the rounding ggml_compute_forward_mul_mat applies before the f16 dot, or f32 as it is).  The 32 chains of
+// ggml_vec_dot_f16 / ggml_vec_dot_f32 (chain l over elements k = l mod 32, sequential in k) are split over the 4 threads of a quad as
+// l in {4u..4u+3} u {16+4u..16+4u+3}: two 16-byte shared loads per operand row and step, and the reduction tree (offsets 16, 8, 4, then the two
+// hadds) is: in-thread, quad shuffle 2, quad shuffle 1, in-thread -- the reference's association exactly.  Inner loop per thread and 32-element
+// step: 12 LDS.128 + 64 FFMA.
 constexpr int FT_A = 16, FT_B = 32, FT_K = 64, FT_STRIDE = FT_K + 4, FT_THREADS = 256;      // stride 68 floats: quads of a quarter-warp hit disjoint banks
 
-__global__ void __launch_bounds__(FT_THREADS) mul_mat_f16_tiled_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
-                                                                       const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
-                                                                       char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+template <bool F32>
+__device__ __forceinline__ void mul_mat_attn_tiled(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                                                   const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                                                   char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+    using T0 = typename AttnSrc0<F32>::T;
+    using RA = typename std::conditional<F32, float4, uint2>::type;                   // one thread's 4 src0 elements
     __shared__ __align__(16) float sa[2][FT_A][FT_STRIDE];
     __shared__ __align__(16) float sb[2][FT_B][FT_STRIDE];
     const int tid = threadIdx.x, u = tid & 3, bq = (tid >> 2) & 7, ap = tid >> 5;        // quad (ap, bq): src0 rows 2ap, 2ap+1 x src1 rows 4bq..4bq+3
@@ -175,23 +211,28 @@ __global__ void __launch_bounds__(FT_THREADS) mul_mat_f16_tiled_kernel(const cha
     const char *A = src0 + i02 * nb02, *Bm = src1 + i2 * nb12;
     const int64_t np = ne00 & ~(int64_t)31;
 
-    // fill plan: src0 tile = 16 rows x 64 halves = 256 x 8 B (one per thread); src1 tile = 32 rows x 64 floats = 512 x 16 B (two per thread)
+    // fill plan: src0 tile = 16 rows x 64 elements = 256 x 4 elements (one per thread); src1 tile = 32 rows x 64 floats = 512 x 16 B (two per thread)
     const int far = tid >> 4, fac = (tid & 15) * 4;                  // src0: row, first of 4 elements
     const int fbr = tid >> 3, fbc = (tid & 7) * 4;                   // src1: rows fbr and fbr (+0) with columns fbc, fbc + 32
     const int64_t arow = a0 + far < ne01 ? a0 + far : ne01 - 1, brow = b0 + fbr < ne11 ? b0 + fbr : ne11 - 1;
-    const __half *ga = (const __half *)(A + arow * nb01);
+    const T0 *ga = (const T0 *)(A + arow * nb01);
     const float *gb = (const float *)(Bm + brow * nb11);
-    uint2 ra; float4 rb0, rb1;
+    RA ra; float4 rb0, rb1;
     auto fetch = [&](int64_t k0) {                                   // elements past np are never used by the main loop: read them as zero
-        ra = k0 + fac < np ? *(const uint2 *)(ga + k0 + fac) : make_uint2(0u, 0u);
+        if constexpr (F32) ra = k0 + fac < np ? *(const float4 *)(ga + k0 + fac) : make_float4(0.f, 0.f, 0.f, 0.f);
+        else ra = k0 + fac < np ? *(const uint2 *)(ga + k0 + fac) : make_uint2(0u, 0u);
         rb0 = k0 + fbc < np ? *(const float4 *)(gb + k0 + fbc) : make_float4(0.f, 0.f, 0.f, 0.f);
         rb1 = k0 + 32 + fbc < np ? *(const float4 *)(gb + k0 + 32 + fbc) : make_float4(0.f, 0.f, 0.f, 0.f);
     };
-    auto r16 = [](float v) { return __half2float(__float2half_rn(v)); };
+    auto r16 = [](float v) { if constexpr (F32) return v; else return __half2float(__float2half_rn(v)); };
     auto stash = [&](int buf) {
-        const __half2 h0 = *(const __half2 *)&ra.x, h1 = *(const __half2 *)&ra.y;
-        const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-        *(float4 *)&sa[buf][far][fac] = make_float4(f0.x, f0.y, f1.x, f1.y);
+        if constexpr (F32) {
+            *(float4 *)&sa[buf][far][fac] = ra;
+        } else {
+            const __half2 h0 = *(const __half2 *)&ra.x, h1 = *(const __half2 *)&ra.y;
+            const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
+            *(float4 *)&sa[buf][far][fac] = make_float4(f0.x, f0.y, f1.x, f1.y);
+        }
         *(float4 *)&sb[buf][fbr][fbc] = make_float4(r16(rb0.x), r16(rb0.y), r16(rb0.z), r16(rb0.w));
         *(float4 *)&sb[buf][fbr][32 + fbc] = make_float4(r16(rb1.x), r16(rb1.y), r16(rb1.z), r16(rb1.w));
     };
@@ -249,34 +290,67 @@ __global__ void __launch_bounds__(FT_THREADS) mul_mat_f16_tiled_kernel(const cha
             const float s = __fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3]));                               // the two hadds
             const int64_t i0 = a0 + 2 * ap + i, i1 = b0 + 4 * bq + j;
             if (u == 0 && i0 < ne01 && i1 < ne11 && !(causal_past >= 0 && i0 > causal_past + i1)) {
-                double sumf = (double)s;
-                if (np < ne00) {                                                                                   // leftovers: double += (double)(f32 product)
-                    const __half *al = (const __half *)(A + i0 * nb01);
-                    const float *bl = (const float *)(Bm + i1 * nb11);
-                    for (int64_t k = np; k < ne00; ++k) sumf += (double)__fmul_rn(__half2float(al[k]), r16(bl[k]));
+                float out;
+                if constexpr (F32) {
+                    const float *al = (const float *)(A + i0 * nb01), *bl = (const float *)(Bm + i1 * nb11);
+                    out = f32_leftovers(s, (int)(ne00 - np), [&](int k) { return al[np + k]; }, [&](int k) { return bl[np + k]; });
+                } else {
+                    double sumf = (double)s;
+                    if (np < ne00) {                                                                               // leftovers: double += (double)(f32 product)
+                        const __half *al = (const __half *)(A + i0 * nb01);
+                        const float *bl = (const float *)(Bm + i1 * nb11);
+                        for (int64_t k = np; k < ne00; ++k) sumf += (double)__fmul_rn(__half2float(al[k]), r16(bl[k]));
+                    }
+                    out = (float)sumf;
                 }
-                *(float *)(dst + i2 * nbd2 + i1 * nbd1 + i0 * 4) = (float)sumf;
+                *(float *)(dst + i2 * nbd2 + i1 * nbd1 + i0 * 4) = out;
             }
         }
+}
+__global__ void __launch_bounds__(FT_THREADS) mul_mat_f16_tiled_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                                                                       const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                                                                       char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+    mul_mat_attn_tiled<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+}
+// (FT_THREADS, 1): without the one-CTA hint ptxas caps the f32 form at 128 registers and spills 24 bytes inside the main loop; it needs 145
+__global__ void __launch_bounds__(FT_THREADS, 1) mul_mat_f32_tiled_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                                                                       const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                                                                       char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+    mul_mat_attn_tiled<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+}
+
+// the tiled kernel wants src0 rows aligned to its 4-element loads (8 bytes f16, 16 bytes f32) and 16-byte aligned src1 rows; a handful of src1
+// rows is cheaper one warp per dot
+template <bool F32>
+static void mul_mat_attn(const void *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                         const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                         float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st) {
+    if (ne01 == 0 || ne11 == 0 || ne12 == 0) return;
+    B200_ASSERT(ne12 % ne02 == 0 && ne11 <= 65535 && ne12 <= 65535);
+    const int64_t al = F32 ? 16 : 8;
+    const bool aligned = ((uintptr_t)src0 % al == 0) && nb01 % al == 0 && nb02 % al == 0 && ((uintptr_t)src1 % 16 == 0) && nb11 % 16 == 0 && nb12 % 16 == 0;
+    if (ne11 >= 8 && aligned) {
+        dim3 grid((unsigned)((ne01 + FT_A - 1) / FT_A), (unsigned)((ne11 + FT_B - 1) / FT_B), (unsigned)ne12);
+        (F32 ? mul_mat_f32_tiled_kernel : mul_mat_f16_tiled_kernel)<<<grid, FT_THREADS, 0, st>>>((const char *)src0, ne00, ne01, ne02, nb01, nb02, (const char *)src1, ne11,
+                                                                                                ne12, nb11, nb12, (char *)dst, nbd1, nbd2, causal_past);
+    } else {
+        dim3 grid((unsigned)((ne01 + F16X_WARPS - 1) / F16X_WARPS), (unsigned)ne11, (unsigned)ne12);
+        (F32 ? mul_mat_f32_exact_kernel : mul_mat_f16_exact_kernel)<<<grid, F16X_WARPS * 32, 0, st>>>((const char *)src0, ne00, ne01, ne02, nb01, nb02, (const char *)src1,
+                                                                                                      ne11, ne12, nb11, nb12, (char *)dst, nbd1, nbd2, causal_past);
+    }
+    B200_CHECK(cudaGetLastError());
 }
 
 void mul_mat_f16_exact(const __half *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                        float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st) {
-    if (ne01 == 0 || ne11 == 0 || ne12 == 0) return;
-    B200_ASSERT(ne12 % ne02 == 0 && ne11 <= 65535 && ne12 <= 65535);
-    // the tiled kernel wants 8-byte aligned src0 rows and 16-byte aligned src1 rows; a handful of src1 rows is cheaper one warp per dot
-    const bool aligned = ((uintptr_t)src0 % 8 == 0) && nb01 % 8 == 0 && nb02 % 8 == 0 && ((uintptr_t)src1 % 16 == 0) && nb11 % 16 == 0 && nb12 % 16 == 0;
-    if (ne11 >= 8 && aligned) {
-        dim3 grid((unsigned)((ne01 + FT_A - 1) / FT_A), (unsigned)((ne11 + FT_B - 1) / FT_B), (unsigned)ne12);
-        mul_mat_f16_tiled_kernel<<<grid, FT_THREADS, 0, st>>>((const char *)src0, ne00, ne01, ne02, nb01, nb02, (const char *)src1, ne11, ne12, nb11, nb12,
-                                                              (char *)dst, nbd1, nbd2, causal_past);
-    } else {
-        dim3 grid((unsigned)((ne01 + F16X_WARPS - 1) / F16X_WARPS), (unsigned)ne11, (unsigned)ne12);
-        mul_mat_f16_exact_kernel<<<grid, F16X_WARPS * 32, 0, st>>>((const char *)src0, ne00, ne01, ne02, nb01, nb02, (const char *)src1, ne11, ne12, nb11, nb12,
-                                                                   (char *)dst, nbd1, nbd2, causal_past);
-    }
-    B200_CHECK(cudaGetLastError());
+    mul_mat_attn<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past, st);
+}
+
+void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                       const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                       float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st) {
+    mul_mat_attn<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past, st);
 }
 
 }  // namespace b200

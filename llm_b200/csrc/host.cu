@@ -116,16 +116,25 @@ int read_slot(const Slot &s, void *host, size_t nbytes) {
     return B200_OK;
 }
 
-void SessionCore::start(int n_batch_, int n_ctx_, int n_vocab_, size_t kv_elems) {
+void SessionCore::start(int n_batch_, int n_ctx_, int n_vocab_, size_t kv_elems_, int kv_type_) {
     n_batch = n_batch_; n_ctx = n_ctx_; n_vocab = n_vocab_;
-    memory_k = device_zeros<__half>(kv_elems * 2);              // offload_no_scratch zero-fills (LC/ggml-cuda.cu:3967-3973)
-    memory_v = device_zeros<__half>(kv_elems * 2);
+    kv_type = kv_type_; kv_elems = kv_elems_;
+    memory_k = device_zeros<char>(kv_bytes());                  // offload_no_scratch zero-fills (LC/ggml-cuda.cu:3967-3973)
+    memory_v = device_zeros<char>(kv_bytes());
     d_tokens = device_alloc<int32_t>((size_t)n_batch * 4);
     h_tokens = pinned_alloc<int32_t>((size_t)n_batch * 4);
     h_logits = pinned_alloc<float>((size_t)n_batch * n_vocab * 4);
     cudaEvent_t ev;
     B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     tokens_uploaded.reset(ev);
+}
+
+int SessionCore::read_kv(int which, void *host_out, size_t nbytes) {
+    if (!host_out) return B200_ERR_BAD_ARG;
+    if (nbytes != kv_bytes()) return B200_ERR_TENSOR_SHAPE;
+    B200_CHECK(cudaStreamSynchronize(rt().stream));
+    B200_CHECK(cudaMemcpy(host_out, which ? memory_v.get() : memory_k.get(), nbytes, cudaMemcpyDeviceToHost));
+    return B200_OK;
 }
 
 int SessionCore::admit(int n) const {

@@ -102,17 +102,26 @@ int64_t ggml_find_tensor(const b200_ggml_file *f, const char *name);        // i
 bool lora_in_patch_set(const b200_ggml_file *f, const char *name);          // some tensor of the adapter is `name` + "." + a last component
 float lora_scaling(const b200_ggml_file *f);                                // (f32)alpha / (f32)r
 
-// ---- what every session keeps: the f16 KV cache, the position, token and logits staging, the decode graphs -------------------------
+// ---- what every session keeps: the KV cache, the position, token and logits staging, the decode graphs -------------------------------
 struct SessionCore {
     int n_batch = 0, n_ctx = 0, n_vocab = 0;
     int n_past = 0, last_launches = 0;
-    DeviceBuf<__half> memory_k, memory_v;
+    // memory_k / memory_v of InferenceSessionConfig::memory_k_type / memory_v_type (one type for both): T_F16 (the default) or T_F32
+    int kv_type = T_F16;
+    size_t kv_elems = 0;                // elements of each
+    DeviceBuf<char> memory_k, memory_v;
     DeviceBuf<int32_t> d_tokens; PinnedBuf<int32_t> h_tokens;
     PinnedBuf<float> h_logits;          // n_batch rows of n_vocab
     Event tokens_uploaded;              // guards reuse of h_tokens by the next evaluate()
     DecodeGraphCache decode;            // the decode graphs and the device copy of n_past they read
 
-    void start(int n_batch, int n_ctx, int n_vocab, size_t kv_elems);   // zero-filled KV cache of kv_elems f16 values each for K and V
+    // zero-filled KV cache of kv_elems values of kv_type (T_F16 / T_F32) each for K and V
+    void start(int n_batch, int n_ctx, int n_vocab, size_t kv_elems, int kv_type);
+    size_t kv_elem_bytes() const { return kv_type == T_F32 ? 4 : 2; }
+    size_t kv_bytes() const { return kv_elems * kv_elem_bytes(); }      // of each of memory_k, memory_v
+    // element offset `elems` into memory_k (which = 0) or memory_v (1), in bytes of the cache's type
+    void *kv_at(int which, size_t elems) const { return (which ? memory_v : memory_k).get() + elems * kv_elem_bytes(); }
+    int read_kv(int which, void *host_out, size_t nbytes);            // the raw cache bytes; B200_ERR_TENSOR_SHAPE unless nbytes == kv_bytes()
     int admit(int n) const;             // B200_ERR_BAD_ARG unless 1 <= n <= n_batch, B200_ERR_CONTEXT_FULL if n more positions do not fit
     int stage_tokens(const int32_t *tokens, int n);   // validates the ids and uploads them to d_tokens
     void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)

@@ -145,5 +145,10 @@ void mul_mat_f16(const __half *src0, int64_t ne00, int64_t ne01, int64_t ne02, i
 void mul_mat_f16_exact(const __half *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                        float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st);
+// the same shape contract and causal skip on an f32 cache: ggml_vec_dot_f32 operation order (f32dot.cuh), src1 as it is (F32 type traits: no
+// rounding, LC/ggml.c:1646-1648, 10504-10520)
+void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                       const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
+                       float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st);
 
 }  // namespace b200

@@ -10,6 +10,7 @@
 // of quant_rules.cuh.  The dots run on CUDA cores in the reference's order (tensor cores cannot reproduce it): each thread keeps the 32 chains of
 // the AVX code (element i of a 32-element step -> chain i % 32) for its two outputs, fed from 32-element slices of A and B staged in shared memory.
 #include "../../include/llm_b200.h"
+#include "f32dot.cuh"
 #include "kernels.cuh"
 #include "quant_rules.cuh"
 
@@ -17,17 +18,7 @@ namespace b200 {
 
 constexpr int LP_ROWS = 16, LP_THREADS = 256, LP_RPW = LP_ROWS / (LP_THREADS / 32), LP_STRIDE = 36;   // stride 36: the float4 reads of a quarter-warp hit disjoint banks
 
-// GGML_F32x8_REDUCE (LC/ggml.c:1897-1915), which ggml_vec_dot_f32 and ggml_vec_dot_f16 share, on the 32 chains held by one thread: chains l and l + 16,
-// then l and l + 8, then the two 128-bit halves (l and l + 4), then two hadds -- the association exact.cu spreads over a warp's lanes
-__device__ __forceinline__ float f32x8_reduce(float (&c)[32]) {
-#pragma unroll
-    for (int l = 0; l < 16; l++) c[l] = __fadd_rn(c[l], c[l + 16]);
-#pragma unroll
-    for (int l = 0; l < 8; l++) c[l] = __fadd_rn(c[l], c[l + 8]);
-#pragma unroll
-    for (int l = 0; l < 4; l++) c[l] = __fadd_rn(c[l], c[l + 4]);
-    return __fadd_rn(__fadd_rn(c[0], c[1]), __fadd_rn(c[2], c[3]));
-}
+// the 32 chains of one output end in f32x8_reduce (f32dot.cuh), the GGML_F32x8_REDUCE that ggml_vec_dot_f32 and ggml_vec_dot_f16 share
 
 // w: N rows of the target in GGML layout (WT = T_F32: N rows of K floats).  a: K rows of r (f32, or f16 when A16); b: NB rows of r floats.
 template <int WT, bool A16>
@@ -97,10 +88,8 @@ __global__ void __launch_bounds__(LP_THREADS) lora_patch_kernel(uint8_t *__restr
                 double sd = (double)s[j];
                 for (int i = 0; i < left; i++) sd += (double)__fmul_rn(sa[lane][i], y[i]);
                 s[j] = (float)sd;
-            } else {                                                  // ggml_vec_dot_f32 as compiled: the products of groups of 8 and then 4 are
-                const int nv = left & ~3;                             // vector multiplies, each added in order; the last left % 4 are scalar FMAs
-                for (int i = 0; i < nv; i++) s[j] = __fadd_rn(s[j], __fmul_rn(sa[lane][i], y[i]));
-                for (int i = nv; i < left; i++) s[j] = __fmaf_rn(sa[lane][i], y[i], s[j]);
+            } else {                                                  // ggml_vec_dot_f32 as compiled (f32dot.cuh)
+                s[j] = f32_leftovers(s[j], left, [&](int i) { return sa[lane][i]; }, [&](int i) { return y[i]; });
             }
         }
     }

@@ -199,7 +199,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     // the graph schedule's attention keeps the whole bucket in shared memory: steps in buckets past 3264 positions run per op below, and the
     // graph cache re-uploads the device n_past when graph steps resume (after a rewind)
     // F16 weights decode per op (exact_f16.cu's mat-vec): the graph schedule is built on Q8 activation records
-    if (n == 1 && hp.wtype != T_F16 && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {
+    if (n == 1 && hp.wtype != T_F16 && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {   // f32 cache: up to 1664 positions
         s->last_launches = s->decode.run(n_kv, n_ctx, true, [s, &hp](int bucket, cudaStream_t st, int *nodes) {
             neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
         }, st);
@@ -207,6 +207,8 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         return;
     }
     const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()};
+    const bool kv32 = s->kv_type == T_F32;
+    const int64_t ke = (int64_t)s->kv_elem_bytes();
     const bool gptj = m->gptj(), parallel = m->parallel;
     const RopeTable *rope = m->rope;
     const int64_t ld3 = 3 * (int64_t)e;
@@ -220,7 +222,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     if (m->wpe) { add_f32(s->x.get(), m->wpe + (size_t)n_past * e, s->x.get(), (int64_t)n * e, (int64_t)n * e, st); L++; }               // gpt2 lib.rs:164-172: + wpe[n_past + i]
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &ly = m->layers[il];
-        __half *Kl = s->memory_k.get() + (size_t)il * n_ctx * e, *Vl = s->memory_v.get() + (size_t)il * n_ctx * e;
+        void *Kl = s->kv_at(0, (size_t)il * n_ctx * e), *Vl = s->kv_at(1, (size_t)il * n_ctx * e);
         layer_norm(s->x.get(), s->cur.get(), ly.ln1_g, ly.ln1_b, e, n, st); L++;                                                  // :192-196
         L += mul_mat_exact_auto(ly.wqkv, s->cur.get(), e, n, s->qkv.get(), ld3, nullptr, 0, acts, st);                                // :199
         if (ly.bqkv) { add_f32(s->qkv.get(), ly.bqkv, s->qkv.get(), (int64_t)n * ld3, ld3, st); L++; }                            // :200 (MPT: no bias)
@@ -229,20 +231,26 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
             rope_f32(s->qkv.get() + koff, s->qkv.get() + koff, hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
         }
         {   // k -> cache rows n_past.., v -> cache columns (transposed; GPT-2's v_trans copy of every evaluate is this layout)       :231-247
-            StridedDesc sk{{hd, n_head, n, 1}, {4, hs * 4, ld3 * 4, 0}}, dk{{hd, n_head, n, 1}, {2, (int64_t)hd * 2, (int64_t)e * 2, 0}};
-            cpy_strided(s->qkv.get() + koff, T_F32, sk, Kl + (size_t)n_past * e, T_F16, dk, st); L++;
-            StridedDesc dv{{hd, n_head, n, 1}, {(int64_t)n_ctx * 2, (int64_t)hd * n_ctx * 2, 2, 0}};
-            cpy_strided(s->qkv.get() + voff, T_F32, sk, Vl + n_past, T_F16, dv, st); L++;
+            StridedDesc sk{{hd, n_head, n, 1}, {4, hs * 4, ld3 * 4, 0}}, dk{{hd, n_head, n, 1}, {ke, (int64_t)hd * ke, (int64_t)e * ke, 0}};
+            cpy_strided(s->qkv.get() + koff, T_F32, sk, (char *)Kl + (size_t)n_past * e * ke, s->kv_type, dk, st); L++;
+            StridedDesc dv{{hd, n_head, n, 1}, {(int64_t)n_ctx * ke, (int64_t)hd * n_ctx * ke, ke, 0}};
+            cpy_strided(s->qkv.get() + voff, T_F32, sk, (char *)Vl + (size_t)n_past * ke, s->kv_type, dv, st); L++;
         }
-        mul_mat_f16_exact(Kl, hd, n_kv, n_head, (int64_t)e * 2, (int64_t)hd * 2, s->qkv.get(), n, n_head, ld3 * 4, hs * 4,
-                          s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st); L++;                          // :250-267
+        if (kv32) mul_mat_f32_exact((const float *)Kl, hd, n_kv, n_head, (int64_t)e * 4, (int64_t)hd * 4, s->qkv.get(), n, n_head, ld3 * 4, hs * 4,
+                                    s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st);
+        else mul_mat_f16_exact((const __half *)Kl, hd, n_kv, n_head, (int64_t)e * 2, (int64_t)hd * 2, s->qkv.get(), n, n_head, ld3 * 4, hs * 4,
+                               s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st);
+        L++;                                                                                                                      // :250-267
         if (m->alibi) soft_max_alibi(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, m->kq_scale, n_past, m->alibi.get(), st);   // MPT / BLOOM: + ALiBi
         else soft_max(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, m->kq_scale, true, n_past, true, true, st);                // :270-279
         L++;
         // GPT-J: cur (ln_1's output, input_sa) still feeds fc_in, so the merged KQV goes to t
         float *kqv = gptj ? s->t.get() : s->cur.get();
-        mul_mat_f16_exact(Vl, n_kv, hd, n_head, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2, s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
-                          kqv, (int64_t)e * 4, (int64_t)hd * 4, -1, st); L++;                                               // :282-298
+        if (kv32) mul_mat_f32_exact((const float *)Vl, n_kv, hd, n_head, (int64_t)n_ctx * 4, (int64_t)n_ctx * hd * 4, s->kq.get(), n, n_head, (int64_t)n_kv * 4,
+                                    (int64_t)n_kv * n * 4, kqv, (int64_t)e * 4, (int64_t)hd * 4, -1, st);
+        else mul_mat_f16_exact((const __half *)Vl, n_kv, hd, n_head, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2, s->kq.get(), n, n_head, (int64_t)n_kv * 4,
+                               (int64_t)n_kv * n * 4, kqv, (int64_t)e * 4, (int64_t)hd * 4, -1, st);
+        L++;                                                                                                                      // :282-298
         L += mul_mat_exact_auto(ly.wdense, kqv, e, n, s->attn.get(), e, nullptr, 0, acts, st);                                        // :301
         if (gptj) {   // gptj lib.rs:265-282: t = (fc_out gelu(fc_in input_sa + b_in) + b_out) + attn; inpL = t + inpL
             L += mul_mat_exact_auto(ly.wfc, s->cur.get(), e, n, s->h4.get(), 4 * (int64_t)e, nullptr, 0, acts, st);
@@ -384,14 +392,16 @@ void b200_neox_free(b200_neox_model *m) {
     delete m;                                           // the slab goes with it
 }
 
-b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) {
-    if (!m || n_batch < 1) return nullptr;
+b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) { return b200_neox_start_session_flags(m, n_batch, 0); }
+
+b200_neox_session *b200_neox_start_session_flags(b200_neox_model *m, int32_t n_batch, int32_t flags) {
+    if (!m || n_batch < 1 || (flags & ~B200_SESSION_KV_F32)) return nullptr;
     if (!m->all_loaded()) { fprintf(stderr, "llm_b200: neox start_session: %d of %d tensors loaded\n", m->n_loaded, (int)m->loaded.size()); return nullptr; }
     b200_neox_session *s = new b200_neox_session();
     s->m = m;
     const b200_neox_hparams &hp = m->hp;
     const size_t e = hp.n_embd, B = n_batch, n_ctx = hp.context_size, V = hp.n_vocab;
-    s->start(n_batch, hp.context_size, hp.n_vocab, (size_t)hp.n_layer * n_ctx * e);
+    s->start(n_batch, hp.context_size, hp.n_vocab, (size_t)hp.n_layer * n_ctx * e, (flags & B200_SESSION_KV_F32) ? T_F32 : T_F16);
     s->x = device_alloc<float>(B * e * 4); s->cur = device_alloc<float>(B * e * 4); s->qkv = device_alloc<float>(B * 3 * e * 4);
     s->kq = device_alloc<float>((size_t)hp.n_head * B * n_ctx * 4); s->attn = device_alloc<float>(B * e * 4);
     s->h4 = device_alloc<float>(B * 4 * e * 4); s->hact = device_alloc<float>(B * 4 * e * 4); s->t = device_alloc<float>(B * e * 4);
@@ -404,11 +414,11 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &L = m->layers[il];
         s->dl[il] = NeoxLayer{L.wqkv, L.wdense, L.wfc, L.wproj, L.ln1_g, L.ln1_b, L.ln2_g, L.ln2_b, L.bqkv, L.bdense, L.bfc, L.bproj,
-                              s->memory_k.get() + (size_t)il * n_ctx * e, s->memory_v.get() + (size_t)il * n_ctx * e};
+                              s->kv_at(0, (size_t)il * n_ctx * e), s->kv_at(1, (size_t)il * n_ctx * e)};
     }
     NeoxParams &P = s->dp;
     P.n_layer = hp.n_layer; P.e = (int)e; P.hd = m->hd; P.n_head = hp.n_head; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab;
-    P.parallel_residual = m->parallel; P.qkv_layout = m->qkv_layout; P.n_rot = m->rope && m->rope->mode ? m->rope->n_dims : 0; P.wpe = m->wpe;
+    P.kv_type = s->kv_type; P.parallel_residual = m->parallel; P.qkv_layout = m->qkv_layout; P.n_rot = m->rope && m->rope->mode ? m->rope->n_dims : 0; P.wpe = m->wpe;
     P.alibi = m->alibi.get(); P.emb_g = m->emb_g; P.emb_b = m->emb_b; P.wte = m->wte; P.lm_head = m->lm_head; P.lnf_g = m->lnf_g; P.lnf_b = m->lnf_b;
     P.gptj = m->gptj() ? 1 : 0; P.lm_head_b = m->lm_head_b;
     P.kq_scale = m->kq_scale; P.rope_cs = m->rope ? m->rope->cs : nullptr; P.rope_half = m->rope ? m->rope->half : 0;
@@ -421,14 +431,7 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch) 
 
 int32_t b200_neox_n_past(const b200_neox_session *s) { return s ? s->n_past : -1; }
 int b200_neox_set_n_past(b200_neox_session *s, int32_t n_past) { return s ? s->set_n_past(n_past) : B200_ERR_BAD_ARG; }
-int b200_neox_read_kv(b200_neox_session *s, int32_t which, void *host_out, size_t nbytes) {
-    if (!s || !host_out) return B200_ERR_BAD_ARG;
-    const size_t kv_bytes = (size_t)s->m->hp.n_layer * s->m->hp.context_size * s->m->hp.n_embd * 2;
-    if (nbytes != kv_bytes) return B200_ERR_TENSOR_SHAPE;
-    B200_CHECK(cudaStreamSynchronize(rt().stream));
-    B200_CHECK(cudaMemcpy(host_out, which ? s->memory_v.get() : s->memory_k.get(), kv_bytes, cudaMemcpyDeviceToHost));
-    return B200_OK;
-}
+int b200_neox_read_kv(b200_neox_session *s, int32_t which, void *host_out, size_t nbytes) { return s ? s->read_kv(which, host_out, nbytes) : B200_ERR_BAD_ARG; }
 int32_t b200_neox_last_launches(const b200_neox_session *s) { return s ? s->last_launches : 0; }
 int b200_neox_sync(b200_neox_session *s) { if (!s) return B200_ERR_BAD_ARG; B200_CHECK(cudaStreamSynchronize(rt().stream)); return B200_OK; }
 

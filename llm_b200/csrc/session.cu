@@ -124,6 +124,8 @@ void forward(b200_session *s, int n, bool all_rows = true) {
     int L = 0;
     const bool tp = m->tp_world > 1;
     const bool fast = !tp && (s->cfg.flags & B200_SESSION_FAST) != 0;
+    const bool kv32 = s->kv_type == T_F32;                                                   // InferenceSessionConfig::memory_k_type / memory_v_type
+    const int64_t ke = (int64_t)s->kv_elem_bytes();
     if (tp && (n != 1 || !s->tp_connected)) { fprintf(stderr, "llm_b200: tensor-parallel sessions decode one token per step, after b200_session_tp_connect\n"); exit(1); }
     if (n == 1 && s->graph_ok && !fast && (tp || (!(s->cfg.flags & B200_SESSION_UNFUSED) && s->tap_layer == -2))) {
         // 7 fused kernels per layer, replayed from one CUDA graph per token (decode_ops.cu)
@@ -144,8 +146,8 @@ void forward(b200_session *s, int n, bool all_rows = true) {
     get_rows_q(m->wte, s->d_tokens.get(), s->x.get(), n, st); L++;                                      // :170
     for (il = 0; il < hp.n_layer; il++) {
         const Layer &ly = m->layers[il];
-        __half *Kl = s->memory_k.get() + (size_t)il * n_ctx * gqa;                                  // :227-231
-        __half *Vl = s->memory_v.get() + (size_t)il * n_ctx * gqa;                                  // :233-239
+        void *Kl = s->kv_at(0, (size_t)il * n_ctx * gqa);                                          // :227-231
+        void *Vl = s->kv_at(1, (size_t)il * n_ctx * gqa);                                          // :233-239
         rms_norm(s->x.get(), s->cur.get(), ly.attention_norm, e, n, 5e-6f, st); L++;                    // :183,186
         TAP(1, s->cur.get(), (size_t)n * e);
         L += matmul(s, ly.wqkv, s->cur.get(), s->qkv.get(), qkv_ld, n, nullptr, 0, st, fast);                // :194,208,223
@@ -153,28 +155,34 @@ void forward(b200_session *s, int n, bool all_rows = true) {
         // RoPE on Q and K heads in place: [hd, n_head + n_head_kv, n] with row stride qkv_ld    :190-217
         rope_f32(s->qkv.get(), s->qkv.get(), hd, n_head + n_head_kv, n, hd, qkv_ld, hd, qkv_ld, n_past, rope, st); L++;
         TAP(3, s->qkv.get(), (size_t)n * qkv_ld);
-        {   // store K (row per position) and V (transposed) into the f16 cache                   :243-244
-            StridedDesc sk{{gqa, n, 1, 1}, {4, (int64_t)qkv_ld * 4, 0, 0}}, dk{{gqa, n, 1, 1}, {2, (int64_t)gqa * 2, 0, 0}};
-            cpy_strided(s->qkv.get() + e, T_F32, sk, Kl + (size_t)n_past * gqa, T_F16, dk, st); L++;
-            StridedDesc sv{{n, gqa, 1, 1}, {(int64_t)qkv_ld * 4, 4, 0, 0}}, dv{{n, gqa, 1, 1}, {2, (int64_t)n_ctx * 2, 0, 0}};
-            cpy_strided(s->qkv.get() + e + gqa, T_F32, sv, Vl + n_past, T_F16, dv, st); L++;
+        {   // store K (row per position) and V (transposed) into the cache (f16, or f32 as it is)   :243-244
+            StridedDesc sk{{gqa, n, 1, 1}, {4, (int64_t)qkv_ld * 4, 0, 0}}, dk{{gqa, n, 1, 1}, {ke, (int64_t)gqa * ke, 0, 0}};
+            cpy_strided(s->qkv.get() + e, T_F32, sk, (char *)Kl + (size_t)n_past * gqa * ke, s->kv_type, dk, st); L++;
+            StridedDesc sv{{n, gqa, 1, 1}, {(int64_t)qkv_ld * 4, 4, 0, 0}}, dv{{n, gqa, 1, 1}, {ke, (int64_t)n_ctx * ke, 0, 0}};
+            cpy_strided(s->qkv.get() + e + gqa, T_F32, sv, (char *)Vl + (size_t)n_past * ke, s->kv_type, dv, st); L++;
         }
-        // KQ[h][i][j] = K[j][h] . f16(Q[i][h])                                                    :246-265
-        if (fast) mul_mat_f16(Kl, hd, n_kv, n_head_kv, (int64_t)gqa * 2, (int64_t)hd * 2,
-                              s->qkv.get(), n, n_head, (int64_t)qkv_ld * 4, (int64_t)hd * 4,
-                              s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, st);
-        else mul_mat_f16_exact(Kl, hd, n_kv, n_head_kv, (int64_t)gqa * 2, (int64_t)hd * 2,
+        // KQ[h][i][j] = K[j][h] . f16(Q[i][h])  (f32 cache: K[j][h] . Q[i][h], also in FAST sessions)        :246-265
+        if (kv32) mul_mat_f32_exact((const float *)Kl, hd, n_kv, n_head_kv, (int64_t)gqa * 4, (int64_t)hd * 4,
+                                    s->qkv.get(), n, n_head, (int64_t)qkv_ld * 4, (int64_t)hd * 4,
+                                    s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st);
+        else if (fast) mul_mat_f16((const __half *)Kl, hd, n_kv, n_head_kv, (int64_t)gqa * 2, (int64_t)hd * 2,
+                                   s->qkv.get(), n, n_head, (int64_t)qkv_ld * 4, (int64_t)hd * 4,
+                                   s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, st);
+        else mul_mat_f16_exact((const __half *)Kl, hd, n_kv, n_head_kv, (int64_t)gqa * 2, (int64_t)hd * 2,
                                s->qkv.get(), n, n_head, (int64_t)qkv_ld * 4, (int64_t)hd * 4,
                                s->kq.get(), (int64_t)n_kv * 4, (int64_t)n_kv * n * 4, n_past, st);
         L++;
         TAP(4, s->kq.get(), (size_t)n_head * n * n_kv);
         soft_max(s->kq.get(), s->kq.get(), n_kv, (int64_t)n_head * n, n, kq_scale, true, n_past, true, true, st); L++;   // :268-281
         TAP(5, s->kq.get(), (size_t)n_head * n * n_kv);
-        // KQV[h][i][c] = V[h][c][:] . f16(P[h][i][:]) written straight into the merged [n][e] layout     :284-307
-        if (fast) mul_mat_f16(Vl, n_kv, hd, n_head_kv, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2,
-                              s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
-                              s->cur.get(), (int64_t)e * 4, (int64_t)hd * 4, st);
-        else mul_mat_f16_exact(Vl, n_kv, hd, n_head_kv, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2,
+        // KQV[h][i][c] = V[h][c][:] . f16(P[h][i][:]) (f32 cache: . P[h][i][:]) written straight into the merged [n][e] layout     :284-307
+        if (kv32) mul_mat_f32_exact((const float *)Vl, n_kv, hd, n_head_kv, (int64_t)n_ctx * 4, (int64_t)n_ctx * hd * 4,
+                                    s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
+                                    s->cur.get(), (int64_t)e * 4, (int64_t)hd * 4, -1, st);
+        else if (fast) mul_mat_f16((const __half *)Vl, n_kv, hd, n_head_kv, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2,
+                                   s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
+                                   s->cur.get(), (int64_t)e * 4, (int64_t)hd * 4, st);
+        else mul_mat_f16_exact((const __half *)Vl, n_kv, hd, n_head_kv, (int64_t)n_ctx * 2, (int64_t)n_ctx * hd * 2,
                                s->kq.get(), n, n_head, (int64_t)n_kv * 4, (int64_t)n_kv * n * 4,
                                s->cur.get(), (int64_t)e * 4, (int64_t)hd * 4, -1, st);
         L++;
@@ -407,7 +415,7 @@ static std::vector<DecodeLayer> decode_layers(const b200_session *s) {
     std::vector<DecodeLayer> hl(m->hp.n_layer);
     for (int il = 0; il < m->hp.n_layer; il++) {
         const Layer &L = m->layers[il];
-        hl[il] = DecodeLayer{L.wqkv, L.wo, L.w13, L.w2, L.attention_norm, L.ffn_norm, s->memory_k.get() + il * slice, s->memory_v.get() + il * slice};
+        hl[il] = DecodeLayer{L.wqkv, L.wo, L.w13, L.w2, L.attention_norm, L.ffn_norm, s->kv_at(0, il * slice), s->kv_at(1, il * slice)};
     }
     return hl;
 }
@@ -417,7 +425,7 @@ static std::vector<DecodeLayer> decode_layers(const b200_session *s) {
 static void start_common(b200_session *s) {
     const b200_model *m = s->m;
     const b200_llama_hparams &hp = m->hp;
-    s->start(s->cfg.n_batch, hp.context_size, hp.n_vocab, (size_t)hp.n_layer * hp.context_size * m->gqa_loc);
+    s->start(s->cfg.n_batch, hp.context_size, hp.n_vocab, (size_t)hp.n_layer * hp.context_size * m->gqa_loc, (s->cfg.flags & B200_SESSION_KV_F32) ? T_F32 : T_F16);
     s->topk = device_alloc<int32_t>(2048 * 4);
     s->h_topk = pinned_alloc<int32_t>(2048 * 4);
     s->qbuf = device_alloc<float>((size_t)m->e_loc * 4);
@@ -459,7 +467,7 @@ static b200_session *start_session_tp(b200_session *s) {
     DecodeParams &P = s->dp;
     P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
     P.e = (int)e; P.f = m->f_loc; P.hd = m->hd; P.gqa = m->gqa_loc; P.n_head = hp.n_head / G; P.n_head_kv = hp.n_head_kv / G; P.n_ctx = (int)n_ctx; P.n_vocab = m->v_loc;
-    P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f;
+    P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f; P.kv_type = s->kv_type;
     P.rope_cs = rt_.cs; P.rope_half = rt_.half;
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
@@ -480,6 +488,8 @@ static b200_session *start_session_tp(b200_session *s) {
 b200_session *b200_model_start_session(b200_model *m, const b200_session_config *cfg) {
     if (!m || !cfg || cfg->n_batch < 1) return nullptr;
     if (!m->all_loaded()) { fprintf(stderr, "llm_b200: start_session: %d of %d tensors loaded\n", m->n_loaded, m->n_slots()); return nullptr; }
+    // the tensor-parallel attention lives in the fused f16 kernel's epilogue: an f32 cache there is not offered
+    if (m->tp_world > 1 && (cfg->flags & B200_SESSION_KV_F32)) { fprintf(stderr, "llm_b200: start_session: B200_SESSION_KV_F32 on a tensor-parallel model\n"); return nullptr; }
     b200_session *s = new b200_session();
     s->m = m; s->cfg = *cfg;
     if (m->tp_world > 1) return start_session_tp(s);
@@ -510,7 +520,7 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     DecodeParams &P = s->dp;
     P.n_layer = hp.n_layer; P.wte = m->wte; P.output = m->output; P.norm = m->norm;
     P.e = (int)e; P.f = (int)f; P.hd = m->hd; P.gqa = m->gqa; P.n_head = hp.n_head; P.n_head_kv = hp.n_head_kv; P.n_ctx = (int)n_ctx; P.n_vocab = hp.n_vocab;
-    P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f;
+    P.kq_scale = 1.0f / sqrtf((float)hp.n_embd / (float)hp.n_head); P.eps = 5e-6f; P.kv_type = s->kv_type;
     P.rope_cs = rt_.cs; P.rope_half = rt_.half;
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
@@ -524,9 +534,10 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     // n_embd <= 6144 and context_size % 128 == 0 are limits of the removed one-kernel decode, kept so that the same geometries decode through the graph.
     QWeight probe; probe.nb = (int64_t)e / QK;
     QWeight probe2; probe2.nb = (int64_t)f / QK;
-    // F16 weights decode through the per-op path (exact_f16.cu's mat-vec): the fused schedule is built on Q8 activation records.
+    // F16 weights decode through the per-op path (exact_f16.cu's mat-vec): the fused schedule is built on Q8 activation records.  So does an f32
+    // cache whose context is longer than its two-kernel attention holds (the schedule's attention past 1664 positions).
     s->graph_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && mmv_exact_stream_supported(probe) && mmv_exact_stream_supported(probe2) &&
-                  e <= 6144 && n_ctx % 128 == 0 && hp.wtype != T_F16;
+                  e <= 6144 && n_ctx % 128 == 0 && hp.wtype != T_F16 && (s->kv_type != T_F32 || (int)n_ctx <= attn_sv_f32_max_ctx());
     B200_CHECK(cudaDeviceSynchronize());   // the memsets / copies above ran on the legacy stream: order them before anything on the backend's non-blocking stream
     return s;
 }
@@ -598,13 +609,9 @@ int b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, 
     return B200_OK;
 }
 
+// n_layer x context_size x the cache width (tensor-parallel: this rank's heads) elements of the cache's type
 int b200_session_read_kv(b200_session *s, int32_t which, void *host_out, size_t nbytes) {
-    if (!s || !host_out) return B200_ERR_BAD_ARG;
-    const size_t kv_bytes = (size_t)s->m->hp.n_layer * s->m->hp.context_size * (s->m->tp_world > 1 ? s->m->gqa_loc : s->m->gqa) * 2;   // tensor-parallel: this rank's heads
-    if (nbytes != kv_bytes) return B200_ERR_TENSOR_SHAPE;
-    B200_CHECK(cudaStreamSynchronize(rt().stream));
-    B200_CHECK(cudaMemcpy(host_out, which ? s->memory_v.get() : s->memory_k.get(), kv_bytes, cudaMemcpyDeviceToHost));
-    return B200_OK;
+    return s ? s->read_kv(which, host_out, nbytes) : B200_ERR_BAD_ARG;
 }
 
 int b200_session_set_tap(b200_session *s, int32_t layer, int32_t stage) {

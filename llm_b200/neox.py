@@ -12,7 +12,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .session import LoraAdapters, _check, _Native, _perplexity, ggml_dims
+from .session import LoraAdapters, ModelKVMemoryType, _check, _Native, _perplexity, ggml_dims, kv_array, kv_flags
 
 
 class NeoxHparams(C.Structure):
@@ -35,6 +35,8 @@ def _bind(L):
     L.b200_neox_free.argtypes = [vp]
     L.b200_neox_start_session.restype = vp
     L.b200_neox_start_session.argtypes = [vp, i32]
+    L.b200_neox_start_session_flags.restype = vp
+    L.b200_neox_start_session_flags.argtypes = [vp, i32, i32]
     L.b200_neox_evaluate.argtypes = [vp, vp, i32, vp, i32]
     L.b200_neox_evaluate_device.argtypes = [vp, i32]
     L.b200_neox_n_past.argtypes = [vp]
@@ -99,8 +101,10 @@ class GptNeoX(_Native):
     def weight_bytes(self) -> int:
         return self.L.b200_neox_weight_bytes(self._m)
 
-    def start_session(self, n_batch: int = 8) -> "NeoxSession":
-        return NeoxSession(self, n_batch)
+    def start_session(self, n_batch: int = 8, memory_k_type: ModelKVMemoryType = ModelKVMemoryType.Float16,
+                      memory_v_type: ModelKVMemoryType = ModelKVMemoryType.Float16) -> "NeoxSession":
+        """InferenceSessionConfig's n_batch and KV types (equal types only: ValueError otherwise)"""
+        return NeoxSession(self, n_batch, kv_flags(memory_k_type, memory_v_type))
 
     def bot_token_id(self) -> Optional[int]:
         """KnownModel::bot_token_id: GPT-NeoX, GPT-2 and GPT-J have none; MPT's is "<|padding|>" and BLOOM's "<s>" when the vocabulary has it
@@ -155,9 +159,10 @@ class GptJ(GptNeoX):
 class NeoxSession(_Native):
     _HANDLE, _FREE = "_s", "b200_neox_session_free"
 
-    def __init__(self, model: GptNeoX, n_batch: int):
+    def __init__(self, model: GptNeoX, n_batch: int, flags: int = 0):
         self.model, self.L = model, model.L
-        self._s = self.L.b200_neox_start_session(model._m, n_batch)
+        self.kv_f32 = flags != 0
+        self._s = self.L.b200_neox_start_session_flags(model._m, n_batch, flags)
         if not self._s:
             raise RuntimeError("b200_neox_start_session failed (all tensors loaded?)")
         self.n_vocab = int(model.hyperparameters["n_vocab"])
@@ -186,11 +191,11 @@ class NeoxSession(_Native):
         _check(self.L.b200_neox_set_n_past(self._s, n_past), "rewind")
 
     def kv(self, which: int) -> np.ndarray:
-        """the f16 cache as raw bits: K [n_layer][n_ctx][n_embd] (which = 0), V [n_layer][n_embd][n_ctx] (which = 1)"""
+        """the cache: K [n_layer][n_ctx][n_embd] (which = 0), V [n_layer][n_embd][n_ctx] (which = 1); float32 values of an f32 cache, else the f16 bits"""
         hp = self.model.hyperparameters
-        out = np.empty(hp["n_layer"] * self.model.context_size * hp["n_embd"], np.uint16)
+        out = np.empty(hp["n_layer"] * self.model.context_size * hp["n_embd"] * (4 if self.kv_f32 else 2), np.uint8)
         _check(self.L.b200_neox_read_kv(self._s, which, out.ctypes.data_as(C.c_void_p), out.nbytes), "read_kv")
-        return out
+        return kv_array(out, self.kv_f32)
 
     def sync(self):
         self.L.b200_neox_sync(self._s)

@@ -9,6 +9,7 @@ Names follow the reference so that the parity tests read like its own integratio
   InferenceError::ContextFull      crates/llm-base/src/inference_session.rs:311-313
 """
 import ctypes as C
+import enum
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
@@ -30,10 +31,36 @@ class ModelParameters:
     lora_adapters: Optional[List[str]] = None   # model/mod.rs:205-206: LoRA adapter files, applied in this order to every tensor they name
 
 
+class ModelKVMemoryType(enum.Enum):
+    """ModelKVMemoryType (inference_session.rs:907-922): the element type of memory_k / memory_v"""
+    Float16 = 1                       # GGML_TYPE_F16, the default
+    Float32 = 0                       # GGML_TYPE_F32 (the CLI's --no-float16): twice the bytes, no fp16 rounding in the attention
+
+
+SESSION_KV_F32 = 8                    # B200_SESSION_KV_F32 (include/llm_b200.h)
+
+
+def kv_flags(memory_k_type: ModelKVMemoryType, memory_v_type: ModelKVMemoryType) -> int:
+    """The B200_SESSION_* bits of a (memory_k_type, memory_v_type) pair: one type for both caches, as the reference CLI always sets them"""
+    if memory_k_type != memory_v_type:
+        raise ValueError(f"memory_k_type {memory_k_type} and memory_v_type {memory_v_type} differ: only equal KV types are supported")
+    return SESSION_KV_F32 if memory_k_type == ModelKVMemoryType.Float32 else 0
+
+
+def kv_array(raw: np.ndarray, kv_f32: bool) -> np.ndarray:
+    """a cache read back as raw bytes: float32 values of an f32 cache, the f16 bits (uint16) otherwise"""
+    return raw.view(np.float32) if kv_f32 else raw.view(np.uint16)
+
+
 @dataclass
 class InferenceSessionConfig:
     n_batch: int = 8                  # inference_session.rs:837
     flags: int = 0
+    memory_k_type: ModelKVMemoryType = ModelKVMemoryType.Float16      # inference_session.rs:838-839
+    memory_v_type: ModelKVMemoryType = ModelKVMemoryType.Float16
+
+    def __post_init__(self):
+        kv_flags(self.memory_k_type, self.memory_v_type)
 
 
 @dataclass
@@ -219,7 +246,8 @@ class InferenceSession(_Native):
 
     def __init__(self, model: Llama, config: InferenceSessionConfig):
         self.model, self.config, self.L = model, config, model.L
-        cfg = _lib.SessionConfig(n_batch=config.n_batch, flags=config.flags)
+        self.kv_f32 = kv_flags(config.memory_k_type, config.memory_v_type) != 0
+        cfg = _lib.SessionConfig(n_batch=config.n_batch, flags=config.flags | (SESSION_KV_F32 if self.kv_f32 else 0))
         self._s = self.L.b200_model_start_session(model._m, C.byref(cfg))
         if not self._s:
             raise RuntimeError("b200_model_start_session failed (all tensors loaded?)")
@@ -269,12 +297,14 @@ class InferenceSession(_Native):
         _check(self.L.b200_session_set_n_past(self._s, n_past), "rewind")
 
     def kv(self, which: int) -> np.ndarray:
+        """memory_k (0) / memory_v (1): float32 values of an f32 cache (or a session started with the B200_SESSION_KV_F32 flag), else the f16 bits"""
         hp = self.model.hyperparameters
         gqa = hp["n_embd"] // (hp["n_head"] // hp["n_head_kv"])
         n = hp["n_layer"] * self.model.params.context_size * gqa
-        out = np.empty(n, np.uint16)
+        f32 = self.kv_f32 or bool(self.config.flags & SESSION_KV_F32)
+        out = np.empty(n * (4 if f32 else 2), np.uint8)
         _check(self.L.b200_session_read_kv(self._s, which, out.ctypes.data_as(C.c_void_p), out.nbytes), "read_kv")
-        return out
+        return kv_array(out, f32)
 
     def sync(self):
         self.L.b200_session_sync(self._s)
