@@ -67,6 +67,7 @@ enum {                            /* return codes (0 = ok).  CUDA failures print
     B200_ERR_UNKNOWN_TENSOR = -3, /* LoadError::UnknownTensor */
     B200_ERR_TENSOR_SHAPE = -4,   /* LoadError::TensorWrongSize */
     B200_ERR_NOT_LOADED = -5,
+    B200_ERR_SAMPLER_FAILURE = -6,/* InferenceError::SamplerFailure: the logits row holds a NaN (Logits::try_from_iter) */
     /* file loading (ggml::format::LoadError, crates/ggml/src/format/loader.rs:38-70; llm_base::LoadError) */
     B200_ERR_IO = -10,
     B200_ERR_INVALID_MAGIC = -11,
@@ -75,6 +76,26 @@ enum {                            /* return codes (0 = ok).  CUDA failures print
     B200_ERR_UNSUPPORTED_ELEMENT_TYPE = -14,
     B200_ERR_QUANTIZATION_VERSION = -15,    /* quantized tensors need quantization version 2 (llm-base loader.rs:481-484) */
 };
+
+/* The reference's default sampler chain (crates/llm-base/src/samplers.rs:97-211, ensure_default_slots), run on the device in this order:
+ *   repetition   penalty on each distinct id of the last `repetition_last_n` tokens of the session's history: l <= 0 ? l * penalty : l / penalty
+ *                (penalty 1.0 or last_n 0: off); the logits row itself is not modified
+ *   top-k        value descending, ties by ascending token id; k capped at min(top_k, n_vocab, 1024)
+ *   top-p        p_i = expf(l_i - l_0) / S over the k candidates (S summed in f32 in order); the shortest prefix whose running sum is >= top_p
+ *   temperature  l_i / temperature
+ *   draw         one uniform u = (z >> 40) * 2^-24, z = the `draw`-th SplitMix64 output of `seed`; weights expf(l_i - l_0), the first candidate
+ *                whose running weight sum is > u * (sum of the weights)
+ * All f32 with glibc's expf (oracle/sampler_oracle.c restates it in plain C).  The caller owns the draw counter, so a rewind can replay the same
+ * draws.  top_k = 1 is greedy decoding.  The random stream is this project's, not the reference's StdRng: only greedy decoding matches it. */
+typedef struct {
+    float    repetition_penalty;   /* 1.30 */
+    int32_t  repetition_last_n;    /* 64 */
+    int32_t  top_k;                /* 40; >= 1 */
+    float    top_p;                /* 0.95 */
+    float    temperature;          /* 0.80; > 0 */
+    uint64_t seed;
+    uint64_t draw;                 /* index of this step's uniform in the seed's stream */
+} b200_sampler;
 
 int  b200_init(int device);                                   /* accelerator::initialize(device), accelerator/mod.rs:68-77 */
 int  b200_device_info(int32_t *sm_count, size_t *free_bytes, size_t *total_bytes);
@@ -157,9 +178,23 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
 int  b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits);
 /* feed_prompt: evaluate in chunks of n_batch; last row of logits returned */
 /* sampler hand-off (SURVEY.md 8f-3): the k (<= 1024) largest logits of the last evaluated row, selected on the device -- descending logit,
- * ties by ascending token id -- so that 8 k bytes cross PCIe instead of n_vocab floats */
+ * ties by ascending token id -- so that 8 k bytes cross PCIe instead of n_vocab floats (the top-k stage of b200_session_infer_next_token's
+ * sampler, penalty off) */
 int  b200_session_top_k(b200_session *s, int32_t k, int32_t *ids_out, float *logits_out);
 int  b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out);
+/* InferenceSession::infer_next_token (inference_session.rs:381-419): sample a token from the last evaluated row with the chain of b200_sampler
+ * (history window: the session's tokens), append it to the history and evaluate it as a one-token step.  The id is returned as soon as the
+ * sampler has run, while the step is still on the device; only the id crosses PCIe, and the next call queues behind the step.  End of text is
+ * the caller's test on *token_out: that token has been evaluated, as in the reference.
+ * B200_ERR_CONTEXT_FULL if n_past + 1 >= context_size (the reference's check, one slot stricter than evaluate's), with nothing enqueued;
+ * B200_ERR_SAMPLER_FAILURE on a NaN in the row: n_past, the history and the last row are restored; B200_ERR_BAD_ARG: no row evaluated yet,
+ * top_k < 1, temperature <= 0, penalty <= 0, a negative last_n, null pointers, a tensor-parallel session.  B200_SESSION_FAST sessions run. */
+int  b200_session_infer_next_token(b200_session *s, const b200_sampler *sampler, int32_t *token_out);
+/* the token ids at positions [0, n_past) -- what every evaluate fed and infer_next_token sampled (InferenceSession::tokens); a rewind truncates
+ * them.  Copies min(n_past, max) ids and returns n_past, or a negative error code. */
+int32_t b200_session_read_tokens(b200_session *s, int32_t *tokens_out, int32_t max);
+/* the last evaluated row of logits (InferenceSession::last_logits), n_vocab f32; B200_ERR_BAD_ARG before the first evaluate */
+int  b200_session_last_logits(b200_session *s, float *logits_out);
 /* InferenceSession::perplexity (crates/llm-base/src/inference_session.rs:514-589) over HOST token ids tokens[0, n), computed on the device.
  * With C = context_size, chunk i covers [iC, (i+1)C) for i < n_chunk = n / C (n < C: zero chunks).  Each chunk is evaluated in batches of n_batch
  * with all logits, its first token replaced by `bos` (the model's bot_token_id, else 1); rows j in [min(512, C/2), C - 1) are scored as
@@ -258,6 +293,10 @@ int32_t b200_neox_last_launches(const b200_neox_session *s);
 int  b200_neox_sync(b200_neox_session *s);
 /* b200_session_perplexity for every architecture of this runtime (bos: 1 for GPT-NeoX, GPT-2 and GPT-J; BLOOM's "<s>", MPT's "<|padding|>") */
 int  b200_neox_perplexity(b200_neox_session *s, const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out);
+/* b200_session_infer_next_token / read_tokens / last_logits for every architecture of this runtime */
+int  b200_neox_infer_next_token(b200_neox_session *s, const b200_sampler *sampler, int32_t *token_out);
+int32_t b200_neox_read_tokens(b200_neox_session *s, int32_t *tokens_out, int32_t max);
+int  b200_neox_last_logits(b200_neox_session *s, float *logits_out);
 void b200_neox_session_free(b200_neox_session *s);
 
 /* ---- single-op entry points on HOST buffers (unit tests, INTEGRATION examples).  Each uploads, runs the kernel, downloads. */
@@ -274,6 +313,11 @@ int  b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_ou
 int  b200_op_lora_patch(int32_t wtype, void *w_ggml_inout, int64_t K, int64_t N, int32_t a_type, const void *a, const float *b, int64_t r, float scaling);
 /* the scoring step of b200_session_perplexity on host rows: terms_out[r] = -ln(softmax(logits row r)[targets[r]]), `rows` rows of n_vocab f32 */
 int  b200_op_nll_rows(const float *logits, int64_t rows, int64_t n_vocab, const int32_t *targets, float *terms_out);
+/* the sampler of b200_session_infer_next_token on one host row of n_vocab logits, with the penalty window history[max(0, n_past - last_n), n_past)
+ * (history may be NULL when n_past is 0).  id_out: the sampled id; n_kept_out: the candidates top-p kept; cand_ids_out / cand_probs_out
+ * (nullable, min(top_k, n_vocab, 1024) entries): the top-k candidates in order and their top-p probabilities.  B200_ERR_SAMPLER_FAILURE on a NaN. */
+int  b200_op_sample(const float *logits, int64_t n_vocab, const int32_t *history, int32_t n_past, const b200_sampler *sampler, int32_t *id_out,
+                    int32_t *n_kept_out, int32_t *cand_ids_out, float *cand_probs_out);
 enum { B200_MM_AUTO = 0, B200_MM_VEC = 1, B200_MM_SIMPLE = 2, B200_MM_TENSOR = 3, B200_MM_EXACT = 4, B200_MM_EXACT_STREAM = 5, B200_MM_EXACT_MMA = 6, B200_MM_EXACT_TC5 = 7, B200_MM_FAST_TC5 = 8 };   /* AUTO = the exact kernel the sessions pick for B rows (the streaming mat-vec at B == 1 where K allows it, EXACT below 16, EXACT_MMA below 96, EXACT_TC5 from 96; K-quants: EXACT); TC5 = the tensor-core prefill GEMMs (the name predates the sm_90a port): wgmma/TMA kernel (exact_tc5.cu); FAST_TC5 = order-free dequant->wgmma GEMM (mmq_tc5.cu, non-conformant) */
 
 #ifdef __cplusplus

@@ -7,6 +7,8 @@ This Python package is only the host-side mirror of that interface over ctypes (
 arithmetic and no fallback path.
 """
 from .session import ContextFull, InferenceSession, InferenceSessionConfig, Llama, ModelKVMemoryType, ModelParameters, OutputRequest  # noqa: F401
+from .session import (EndOfText, InferenceFeedback, InferenceParameters, InferenceRequest, InferenceStats, Rng, Sampler,  # noqa: F401
+                      SamplerFailure)
 from . import ggml  # noqa: F401
 
 # enum ggml_type values of the five block formats on the hot path (LC/ggml.h:262-285)

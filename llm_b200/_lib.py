@@ -29,6 +29,12 @@ class SessionConfig(C.Structure):
     _fields_ = [("n_batch", C.c_int32), ("flags", C.c_int32)]
 
 
+class SamplerParams(C.Structure):
+    """b200_sampler (include/llm_b200.h) <- the default chain of crates/llm-base/src/samplers.rs:97-211, with the caller's seed and draw index."""
+    _fields_ = [("repetition_penalty", C.c_float), ("repetition_last_n", C.c_int32), ("top_k", C.c_int32), ("top_p", C.c_float),
+                ("temperature", C.c_float), ("seed", C.c_uint64), ("draw", C.c_uint64)]
+
+
 def lib():
     global _lib
     if _lib is not None:
@@ -65,6 +71,11 @@ def lib():
     L.b200_session_perplexity.argtypes = [vp, vp, i64, i32, vp, vp, C.POINTER(i32)]
     L.b200_op_nll_rows.argtypes = [vp, i64, i64, vp, vp]
     L.b200_session_top_k.argtypes = [vp, i32, vp, vp]
+    L.b200_session_infer_next_token.argtypes = [vp, C.POINTER(SamplerParams), C.POINTER(i32)]
+    L.b200_session_read_tokens.restype = i32
+    L.b200_session_read_tokens.argtypes = [vp, vp, i32]
+    L.b200_session_last_logits.argtypes = [vp, vp]
+    L.b200_op_sample.argtypes = [vp, i64, vp, i32, C.POINTER(SamplerParams), C.POINTER(i32), C.POINTER(i32), vp, vp]
     L.b200_session_evaluate_device.argtypes = [vp, vp, i32]
     L.b200_session_device_logits.restype = vp
     L.b200_session_device_logits.argtypes = [vp]

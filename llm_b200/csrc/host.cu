@@ -127,6 +127,82 @@ void SessionCore::start(int n_batch_, int n_ctx_, int n_vocab_, size_t kv_elems_
     cudaEvent_t ev;
     B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     tokens_uploaded.reset(ev);
+    B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    sampled.reset(ev);
+    history = device_zeros<int32_t>((size_t)n_ctx * 4);
+    sample_keys = device_alloc<uint64_t>(2 * sample_key_bytes(n_vocab));
+    sample_fail = device_zeros<int>(sizeof(int));
+    sample_backup = device_alloc<float>((size_t)n_vocab * 4);
+    topk = device_alloc<int32_t>(2048 * 4);
+    h_topk = pinned_alloc<int32_t>(2048 * 4);
+    void *p = nullptr;
+    B200_CHECK(cudaHostAlloc(&p, sizeof(SampleResult), cudaHostAllocMapped));    // the kernel writes the result straight into host memory
+    h_sample.reset((SampleResult *)p);
+    memset(p, 0, sizeof(SampleResult));
+    B200_CHECK(cudaHostGetDevicePointer((void **)&d_sample, p, 0));
+}
+
+bool sampler_args(const b200_sampler *s, SampleArgs &a) {
+    if (!s || s->top_k < 1 || s->repetition_last_n < 0 || !(s->temperature > 0.0f) || !(s->repetition_penalty > 0.0f) || s->top_p != s->top_p) return false;
+    a = SampleArgs{s->repetition_penalty, s->repetition_last_n, s->top_k, s->top_p, s->temperature, s->seed, s->draw};
+    return true;
+}
+
+// inference_session.rs:381-419.  The sampler's event is recorded before the step is enqueued, so the host learns the id while the step runs
+// and the next call's sampler queues right behind it.
+int SessionCore::infer_next_token(const SampleArgs &a, float *logits, const std::function<void()> &forward1, int32_t *token) {
+    if (!token || last_n < 1) return B200_ERR_BAD_ARG;
+    if (n_past + 1 >= n_ctx) return B200_ERR_CONTEXT_FULL;                                         // :388-390
+    cudaStream_t st = rt().stream;
+    const int row_n = last_n;
+    float *row = logits + (size_t)(row_n - 1) * n_vocab;
+    const SampleBufs b{{sample_keys.get(), sample_keys.get() + sample_key_bytes(n_vocab) / 8}, sample_fail.get(), sample_backup.get()};
+    sample_row(row, n_vocab, history.get(), n_past, a, b, d_tokens.get(), history.get() + n_past, d_sample, nullptr, nullptr, nullptr, st);
+    B200_CHECK(cudaEventRecord(sampled.get(), st));
+    forward1();                                                                                    // :400 model.evaluate(self, &[next_token])
+    B200_CHECK(cudaEventSynchronize(sampled.get()));
+    const volatile SampleResult *r = h_sample.get();
+    if (r->status != 0) {                                                                          // :392-397 SamplerFailure: undo the step
+        B200_CHECK(cudaStreamSynchronize(st));
+        n_past -= 1;                                                                               // the decode graphs re-upload their n_past
+        last_n = row_n;
+        B200_CHECK(cudaMemcpyAsync(row, sample_backup.get(), (size_t)n_vocab * 4, cudaMemcpyDeviceToDevice, st));
+        B200_CHECK(cudaStreamSynchronize(st));
+        return B200_ERR_SAMPLER_FAILURE;
+    }
+    *token = r->id;
+    return B200_OK;
+}
+
+int SessionCore::top_k(const float *logits, int k, int32_t *ids_out, float *vals_out) {
+    if (!ids_out || !vals_out || k < 1 || k > 1024 || k > n_vocab || last_n < 1) return B200_ERR_BAD_ARG;
+    cudaStream_t st = rt().stream;
+    const SampleArgs a{1.0f, 0, k, 1.0f, 1.0f, 0, 0};                                              // the top-k stage alone
+    const SampleBufs b{{sample_keys.get(), sample_keys.get() + sample_key_bytes(n_vocab) / 8}, sample_fail.get(), nullptr};
+    int32_t *d_ids = topk.get();
+    float *d_vals = (float *)(topk.get() + 1024);
+    sample_row(logits + (size_t)(last_n - 1) * n_vocab, n_vocab, nullptr, n_past, a, b, nullptr, nullptr, nullptr, d_ids, d_vals, nullptr, st);
+    B200_CHECK(cudaMemcpyAsync(h_topk.get(), d_ids, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaMemcpyAsync(h_topk.get() + 1024, d_vals, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    memcpy(ids_out, h_topk.get(), (size_t)k * 4);
+    memcpy(vals_out, h_topk.get() + 1024, (size_t)k * 4);
+    return B200_OK;
+}
+
+int32_t SessionCore::read_tokens(int32_t *out, int32_t max) {
+    if (max < 0 || (!out && max > 0)) return B200_ERR_BAD_ARG;
+    const int32_t n = n_past < max ? n_past : max;
+    B200_CHECK(cudaStreamSynchronize(rt().stream));
+    if (n > 0) B200_CHECK(cudaMemcpy(out, history.get(), (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return n_past;
+}
+
+int SessionCore::last_logits(const float *logits, float *out) {
+    if (!out || last_n < 1) return B200_ERR_BAD_ARG;
+    B200_CHECK(cudaStreamSynchronize(rt().stream));
+    B200_CHECK(cudaMemcpy(out, logits + (size_t)(last_n - 1) * n_vocab, (size_t)n_vocab * 4, cudaMemcpyDeviceToHost));
+    return B200_OK;
 }
 
 int SessionCore::read_kv(int which, void *host_out, size_t nbytes) {
@@ -149,8 +225,13 @@ int SessionCore::stage_tokens(const int32_t *tokens, int n) {
     B200_CHECK(cudaEventSynchronize(tokens_uploaded.get()));   // the previous (feed-only) call may still be reading the staging buffer
     memcpy(h_tokens.get(), tokens, (size_t)n * 4);
     B200_CHECK(cudaMemcpyAsync(d_tokens.get(), h_tokens.get(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(history.get() + n_past, h_tokens.get(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
     B200_CHECK(cudaEventRecord(tokens_uploaded.get(), st));
     return B200_OK;
+}
+
+void SessionCore::record_tokens(int n) {
+    B200_CHECK(cudaMemcpyAsync(history.get() + n_past, d_tokens.get(), (size_t)n * 4, cudaMemcpyDeviceToDevice, rt().stream));
 }
 
 void SessionCore::copy_logits(float *out, const float *logits, int n, bool all_rows) {

@@ -6,11 +6,10 @@
 #include <type_traits>
 #include <vector>
 
+#include "../../include/llm_b200.h"
 #include "decode.h"
 #include "kernels.cuh"
 #include "runtime.h"
-
-struct b200_ggml_file;
 
 namespace b200 {
 
@@ -106,6 +105,7 @@ float lora_scaling(const b200_ggml_file *f);                                // (
 struct SessionCore {
     int n_batch = 0, n_ctx = 0, n_vocab = 0;
     int n_past = 0, last_launches = 0;
+    int last_n = 0;                     // rows of the last evaluate: its last row (last_n - 1) is InferenceSession::last_logits
     // memory_k / memory_v of InferenceSessionConfig::memory_k_type / memory_v_type (one type for both): T_F16 (the default) or T_F32
     int kv_type = T_F16;
     size_t kv_elems = 0;                // elements of each
@@ -114,6 +114,12 @@ struct SessionCore {
     PinnedBuf<float> h_logits;          // n_batch rows of n_vocab
     Event tokens_uploaded;              // guards reuse of h_tokens by the next evaluate()
     DecodeGraphCache decode;            // the decode graphs and the device copy of n_past they read
+    DeviceBuf<int32_t> history;         // InferenceSession::tokens: the ids at positions [0, n_past) (n_ctx slots; a rewind truncates implicitly)
+    // the sampler (sample.cu): key buffers, fail word, the row kept on a failure, top-k output; its result word in mapped pinned memory
+    DeviceBuf<uint64_t> sample_keys; DeviceBuf<int> sample_fail; DeviceBuf<float> sample_backup;
+    DeviceBuf<int32_t> topk; PinnedBuf<int32_t> h_topk;                 // 1024 ids + 1024 logits each (top_k)
+    PinnedBuf<SampleResult> h_sample; SampleResult *d_sample = nullptr;
+    Event sampled;                      // recorded after the sampler, before the step it feeds
 
     // zero-filled KV cache of kv_elems values of kv_type (T_F16 / T_F32) each for K and V
     void start(int n_batch, int n_ctx, int n_vocab, size_t kv_elems, int kv_type);
@@ -123,7 +129,8 @@ struct SessionCore {
     void *kv_at(int which, size_t elems) const { return (which ? memory_v : memory_k).get() + elems * kv_elem_bytes(); }
     int read_kv(int which, void *host_out, size_t nbytes);            // the raw cache bytes; B200_ERR_TENSOR_SHAPE unless nbytes == kv_bytes()
     int admit(int n) const;             // B200_ERR_BAD_ARG unless 1 <= n <= n_batch, B200_ERR_CONTEXT_FULL if n more positions do not fit
-    int stage_tokens(const int32_t *tokens, int n);   // validates the ids and uploads them to d_tokens
+    int stage_tokens(const int32_t *tokens, int n);   // validates the ids and uploads them to d_tokens (and to the history at n_past)
+    void record_tokens(int n);          // d_tokens[0, n) -> history at n_past (evaluate entry points whose ids are already in HBM)
     void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)
     int set_n_past(int v);
     // InferenceSession::perplexity over tokens[0, n) with C = n_ctx: chunk i = [iC, (i+1)C) is evaluated from n_past 0 in batches of n_batch, its
@@ -132,6 +139,16 @@ struct SessionCore {
     // them.  ppl_out: n_chunk values; terms_out (nullable): n_chunk x scored rows.  n_past ends at C (unchanged when n < C).
     int perplexity(const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out, const float *logits,
                    const std::function<void(int)> &forward);
+    // InferenceSession::infer_next_token: the sampler on the last row of `logits` writes the id into d_tokens[0] and the history, then
+    // forward1() enqueues the one-token step (it reads d_tokens and advances n_past); the host waits on the sampler's event only.
+    // B200_ERR_CONTEXT_FULL (nothing enqueued), B200_ERR_SAMPLER_FAILURE (n_past, history and the row restored), B200_ERR_BAD_ARG.
+    int infer_next_token(const SampleArgs &a, float *logits, const std::function<void()> &forward1, int32_t *token);
+    // the k (<= 1024, <= n_vocab) largest logits of the last row, descending, ties by ascending id
+    int top_k(const float *logits, int k, int32_t *ids_out, float *vals_out);
+    int32_t read_tokens(int32_t *out, int32_t max);                    // min(n_past, max) ids of the history; returns n_past
+    int last_logits(const float *logits, float *out);                 // the last evaluated row, n_vocab floats
 };
+// a b200_sampler as the kernels take it; false if it is out of range (top_k < 1, temperature or penalty <= 0 or NaN, last_n < 0, top_p NaN)
+bool sampler_args(const b200_sampler *s, SampleArgs &a);
 
 }  // namespace b200

@@ -103,13 +103,31 @@ struct PplState { float nll; int64_t count; };        // the running f32 nll and
 // state += terms[0..n) in order; *ppl = expf(nll / (f32)count)
 void nll_fold(const float *terms, int64_t n, PplState *state, float *ppl, cudaStream_t st);
 
+// ---- sample.cu : the reference's default sampler chain (repetition, top-k, top-p, temperature, one draw) on a logits row in HBM -----------
+// the draw-th output of SplitMix64 seeded with seed (the draw's uniform is (z >> 40) * 2^-24)
+__host__ __device__ inline uint64_t splitmix64(uint64_t seed, uint64_t draw) {
+    uint64_t z = seed + (draw + 1) * 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+struct SampleArgs { float penalty; int last_n, top_k; float top_p, temperature; uint64_t seed, draw; };   // b200_sampler, checked by the caller
+struct SampleResult { int32_t id, status, n_cand, n_kept; };      // status 0, or 1: a NaN in the row (the id is then -1)
+// device scratch: two key buffers of sample_key_bytes(n_vocab), a zero-initialised fail word, and (nullable) n_vocab floats that receive the
+// row when it fails
+struct SampleBufs { uint64_t *keys[2]; int *fail; float *backup; };
+size_t sample_key_bytes(int n_vocab);
+// The chain on row[0, n_vocab) with the penalty window hist[max(0, n_past - last_n), n_past).  The id goes to *tok_dst and *hist_dst, the
+// result to *res (mapped host memory: written last, after a system fence); each nullable.  cand_* (nullable): the min(k, n_vocab, 1024)
+// candidates in order -- ids, their unpenalized logits row[id], and their top-p probabilities.  Nothing is written to row.
+void sample_row(const float *row, int n_vocab, const int32_t *hist, int n_past, const SampleArgs &a, const SampleBufs &b, int32_t *tok_dst, int32_t *hist_dst,
+                SampleResult *res, int32_t *cand_ids, float *cand_vals, float *cand_probs, cudaStream_t st);
+
 // ---- rowops.cu : warp/block-reduce kernels ------------------------------------------------------------------------
 struct Luts { const uint16_t *silu, *gelu, *exp; };   // 3 x 64 Ki fp16 tables built on the host with libm (LC/ggml.c:4313-4326)
 const Luts &luts();                                   // uploaded on first use
 // y = x / sqrt(mean(x^2) + eps) [* gain]   (LC/ggml.c:10129-10175 + the following ggml_mul node)
 void rms_norm(const float *x, float *y, const float *gain, int64_t n, int64_t rows, float eps, cudaStream_t st);
-// the k largest of x[0..n) in descending order (ties: smaller index first); k <= 1024
-void top_k_rows(const float *x, int64_t n, int k, int32_t *ids, float *vals, cudaStream_t st);
 // y = (x - mean) / sqrt(var + 1e-5) [* gain] [+ bias]   (LC/ggml.c:10063-10111)
 void layer_norm(const float *x, float *y, const float *gain, const float *bias, int64_t n, int64_t rows, cudaStream_t st);
 // rows of nc: optional scale, optional causal mask (col > n_past + (row % nr) -> -inf), softmax through the fp16 exp table

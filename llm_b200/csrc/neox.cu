@@ -204,6 +204,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
             neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
         }, st);
         s->n_past += 1;
+        s->last_n = 1;
         return;
     }
     const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()};
@@ -287,6 +288,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         if (m->lm_head_b) { add_f32(row, m->lm_head_b, row, hp.n_vocab, hp.n_vocab, st); L++; }
     }
     s->last_launches = L;
+    s->last_n = n;
     s->n_past += n;
 }
 
@@ -439,6 +441,7 @@ int b200_neox_sync(b200_neox_session *s) { if (!s) return B200_ERR_BAD_ARG; B200
 int b200_neox_evaluate_device(b200_neox_session *s, int32_t n) {
     if (!s) return B200_ERR_BAD_ARG;
     if (const int rc = s->admit(n)) return rc;
+    s->record_tokens(n);
     forward(s, n, true);
     return B200_OK;
 }
@@ -456,6 +459,15 @@ int b200_neox_perplexity(b200_neox_session *s, const int32_t *tokens, int64_t n,
     if (!s) return B200_ERR_BAD_ARG;
     return s->perplexity(tokens, n, bos, ppl_out, terms_out, n_chunk_out, s->logits.get(), [s](int rows) { forward(s, rows, true); });
 }
+
+int b200_neox_infer_next_token(b200_neox_session *s, const b200_sampler *sampler, int32_t *token_out) {
+    SampleArgs a;
+    if (!s || !sampler_args(sampler, a)) return B200_ERR_BAD_ARG;
+    return s->infer_next_token(a, s->logits.get(), [s]() { forward(s, 1, true); }, token_out);
+}
+
+int32_t b200_neox_read_tokens(b200_neox_session *s, int32_t *tokens_out, int32_t max) { return s ? s->read_tokens(tokens_out, max) : B200_ERR_BAD_ARG; }
+int b200_neox_last_logits(b200_neox_session *s, float *logits_out) { return s ? s->last_logits(s->logits.get(), logits_out) : B200_ERR_BAD_ARG; }
 
 void b200_neox_session_free(b200_neox_session *s) {
     if (!s) return;

@@ -1,8 +1,11 @@
 // llm_b200/csrc/ops.cu -- single-op entry points on host buffers (include/llm_b200.h: b200_op_*): one kernel family per call, for tests and
 // kernel benchmarks
+#include <string.h>
+
 #include <vector>
 
 #include "../../include/llm_b200.h"
+#include "host.h"
 #include "kernels.cuh"
 #include "runtime.h"
 
@@ -204,6 +207,39 @@ int b200_op_nll_rows(const float *logits, int64_t rows, int64_t n_vocab, const i
     nll_rows(dl, rows, n_vocab, dtg, dt, st);
     B200_CHECK(cudaMemcpyAsync(terms_out, dt, (size_t)rows * 4, cudaMemcpyDeviceToHost, st));
     B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
+int b200_op_sample(const float *logits, int64_t n_vocab, const int32_t *history, int32_t n_past, const b200_sampler *sampler, int32_t *id_out,
+                   int32_t *n_kept_out, int32_t *cand_ids_out, float *cand_probs_out) {
+    SampleArgs a;
+    if (!logits || !id_out || n_vocab < 1 || n_vocab > INT32_MAX / 2 || n_past < 0 || (n_past > 0 && !history) || !sampler_args(sampler, a)) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    const int V = (int)n_vocab, kk = a.top_k < V ? (a.top_k < 1024 ? a.top_k : 1024) : (V < 1024 ? V : 1024);
+    float *dl = (float *)R.op_arena.get((size_t)V * 4, st);
+    int32_t *dh = (int32_t *)R.op_arena.get((size_t)(n_past > 0 ? n_past : 1) * 4, st);
+    int32_t *dids = (int32_t *)R.op_arena.get((size_t)kk * 4, st);
+    float *dprobs = (float *)R.op_arena.get((size_t)kk * 4, st);
+    SampleResult *dres = (SampleResult *)R.op_arena.get(sizeof(SampleResult), st);
+    SampleBufs b{{(uint64_t *)R.op_arena.get(sample_key_bytes(V), st), (uint64_t *)R.op_arena.get(sample_key_bytes(V), st)},
+                 (int *)R.op_arena.get(sizeof(int), st), nullptr};
+    B200_CHECK(cudaMemcpyAsync(dl, logits, (size_t)V * 4, cudaMemcpyHostToDevice, st));
+    if (n_past > 0) B200_CHECK(cudaMemcpyAsync(dh, history, (size_t)n_past * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemsetAsync(b.fail, 0, sizeof(int), st));
+    sample_row(dl, V, dh, n_past, a, b, nullptr, nullptr, dres, dids, nullptr, dprobs, st);
+    SampleResult r;
+    std::vector<int32_t> ids(kk);
+    std::vector<float> probs(kk);
+    B200_CHECK(cudaMemcpyAsync(&r, dres, sizeof(r), cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaMemcpyAsync(ids.data(), dids, (size_t)kk * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaMemcpyAsync(probs.data(), dprobs, (size_t)kk * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    if (r.status != 0) return B200_ERR_SAMPLER_FAILURE;
+    *id_out = r.id;
+    if (n_kept_out) *n_kept_out = r.n_kept;
+    if (cand_ids_out) memcpy(cand_ids_out, ids.data(), (size_t)kk * 4);
+    if (cand_probs_out) memcpy(cand_probs_out, probs.data(), (size_t)kk * 4);
     return B200_OK;
 }
 

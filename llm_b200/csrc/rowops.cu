@@ -107,50 +107,6 @@ __global__ void rms_norm_kernel(const float *__restrict__ x, float *__restrict__
         yr[i] = v;
     }
 }
-// ---- top-k of one row: k selection passes over a strict total order (value descending, index ascending); nothing is modified, an element is
-//      eligible in pass p iff it comes after the element selected in pass p-1 ----------------------------------------------------------------
-__global__ void __launch_bounds__(1024) top_k_kernel(const float *__restrict__ x, int64_t n, int k, int32_t *__restrict__ ids, float *__restrict__ vals) {
-    __shared__ float sv[32];
-    __shared__ int si[32];
-    __shared__ float last_v;
-    __shared__ int last_i;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) { last_v = INFINITY; last_i = -1; }
-    __syncthreads();
-    for (int p = 0; p < k; p++) {
-        const float lv = last_v; const int li = last_i;
-        float bv = -INFINITY; int bi = 0x7fffffff;
-        for (int64_t i = tid; i < n; i += 1024) {
-            const float v = x[i];
-            const bool eligible = v < lv || (v == lv && (int)i > li);
-            if (eligible && (v > bv || (v == bv && (int)i < bi))) { bv = v; bi = (int)i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-        }
-        if (lane == 0) { sv[warp] = bv; si[warp] = bi; }
-        __syncthreads();
-        if (warp == 0) {
-            bv = sv[lane]; bi = si[lane];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-            }
-            if (lane == 0) { last_v = bv; last_i = bi; ids[p] = bi; vals[p] = bv; }
-        }
-        __syncthreads();
-    }
-}
-
-void top_k_rows(const float *x, int64_t n, int k, int32_t *ids, float *vals, cudaStream_t st) {
-    B200_ASSERT(k >= 1 && k <= 1024 && n >= k && n < 0x7fffffff);
-    top_k_kernel<<<1, 1024, 0, st>>>(x, n, k, ids, vals);
-    B200_CHECK(cudaGetLastError());
-}
-
 void rms_norm(const float *x, float *y, const float *gain, int64_t n, int64_t rows, float eps, cudaStream_t st) {
     if (rows == 0) return;
     const int threads = n >= 4096 ? 512 : 256;

@@ -45,10 +45,7 @@ struct b200_session : SessionCore {     // memory_k [n_layer][n_ctx][gqa], memor
     b200_session_config cfg;
     // activations (sized for n_batch rows)
     DeviceBuf<float> x, cur, ff, qkv, kq, h13, hmul, logits;
-    DeviceBuf<int32_t> topk;            // 1024 ids + 1024 logits (b200_session_top_k)
     DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh;
-    PinnedBuf<int32_t> h_topk;
-    int last_n = 0;
     // the graph decode schedule (decode_ops.cu)
     DeviceBuf<unsigned long long> d_prof;
     DeviceBuf<float> qbuf; DeviceBuf<int4> xpack_d, xpack_f;
@@ -420,14 +417,12 @@ static std::vector<DecodeLayer> decode_layers(const b200_session *s) {
     return hl;
 }
 
-// what single-GPU and tensor-parallel sessions both allocate: the KV cache (this rank's heads), token and logits staging, top-k, and the decode
-// schedules' q vector, activation records and timeline slots
+// what single-GPU and tensor-parallel sessions both allocate: the KV cache (this rank's heads), token and logits staging, the sampler's
+// buffers, and the decode schedules' q vector, activation records and timeline slots
 static void start_common(b200_session *s) {
     const b200_model *m = s->m;
     const b200_llama_hparams &hp = m->hp;
     s->start(s->cfg.n_batch, hp.context_size, hp.n_vocab, (size_t)hp.n_layer * hp.context_size * m->gqa_loc, (s->cfg.flags & B200_SESSION_KV_F32) ? T_F32 : T_F16);
-    s->topk = device_alloc<int32_t>(2048 * 4);
-    s->h_topk = pinned_alloc<int32_t>(2048 * 4);
     s->qbuf = device_alloc<float>((size_t)m->e_loc * 4);
     s->xpack_a = device_alloc<int4>((size_t)(hp.n_embd / QK) * 64);
     s->d_prof = device_zeros<unsigned long long>(B200_PROF_SLOTS * 8 * sizeof(unsigned long long));
@@ -551,6 +546,7 @@ int b200_session_evaluate_device(b200_session *s, const int32_t *d_tokens, int32
     if (const int rc = s->admit(n)) return rc;
     if (d_tokens && d_tokens != s->d_tokens.get())
         B200_CHECK(cudaMemcpyAsync(s->d_tokens.get(), d_tokens, (size_t)n * 4, cudaMemcpyDeviceToDevice, rt().stream));
+    s->record_tokens(n);
     forward(s, n);
     return B200_OK;
 }
@@ -580,22 +576,22 @@ int b200_session_perplexity(b200_session *s, const int32_t *tokens, int64_t n, i
     return s->perplexity(tokens, n, bos, ppl_out, terms_out, n_chunk_out, s->logits.get(), [s](int rows) { forward(s, rows); });
 }
 
-// Sampler hand-off (SURVEY.md §8f-3): the k largest logits of the last evaluated row, selected on the device; 8 k bytes cross PCIe instead of
-// n_vocab floats.  Order = descending logit, ties by ascending token id (what a stable descending sort of (id, logit) pairs yields: llm-samplers top-k).
+// Sampler hand-off (SURVEY.md §8f-3): the k largest logits of the last evaluated row, selected on the device (the sampler's top-k stage, sample.cu);
+// 8 k bytes cross PCIe instead of n_vocab floats.  Order = descending logit, ties by ascending token id (what a stable descending sort of
+// (id, logit) pairs yields: llm-samplers top-k).
 int b200_session_top_k(b200_session *s, int32_t k, int32_t *ids_out, float *logits_out) {
-    if (!s || !ids_out || !logits_out || k < 1 || k > 1024 || k > s->m->hp.n_vocab || s->last_n < 1) return B200_ERR_BAD_ARG;
-    cudaStream_t st = rt().stream;
-    const size_t V = s->m->hp.n_vocab;
-    int32_t *d_ids = s->topk.get();
-    float *d_vals = (float *)(s->topk.get() + 1024);
-    top_k_rows(s->logits.get() + (size_t)(s->last_n - 1) * V, (int64_t)V, k, d_ids, d_vals, st);
-    B200_CHECK(cudaMemcpyAsync(s->h_topk.get(), d_ids, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
-    B200_CHECK(cudaMemcpyAsync(s->h_topk.get() + 1024, d_vals, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
-    B200_CHECK(cudaStreamSynchronize(st));
-    memcpy(ids_out, s->h_topk.get(), (size_t)k * 4);
-    memcpy(logits_out, s->h_topk.get() + 1024, (size_t)k * 4);
-    return B200_OK;
+    return s ? s->top_k(s->logits.get(), k, ids_out, logits_out) : B200_ERR_BAD_ARG;
 }
+
+// InferenceSession::infer_next_token (SessionCore::infer_next_token): tensor-parallel sessions are refused, FAST sessions run
+int b200_session_infer_next_token(b200_session *s, const b200_sampler *sampler, int32_t *token_out) {
+    SampleArgs a;
+    if (!s || s->m->tp_world > 1 || !sampler_args(sampler, a)) return B200_ERR_BAD_ARG;
+    return s->infer_next_token(a, s->logits.get(), [s]() { forward(s, 1); }, token_out);
+}
+
+int32_t b200_session_read_tokens(b200_session *s, int32_t *tokens_out, int32_t max) { return s ? s->read_tokens(tokens_out, max) : B200_ERR_BAD_ARG; }
+int b200_session_last_logits(b200_session *s, float *logits_out) { return s ? s->last_logits(s->logits.get(), logits_out) : B200_ERR_BAD_ARG; }
 
 int b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out) {
     if (!s || !tokens || n < 0) return B200_ERR_BAD_ARG;

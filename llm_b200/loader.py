@@ -194,6 +194,7 @@ def load(path: str, params: ModelParameters = None, device: int = 0) -> Llama:
         raise RuntimeError(f"b200_init failed with code {rc}")
     with_hp = GgmlFile(path)
     hp = with_hp.llama_hyperparameters()
+    vocabulary = [t for t, _ in with_hp.vocabulary()]
     with_hp.close()
     err = C.c_int(0)
     if params.lora_adapters:
@@ -206,4 +207,5 @@ def load(path: str, params: ModelParameters = None, device: int = 0) -> Llama:
         raise LoadError(err.value, f"load {path}")
     model = Llama.__new__(Llama)
     model.L, model.hyperparameters, model.params, model._m = L, hp, params, m
+    model.vocabulary = vocabulary                                  # eot_token_id()
     return model

@@ -12,7 +12,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .session import LoraAdapters, ModelKVMemoryType, _check, _Native, _perplexity, ggml_dims, kv_array, kv_flags
+from .session import ContextFull, LoraAdapters, ModelKVMemoryType, _check, _Generation, _Native, _perplexity, _vocab_id, ggml_dims, kv_array, kv_flags
 
 
 class NeoxHparams(C.Structure):
@@ -45,6 +45,10 @@ def _bind(L):
     L.b200_neox_last_launches.argtypes = [vp]
     L.b200_neox_sync.argtypes = [vp]
     L.b200_neox_perplexity.argtypes = [vp, vp, C.c_int64, i32, vp, vp, C.POINTER(i32)]
+    L.b200_neox_infer_next_token.argtypes = [vp, C.POINTER(_lib.SamplerParams), C.POINTER(i32)]
+    L.b200_neox_read_tokens.restype = i32
+    L.b200_neox_read_tokens.argtypes = [vp, vp, i32]
+    L.b200_neox_last_logits.argtypes = [vp, vp]
     L.b200_neox_session_free.argtypes = [vp]
     L._neox_ready = True
     return L
@@ -58,6 +62,7 @@ class GptNeoX(_Native):
     _HANDLE, _FREE = "_m", "b200_neox_free"
 
     BOT_TOKEN: Optional[bytes] = None       # the vocabulary entry bot_token_id() names (MPT, BLOOM); None: the model has no BOS token
+    EOT_TOKEN: bytes = b"<|endoftext|>"     # the entry eot_token_id() names (gptneox lib.rs:376-378, gpt2 :353-355, gptj :329-331, mpt :277-279)
 
     def __init__(self, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray] = None, context_size: int = None, device: int = 0,
                  lora_adapters: Optional[List[str]] = None, vocabulary: Optional[Sequence] = None):
@@ -111,10 +116,12 @@ class GptNeoX(_Native):
         (mpt lib.rs:273-275, bloom lib.rs:356-358).  Without a vocabulary there is nothing to look up: None."""
         if self.BOT_TOKEN is None or self.vocabulary is None:
             return None
-        try:
-            return self.vocabulary.index(self.BOT_TOKEN)
-        except ValueError:
-            return None
+        return _vocab_id(self.vocabulary, self.BOT_TOKEN)
+
+    def eot_token_id(self) -> Optional[int]:
+        """KnownModel::eot_token_id: "<|endoftext|>" (BLOOM: "</s>") in the vocabulary.  The reference panics when it is missing; here that, and
+        a model without a vocabulary, give None (no end of text)."""
+        return None if self.vocabulary is None else _vocab_id(self.vocabulary, self.EOT_TOKEN)
 
 
 class Gpt2(GptNeoX):
@@ -144,6 +151,7 @@ class Bloom(Mpt):
     "layers.N.attention.{query_key_value,wo}.{weight,bias}", "layers.N.feed_forward.{w1,w2}.{weight,bias}"."""
     ARCH = 3
     BOT_TOKEN = b"<s>"
+    EOT_TOKEN = b"</s>"                     # bloom lib.rs:360-362
 
     def _alibi_bias_max(self):
         return 8.0
@@ -156,16 +164,19 @@ class GptJ(GptNeoX):
     ARCH = 4
 
 
-class NeoxSession(_Native):
+class NeoxSession(_Generation, _Native):
     _HANDLE, _FREE = "_s", "b200_neox_session_free"
+    _INFER, _TOKENS, _LAST = "b200_neox_infer_next_token", "b200_neox_read_tokens", "b200_neox_last_logits"
 
     def __init__(self, model: GptNeoX, n_batch: int, flags: int = 0):
         self.model, self.L = model, model.L
         self.kv_f32 = flags != 0
+        self.n_batch = n_batch
         self._s = self.L.b200_neox_start_session_flags(model._m, n_batch, flags)
         if not self._s:
             raise RuntimeError("b200_neox_start_session failed (all tensors loaded?)")
         self.n_vocab = int(model.hyperparameters["n_vocab"])
+        self._last_logits = np.zeros(self.n_vocab, np.float32)
 
     @property
     def n_past(self) -> int:
@@ -179,12 +190,26 @@ class NeoxSession(_Native):
         tokens = np.ascontiguousarray(tokens, np.int32)
         out = np.empty((tokens.size if all_logits else 1, self.n_vocab), np.float32)
         _check(self.L.b200_neox_evaluate(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size, out.ctypes.data_as(C.c_void_p), 1 if all_logits else 0), "evaluate")
+        self._last_logits = out[-1].copy()
         return out if all_logits else out[0]
+
+    def feed_prompt(self, tokens) -> np.ndarray:
+        """InferenceSession::feed_prompt (inference_session.rs:299-350): the prompt in chunks of n_batch; returns last_logits.  ContextFull if
+        it does not fit (nothing is evaluated then); an empty prompt leaves last_logits untouched."""
+        tokens = np.ascontiguousarray(tokens, np.int32).ravel()
+        if tokens.size == 0:
+            return self.last_logits
+        if self.n_past + tokens.size > self.model.context_size:
+            raise ContextFull("feed_prompt")
+        for i in range(0, tokens.size, self.n_batch):
+            self.evaluate(tokens[i:i + self.n_batch])
+        return self.last_logits
 
     def perplexity(self, tokens, callback=None, bos: Optional[int] = None, return_terms: bool = False):
         """InferenceSession::perplexity on the device (see InferenceSession.perplexity); bos defaults to bot_token_id() or 1"""
         bot = self.model.bot_token_id()
         bos = (1 if bot is None else bot) if bos is None else bos
+        self._last_logits = None
         return _perplexity(self.L.b200_neox_perplexity, self._s, tokens, bos, self.model.context_size, callback, return_terms)
 
     def rewind(self, n_past: int):

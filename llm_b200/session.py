@@ -7,11 +7,14 @@ Names follow the reference so that the parity tests read like its own integratio
   InferenceSession                 crates/llm-base/src/inference_session.rs:43-512  feed_prompt / n_past / last_logits
   OutputRequest                    crates/llm-base/src/lib.rs (all_logits), model/common.rs:22-39
   InferenceError::ContextFull      crates/llm-base/src/inference_session.rs:311-313
+  infer_next_token / infer         crates/llm-base/src/inference_session.rs:381-512, InferenceRequest / InferenceStats / InferenceFeedback
+  InferenceParameters / Sampler    crates/llm-base/src/inference_session.rs, samplers.rs:97-211 (the default chain, run on the device)
 """
 import ctypes as C
 import enum
+import time
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional
+from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -20,6 +23,64 @@ from . import _lib
 
 class ContextFull(Exception):
     """InferenceError::ContextFull."""
+
+
+class EndOfText(Exception):
+    """InferenceError::EndOfText: the sampled token is the model's end-of-text token.  It has been evaluated (n_past counts it), as in the
+    reference; `token` is its id."""
+
+    def __init__(self, token: int):
+        super().__init__(f"end of text (token {token})")
+        self.token = token
+
+
+class SamplerFailure(Exception):
+    """InferenceError::SamplerFailure: the last logits row holds a NaN.  n_past, tokens() and last_logits are as they were before the call."""
+
+
+@dataclass
+class Sampler:
+    """The reference's default sampler chain (samplers.rs:97-211, ensure_default_slots), in this order: repetition penalty over the last
+    `repetition_last_n` tokens, top-k, top-p, temperature, one random draw.  Its arithmetic is fixed in include/llm_b200.h (b200_sampler);
+    top_k = 1 is greedy decoding."""
+    repetition_penalty: float = 1.30
+    repetition_last_n: int = 64
+    top_k: int = 40
+    top_p: float = 0.95
+    temperature: float = 0.80
+
+
+@dataclass
+class InferenceParameters:
+    sampler: Sampler = field(default_factory=Sampler)
+
+
+class Rng:
+    """The random stream of the draw: SplitMix64 seeded with `seed`; `draw` is the index of the next uniform.  The caller owns the counter:
+    after a rewind by r tokens, `draw -= r` replays the same draws."""
+
+    def __init__(self, seed: int = 0):
+        self.seed, self.draw = int(seed) & 0xFFFFFFFFFFFFFFFF, 0
+
+
+@dataclass
+class InferenceRequest:
+    prompt: Sequence[int] = ()                      # token ids (tokenization is the caller's)
+    parameters: InferenceParameters = field(default_factory=InferenceParameters)
+    maximum_token_count: Optional[int] = None       # None: until end of text (or ContextFull)
+
+
+@dataclass
+class InferenceStats:
+    feed_prompt_duration: float = 0.0               # seconds
+    prompt_tokens: int = 0                          # n_past after the prompt
+    predict_duration: float = 0.0                   # seconds, from the start of infer
+    predict_tokens: int = 0                         # n_past at the end
+
+
+class InferenceFeedback(enum.Enum):
+    Continue = 0
+    Halt = 1
 
 
 @dataclass
@@ -89,6 +150,8 @@ def llama_tensor_shapes(hp: Dict[str, int]) -> Dict[str, tuple]:
 def _check(rc, what):
     if rc == -1:
         raise ContextFull(what)
+    if rc == -6:
+        raise SamplerFailure(what)
     if rc != 0:
         raise RuntimeError(f"{what} failed with code {rc}")
 
@@ -128,6 +191,78 @@ class _Native:
             self.close()
         except Exception:
             pass
+
+
+class _Generation:
+    """Text generation on a native session (InferenceSession::infer_next_token / infer): `_INFER`, `_TOKENS` and `_LAST` name the library's
+    entry points; the session keeps `model`, `n_vocab`, `L`, `_s`, `_last_logits` (host copy of the last row, None: read it from the device)."""
+    _INFER, _TOKENS, _LAST = "", "", ""
+
+    @property
+    def last_logits(self) -> np.ndarray:
+        """the last evaluated row (zeros before the first evaluate); read from the device on access after generation"""
+        if self._last_logits is None:
+            out = np.zeros(self.n_vocab, np.float32)
+            if getattr(self.L, self._LAST)(self._s, out.ctypes.data_as(C.c_void_p)) != 0:
+                out[:] = 0.0                        # nothing evaluated yet
+            self._last_logits = out
+        return self._last_logits
+
+    def tokens(self) -> np.ndarray:
+        """InferenceSession::tokens: the ids at positions [0, n_past)"""
+        n = self.n_past
+        out = np.empty(max(n, 1), np.int32)
+        got = getattr(self.L, self._TOKENS)(self._s, out.ctypes.data_as(C.c_void_p), n)
+        if got < 0:
+            _check(got, "read_tokens")
+        return out[:min(got, n)].copy()
+
+    def infer_next_token(self, params: Optional[InferenceParameters], rng: Rng) -> int:
+        """Sample the next token from last_logits on the device, append it and evaluate it; returns its id and advances rng.draw.
+        Raises ContextFull (n_past + 1 >= context size; nothing changes), SamplerFailure (nothing changes), or EndOfText (the token is the
+        model's eot_token_id(); it has been evaluated and rng.draw advanced)."""
+        sp = (params or InferenceParameters()).sampler
+        c = _lib.SamplerParams(repetition_penalty=sp.repetition_penalty, repetition_last_n=sp.repetition_last_n, top_k=sp.top_k, top_p=sp.top_p,
+                               temperature=sp.temperature, seed=rng.seed, draw=rng.draw)
+        tok = C.c_int32(-1)
+        _check(getattr(self.L, self._INFER)(self._s, C.byref(c), C.byref(tok)), "infer_next_token")
+        rng.draw += 1
+        self._last_logits = None
+        eot = self.model.eot_token_id()
+        if eot is not None and tok.value == eot:
+            raise EndOfText(tok.value)
+        return tok.value
+
+    def infer(self, request: InferenceRequest, rng: Rng, callback: Optional[Callable[[int], Optional[InferenceFeedback]]] = None) -> InferenceStats:
+        """InferenceSession::infer: feed the prompt, then generate until end of text, maximum_token_count tokens or a callback that returns
+        InferenceFeedback.Halt.  callback(token_id) is called for each generated token but the end-of-text one.  ContextFull is raised, as the
+        reference returns it."""
+        stats = InferenceStats()
+        t0 = time.perf_counter()
+        if len(request.prompt):
+            self.feed_prompt(request.prompt)
+        stats.feed_prompt_duration = time.perf_counter() - t0
+        stats.prompt_tokens = self.n_past
+        limit = request.maximum_token_count
+        done = 0
+        while limit is None or done < limit:
+            try:
+                tok = self.infer_next_token(request.parameters, rng)
+            except EndOfText:
+                break
+            if callback is not None and callback(tok) == InferenceFeedback.Halt:
+                break
+            done += 1
+        stats.predict_duration = time.perf_counter() - t0
+        stats.predict_tokens = self.n_past
+        return stats
+
+
+def _vocab_id(vocabulary, token: bytes) -> Optional[int]:
+    try:
+        return vocabulary.index(token)
+    except ValueError:
+        return None
 
 
 class LoraAdapters:
@@ -175,8 +310,10 @@ class Llama(_Native):
     _HANDLE, _FREE = "_m", "b200_model_free"
 
     def __init__(self, hyperparameters: Dict[str, int], params: ModelParameters = None, tensors: Dict[str, np.ndarray] = None,
-                 device: int = 0):
+                 device: int = 0, vocabulary: Optional[Sequence] = None):
+        """vocabulary: the model file's tokens ((bytes, score) pairs, or bytes), consulted by eot_token_id()"""
         params = params or ModelParameters()
+        self.vocabulary = [t[0] if isinstance(t, tuple) else bytes(t) for t in vocabulary] if vocabulary is not None else None
         if not params.use_gpu:
             raise ValueError("llm_b200 has no CPU path: ModelParameters.use_gpu must be True")
         self.L = _lib.lib()
@@ -240,9 +377,18 @@ class Llama(_Native):
         """KnownModel::bot_token_id: LLaMA has none (llama lib.rs:382-384)"""
         return None
 
+    def eot_token_id(self) -> Optional[int]:
+        """KnownModel::eot_token_id: "</s>" in the vocabulary, else 2 (llama lib.rs:386-388).  Without a vocabulary: None (no end of text)."""
+        vocab = getattr(self, "vocabulary", None)
+        if vocab is None:
+            return None
+        eot = _vocab_id(vocab, b"</s>")
+        return 2 if eot is None else eot
 
-class InferenceSession(_Native):
+
+class InferenceSession(_Generation, _Native):
     _HANDLE, _FREE = "_s", "b200_session_free"
+    _INFER, _TOKENS, _LAST = "b200_session_infer_next_token", "b200_session_read_tokens", "b200_session_last_logits"
 
     def __init__(self, model: Llama, config: InferenceSessionConfig):
         self.model, self.config, self.L = model, config, model.L
@@ -252,7 +398,7 @@ class InferenceSession(_Native):
         if not self._s:
             raise RuntimeError("b200_model_start_session failed (all tensors loaded?)")
         self.n_vocab = int(model.hyperparameters["n_vocab"])
-        self.last_logits = np.zeros(self.n_vocab, np.float32)
+        self._last_logits = np.zeros(self.n_vocab, np.float32)
 
     @property
     def n_past(self) -> int:
@@ -272,7 +418,7 @@ class InferenceSession(_Native):
         out = np.empty((n if all_logits else 1, self.n_vocab), np.float32)
         _check(self.L.b200_session_evaluate(self._s, tokens.ctypes.data_as(C.c_void_p), n, out.ctypes.data_as(C.c_void_p),
                                             1 if all_logits else 0), "evaluate")
-        self.last_logits = out[-1].copy()
+        self._last_logits = out[-1].copy()
         return out if all_logits else out[0]
 
     def feed_prompt(self, tokens) -> np.ndarray:
@@ -282,7 +428,7 @@ class InferenceSession(_Native):
         out = np.empty(self.n_vocab, np.float32)
         _check(self.L.b200_session_feed_prompt(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size,
                                                out.ctypes.data_as(C.c_void_p)), "feed_prompt")
-        self.last_logits = out
+        self._last_logits = out
         return out
 
     def perplexity(self, tokens, callback=None, bos: Optional[int] = None, return_terms: bool = False):
@@ -291,6 +437,7 @@ class InferenceSession(_Native):
         starts at n_past 0; afterwards n_past is context_size (unchanged when there are fewer tokens than that).  See include/llm_b200.h."""
         bot = self.model.bot_token_id()
         bos = (1 if bot is None else bot) if bos is None else bos
+        self._last_logits = None
         return _perplexity(self.L.b200_session_perplexity, self._s, tokens, bos, self.model.params.context_size, callback, return_terms)
 
     def rewind(self, n_past: int):
