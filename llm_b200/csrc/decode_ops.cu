@@ -1,10 +1,11 @@
 // llm_b200/csrc/decode_ops.cu -- the default decode schedule: 7 fused kernels per layer, replayed from ONE CUDA graph per token.
 //
 //   1 norm_pack        rms_norm(x) * attn_norm -> Q8 activation records                       (llama lib.rs:183-186 + mul_mat INIT)
-//   2 mmv<QKV>         [wq|wk|wv] x, epilogue: RoPE on Q/K rows, K/V rows -> f16 cache at n_past (:190-244)
+//   2 mmv<QKV>         [wq|wk|wv] x, epilogue: RoPE on Q/K rows, K/V rows -> cache at n_past (:190-244)
 //   3 attn_fused       KQ = K . f16(Q), scale + soft_max, V^T . f16(P), epilogue: quantize the merged row -- one cluster of hd/32 CTAs per
 //                      head, scores exchanged through distributed shared memory                (:246-307)
-//                      (buckets past 3264 positions: the two-kernel variant attn_kq + attn_sv)
+//                      (buckets past 3264 positions, 1664 on an f32 cache: the two-kernel variant attn_kq + attn_sv)
+// Each attention kernel is one template over the cache's element type KT: __half, or float for an f32 cache (Q and P then stay f32).
 //   4 mmv<RES>         wo x + inpSA                                                           (:310-314)
 //   5 norm_pack        rms_norm(inpFF) * ffn_norm                                             (:318-321)
 //   6 mmv<SILU>        [w1|w3] x (rows interleaved in 32-row pieces), epilogue: silu(w1 x) * (w3 x) quantized (:323-330)
@@ -68,6 +69,11 @@ __device__ __forceinline__ float f16dot_tree(float s) {          // ggml_vec_dot
     s = __fadd_rn(s, __shfl_down_sync(0xffffffffu, s, 2));
     return s;
 }
+// the KV cache's element type KT (__half or float): a float converted to it (f16: rounded to nearest), and one read back as a float
+template <typename KT>
+__device__ __forceinline__ KT kv_cast(float v) { if constexpr (sizeof(KT) == 2) return __float2half_rn(v); else return v; }
+__device__ __forceinline__ float kv_load(__half v) { return __half2float(v); }
+__device__ __forceinline__ float kv_load(float v) { return v; }
 
 // ---- 1 / 6: rms_norm * gain -> records.  grid = e/128 CTAs of 256 threads; every CTA reduces the whole row (16 KB from L2) and
 //      quantizes its own 4 blocks per warp pass. ------------------------------------------------------------------------------------
@@ -288,12 +294,14 @@ __global__ void __launch_bounds__(STHREADS) mmv_fused_kernel(const QWeight w, co
 }
 
 // ---- 3: KQ.  CTA = (64 cached positions, head); CTAs past n_kv exit at once (the grid is sized for the context bucket).  All
-//      16-byte loads of the K tile are issued before the first one is consumed. ---------------------------------------------------------
-template <int HD>
-__global__ void __launch_bounds__(128) attn_kq_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, float *__restrict__ kq,
+//      16-byte loads of the K tile are issued before the first one is consumed.
+//      KT, the cache's element type: f16 rounds q to f16 (ggml_vec_dot_f16); f32 takes q as it is (ggml_vec_dot_f32: the chains and tree of
+//      the f16 dot; hd % 32 == 0 leaves no leftovers). ------------------------------------------------------------------------------------
+template <int HD, typename KT>
+__global__ void __launch_bounds__(128) attn_kq_kernel(const float *__restrict__ q, const KT *__restrict__ Kl, float *__restrict__ kq,
                                                       const int *__restrict__ n_past, int gqa, int n_head, int n_head_kv, int n_ctx, unsigned long long *prof) {
-    __shared__ __align__(16) __half q16[HD];
-    __shared__ __align__(16) __half kt[64 * HD];
+    __shared__ __align__(16) KT qs[HD];
+    __shared__ __align__(16) KT kt[64 * HD];
     pdl_trigger();
     pdl_wait();
     prof_begin(prof);
@@ -303,7 +311,7 @@ __global__ void __launch_bounds__(128) attn_kq_kernel(const float *__restrict__ 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int hk = h / (n_head / n_head_kv);
     const int rows = n_kv - j0 < 64 ? n_kv - j0 : 64;
-    constexpr int VPR = HD / 8;                       // 16-byte vectors per K row
+    constexpr int VPR = HD * (int)sizeof(KT) / 16;    // 16-byte vectors per K row
     constexpr int NV = 64 * VPR / 128;                // vectors per thread
     int4 v[NV];
 #pragma unroll
@@ -311,64 +319,37 @@ __global__ void __launch_bounds__(128) attn_kq_kernel(const float *__restrict__ 
         const int i = tid + u * 128, rr = i / VPR, cc = i % VPR;
         v[u] = rr < rows ? __ldcg((const int4 *)(Kl + (int64_t)(j0 + rr) * gqa + hk * HD) + cc) : make_int4(0, 0, 0, 0);
     }
-    for (int i = tid; i < HD; i += 128) q16[i] = __float2half_rn(__ldcg(q + h * HD + i));
+    for (int i = tid; i < HD; i += 128) qs[i] = kv_cast<KT>(__ldcg(q + h * HD + i));
 #pragma unroll
     for (int u = 0; u < NV; u++) ((int4 *)kt)[tid + u * 128] = v[u];
     __syncthreads();
     for (int jj = warp; jj < rows; jj += 4) {
-        const __half *krow = kt + jj * HD;
+        const KT *krow = kt + jj * HD;
         float s = 0.f;
 #pragma unroll
-        for (int k = 0; k < HD; k += 32) s = __fmaf_rn(__half2float(krow[k + lane]), __half2float(q16[k + lane]), s);
-        s = f16dot_tree(s);
-        if (lane == 0) kq[(int64_t)h * n_ctx + j0 + jj] = (float)(double)s;
-    }
-    prof_end(prof);
-}
-
-// the f32 cache's form: K rows and q as they are (ggml_vec_dot_f32: the chains and tree of the f16 dot; hd % 32 == 0 leaves no leftovers)
-template <int HD>
-__global__ void __launch_bounds__(128) attn_kq_f32_kernel(const float *__restrict__ q, const float *__restrict__ Kl, float *__restrict__ kq,
-                                                          const int *__restrict__ n_past, int gqa, int n_head, int n_head_kv, int n_ctx, unsigned long long *prof) {
-    __shared__ __align__(16) float qs[HD];
-    __shared__ __align__(16) float kt[64 * HD];
-    pdl_trigger();
-    pdl_wait();
-    prof_begin(prof);
-    const int n_kv = __ldcg(n_past) + 1;
-    const int j0 = blockIdx.x * 64, h = blockIdx.y;
-    if (j0 >= n_kv) return;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int hk = h / (n_head / n_head_kv);
-    const int rows = n_kv - j0 < 64 ? n_kv - j0 : 64;
-    constexpr int VPR = HD / 4;                       // 16-byte vectors per K row
-    constexpr int NV = 64 * VPR / 128;                // vectors per thread
-    int4 v[NV];
-#pragma unroll
-    for (int u = 0; u < NV; u++) {
-        const int i = tid + u * 128, rr = i / VPR, cc = i % VPR;
-        v[u] = rr < rows ? __ldcg((const int4 *)(Kl + (int64_t)(j0 + rr) * gqa + hk * HD) + cc) : make_int4(0, 0, 0, 0);
-    }
-    for (int i = tid; i < HD; i += 128) qs[i] = __ldcg(q + h * HD + i);
-#pragma unroll
-    for (int u = 0; u < NV; u++) ((int4 *)kt)[tid + u * 128] = v[u];
-    __syncthreads();
-    for (int jj = warp; jj < rows; jj += 4) {
-        const float *krow = kt + jj * HD;
-        float s = 0.f;
-#pragma unroll
-        for (int k = 0; k < HD; k += 32) s = __fmaf_rn(krow[k + lane], qs[k + lane], s);
-        s = f16dot_tree(s);                           // GGML_F32x8_REDUCE, the tree both dots share
+        for (int k = 0; k < HD; k += 32) s = __fmaf_rn(kv_load(krow[k + lane]), kv_load(qs[k + lane]), s);
+        s = f16dot_tree(s);                           // GGML_F32x8_REDUCE is the same tree
         if (lane == 0) kq[(int64_t)h * n_ctx + j0 + jj] = s;
     }
     prof_end(prof);
 }
 
 // ---- 4: scale + soft_max + KQV for 32 channels of one head, then quantize those 32 outputs (one block of wo's input) ---------------
+//      KT, the cache's element type, is also that of the probabilities (f16: rounded, ggml_vec_dot_f16).  V tiles are 32 rows of 256 bytes
+//      (KC = 128 f16 or 64 f32 positions: 4 vectors per thread); the positions past the last whole 32 are added in double (f16) or by the
+//      f32 leftover rule (f32dot.cuh).  Dynamic shared memory: scores and probabilities for the whole context, a V tile, 32 leftover columns.
 constexpr int KC = 128;
-__global__ void __launch_bounds__(128) attn_sv_kernel(const float *__restrict__ kq, const __half *__restrict__ Vl, int4 *__restrict__ xpack_out,
+constexpr size_t attn_sv_smem(int n_ctx, int kv_type) {
+    const size_t es = kv_type == T_F32 ? 4 : 2;
+    return (size_t)n_ctx * (4 + es) + 32 * KC * 2 + 32 * 32 * es;
+}
+template <typename KT>
+__global__ void __launch_bounds__(128) attn_sv_kernel(const float *__restrict__ kq, const KT *__restrict__ Vl, int4 *__restrict__ xpack_out,
                                                       const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp, float kq_scale,
                                                       int hd, int n_head, int n_head_kv, int n_ctx, int q81, int off, int scale16, unsigned long long *prof) {
+    constexpr bool F32 = sizeof(KT) == 4;
+    constexpr int TC = KC * 2 / (int)sizeof(KT);      // positions per V tile
+    constexpr int TV = TC * (int)sizeof(KT) / 16;     // 16-byte vectors per row of a tile
     extern __shared__ __align__(16) uint8_t sm[];
     __shared__ double shd[8];
     __shared__ float shf[4], stash[32];
@@ -380,114 +361,21 @@ __global__ void __launch_bounds__(128) attn_sv_kernel(const float *__restrict__ 
     const int hk = h / (n_head / n_head_kv);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     float *sc = (float *)sm;
-    __half *p16 = (__half *)(sm + (size_t)n_ctx * 4);
-    __half *vt = (__half *)(sm + (size_t)n_ctx * 6);
-    __half *vleft = vt + 32 * KC;
+    KT *p = (KT *)(sm + (size_t)n_ctx * 4);
+    KT *vt = (KT *)(sm + (size_t)n_ctx * (4 + sizeof(KT)));
+    KT *vleft = vt + 32 * TC;
     // leftover V columns and the first V tile are requested before anything else so that their latency hides behind the soft_max
     const int np = n_kv & ~31;
     if (np < n_kv) {
-        const int rr = tid >> 2, part = tid & 3;
-        ((int4 *)vleft)[tid] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + rr) * n_ctx + np) + part);
-    }
-    int4 pre[KC / 32];
-    auto fetch = [&](int k0) {
+        if constexpr (F32) {
+            constexpr int VL = 8;                     // 16-byte vectors of 32 positions
 #pragma unroll
-        for (int u = 0; u < KC / 32; u++) {
-            const int i = tid + u * 128, rr = i / (KC / 8), cc = i - rr * (KC / 8);
-            pre[u] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + rr) * n_ctx + k0) + cc);
-        }
-    };
-    if (np > 0) fetch(0);
-    float mx = -INFINITY;
-    constexpr int SB = 8;                              // scores per thread per pass: 8 loads in flight
-    for (int jb = 0; jb < n_kv; jb += SB * 128) {
-        float sv[SB];
-#pragma unroll
-        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; sv[u] = j < n_kv ? __ldcg(kq + (int64_t)h * n_ctx + j) : 0.f; }
-#pragma unroll
-        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; if (j < n_kv) { const float v = __fmul_rn(sv[u], kq_scale); sc[j] = v; mx = fmaxf(mx, v); } }
-    }
-    mx = warp_max(mx);
-    if (lane == 0) shf[warp] = mx;
-    __syncthreads();
-    mx = fmaxf(fmaxf(shf[0], shf[1]), fmaxf(shf[2], shf[3]));
-    double s = 0.0;
-    for (int jb = 0; jb < n_kv; jb += SB * 128) {
-        uint16_t ev16[SB];
-#pragma unroll
-        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; ev16[u] = j < n_kv ? __ldg(lut_exp + f32_to_f16_bits(__fsub_rn(sc[j], mx))) : (uint16_t)0; }
-#pragma unroll
-        for (int u = 0; u < SB; u++) { const int j = jb + tid + u * 128; if (j < n_kv) { const float ev = f16_bits_to_f32(ev16[u]); sc[j] = ev; s += (double)ev; } }
-    }
-    s = warp_sum(s);
-    if (lane == 0) shd[warp] = s;
-    __syncthreads();
-    const float inv = (float)(1.0 / ((shd[0] + shd[1]) + (shd[2] + shd[3])));
-    for (int j = tid; j < n_kv; j += 128) p16[j] = __float2half_rn(__fmul_rn(sc[j], inv));
-    float acc[8];
-#pragma unroll
-    for (int cc = 0; cc < 8; cc++) acc[cc] = 0.f;
-    for (int k0 = 0; k0 < np; k0 += KC) {
-        __syncthreads();
-#pragma unroll
-        for (int u = 0; u < KC / 32; u++) ((int4 *)vt)[tid + u * 128] = pre[u];
-        __syncthreads();
-        if (k0 + KC < np) fetch(k0 + KC);
-        const int kend = np - k0 < KC ? np - k0 : KC;
-#pragma unroll
-        for (int cc = 0; cc < 8; cc++) {
-            const __half *vrow = vt + (warp * 8 + cc) * KC;
-            for (int k = lane; k < kend; k += 32) acc[cc] = __fmaf_rn(__half2float(vrow[k]), __half2float(p16[k0 + k]), acc[cc]);
+            for (int i = tid; i < 32 * VL; i += 128) ((int4 *)vleft)[i] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + i / VL) * n_ctx + np) + i % VL);
+        } else {
+            const int rr = tid >> 2, part = tid & 3;
+            ((int4 *)vleft)[tid] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + rr) * n_ctx + np) + part);
         }
     }
-    __syncthreads();
-#pragma unroll
-    for (int cc = 0; cc < 8; cc++) {
-        const float a = f16dot_tree(acc[cc]);
-        if (lane == 0) {
-            const __half *vrow = vleft + (warp * 8 + cc) * 32;
-            double sumf = (double)a;
-            for (int k = np; k < n_kv; k++) sumf += (double)__fmul_rn(__half2float(vrow[k - np]), __half2float(p16[k]));
-            stash[warp * 8 + cc] = (float)sumf;
-        }
-    }
-    __syncthreads();
-    if (warp == 0) pack_quad(((const float4 *)stash)[lane & 7], xpack_out + (int64_t)((h * hd + c0) / QK) * 4, lane, lane < 8, q81, off, scale16);
-    prof_end(prof);
-}
-
-
-// the f32 cache's form: probabilities kept f32, V tiles of KC_F32 = 64 positions (the same 16 KB and 4 vectors per thread as the f16 kernel's
-// 128), leftovers added in float (f32dot.cuh).  Dynamic shared memory: scores and probabilities, a V tile, 32 leftover columns -- it holds the
-// context of n_ctx positions up to attn_sv_f32_max_ctx()
-constexpr int KC_F32 = KC / 2;
-constexpr size_t attn_sv_f32_smem(int n_ctx) { return (size_t)n_ctx * 8 + (size_t)(32 * KC_F32 + 32 * 32) * 4; }
-__global__ void __launch_bounds__(128) attn_sv_f32_kernel(const float *__restrict__ kq, const float *__restrict__ Vl, int4 *__restrict__ xpack_out,
-                                                          const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp, float kq_scale,
-                                                          int hd, int n_head, int n_head_kv, int n_ctx, int q81, int off, int scale16, unsigned long long *prof) {
-    constexpr int TC = KC_F32;
-    constexpr int VL = 8;                             // 16-byte vectors of 32 positions
-    extern __shared__ __align__(16) uint8_t sm[];
-    __shared__ double shd[8];
-    __shared__ float shf[4], stash[32];
-    pdl_trigger();
-    pdl_wait();
-    prof_begin(prof);
-    const int n_kv = __ldcg(n_past) + 1;
-    const int per_head = hd / 32, h = blockIdx.x / per_head, c0 = (blockIdx.x - h * per_head) * 32;
-    const int hk = h / (n_head / n_head_kv);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    float *sc = (float *)sm;
-    float *p = (float *)(sm + (size_t)n_ctx * 4);
-    float *vt = (float *)(sm + (size_t)n_ctx * 8);
-    float *vleft = vt + 32 * TC;
-    // leftover V columns and the first V tile are requested before anything else so that their latency hides behind the soft_max
-    const int np = n_kv & ~31;
-    if (np < n_kv) {
-#pragma unroll
-        for (int i = tid; i < 32 * VL; i += 128) ((int4 *)vleft)[i] = __ldcg((const int4 *)(Vl + (int64_t)(hk * hd + c0 + i / VL) * n_ctx + np) + i % VL);
-    }
-    constexpr int TV = TC / 4;                        // 16-byte vectors per row of a tile
     int4 pre[32 * TV / 128];
     auto fetch = [&](int k0) {
 #pragma unroll
@@ -522,7 +410,7 @@ __global__ void __launch_bounds__(128) attn_sv_f32_kernel(const float *__restric
     if (lane == 0) shd[warp] = s;
     __syncthreads();
     const float inv = (float)(1.0 / ((shd[0] + shd[1]) + (shd[2] + shd[3])));
-    for (int j = tid; j < n_kv; j += 128) p[j] = __fmul_rn(sc[j], inv);             // the probabilities stay f32
+    for (int j = tid; j < n_kv; j += 128) p[j] = kv_cast<KT>(__fmul_rn(sc[j], inv));
     float acc[8];
 #pragma unroll
     for (int cc = 0; cc < 8; cc++) acc[cc] = 0.f;
@@ -535,8 +423,8 @@ __global__ void __launch_bounds__(128) attn_sv_f32_kernel(const float *__restric
         const int kend = np - k0 < TC ? np - k0 : TC;
 #pragma unroll
         for (int cc = 0; cc < 8; cc++) {
-            const float *vrow = vt + (warp * 8 + cc) * TC;
-            for (int k = lane; k < kend; k += 32) acc[cc] = __fmaf_rn(vrow[k], p[k0 + k], acc[cc]);
+            const KT *vrow = vt + (warp * 8 + cc) * TC;
+            for (int k = lane; k < kend; k += 32) acc[cc] = __fmaf_rn(kv_load(vrow[k]), kv_load(p[k0 + k]), acc[cc]);
         }
     }
     __syncthreads();
@@ -544,8 +432,14 @@ __global__ void __launch_bounds__(128) attn_sv_f32_kernel(const float *__restric
     for (int cc = 0; cc < 8; cc++) {
         const float a = f16dot_tree(acc[cc]);
         if (lane == 0) {
-            const float *vrow = vleft + (warp * 8 + cc) * 32;
-            stash[warp * 8 + cc] = f32_leftovers(a, n_kv - np, [&](int i) { return vrow[i]; }, [&](int i) { return p[np + i]; });
+            const KT *vrow = vleft + (warp * 8 + cc) * 32;
+            if constexpr (F32) {
+                stash[warp * 8 + cc] = f32_leftovers(a, n_kv - np, [&](int i) { return vrow[i]; }, [&](int i) { return p[np + i]; });
+            } else {
+                double sumf = (double)a;
+                for (int k = np; k < n_kv; k++) sumf += (double)__fmul_rn(__half2float(vrow[k - np]), __half2float(p[k]));
+                stash[warp * 8 + cc] = (float)sumf;
+            }
         }
     }
     __syncthreads();
@@ -593,12 +487,15 @@ __device__ __forceinline__ void fma8(float (&acc)[8], const int4 &a0, const int4
 //
 // KT = float (an f32 cache, ggml_vec_dot_f32): a step of a quad thread is two 16-byte K vectors (CW = 2, so half the positions per pass); q and
 // the probabilities stay f32 in shared memory, the V rows take twice the bytes, and the KQV leftovers are added in float (f32dot.cuh).
+//
+// TP: the merged row goes to every rank's exchange buffer (tp.cuh); head0 is this rank's first head.  alibi: the per-head slopes [n_head], read
+// only by the ALIBI instances.  The instances that launch are listed in attn_fused_instances.
 constexpr int ATH = 256;
-template <bool TP, bool ALIBI, int NV = 4, typename KT = __half>
-__device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, const KT *__restrict__ Kl, const KT *__restrict__ Vl,
-                                                int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
-                                                float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                                                unsigned long long *prof, const TpSync &S, int head0, const float *__restrict__ alibi) {
+template <bool TP, bool ALIBI, int NV, typename KT>
+__global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict__ q, const KT *__restrict__ Kl, const KT *__restrict__ Vl,
+                                                         int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
+                                                         float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
+                                                         unsigned long long *prof, const TpSync S, int head0, const float *__restrict__ alibi) {
     const TpCtx &T = c_tp;
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
@@ -773,35 +670,6 @@ __device__ __forceinline__ void attn_fused_body(const float *__restrict__ q, con
     }
     prof_end(prof);
 }
-template <bool TP>
-__global__ void __launch_bounds__(ATH) attn_fused_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
-                                                         int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
-                                                         float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                                                         unsigned long long *prof, const TpSync S, int head0) {
-    attn_fused_body<TP, false>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, nullptr);
-}
-// the ALiBi form (single GPU): alibi = the per-head slopes [n_head]
-__global__ void __launch_bounds__(ATH) attn_fused_alibi_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
-                                                               int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
-                                                               float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                                                               unsigned long long *prof, const TpSync S, int head0, const float *__restrict__ alibi) {
-    attn_fused_body<false, true>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, alibi);
-}
-// the wide form (single GPU, no ALiBi): head sizes 128 < hd <= 256, hd % 32 == 0 -- one cluster of hd/32 = 5..8 CTAs per head (GPT-J)
-__global__ void __launch_bounds__(ATH) attn_fused_wide_kernel(const float *__restrict__ q, const __half *__restrict__ Kl, const __half *__restrict__ Vl,
-                                                              int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
-                                                              float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                                                              unsigned long long *prof, const TpSync S, int head0) {
-    attn_fused_body<false, false, 8>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, nullptr);
-}
-// the three single-GPU forms on an f32 cache (MHA / GQA, ALiBi, wide); alibi: nullptr except for the ALiBi form
-template <bool ALIBI, int NV>
-__global__ void __launch_bounds__(ATH) attn_fused_f32_kernel(const float *__restrict__ q, const float *__restrict__ Kl, const float *__restrict__ Vl,
-                                                             int4 *__restrict__ xpack_out, const int *__restrict__ n_past, const uint16_t *__restrict__ lut_exp,
-                                                             float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int nlay, int q81, int off, int scale16,
-                                                             unsigned long long *prof, const TpSync S, int head0, const float *__restrict__ alibi) {
-    attn_fused_body<false, ALIBI, NV, float>(q, Kl, Vl, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay, q81, off, scale16, prof, S, head0, alibi);
-}
 
 // ---- ring and grid plan of the decode mat-vecs ------------------------------------------------------------------------------------------------
 // What one CTA takes from an SM while it is resident: shared memory (static + dynamic + the per-CTA reservation), registers as the SM allocates
@@ -824,8 +692,8 @@ const SmLimits &sm_limits() {
     }
     return L;
 }
-template <typename... KArgs>
-CtaFootprint footprint_of(void (*kern)(KArgs...), int threads, size_t dyn_smem) {
+template <typename K>
+CtaFootprint footprint_of(K *kern, int threads, size_t dyn_smem) {
     cudaFuncAttributes fa;
     B200_CHECK(cudaFuncGetAttributes(&fa, (const void *)kern));
     const int warps = (threads + 31) / 32;
@@ -920,26 +788,42 @@ void launch_mmv(const QWeight &w, MmvArgs A, const MmvPlan &plan, cudaStream_t s
     launch_k(mmv_fused_kernel<TYPE, EPI, TP>, dim3((unsigned)plan.grid), dim3(STHREADS), (size_t)plan.smem, st, w, A);
 }
 
+// The instances of attn_fused_kernel that launch, in one list: attn_fused_pick chooses from it and attn_fused_reserve opts every entry in, so no
+// instance launches without its shared-memory reservation.  All of them take one parameter list; Kl and Vl point to the cache's element type.
+struct AttnFusedInstance { bool tp, alibi; int nv, kv_type; const void *kern; };
+template <bool TP, bool ALIBI, int NV, typename KT>
+AttnFusedInstance attn_fused_entry() { return {TP, ALIBI, NV, sizeof(KT) == 4 ? T_F32 : T_F16, (const void *)attn_fused_kernel<TP, ALIBI, NV, KT>}; }
+const AttnFusedInstance attn_fused_instances[] = {
+    attn_fused_entry<false, false, 4, __half>(), attn_fused_entry<true, false, 4, __half>(), attn_fused_entry<false, true, 4, __half>(),
+    attn_fused_entry<false, false, 8, __half>(),
+    attn_fused_entry<false, false, 4, float>(), attn_fused_entry<false, true, 4, float>(), attn_fused_entry<false, false, 8, float>(),
+};
+// the instance for a geometry: heads of up to 256 in 32-wide slices (NV 8 past 128), ALiBi only up to 128, tensor-parallel only on an f16
+// cache with heads of up to 128 and no ALiBi
+const void *attn_fused_pick(bool tp, int hd, bool alibi, int kv_type) {
+    B200_ASSERT(hd <= 256 && hd % 32 == 0);
+    B200_ASSERT(!alibi || hd <= 128);
+    B200_ASSERT(!tp || (kv_type == T_F16 && hd <= 128 && !alibi));
+    const int nv = hd > 128 ? 8 : 4;
+    for (const AttnFusedInstance &I : attn_fused_instances)
+        if (I.tp == tp && I.alibi == alibi && I.nv == nv && I.kv_type == kv_type) return I.kern;
+    B200_ASSERT(!"attn_fused_pick: no instance for this geometry");
+    return nullptr;
+}
 // dynamic shared memory opt-in of the cluster attention kernels: one high-water mark for all of them (the attribute is per function, not per caller)
 static void attn_fused_reserve(size_t bytes) {
     static size_t set = 48 * 1024;
     if (bytes <= set) return;
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_alibi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_f32_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_f32_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_fused_f32_kernel<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    for (const AttnFusedInstance &I : attn_fused_instances) B200_CHECK(cudaFuncSetAttribute(I.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
-// the same for attn_sv_kernel (and its f32 form): one record per process.  Every decode_ops_t<TYPE, TP> launches this one kernel, so a record per
+// the same for attn_sv_kernel (both instances): one record per process.  Every decode_ops_t<TYPE, TP> launches this one kernel, so a record per
 // instantiation would let a session of another weight type with a shorter context LOWER the attribute under a session that already relies on more.
 static void attn_sv_reserve(size_t bytes) {
     static size_t set = 48 * 1024;
     if (bytes <= set) return;
-    B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    B200_CHECK(cudaFuncSetAttribute(attn_sv_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    B200_CHECK(cudaFuncSetAttribute(attn_sv_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     set = bytes;
 }
 // the positions attn_fused_kernel holds for a context bucket: the bucket rounded up to whole 64-position tiles
@@ -953,15 +837,15 @@ size_t attn_fused_smem(int n_kv_bucket, int hd, int kv_type = T_F16) {
 }
 }  // namespace
 bool attn_fused_fits(int n_kv_bucket, int hd, int kv_type) { return attn_fused_smem(n_kv_bucket, hd, kv_type) <= 227 * 1024; }
-int attn_sv_f32_max_ctx() { return (int)((227 * 1024 - attn_sv_f32_smem(0)) / 8); }
+int attn_sv_f32_max_ctx() { return (int)((227 * 1024 - attn_sv_smem(0, T_F32)) / 8); }
 namespace {
 // one cluster of hd/32 CTAs per head, a programmatic dependent of its predecessor.  alibi: per-head slopes (the ALiBi form, single GPU only)
 // or nullptr.  kv_type T_F32: Kl / Vl are an f32 cache (single GPU only)
-template <bool TP>
-void launch_attn_fused(cudaStream_t st, const float *q, const void *Kl, const void *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
+void launch_attn_fused(cudaStream_t st, bool tp, const float *q, const void *Kl, const void *Vl, int4 *xpack_out, const int *n_past, const uint16_t *lut_exp,
                        float kq_scale, int hd, int n_head, int n_head_kv, int gqa, int n_ctx, int n_kv_bucket, int q81, int off, int scale16,
-                       unsigned long long *prof, const TpSync &S, int head0, const float *alibi = nullptr, int kv_type = T_F16) {
-    const int nlay = attn_fused_rows(n_kv_bucket);
+                       unsigned long long *prof, TpSync S, int head0, const float *alibi, int kv_type) {
+    const void *kern = attn_fused_pick(tp, hd, alibi != nullptr, kv_type);
+    int nlay = attn_fused_rows(n_kv_bucket);
     const size_t smem = attn_fused_smem(n_kv_bucket, hd, kv_type);
     attn_fused_reserve(smem);
     cudaLaunchConfig_t cfg{};
@@ -972,37 +856,16 @@ void launch_attn_fused(cudaStream_t st, const float *q, const void *Kl, const vo
     at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 2;
-    if (kv_type == T_F32) {
-        B200_ASSERT(!TP && hd <= 256 && hd % 32 == 0 && (!alibi || hd <= 128));
-        const float *K32 = (const float *)Kl, *V32 = (const float *)Vl;
-        auto kern = alibi ? attn_fused_f32_kernel<true, 4> : hd > 128 ? attn_fused_f32_kernel<false, 8> : attn_fused_f32_kernel<false, 4>;
-        B200_CHECK(cudaLaunchKernelEx(&cfg, kern, q, K32, V32, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
-                                      q81, off, scale16, prof, S, head0, alibi));
-        return;
-    }
-    const __half *K16 = (const __half *)Kl, *V16 = (const __half *)Vl;
-    if (alibi) {
-        B200_ASSERT(!TP && hd <= 128);
-        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_alibi_kernel, q, K16, V16, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
-                                      q81, off, scale16, prof, S, head0, alibi));
-        return;
-    }
-    if (hd > 128) {                                              // 5..8 CTAs per head
-        B200_ASSERT(!TP && hd <= 256 && hd % 32 == 0);
-        B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_wide_kernel, q, K16, V16, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
-                                      q81, off, scale16, prof, S, head0));
-        return;
-    }
-    B200_CHECK(cudaLaunchKernelEx(&cfg, attn_fused_kernel<TP>, q, K16, V16, xpack_out, n_past, lut_exp, kq_scale, hd, n_head, n_head_kv, gqa, n_ctx, nlay,
-                                  q81, off, scale16, prof, S, head0));
+    // attn_fused_kernel's parameters in order (Kl and Vl as the untyped pointers they are here)
+    void *args[] = {&q, &Kl, &Vl, &xpack_out, &n_past, &lut_exp, &kq_scale, &hd, &n_head, &n_head_kv, &gqa, &n_ctx, &nlay, &q81, &off, &scale16, &prof, &S, &head0, &alibi};
+    B200_CHECK(cudaLaunchKernelExC(&cfg, kern, args));
 }
 // the footprint of the cluster attention launch_attn_fused picks for the geometry (the successor the qkv node's ring is planned against)
-CtaFootprint attn_fused_footprint(bool tp, int hd, bool alibi, int kv_type, size_t smem) {
-    if (kv_type == T_F32) return footprint_of(alibi ? attn_fused_f32_kernel<true, 4> : hd > 128 ? attn_fused_f32_kernel<false, 8> : attn_fused_f32_kernel<false, 4>, ATH, smem);
-    if (alibi) return footprint_of(attn_fused_alibi_kernel, ATH, smem);
-    if (hd > 128) return footprint_of(attn_fused_wide_kernel, ATH, smem);
-    return tp ? footprint_of(attn_fused_kernel<true>, ATH, smem) : footprint_of(attn_fused_kernel<false>, ATH, smem);
-}
+CtaFootprint attn_fused_footprint(bool tp, int hd, bool alibi, int kv_type, size_t smem) { return footprint_of(attn_fused_pick(tp, hd, alibi, kv_type), ATH, smem); }
+
+// f(KT()) for the KV cache's element type KT: the choice between the f16 and f32 instances of a kernel
+template <typename F>
+auto with_kv_type(int kv_type, F &&f) { return kv_type == T_F32 ? f(float()) : f(__half()); }
 
 // tensor-parallel helpers (tp.cuh).  spread: the embedding row every rank computed for itself -> the X exchange buffer's unit form (stamp 0);
 // collect: the gathered logits units -> the plain f32 logits array the host reads; bump: the token is complete, the epoch moves on.
@@ -1067,18 +930,19 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     // attention: one cluster launch per layer, or the two-kernel variant for head sizes a cluster cannot cover and for buckets whose scores
     // and V rows do not fit one CTA's shared memory (an f32 cache: past 1664 positions)
     const bool kv32 = !TP && P.kv_type == T_F32;                // sessions of a tensor-parallel model keep an f16 cache
+    const int kv_type = kv32 ? T_F32 : T_F16;
     const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd, P.kv_type);
     const bool fused_attn = P.hd % 32 == 0 && P.hd <= 128 && P.n_ctx % 8 == 0 && attn_fused_fits(n_kv_bucket, P.hd, P.kv_type);
     B200_ASSERT(fused_attn || !tp);                              // the tensor-parallel exchange lives in the fused attention kernel's epilogue (start_session_tp checks the size)
-    const size_t sv_smem = kv32 ? attn_sv_f32_smem(P.n_ctx) : (size_t)P.n_ctx * 6 + 32 * KC * 2 + 32 * 32 * 2;
+    const size_t sv_smem = attn_sv_smem(P.n_ctx, kv_type);
     attn_sv_reserve(sv_smem);
+    // the two-kernel attention's KQ instance for the cache's element type (heads of 64 or 128)
+    auto attn_kq_of = [&](auto kt) { return P.hd == 128 ? attn_kq_kernel<128, decltype(kt)> : attn_kq_kernel<64, decltype(kt)>; };
     // mat-vec plans, each leaving room for what follows it (planned from the successor backwards; every layer has the same shapes): the norm
     // kernels release their dependents at entry, so beside wo and w2 there has to be room for the norm AND the next mat-vec
     const CtaFootprint f_norm = TP ? footprint_of(norm_pack_tp_kernel, 256, 0) : footprint_of(norm_pack_kernel, 256, 0);
-    const CtaFootprint f_attn = kv32 ? (fused_attn ? attn_fused_footprint(false, P.hd, false, T_F32, fa_smem)
-                                                   : footprint_of(P.hd == 128 ? attn_kq_f32_kernel<128> : attn_kq_f32_kernel<64>, 128, 0))
-                              : fused_attn ? footprint_of(attn_fused_kernel<TP>, ATH, fa_smem)
-                                           : footprint_of(P.hd == 128 ? attn_kq_kernel<128> : attn_kq_kernel<64>, 128, 0);
+    const CtaFootprint f_attn = fused_attn ? attn_fused_footprint(TP, P.hd, false, kv_type, fa_smem)
+                                           : with_kv_type(kv_type, [&](auto kt) { return footprint_of(attn_kq_of(kt), 128, 0); });
     const MmvPlan &p_qkv = qkv_plan<TYPE, TP>(kv32, layers[0].wqkv, f_attn);
     const MmvPlan &p_w2 = mmv_plan<TYPE, EPI_RES, TP>(layers[0].w2, f_norm + p_qkv.cta);
     const MmvPlan &p_w13 = mmv_plan<TYPE, EPI_SILU, TP>(layers[0].w13, p_w2.cta);
@@ -1092,22 +956,17 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
         A.prof = pr(); launch_qkv<TYPE, TP>(kv32, L.wqkv, A, p_qkv, st); n++;
         if (fused_attn) {
-            launch_attn_fused<TP>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, n_kv_bucket, q81, off, s16, pr(),
-                                  ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0, nullptr, kv32 ? T_F32 : T_F16);
+            launch_attn_fused(st, TP, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head_kv, P.gqa, P.n_ctx, n_kv_bucket, q81, off, s16, pr(),
+                              ts(-1, 0, -1, 0, TPB_XD, v), tp ? P.head0 : 0, nullptr, kv_type);
             n++;
-        } else if (kv32) {
-            launch_k(P.hd == 128 ? attn_kq_f32_kernel<128> : attn_kq_f32_kernel<64>, dim3((n_kv_bucket + 63) / 64, P.n_head), dim3(128), 0, st,
-                     P.q, (const float *)L.K, P.kq, P.n_past, P.gqa, P.n_head, P.n_head_kv, P.n_ctx, pr());
+        } else with_kv_type(kv_type, [&](auto kt) {
+            using KT = decltype(kt);
+            launch_k(attn_kq_of(kt), dim3((n_kv_bucket + 63) / 64, P.n_head), dim3(128), 0, st,
+                     P.q, (const KT *)L.K, P.kq, P.n_past, P.gqa, P.n_head, P.n_head_kv, P.n_ctx, pr());
             n++;
-            launch_k(attn_sv_f32_kernel, dim3(P.n_head * (P.hd / 32)), dim3(128), sv_smem, st, P.kq, (const float *)L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale,
+            launch_k(attn_sv_kernel<KT>, dim3(P.n_head * (P.hd / 32)), dim3(128), sv_smem, st, P.kq, (const KT *)L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale,
                      P.hd, P.n_head, P.n_head_kv, P.n_ctx, q81, off, s16, pr()); n++;
-        } else {
-            launch_k(P.hd == 128 ? attn_kq_kernel<128> : attn_kq_kernel<64>, dim3((n_kv_bucket + 63) / 64, P.n_head), dim3(128), 0, st,
-                     P.q, (const __half *)L.K, P.kq, P.n_past, P.gqa, P.n_head, P.n_head_kv, P.n_ctx, pr());
-            n++;
-            launch_k(attn_sv_kernel, dim3(P.n_head * (P.hd / 32)), dim3(128), sv_smem, st, P.kq, (const __half *)L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head,
-                     P.n_head_kv, P.n_ctx, q81, off, s16, pr()); n++;
-        }
+        });
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.ff; Bo.addend = P.x;
         Bo.ts = ts(TPB_XD, v, TPB_X, (unsigned)il, TPB_FF, v); Bo.row0 = tp ? P.row0_e : 0;
         Bo.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.wo, Bo, p_wo, st); n++;
@@ -1196,12 +1055,10 @@ __global__ void __launch_bounds__(256) ln_pack_nobias_kernel(const float *__rest
 // (head stride 3 hd) and q, k get RoPE mode 2 -- the ggml neox branch (LC/ggml.c:11876-11897) rotates EVERY block of n_rot dims of the head, pairs
 // (c, c + n_rot/2).  GPT-2 (gpt2 lib.rs:190-210): the three thirds of the row, no rotation (n_rot = 0).  One thread per channel.
 // KT: the cache's element type (float: K and V stored as they are)
-__device__ __forceinline__ void kv_store(__half *p, float v) { *p = __float2half_rn(v); }
-__device__ __forceinline__ void kv_store(float *p, float v) { *p = v; }
 template <typename KT>
-__device__ __forceinline__ void neox_rope_store_body(const float *__restrict__ qkv, float *__restrict__ q, KT *__restrict__ Kl, KT *__restrict__ Vl,
-                                                     const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e, int n_ctx,
-                                                     int head_stride, int k_off, int v_off) {
+__global__ void __launch_bounds__(256) neox_rope_store_kernel(const float *__restrict__ qkv, float *__restrict__ q, KT *__restrict__ Kl, KT *__restrict__ Vl,
+                                                              const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e, int n_ctx,
+                                                              int head_stride, int k_off, int v_off) {
     pdl_trigger();
     pdl_wait();
     const int i = blockIdx.x * 256 + threadIdx.x;
@@ -1223,18 +1080,8 @@ __device__ __forceinline__ void neox_rope_store_body(const float *__restrict__ q
         }
     }
     q[i] = qo;
-    kv_store(Kl + (int64_t)p * e + i, ko);
-    kv_store(Vl + (int64_t)i * n_ctx + p, __ldcg(base + v_off + c));
-}
-__global__ void __launch_bounds__(256) neox_rope_store_kernel(const float *__restrict__ qkv, float *__restrict__ q, __half *__restrict__ Kl, __half *__restrict__ Vl,
-                                                              const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e, int n_ctx,
-                                                              int head_stride, int k_off, int v_off) {
-    neox_rope_store_body(qkv, q, Kl, Vl, n_past, rope_cs, rope_half, n_rot, hd, e, n_ctx, head_stride, k_off, v_off);
-}
-__global__ void __launch_bounds__(256) neox_rope_store_f32_kernel(const float *__restrict__ qkv, float *__restrict__ q, float *__restrict__ Kl, float *__restrict__ Vl,
-                                                                  const int *__restrict__ n_past, const float2 *__restrict__ rope_cs, int rope_half, int n_rot, int hd, int e,
-                                                                  int n_ctx, int head_stride, int k_off, int v_off) {
-    neox_rope_store_body(qkv, q, Kl, Vl, n_past, rope_cs, rope_half, n_rot, hd, e, n_ctx, head_stride, k_off, v_off);
+    Kl[(int64_t)p * e + i] = kv_cast<KT>(ko);
+    Vl[(int64_t)i * n_ctx + p] = kv_cast<KT>(__ldcg(base + v_off + c));
 }
 
 // GPT-2: inpL = wte[token] + wpe[n_past]  (gpt2 lib.rs:164-172), position read from device memory
@@ -1259,7 +1106,6 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     }
     if (P.wpe) { launch_k(gpt2_add_pos_kernel, dim3((e + 255) / 256), dim3(256), 0, st, P.x, P.wpe, (const int *)P.n_past, e); n++; }
     B200_ASSERT(neox_decode_fits(P, n_kv_bucket));
-    const bool kv32 = P.kv_type == T_F32;
     const size_t fa_smem = attn_fused_smem(n_kv_bucket, P.hd, P.kv_type);
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
@@ -1267,9 +1113,8 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     const bool biased = layers[0].ln1_b != nullptr, fc_bias = layers[0].bfc != nullptr;
     auto ln_kernel = biased ? ln_pack_kernel : ln_pack_nobias_kernel;
     const CtaFootprint f_ln = footprint_of(ln_kernel, 256, 0);
-    const CtaFootprint f_attn = kv32 ? attn_fused_footprint(false, P.hd, P.alibi != nullptr, T_F32, fa_smem)
-                              : P.alibi ? footprint_of(attn_fused_alibi_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
-    const CtaFootprint f_store = kv32 ? footprint_of(neox_rope_store_f32_kernel, 256, 0) : footprint_of(neox_rope_store_kernel, 256, 0);
+    const CtaFootprint f_attn = attn_fused_footprint(false, P.hd, P.alibi != nullptr, P.kv_type, fa_smem);
+    const CtaFootprint f_store = with_kv_type(P.kv_type, [](auto kt) { return footprint_of(neox_rope_store_kernel<decltype(kt)>, 256, 0); });
     const MmvPlan &p_qkv = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wqkv, f_store + f_attn);
     const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
     const MmvPlan &p_fc = fc_bias ? mmv_plan<TYPE, EPI_GELU, false>(layers[0].wfc, p_proj.cta) : mmv_plan<TYPE, EPI_GELU_NB, false>(layers[0].wfc, p_proj.cta);
@@ -1280,13 +1125,14 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         launch_k(ln_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, L.ln1_g, L.ln1_b, P.xpack_a, e, q81, off, s16); n++;               // :192-196
         MmvArgs A{}; A.xpack = P.xpack_a; A.dst = P.qkv; A.bias = L.bqkv;
         launch_mmv<TYPE, EPI_BIAS>(L.wqkv, A, p_qkv, st); n++;                                                                                      // :199-200
-        if (kv32) launch_k(neox_rope_store_f32_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, (float *)L.K, (float *)L.V, (const int *)P.n_past,
-                           P.rope_cs, P.rope_half, P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off);
-        else launch_k(neox_rope_store_kernel, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, (__half *)L.K, (__half *)L.V, (const int *)P.n_past,
-                      P.rope_cs, P.rope_half, P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off);
+        with_kv_type(P.kv_type, [&](auto kt) {
+            using KT = decltype(kt);
+            launch_k(neox_rope_store_kernel<KT>, dim3((e + 255) / 256), dim3(256), 0, st, (const float *)P.qkv, P.q, (KT *)L.K, (KT *)L.V, (const int *)P.n_past,
+                     P.rope_cs, P.rope_half, P.n_rot, P.hd, e, P.n_ctx, P.qkv_layout.head_stride, P.qkv_layout.k_off, P.qkv_layout.v_off);
+        });
         n++;                                                                                                                                  // :205-247
-        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
-                                 nullptr, S, 0, P.alibi, P.kv_type); n++;                                                                 // :250-298
+        launch_attn_fused(st, false, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
+                          nullptr, S, 0, P.alibi, P.kv_type); n++;                                                                        // :250-298
         // attention.dense (+bias); sequential residual: ff_in = that + inpL                                                                    :301-312
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out; Bo.bias = L.bdense; Bo.add1 = P.parallel_residual ? nullptr : P.x;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;
@@ -1323,8 +1169,7 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     const dim3 ln_grid((e / 4 + 255) / 256);
     const TpSync S{};
     const CtaFootprint f_ln = footprint_of(ln_pack_kernel, 256, 0);
-    const CtaFootprint f_attn = kv32 ? attn_fused_footprint(false, P.hd, false, T_F32, fa_smem)
-                              : P.hd > 128 ? footprint_of(attn_fused_wide_kernel, ATH, fa_smem) : footprint_of(attn_fused_kernel<false>, ATH, fa_smem);
+    const CtaFootprint f_attn = attn_fused_footprint(false, P.hd, false, P.kv_type, fa_smem);
     // each ring planned against the node launched after it: qkv -> attention, out_proj -> fc_in, fc_in -> fc_out, fc_out -> next layer's ln_1 + qkv
     const MmvPlan &p_qkv = qkv_plan<TYPE, false>(kv32, layers[0].wqkv, f_attn);
     const MmvPlan &p_proj = mmv_plan<TYPE, EPI_BIAS, false>(layers[0].wproj, f_ln + p_qkv.cta);
@@ -1337,8 +1182,8 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         MmvArgs A{}; A.xpack = P.xpack_a; A.q = P.q; A.K = L.K; A.V = L.V; A.rope_cs = P.rope_cs; A.rope_half = P.rope_half; A.hd = P.hd; A.e = e; A.gqa = e;
         A.n_ctx = P.n_ctx; A.n_past = P.n_past;
         launch_qkv<TYPE, false>(kv32, L.wqkv, A, p_qkv, st); n++;                                                                                     // :178-220
-        launch_attn_fused<false>(st, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
-                                 nullptr, S, 0, nullptr, P.kv_type); n++;                                                                               // :222-262
+        launch_attn_fused(st, false, P.q, L.K, L.V, P.xpack_d, P.n_past, P.lut_exp, P.kq_scale, P.hd, P.n_head, P.n_head, e, P.n_ctx, n_kv_bucket, q81, off, s16,
+                          nullptr, S, 0, nullptr, P.kv_type); n++;                                                                                      // :222-262
         MmvArgs Bo{}; Bo.xpack = P.xpack_d; Bo.dst = P.attn_out;
         launch_mmv<TYPE, EPI_BIAS>(L.wdense, Bo, p_dense, st); n++;                                                                                    // :265
         MmvArgs C{}; C.xpack = P.xpack_a; C.xpack_out = P.xpack_f; C.bias = L.bfc; C.lut_gelu = P.lut_gelu; C.q81 = q81; C.off = off; C.scale16 = s16;

@@ -103,7 +103,7 @@ def short_sequence(s, cpu, hp, want, seed):
 
 
 # ---- 1. the cluster attention at every cluster size --------------------------------------------------------------------------------------------
-# attn_fused_body runs one cluster of hd / 32 CTAs per head.  GPT-J's wide form (hd > 128, NV = 8) covers clusters of 5..8: thread u of a quad
+# attn_fused_kernel runs one cluster of hd / 32 CTAs per head.  GPT-J's wide form (hd > 128, NV = 8) covers clusters of 5..8: thread u of a quad
 # feeds the scores to CTA u and, where u + 4 < hd / 32, to CTA u + 4 -- clusters of 5 and 7 send from only one or three of the four threads.
 # 8 heads keep n_embd a multiple of 256: with 4 heads of 160 (n_embd 640, nb 20) mmv_exact_stream_supported refuses the rows and the model
 # decodes per op, which the launch counts would catch.
@@ -133,7 +133,7 @@ def test_gptj_cluster_sizes(orc, cfg, qname):
 
 
 def second_kq_pass(hd):
-    """the first n_past at which attn_fused_body makes a second KQ pass: each of the hd / 32 CTAs takes per = ceil(n_kv / (hd / 32)) positions
+    """the first n_past at which attn_fused_kernel (f16 cache) makes a second KQ pass: each of the hd / 32 CTAs takes per = ceil(n_kv / (hd / 32)) positions
     and one pass covers PU * ATH / 4 of them (PU = 16 / NV; NV = 8 for hd > 128, else 4; ATH = 256): 128 or 256 positions per CTA per pass"""
     per_pass = (16 // (8 if hd > 128 else 4)) * 256 // 4
     return per_pass * (hd // 32)            # n_kv > per_pass * hd / 32, i.e. n_past >= that

@@ -52,7 +52,7 @@ def llama_kv_equal(s, cpu):
         assert np.array_equal(a.view(np.uint32), kv32.kv_f32(cpu, which)[:a.size].view(np.uint32)), which
 
 
-# hd128: the LLaMA-7B head size (4-CTA clusters, attn_kq_f32_kernel<128>); the others have 64-wide heads
+# hd128: the LLaMA-7B head size (4-CTA clusters, attn_kq_kernel<128, float>); the others have 64-wide heads
 LLAMA_CFGS = dict(synth.CONFIGS, hd128=dict(synth.CONFIGS["tiny8"], n_head=2, n_head_kv=2, n_rot=128))
 
 

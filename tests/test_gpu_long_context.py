@@ -1,7 +1,7 @@
 """Long-context decode: logits bit-identical to the CPU model at every step up to the last slot of the context, and both KV caches at the end.
 
 Where the decode schedules change what they run, by position:
-  - attn_fused_kernel makes more than one KQ pass once a CTA's share of the positions is over 256 (n_kv > 256 * hd / 32), and its soft_max
+  - attn_fused_kernel on an f16 cache with heads of up to 128 makes more than one KQ pass once a CTA's share of the positions is over 256 (n_kv > 256 * hd / 32), and its soft_max
     makes a second pass at n_kv > 1024;
   - a context bucket (n_kv rounded up to 256, at most n_ctx) past 3264 positions does not fit that kernel's shared memory: from n_past 3072
     on, LLaMA decodes with the two-kernel attention (attn_kq + attn_sv, 8 launches per layer instead of 7) and GPT-NeoX / GPT-2 per op;
