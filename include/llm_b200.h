@@ -75,6 +75,9 @@ enum {                            /* return codes (0 = ok).  CUDA failures print
     B200_ERR_INVARIANT_BROKEN = -13,        /* n_dims > 2, negative sizes, Q4_0/Q4_1 rows with ne0 % 64 != 0 */
     B200_ERR_UNSUPPORTED_ELEMENT_TYPE = -14,
     B200_ERR_QUANTIZATION_VERSION = -15,    /* quantized tensors need quantization version 2 (llm-base loader.rs:481-484) */
+    /* model quantization (llm_base::QuantizeError, crates/llm-base/src/quantize.rs:69-121) */
+    B200_ERR_INVALID_QUANTIZATION_TARGET = -16,         /* InvalidQuantizationTarget: a target other than Q4_0 / Q4_1 / Q5_0 / Q5_1 / Q8_0 */
+    B200_ERR_VOCABULARY_SCORING_NOT_SUPPORTED = -17,    /* VocabularyScoringNotSupported: the GGML container with a non-zero token score */
 };
 
 /* The reference's default sampler chain (crates/llm-base/src/samplers.rs:97-211, ensure_default_slots), run on the device in this order:
@@ -170,6 +173,30 @@ int  b200_model_load_tensor_lora(b200_model *m, const char *name, int32_t type, 
 /* b200_llama_load_file_gqa with the adapter files lora_paths[0..n_lora), opened and closed here */
 b200_model *b200_llama_load_file_lora(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa,
                                       const char *const *lora_paths, int32_t n_lora, int *err);
+
+/* ---- model quantization: llm_base::quantize (crates/llm-base/src/quantize.rs:139-414) + ggml::format::save (saver.rs:86-163) --------------------
+ * src_path (an F16 / F32 file of architecture `arch`, B200_ARCH_LLAMA .. B200_ARCH_GPTJ) -> dst_path with every selected tensor quantized to
+ * target_type (2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0) on the GPU, byte-identical with the reference given the same tensor order.  Selected: n_dims == 2
+ * and a name matching the architecture's quantize_tensors() (".*weight"; GPT-2: model/wte, model/lm_head and the c_attn, c_proj, c_fc and mlp c_proj
+ * weights of each layer), unanchored.
+ * Every other tensor is copied byte for byte.  Tensors are written in the source file's order; the header words are the source's except the file
+ * type, 2000 + llama_ftype(target); the vocabulary is the source's.  container: 0 GGJT v3 (scores, 32-byte aligned data), 1 unversioned GGML (no
+ * scores, no padding; B200_ERR_VOCABULARY_SCORING_NOT_SUPPORTED if a score is non-zero).
+ * Everything is checked before dst_path is created: B200_ERR_INVALID_QUANTIZATION_TARGET; B200_ERR_UNSUPPORTED_ELEMENT_TYPE for a selected tensor that
+ * is not F32 / F16; B200_ERR_INVARIANT_BROKEN for a selected tensor with ne0 % 32 != 0, or ne0 % 64 != 0 for a Q4_0 / Q4_1 target; B200_ERR_BAD_ARG
+ * for B200_ARCH_LORA, another container, or a destination that is the source file; the source's LoadError.  On a write error (B200_ERR_IO) the
+ * partial output is removed.  cb (nullable) runs once per tensor, in file order, after the tensor's bytes are written.  The totals and the sum of
+ * the histograms go to the nullable *_out pointers (hist_out: 16 values). */
+typedef struct {
+    char    name[96];
+    int32_t n_dims, src_type, dst_type;    /* dst_type == src_type: copied, not quantized */
+    int64_t ne[2], n_elements, original_size, reduced_size;
+    int64_t hist[16];                      /* ggml_quantize_* histogram; zero when copied */
+} b200_quantize_report;
+typedef void (*b200_quantize_callback)(void *user, const b200_quantize_report *r);
+int  b200_quantize_file(const char *src_path, const char *dst_path, int32_t arch, int32_t target_type,
+                        int32_t container /* 0 GGJT v3, 1 GGML */, b200_quantize_callback cb, void *user,
+                        int64_t *original_size_out, int64_t *reduced_size_out, int64_t *hist_out /* [16] */);
 
 b200_session *b200_model_start_session(b200_model *m, const b200_session_config *cfg);
 /* One forward pass over `n` tokens appended at n_past (InferenceSession::compute + Llama::evaluate).  tokens: HOST int32.
@@ -303,6 +330,9 @@ void b200_neox_session_free(b200_neox_session *s);
 int  b200_op_quantize_act(int32_t vec_dot_type, const float *x, int64_t K, int64_t B, int8_t *qs_out, float *d_out, float *aux_out);
 /* ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} (LC/ggml.c:18083-18230) on the GPU: w_host f32 [N][K] -> N rows of GGML blocks, bit-exact with the reference */
 int  b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int64_t N, void *ggml_blocks_out);
+/* the kernel of b200_quantize_file on DEVICE buffers, enqueued on b200_stream() without a sync (for kernel timing): nblk 32-element blocks of
+ * d_src (src_type 0 F32 / 1 F16) -> GGML blocks of target at d_dst (16-byte aligned); d_hist (nullable): 16 uint64 counters, added to */
+int  b200_op_quantize_blocks_device(int32_t target, int32_t src_type, const void *d_src, int64_t nblk, void *d_dst, void *d_hist);
 /* wtype: GGML_TYPE_F16 (1; K % 64 == 0, impl AUTO or EXACT = mul_mat_f16_exact), GGML_TYPE_Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 (2,3,6,7,8; K % 64 == 0), or the K-quants Q2_K..Q6_K (10..14; K % 256 == 0, impl AUTO or EXACT:
  * ggml_vec_dot_q{2,3,4,5,6}_K_q8_K of LC/k_quants.c:1240,1763,2492,3023,3592 on quantize_row_q8_K activations, bit-exact with the reference's AVX2 build) */
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);

@@ -15,5 +15,6 @@ from . import ggml  # noqa: F401
 Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 = 2, 3, 6, 7, 8
 F32, F16 = 0, 1
 from . import loader  # noqa: F401
+from .quantize import QuantizeError, quantize  # noqa: F401
 from . import tp  # noqa: F401
 from .neox import GptJ  # noqa: F401

@@ -35,6 +35,15 @@ class SamplerParams(C.Structure):
                 ("temperature", C.c_float), ("seed", C.c_uint64), ("draw", C.c_uint64)]
 
 
+class QuantizeReport(C.Structure):
+    """b200_quantize_report (include/llm_b200.h): one tensor of b200_quantize_file, as written."""
+    _fields_ = [("name", C.c_char * 96), ("n_dims", C.c_int32), ("src_type", C.c_int32), ("dst_type", C.c_int32), ("ne", C.c_int64 * 2),
+                ("n_elements", C.c_int64), ("original_size", C.c_int64), ("reduced_size", C.c_int64), ("hist", C.c_int64 * 16)]
+
+
+QUANTIZE_CALLBACK = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(QuantizeReport))
+
+
 def lib():
     global _lib
     if _lib is not None:
@@ -116,11 +125,13 @@ def lib():
     L.b200_llama_load_file.argtypes = [C.c_char_p, i32, C.c_float, C.c_float, C.POINTER(C.c_int)]
     L.b200_op_quantize_act.argtypes = [i32, vp, i64, i64, vp, vp, vp]
     L.b200_op_quantize_weights.argtypes = [i32, vp, i64, i64, vp]
+    L.b200_op_quantize_blocks_device.argtypes = [i32, i32, vp, i64, vp, vp]
     L.b200_op_mul_mat.argtypes = [i32, vp, i64, i64, vp, i64, vp, i32]
     L.b200_op_quantize_q8_K.argtypes = [vp, i64, i64, vp]
     L.b200_op_lora_patch.argtypes = [i32, vp, i64, i64, i32, vp, vp, i64, C.c_float]
     L.b200_model_load_tensor_lora.argtypes = [vp, C.c_char_p, i32, i32, i64, i64, vp, sz, C.POINTER(vp), i32]
     L.b200_llama_load_file_lora.restype = vp
     L.b200_llama_load_file_lora.argtypes = [C.c_char_p, i32, C.c_float, C.c_float, i32, C.POINTER(C.c_char_p), i32, C.POINTER(C.c_int)]
+    L.b200_quantize_file.argtypes = [C.c_char_p, C.c_char_p, i32, i32, i32, QUANTIZE_CALLBACK, vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64 * 16)]
     _lib = L
     return L

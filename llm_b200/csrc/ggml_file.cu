@@ -87,6 +87,29 @@ bool b200::lora_in_patch_set(const b200_ggml_file *f, const char *name) {     //
 }
 float b200::lora_scaling(const b200_ggml_file *f) { return (float)f->hp[1] / (float)f->hp[0]; }    // LoraParameters::calculate_scaling
 
+// ---- the writers' view (host.h) ----
+const char *b200::ggml_tensor_name(const b200_ggml_file *f, int64_t i, size_t *len) {
+    const std::string &n = f->tensors[(size_t)i].name;
+    *len = n.size();
+    return n.data();
+}
+// one tensor record of ggml::format::save (saver.rs:136-153): n_dims, name length, element type, ne[0..n_dims), the name, and with `align`
+// (GGJT) zeros up to the next multiple of 32 bytes of the file; the caller writes the data
+bool b200::ggml_write_record(FILE *fp, const char *name, size_t name_len, int32_t n_dims, int32_t type, const int64_t *ne, bool align) {
+    bool ok = true;
+    auto w32 = [&](uint32_t v) { ok &= fwrite(&v, 4, 1, fp) == 1; };
+    w32((uint32_t)n_dims); w32((uint32_t)name_len); w32((uint32_t)type);
+    for (int d = 0; d < n_dims; d++) w32((uint32_t)ne[d]);
+    ok &= fwrite(name, 1, name_len, fp) == name_len;
+    if (align) {
+        const long pos = ftell(fp);
+        static const uint8_t zeros[32] = {0};
+        const size_t pad = (size_t)(((pos + 31) & ~31L) - pos);
+        if (pad) ok &= fwrite(zeros, 1, pad, fp) == pad;
+    }
+    return ok;
+}
+
 extern "C" {
 
 void b200_ggml_close(b200_ggml_file *f) {
@@ -265,14 +288,7 @@ int b200_ggml_write(const char *path, const int32_t *hparam_words, int32_t n_wor
     }
     for (int64_t i = 0; i < n_tensors && ok; i++) {
         const b200_ggml_tensor_info &t = tensors[i];
-        const uint32_t name_len = (uint32_t)strnlen(t.name, sizeof(t.name));
-        w32((uint32_t)t.n_dims); w32(name_len); w32((uint32_t)t.type);
-        for (int d = 0; d < t.n_dims; d++) w32((uint32_t)t.ne[d]);
-        ok &= fwrite(t.name, 1, name_len, fp) == name_len;
-        const long pos = ftell(fp);
-        static const uint8_t zeros[32] = {0};
-        const size_t pad = (size_t)(((pos + 31) & ~31L) - pos);
-        if (pad) ok &= fwrite(zeros, 1, pad, fp) == pad;
+        ok &= b200::ggml_write_record(fp, t.name, strnlen(t.name, sizeof(t.name)), t.n_dims, t.type, t.ne, true);
         if (t.nbytes) ok &= fwrite(data[i], 1, (size_t)t.nbytes, fp) == (size_t)t.nbytes;
     }
     ok &= fclose(fp) == 0;

@@ -100,6 +100,10 @@ int read_slot(const Slot &s, void *host, size_t nbytes);                       /
 int64_t ggml_find_tensor(const b200_ggml_file *f, const char *name);        // index in the tensor table, -1 if absent
 bool lora_in_patch_set(const b200_ggml_file *f, const char *name);          // some tensor of the adapter is `name` + "." + a last component
 float lora_scaling(const b200_ggml_file *f);                                // (f32)alpha / (f32)r
+// ---- model files written by b200_ggml_write and the quantizer (ggml_file.cu) ----
+const char *ggml_tensor_name(const b200_ggml_file *f, int64_t i, size_t *len);     // tensor i's whole name (not NUL-terminated)
+// a tensor record: header, name and (GGJT) the zero padding to the next 32-byte offset of the file; false on a write error
+bool ggml_write_record(FILE *fp, const char *name, size_t name_len, int32_t n_dims, int32_t type, const int64_t *ne, bool align);
 
 // ---- what every session keeps: the KV cache, the position, token and logits staging, the decode graphs -------------------------------
 struct SessionCore {

@@ -86,8 +86,12 @@ void mul_mat_kq_exact(int type, const void *w_raw, const void *xq8k, float *dst,
 // ---- synth.cu : seeded synthetic tensors generated in HBM (bench / tests) ------------------------------------------------------------
 void synth_qweight(const QWeight &w, uint64_t seed, cudaStream_t st);
 void synth_gain(float *g, int64_t n, uint64_t seed, cudaStream_t st);                       // 1 + 0.1 N(0,1)
-void quantize_weights(const QWeight &w, const float *src, cudaStream_t st);                  // ggml_quantize_q* on the GPU: f32 [N][K] -> planes, bit-exact
 void scale_shift_f32(float *p, int64_t n, float a, float b, cudaStream_t st);                // p = p * a + b
+
+// ---- quantize_file.cu : ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} on the GPU, bit-exact (LC/ggml.c:18083-18208) -------------------------------------
+// nblk 32-element blocks of src (src_type T_F32 or T_F16, contiguous) -> nblk GGML blocks of `type` in file layout at dst (16-byte aligned);
+// hist (nullable): += the reference's 16-bin histogram of the quants
+void quantize_blocks(int type, int src_type, const void *src, int64_t nblk, void *dst, unsigned long long *hist, cudaStream_t st);
 
 // ---- lora.cu : LoRA adapters patched into a weight at load time, bit-exact with the reference's CPU graph (LoraAdapter::patch) ----------------------
 // B200_OK, or the LoadError (TensorWrongSize / UnsupportedElementType) for factors A [a_ne0 = r, a_ne1] and B [b_ne0, b_ne1] on a target [K, N] of wtype

@@ -156,22 +156,27 @@ int b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, con
     return B200_OK;
 }
 
-// ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} on the GPU (crates/llm-base/src/quantize.rs:320-414 calls them per tensor): f32 rows in, GGML blocks out
+// ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} on the GPU (crates/llm-base/src/quantize.rs:320-414 calls them per tensor): f32 rows in, GGML blocks out,
+// through the kernel of b200_quantize_file
 int b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int64_t N, void *ggml_blocks_out) {
     if (!is_quant(wtype) || !w_host || !ggml_blocks_out || K % QK) return B200_ERR_BAD_ARG;
     Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
     cudaStream_t st = R.stream;
     float *dw = (float *)R.op_arena.get((size_t)N * K * 4, st);
     B200_CHECK(cudaMemcpyAsync(dw, w_host, (size_t)N * K * 4, cudaMemcpyHostToDevice, st));
-    QWeight w;
-    const size_t pb = qweight_layout(w, wtype, K, N, nullptr);
-    qweight_layout(w, wtype, K, N, R.op_arena.get(pb, st));
-    quantize_weights(w, dw, st);
     const size_t raw_bytes = (size_t)N * (K / QK) * ggml_block_bytes(wtype);
     void *raw = R.op_arena.get(raw_bytes, st);
-    unpack_weights(w, raw, st);
+    quantize_blocks(wtype, T_F32, dw, N * (K / QK), raw, nullptr, st);
     B200_CHECK(cudaMemcpyAsync(ggml_blocks_out, raw, raw_bytes, cudaMemcpyDeviceToHost, st));
     B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
+// the same kernel on device buffers, enqueued on the backend's stream without a sync (kernel timing with b200_timing_begin / end_ms)
+int b200_op_quantize_blocks_device(int32_t target, int32_t src_type, const void *d_src, int64_t nblk, void *d_dst, void *d_hist) {
+    if (!is_quant(target) || (src_type != T_F32 && src_type != T_F16) || !d_src || !d_dst || nblk < 0 || ((uintptr_t)d_dst & 15)) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init();
+    quantize_blocks(target, src_type, d_src, nblk, d_dst, (unsigned long long *)d_hist, R.stream);
     return B200_OK;
 }
 

@@ -34,25 +34,33 @@ __device__ __forceinline__ void dequant_block(int type, const uint8_t *qs, uint3
 
 // quantize_row_q{4_0,4_1,5_0,5_1,8_0}_reference (LC/ggml.c:943-1145), what ggml_quantize_* calls: the lane's quant q (the 5-bit value for Q5_x),
 // and the block's d and min (Q4_1 / Q5_1), in f32 before the fp16 store.  All 32 lanes take part.
+// FMA: `x0 = x*id; (int8_t)(x0 + 8.5f)` (16.5f, and `(x - min)*id + 0.5f` for Q4_1 / Q5_1) is one fused multiply-add, as the reference's release
+// build executes it (gcc -O3 -mfma contracts across the two statements; oracle/_ref/libggml_ref.so has vfmadd there): the file quantizer.  Without
+// it each step is rounded, as oracle/ggml_oracle.c restates the rule: the synthetic weights and the LoRA patch.  The two differ only where the
+// sum lands within an ulp of an integer (about one block in 400 of F16 values).  Signed zeros follow the reference's scans in both forms.
+template <bool FMA = false>
 __device__ __forceinline__ int quantize_block_ref(int type, float v, float &d, float &mn) {
     int q = 0;
     d = 0.f; mn = 0.f;
     if (type == T_Q4_0 || type == T_Q5_0) {
         const float amax = warp_max(fabsf(v));
         const unsigned who = __ballot_sync(0xffffffffu, fabsf(v) == amax);
-        const float mx = __shfl_sync(0xffffffffu, v, __ffs(who) - 1);           // first element attaining amax (strict `<` scan)
+        // the first element attaining amax (strict `<` scan from max = 0.0f: an all-zero block keeps +0, whatever the signs of its zeros)
+        const float mx = amax == 0.f ? 0.f : __shfl_sync(0xffffffffu, v, __ffs(who) - 1);
         const float div = type == T_Q4_0 ? -8.f : -16.f;
         d = __fdiv_rn(mx, div);
         const float id = d != 0.f ? __fdiv_rn(1.0f, d) : 0.f;
         const float off = type == T_Q4_0 ? 8.5f : 16.5f;
-        q = min(type == T_Q4_0 ? 15 : 31, (int)(int8_t)__float2int_rz(__fadd_rn(__fmul_rn(v, id), off)));
+        q = min(type == T_Q4_0 ? 15 : 31, (int)(int8_t)__float2int_rz(FMA ? __fmaf_rn(v, id, off) : __fadd_rn(__fmul_rn(v, id), off)));
     } else if (type == T_Q4_1 || type == T_Q5_1) {
-        mn = -warp_max(-v);
-        const float mx = warp_max(v);
+        // the first element equal to the minimum / maximum (strict `<` / `>` scans): the sign of a zero extreme is that element's
+        const float lo = -warp_max(-v), hi = warp_max(v);
+        mn = __shfl_sync(0xffffffffu, v, __ffs(__ballot_sync(0xffffffffu, v == lo)) - 1);
+        const float mx = __shfl_sync(0xffffffffu, v, __ffs(__ballot_sync(0xffffffffu, v == hi)) - 1);
         const int levels = type == T_Q4_1 ? 15 : 31;
         d = __fdiv_rn(__fsub_rn(mx, mn), (float)levels);
         const float id = d != 0.f ? __fdiv_rn(1.0f, d) : 0.f;
-        q = __float2int_rz(__fadd_rn(__fmul_rn(__fsub_rn(v, mn), id), 0.5f));
+        q = __float2int_rz(FMA ? __fmaf_rn(__fsub_rn(v, mn), id, 0.5f) : __fadd_rn(__fmul_rn(__fsub_rn(v, mn), id), 0.5f));
         if (type == T_Q4_1) q = min(15, q);
         q &= 0xff;
     } else {   // Q8_0

@@ -20,13 +20,13 @@ __device__ __forceinline__ float gauss(uint64_t seed, uint64_t idx) {
     return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
 }
 
-// one warp per quant block, lane j <-> element j.  src == nullptr: seeded gaussians; else the f32 matrix [N][K] to quantize -- the GPU form of
-// ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} (LC/ggml.c:18083-18230 -> quantize_row_*_reference :943-1145), bit-exact (tests/test_gpu_ops.py)
-__global__ void __launch_bounds__(256) synth_q_kernel(QWeight w, uint64_t seed, float sigma, const float *__restrict__ src) {
+// one warp per quant block, lane j <-> element j: seeded gaussians quantized by the reference's rule (quantize_row_*_reference,
+// LC/ggml.c:943-1145) straight into the planes
+__global__ void __launch_bounds__(256) synth_q_kernel(QWeight w, uint64_t seed, float sigma) {
     const int64_t blk = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
     if (blk >= w.N * w.nb) return;
     const int lane = threadIdx.x & 31;
-    const float v = src ? src[blk * 32 + lane] : gauss(seed, (uint64_t)blk * 32 + lane) * sigma;
+    const float v = gauss(seed, (uint64_t)blk * 32 + lane) * sigma;
     float d, mn;
     const int q = quantize_block_ref(w.type, v, d, mn);
     if (w.type == T_Q8_0) {
@@ -65,14 +65,7 @@ void synth_qweight(const QWeight &w, uint64_t seed, cudaStream_t st) {
         B200_CHECK(cudaGetLastError());
         return;
     }
-    synth_q_kernel<<<(unsigned)((nblk + 7) / 8), 256, 0, st>>>(w, seed, 1.0f / sqrtf((float)w.K), nullptr);
-    B200_CHECK(cudaGetLastError());
-}
-// weight quantizer: f32 [N][K] (device, contiguous) -> the planes of w
-void quantize_weights(const QWeight &w, const float *src, cudaStream_t st) {
-    const int64_t nblk = w.N * w.nb;
-    if (nblk == 0) return;
-    synth_q_kernel<<<(unsigned)((nblk + 7) / 8), 256, 0, st>>>(w, 0, 0.f, src);
+    synth_q_kernel<<<(unsigned)((nblk + 7) / 8), 256, 0, st>>>(w, seed, 1.0f / sqrtf((float)w.K));
     B200_CHECK(cudaGetLastError());
 }
 __global__ void scale_shift_kernel(float *p, int64_t n, float a, float b) {
