@@ -78,6 +78,9 @@ enum {                            /* return codes (0 = ok).  CUDA failures print
     /* model quantization (llm_base::QuantizeError, crates/llm-base/src/quantize.rs:69-121) */
     B200_ERR_INVALID_QUANTIZATION_TARGET = -16,         /* InvalidQuantizationTarget: a target other than Q4_0 / Q4_1 / Q5_0 / Q5_1 / Q8_0 */
     B200_ERR_VOCABULARY_SCORING_NOT_SUPPORTED = -17,    /* VocabularyScoringNotSupported: the GGML container with a non-zero token score */
+    /* session snapshots (b200_snapshot below) */
+    B200_ERR_SNAPSHOT_SIZE_MISMATCH = -18,  /* SnapshotError::MemorySizeMismatch: another model geometry, context size or KV type */
+    B200_ERR_SNAPSHOT_FORMAT = -19,         /* a session file this library cannot read (see b200_snapshot) */
 };
 
 /* The reference's default sampler chain (crates/llm-base/src/samplers.rs:97-211, ensure_default_slots), run on the device in this order:
@@ -326,6 +329,57 @@ int32_t b200_neox_read_tokens(b200_neox_session *s, int32_t *tokens_out, int32_t
 int  b200_neox_last_logits(b200_neox_session *s, float *logits_out);
 void b200_neox_session_free(b200_neox_session *s);
 
+/* ---- session snapshots: InferenceSession::get_snapshot / from_snapshot (crates/llm-base/src/inference_session.rs:591-646, types :733-792) and the
+ * CLI's session files (--save-session / --load-session / --persist-session, binaries/llm-cli/src/snapshot.rs) ------------------------------------
+ * memory_k / memory_v are the reference's bytes: n_layer x context_size x n_embd values of the cache's type each (for LLaMA with grouped-query
+ * attention the reference sizes them by n_embd and uses the first n_layer x context_size x n_embd_gqa values; the rest is written as zeros and
+ * ignored when read).  K is [n_layer][context_size][width]; V is [n_layer][width][context_size] for LLaMA, GPT-NeoX and GPT-J, and
+ * [n_layer][context_size][n_embd] (by position) for GPT-2, MPT and BLOOM, whose native cache keeps V by channel: those are transposed on the GPU
+ * on the way out and back in.  The cache slots past npast are part of the bytes and are kept.
+ *
+ * Session file: bincode 1.3.3 (default options: little-endian, fixed-width integers, usize as u64, enum variant as u32, Vec / bytes as a u64
+ * count and the elements) of InferenceSnapshotRef -- npast u64, memory_k_type u32, memory_v_type u32, n_batch u64, n_threads u64, tokens (u64 +
+ * u32 each), last_logits (u64 + f32 each), memory_k (u64 + bytes), memory_v (u64 + bytes) -- inside one zstd frame.  Written: magic 28 B5 2F FD,
+ * frame header descriptor 0xC0 (8-byte content size, not single-segment, no checksum, no dictionary), window descriptor 0x38 (128 KiB), the
+ * content size, then 128 KiB raw (stored) blocks, the last one flagged: no compressor is needed and every zstd decoder reads it.  Read: one zstd
+ * frame whose blocks are raw or RLE (its checksum, if any, is not verified).  This library has no zstd decoder, so compressed blocks -- what the
+ * reference CLI writes at level 1 -- are refused with B200_ERR_SNAPSHOT_FORMAT, as are a truncated file, a bad magic, a reserved bit, a block
+ * larger than the window or 128 KiB, a content size that is not the blocks', a length field that overruns the content, content after
+ * memory_v, and bytes after the frame.  The cache streams between HBM and the file through a ring of a few 8 MiB pinned and device buffers: the
+ * host never holds a copy of the cache.  A failed write removes the partial file.
+ *
+ * from_snapshot starts a session with the snapshot's n_batch and KV type, then writes the cache, n_past, the history and the last row, which the
+ * next infer_next_token samples from (even when it is the reference's initial zeros).  Refusals, all checked before anything is allocated:
+ * B200_ERR_SNAPSHOT_SIZE_MISMATCH when memory_k or memory_v is not the bytes this model's cache has with the snapshot's KV type; B200_ERR_BAD_ARG for
+ * KV types other than 0 / 1 or unequal ones, npast < 0 or > context_size, n_tokens != npast, a token id outside [0, n_vocab), n_logits !=
+ * n_vocab, n_batch outside [1, 65536], null pointers, and tensor-parallel sessions and models.
+ * Deviations: tokens must hold exactly npast ids (the reference does not check it, and its direct evaluate calls push no tokens; here the history
+ * is positional and every evaluate records it); compressed zstd blocks are refused; a GPT-2 model's context is its n_ctx, so a reference GPT-2
+ * session at another context_size is a size mismatch. */
+typedef struct {
+    int64_t  npast;
+    int32_t  memory_k_type, memory_v_type;   /* ModelKVMemoryType variant index: 0 Float16, 1 Float32 (not enum ggml_type) */
+    int64_t  n_batch, n_threads;             /* n_threads: written as 8 (the reference default), ignored when read */
+    int64_t  n_tokens;  uint32_t *tokens;
+    int64_t  n_logits;  float    *last_logits;
+    uint64_t memory_k_bytes, memory_v_bytes; void *memory_k, *memory_v;   /* the reference's layout and size */
+} b200_snapshot;
+/* get_snapshot: with tokens, last_logits, memory_k and memory_v all NULL it fills in the scalars, counts and sizes only; with all four set it also
+ * copies into them, and the counts and sizes must be the session's (B200_ERR_BAD_ARG otherwise).  Ordered after the work queued on the stream. */
+int  b200_session_get_snapshot(b200_session *s, b200_snapshot *snap);
+/* from_snapshot on model m; flags may add B200_SESSION_NO_GRAPH / UNFUSED / FAST, the KV bit comes from the snapshot (a conflicting
+ * B200_SESSION_KV_F32 is B200_ERR_BAD_ARG).  NULL and *err (nullable) on a refusal. */
+b200_session *b200_model_session_from_snapshot(b200_model *m, const b200_snapshot *snap, int32_t flags, int *err);
+int  b200_session_write_snapshot(b200_session *s, const char *path);          /* get_snapshot as a session file; B200_ERR_IO on a write error */
+b200_session *b200_model_session_read_snapshot(b200_model *m, const char *path, int32_t flags, int *err);   /* from_snapshot of a session file */
+/* the scalars, counts and sizes of a session file (the pointers are set to NULL); B200_ERR_IO, B200_ERR_SNAPSHOT_FORMAT */
+int  b200_snapshot_read_header(const char *path, b200_snapshot *snap);
+/* the same for every architecture of the GPT-NeoX / GPT-2 runtime (no flags, as b200_neox_start_session_flags) */
+int  b200_neox_get_snapshot(b200_neox_session *s, b200_snapshot *snap);
+b200_neox_session *b200_neox_session_from_snapshot(b200_neox_model *m, const b200_snapshot *snap, int *err);
+int  b200_neox_write_snapshot(b200_neox_session *s, const char *path);
+b200_neox_session *b200_neox_session_read_snapshot(b200_neox_model *m, const char *path, int *err);
+
 /* ---- single-op entry points on HOST buffers (unit tests, INTEGRATION examples).  Each uploads, runs the kernel, downloads. */
 int  b200_op_quantize_act(int32_t vec_dot_type, const float *x, int64_t K, int64_t B, int8_t *qs_out, float *d_out, float *aux_out);
 /* ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} (LC/ggml.c:18083-18230) on the GPU: w_host f32 [N][K] -> N rows of GGML blocks, bit-exact with the reference */
@@ -333,6 +387,9 @@ int  b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int
 /* the kernel of b200_quantize_file on DEVICE buffers, enqueued on b200_stream() without a sync (for kernel timing): nblk 32-element blocks of
  * d_src (src_type 0 F32 / 1 F16) -> GGML blocks of target at d_dst (16-byte aligned); d_hist (nullable): 16 uint64 counters, added to */
 int  b200_op_quantize_blocks_device(int32_t target, int32_t src_type, const void *d_src, int64_t nblk, void *d_dst, void *d_hist);
+/* the snapshot's transpose kernel on DEVICE buffers, enqueued on b200_stream() without a sync (for kernel timing): d_dst[c][r] = d_src[r][c] for
+ * r < rows, c < cols, elements of elem_bytes (2 or 4) bytes, row strides src_ld / dst_ld elements; bit patterns are copied as they are */
+int  b200_op_transpose_device(int32_t elem_bytes, const void *d_src, int64_t src_ld, void *d_dst, int64_t dst_ld, int64_t rows, int64_t cols);
 /* wtype: GGML_TYPE_F16 (1; K % 64 == 0, impl AUTO or EXACT = mul_mat_f16_exact), GGML_TYPE_Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 (2,3,6,7,8; K % 64 == 0), or the K-quants Q2_K..Q6_K (10..14; K % 256 == 0, impl AUTO or EXACT:
  * ggml_vec_dot_q{2,3,4,5,6}_K_q8_K of LC/k_quants.c:1240,1763,2492,3023,3592 on quantize_row_q8_K activations, bit-exact with the reference's AVX2 build) */
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);

@@ -9,6 +9,7 @@ arithmetic and no fallback path.
 from .session import ContextFull, InferenceSession, InferenceSessionConfig, Llama, ModelKVMemoryType, ModelParameters, OutputRequest  # noqa: F401
 from .session import (EndOfText, InferenceFeedback, InferenceParameters, InferenceRequest, InferenceStats, Rng, Sampler,  # noqa: F401
                       SamplerFailure)
+from .session import InferenceSnapshot, MemorySizeMismatch, SnapshotError  # noqa: F401
 from . import ggml  # noqa: F401
 
 # enum ggml_type values of the five block formats on the hot path (LC/ggml.h:262-285)
@@ -17,4 +18,4 @@ F32, F16 = 0, 1
 from . import loader  # noqa: F401
 from .quantize import QuantizeError, quantize  # noqa: F401
 from . import tp  # noqa: F401
-from .neox import GptJ  # noqa: F401
+from .neox import GptJ, NeoxSession  # noqa: F401

@@ -41,6 +41,13 @@ class QuantizeReport(C.Structure):
                 ("n_elements", C.c_int64), ("original_size", C.c_int64), ("reduced_size", C.c_int64), ("hist", C.c_int64 * 16)]
 
 
+class Snapshot(C.Structure):
+    """b200_snapshot (include/llm_b200.h) <- InferenceSnapshot, crates/llm-base/src/inference_session.rs:733-792."""
+    _fields_ = [("npast", C.c_int64), ("memory_k_type", C.c_int32), ("memory_v_type", C.c_int32), ("n_batch", C.c_int64), ("n_threads", C.c_int64),
+                ("n_tokens", C.c_int64), ("tokens", C.c_void_p), ("n_logits", C.c_int64), ("last_logits", C.c_void_p),
+                ("memory_k_bytes", C.c_uint64), ("memory_v_bytes", C.c_uint64), ("memory_k", C.c_void_p), ("memory_v", C.c_void_p)]
+
+
 QUANTIZE_CALLBACK = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(QuantizeReport))
 
 
@@ -133,5 +140,13 @@ def lib():
     L.b200_llama_load_file_lora.restype = vp
     L.b200_llama_load_file_lora.argtypes = [C.c_char_p, i32, C.c_float, C.c_float, i32, C.POINTER(C.c_char_p), i32, C.POINTER(C.c_int)]
     L.b200_quantize_file.argtypes = [C.c_char_p, C.c_char_p, i32, i32, i32, QUANTIZE_CALLBACK, vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64 * 16)]
+    L.b200_session_get_snapshot.argtypes = [vp, C.POINTER(Snapshot)]
+    L.b200_session_write_snapshot.argtypes = [vp, C.c_char_p]
+    L.b200_model_session_from_snapshot.restype = vp
+    L.b200_model_session_from_snapshot.argtypes = [vp, C.POINTER(Snapshot), i32, C.POINTER(C.c_int)]
+    L.b200_model_session_read_snapshot.restype = vp
+    L.b200_model_session_read_snapshot.argtypes = [vp, C.c_char_p, i32, C.POINTER(C.c_int)]
+    L.b200_snapshot_read_header.argtypes = [C.c_char_p, C.POINTER(Snapshot)]
+    L.b200_op_transpose_device.argtypes = [i32, vp, i64, vp, i64, i64, i64]
     _lib = L
     return L

@@ -116,6 +116,31 @@ int read_slot(const Slot &s, void *host, size_t nbytes) {
     return B200_OK;
 }
 
+StreamRing::StreamRing(int n, size_t host_bytes, size_t dev_bytes) : slots((size_t)n) {
+    rt().ensure_init();
+    for (Slot &s : slots) {
+        B200_CHECK(cudaStreamCreateWithFlags(&s.st, cudaStreamNonBlocking));
+        B200_CHECK(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+        B200_CHECK(cudaHostAlloc((void **)&s.h, host_bytes, cudaHostAllocDefault));
+        if (dev_bytes) B200_CHECK(cudaMalloc((void **)&s.d, dev_bytes));
+    }
+}
+
+StreamRing::~StreamRing() {                 // no exit() here: it also runs while an exception unwinds
+    for (Slot &s : slots) {
+        cudaStreamSynchronize(s.st); cudaStreamDestroy(s.st); cudaEventDestroy(s.done);
+        cudaFreeHost(s.h); if (s.d) cudaFree(s.d);
+    }
+}
+
+void StreamRing::after(cudaStream_t st) {
+    cudaEvent_t ev;
+    B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    B200_CHECK(cudaEventRecord(ev, st));
+    for (Slot &s : slots) B200_CHECK(cudaStreamWaitEvent(s.st, ev, 0));
+    B200_CHECK(cudaEventDestroy(ev));        // released once the waits it feeds have completed
+}
+
 void SessionCore::start(int n_batch_, int n_ctx_, int n_vocab_, size_t kv_elems_, int kv_type_) {
     n_batch = n_batch_; n_ctx = n_ctx_; n_vocab = n_vocab_;
     kv_type = kv_type_; kv_elems = kv_elems_;

@@ -1,6 +1,8 @@
 // llm_b200/csrc/host.h -- host plumbing shared by the LLaMA (session.cu) and GPT-NeoX / GPT-2 (neox.cu) runtimes: owned device and pinned
 // buffers, the weight slab and its named tensor slots, seeded synthesis, and the state every session keeps (KV cache, token / logits staging).
 #pragma once
+#include <string.h>
+
 #include <functional>
 #include <memory>
 #include <type_traits>
@@ -105,6 +107,35 @@ const char *ggml_tensor_name(const b200_ggml_file *f, int64_t i, size_t *len);  
 // a tensor record: header, name and (GGJT) the zero padding to the next 32-byte offset of the file; false on a write error
 bool ggml_write_record(FILE *fp, const char *name, size_t name_len, int32_t n_dims, int32_t type, const int64_t *ne, bool align);
 
+// ---- streaming between host files and HBM in bounded memory (the model quantizer, session snapshots) ------------------------------------
+// `n` slots, each with its own stream, a completion event and a pinned and a device buffer.  Chunk c uses slot c % n: the caller waits for the
+// slot's previous chunk (retire) before refilling it, so chunk c's copies overlap the host work on chunks c - n + 1 .. c - 1.
+struct StreamRing {
+    struct Slot {
+        cudaStream_t st = nullptr; cudaEvent_t done = nullptr;
+        char *h = nullptr, *d = nullptr;
+        size_t bytes = 0;               // the chunk's payload (the caller's bookkeeping)
+        bool busy = false;              // work recorded on `done` has not been retired
+    };
+    std::vector<Slot> slots;
+    StreamRing(int n, size_t host_bytes, size_t dev_bytes);
+    ~StreamRing();                      // waits for every slot, then frees
+    StreamRing(const StreamRing &) = delete;
+    StreamRing &operator=(const StreamRing &) = delete;
+    Slot &at(int64_t chunk) { return slots[(size_t)(chunk % (int64_t)slots.size())]; }
+    void after(cudaStream_t st);        // every slot's later work is ordered after what `st` has queued so far
+    static void wait(Slot &s) { if (s.busy) { B200_CHECK(cudaEventSynchronize(s.done)); s.busy = false; } }
+    void drain() { for (Slot &s : slots) wait(s); }
+};
+
+// ---- session snapshots (snapshot.cu): the reference's cache layout, which a front end describes ----------------------------------------
+// The reference sizes memory_k / memory_v as n_layer x n_ctx x ref_width values and uses the first n_layer x n_ctx x width of them: K as
+// [n_layer][n_ctx][width], V as [n_layer][width][n_ctx], or [n_layer][n_ctx][width] when v_by_position (GPT-2, MPT, BLOOM).  The native cache is
+// [n_layer][n_ctx][width] and [n_layer][width][n_ctx] for every architecture.
+struct RefKvLayout { int n_layer; int64_t width, ref_width; bool v_by_position; };
+// one source of snapshot bytes (a caller's buffer or a session file), read in order; false on a read error
+using SnapshotSource = std::function<bool(void *dst, size_t n)>;
+
 // ---- what every session keeps: the KV cache, the position, token and logits staging, the decode graphs -------------------------------
 struct SessionCore {
     int n_batch = 0, n_ctx = 0, n_vocab = 0;
@@ -151,7 +182,53 @@ struct SessionCore {
     int top_k(const float *logits, int k, int32_t *ids_out, float *vals_out);
     int32_t read_tokens(int32_t *out, int32_t max);                    // min(n_past, max) ids of the history; returns n_past
     int last_logits(const float *logits, float *out);                 // the last evaluated row, n_vocab floats
+
+    // InferenceSession::get_snapshot (snapshot.cu): the scalars and counts always; with the four pointers set, their contents (the counts must be
+    // the session's), ordered after the work queued on the backend stream.  last_logits: the last row of `logits`, zeros before any evaluate.
+    int get_snapshot(const RefKvLayout &L, const float *logits, b200_snapshot *snap);
+    int write_snapshot(const RefKvLayout &L, const float *logits, const char *path);   // the same as a session file, streamed
+    // the second half of InferenceSession::from_snapshot on a fresh session whose type and n_batch are the snapshot's (checked by
+    // snapshot_check): the cache from k / v (the reference's bytes, in order), n_past, the history and the last row (row 0 of `logits`, last_n 1)
+    int restore_snapshot(const RefKvLayout &L, float *logits, const b200_snapshot &h, const SnapshotSource &k, const SnapshotSource &v);
 };
+
+// ---- InferenceSession::from_snapshot for a front end (snapshot.cu) ------------------------------------------------------------------------
+// A parsed session file: its scalars and counts in `h` (tokens / last_logits point into the vectors below, the memory pointers are null), and
+// the cache bytes, read on demand.
+struct SnapshotFile {
+    b200_snapshot h{};
+    std::vector<uint32_t> tokens; std::vector<float> last_logits;
+    std::shared_ptr<void> reader;       // the zstd frame reader, positioned at memory_k's bytes
+    SnapshotSource k, v;
+};
+int snapshot_read_file(const char *path, SnapshotFile &f, bool with_data);    // B200_OK, B200_ERR_IO, B200_ERR_SNAPSHOT_FORMAT
+// every refusal of from_snapshot for a model of context n_ctx, n_vocab ids and cache layout L: BAD_ARG, SNAPSHOT_SIZE_MISMATCH
+int snapshot_check(const b200_snapshot &h, int n_ctx, int n_vocab, const RefKvLayout &L);
+// start(n_batch, kv_f32, logits) starts the front end's session (nullptr: refused) and sets `logits` to its logits buffer; release(s) frees it
+// when a session file fails to read after it was started.  snap (in memory) or path (a session file) is checked before the session is started.
+template <class Sess, class Start, class Release>
+Sess *session_from_snapshot(const b200_snapshot *snap, const char *path, int n_ctx, int n_vocab, const RefKvLayout &L, int *err, Start &&start,
+                            Release &&release) {
+    SnapshotFile file;
+    int rc = B200_OK;
+    if (path) rc = snapshot_read_file(path, file, true);
+    else if (!snap) rc = B200_ERR_BAD_ARG;
+    const b200_snapshot &h = path ? file.h : *snap;
+    if (rc == B200_OK) rc = snapshot_check(h, n_ctx, n_vocab, L);
+    if (rc == B200_OK && !path && (!h.memory_k || !h.memory_v)) rc = B200_ERR_BAD_ARG;
+    Sess *s = nullptr;
+    float *logits = nullptr;
+    if (rc == B200_OK && !(s = start((int)h.n_batch, h.memory_k_type == 1, logits))) rc = B200_ERR_BAD_ARG;
+    if (rc == B200_OK) {
+        size_t ko = 0, vo = 0;
+        const SnapshotSource mk = [&](void *d, size_t n) { memcpy(d, (const char *)h.memory_k + ko, n); ko += n; return true; };
+        const SnapshotSource mv = [&](void *d, size_t n) { memcpy(d, (const char *)h.memory_v + vo, n); vo += n; return true; };
+        rc = s->restore_snapshot(L, logits, h, path ? file.k : mk, path ? file.v : mv);
+        if (rc != B200_OK) { release(s); s = nullptr; }
+    }
+    if (err) *err = rc;
+    return rc == B200_OK ? s : nullptr;
+}
 // a b200_sampler as the kernels take it; false if it is out of range (top_k < 1, temperature or penalty <= 0 or NaN, last_n < 0, top_p NaN)
 bool sampler_args(const b200_sampler *s, SampleArgs &a);
 

@@ -475,4 +475,37 @@ void b200_neox_session_free(b200_neox_session *s) {
     delete s;                                           // every buffer, the decode graphs and n_past words go with it
 }
 
+// ---- snapshots (snapshot.cu): GPT-2, MPT and BLOOM keep V by position in the reference (gpt2 lib.rs:197-211, mpt :139-148, bloom :188-203) ---------
+static RefKvLayout ref_layout(const b200_neox_model *m) {
+    return RefKvLayout{m->hp.n_layer, m->hp.n_embd, m->hp.n_embd, m->hp.arch == 1 || m->mpt() || m->bloom()};
+}
+
+int b200_neox_get_snapshot(b200_neox_session *s, b200_snapshot *snap) {
+    return s ? s->get_snapshot(ref_layout(s->m), s->logits.get(), snap) : B200_ERR_BAD_ARG;
+}
+
+int b200_neox_write_snapshot(b200_neox_session *s, const char *path) {
+    return s ? s->write_snapshot(ref_layout(s->m), s->logits.get(), path) : B200_ERR_BAD_ARG;
+}
+
+static b200_neox_session *neox_session_from(b200_neox_model *m, const b200_snapshot *snap, const char *path, int *err) {
+    if (!m) { if (err) *err = B200_ERR_BAD_ARG; return nullptr; }
+    return session_from_snapshot<b200_neox_session>(snap, path, m->hp.context_size, m->hp.n_vocab, ref_layout(m), err,
+        [m](int n_batch, bool kv32, float *&logits) -> b200_neox_session * {
+            b200_neox_session *s = b200_neox_start_session_flags(m, n_batch, kv32 ? B200_SESSION_KV_F32 : 0);
+            if (s) logits = s->logits.get();
+            return s;
+        },
+        [](b200_neox_session *s) { b200_neox_session_free(s); });
+}
+
+b200_neox_session *b200_neox_session_from_snapshot(b200_neox_model *m, const b200_snapshot *snap, int *err) {
+    return neox_session_from(m, snap, nullptr, err);
+}
+
+b200_neox_session *b200_neox_session_read_snapshot(b200_neox_model *m, const char *path, int *err) {
+    if (!path) { if (err) *err = B200_ERR_BAD_ARG; return nullptr; }
+    return neox_session_from(m, nullptr, path, err);
+}
+
 }  // extern "C"

@@ -129,16 +129,6 @@ int llama_ftype(int32_t target) {
 
 struct Plan { b200_ggml_tensor_info info; bool quantize; int64_t out_bytes; };
 
-struct Slot {
-    cudaStream_t st;
-    cudaEvent_t done;
-    void *h_in, *d_in;
-    uint8_t *h_out, *d_out;
-    unsigned long long *d_hist;                // this slot's 16 counters of the current tensor
-    size_t out_bytes;
-    bool busy;
-};
-
 int quantize_file_impl(const char *src_path, const char *dst_path, int32_t arch, int32_t target, int32_t container, b200_quantize_callback cb,
                        void *user, int64_t *original_size_out, int64_t *reduced_size_out, int64_t *hist_out, bool &created) {
     if (llama_ftype(target) < 0) return B200_ERR_INVALID_QUANTIZATION_TARGET;
@@ -178,34 +168,15 @@ int quantize_file_impl(const char *src_path, const char *dst_path, int32_t arch,
     b200_ggml_hparams(f, nullptr, words, &n_words);
     words[file_type_word(arch)] = 2 * 1000 + llama_ftype(target);           // quantization_version ggml::QNT_VERSION, format MostlyQ*
 
-    std::vector<Slot> slots;
+    // each slot's buffers: the source chunk (IN bytes), then its blocks; d_hist: 16 counters per slot for the current tensor
+    constexpr size_t IN = CHUNK_BLOCKS * QK * 4, OUT = CHUNK_BLOCKS * 34;
     unsigned long long *d_hist = nullptr;
+    struct Release { unsigned long long *&d_hist; ~Release() { if (d_hist) cudaFree(d_hist); } } release{d_hist};
+    std::unique_ptr<StreamRing> ring;             // destroyed first: its streams are idle before d_hist goes
     if (any_quantized) {
-        rt().ensure_init();
+        ring.reset(new StreamRing(RING, IN + OUT, IN + OUT));
         B200_CHECK(cudaMalloc(&d_hist, RING * 16 * sizeof(unsigned long long)));
-        slots.resize(RING);
-        for (int s = 0; s < RING; s++) {
-            Slot &sl = slots[s];
-            B200_CHECK(cudaStreamCreateWithFlags(&sl.st, cudaStreamNonBlocking));
-            B200_CHECK(cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
-            B200_CHECK(cudaHostAlloc(&sl.h_in, CHUNK_BLOCKS * QK * 4, cudaHostAllocDefault));
-            B200_CHECK(cudaHostAlloc((void **)&sl.h_out, CHUNK_BLOCKS * 34, cudaHostAllocDefault));
-            B200_CHECK(cudaMalloc(&sl.d_in, CHUNK_BLOCKS * QK * 4));
-            B200_CHECK(cudaMalloc((void **)&sl.d_out, CHUNK_BLOCKS * 34));
-            sl.d_hist = d_hist + s * 16;
-            sl.busy = false;
-        }
     }
-    struct Release {
-        std::vector<Slot> &slots; unsigned long long *d_hist;
-        ~Release() {
-            for (Slot &sl : slots) {
-                cudaStreamSynchronize(sl.st); cudaStreamDestroy(sl.st); cudaEventDestroy(sl.done);
-                cudaFreeHost(sl.h_in); cudaFreeHost(sl.h_out); cudaFree(sl.d_in); cudaFree(sl.d_out);
-            }
-            if (d_hist) cudaFree(d_hist);
-        }
-    } release{slots, d_hist};
 
     FILE *fp = fopen(dst_path, "wb");
     if (!fp) return B200_ERR_IO;
@@ -224,10 +195,9 @@ int quantize_file_impl(const char *src_path, const char *dst_path, int32_t arch,
     }
 
     int64_t total_in = 0, total_out = 0, hist_all[16] = {0};
-    auto retire = [&](Slot &sl) {
-        B200_CHECK(cudaEventSynchronize(sl.done));
-        ok &= fwrite(sl.h_out, 1, sl.out_bytes, fp) == sl.out_bytes;
-        sl.busy = false;
+    auto retire = [&](StreamRing::Slot &sl) {
+        StreamRing::wait(sl);
+        ok &= fwrite(sl.h + IN, 1, sl.bytes, fp) == sl.bytes;
     };
     for (size_t i = 0; i < plan.size() && ok; i++) {
         const Plan &p = plan[i];
@@ -242,22 +212,22 @@ int quantize_file_impl(const char *src_path, const char *dst_path, int32_t arch,
             if (p.info.nbytes) ok &= fwrite(data, 1, (size_t)p.info.nbytes, fp) == (size_t)p.info.nbytes;
         } else {
             const int64_t nblk = p.info.ne[0] * p.info.ne[1] / QK, es = p.info.type == T_F16 ? 2 : 4;
-            for (Slot &sl : slots) B200_CHECK(cudaMemsetAsync(sl.d_hist, 0, 16 * sizeof(unsigned long long), sl.st));
+            for (int k = 0; k < RING; k++) B200_CHECK(cudaMemsetAsync(d_hist + k * 16, 0, 16 * sizeof(unsigned long long), ring->at(k).st));
             int64_t c = 0;
             for (int64_t b0 = 0; b0 < nblk && ok; b0 += CHUNK_BLOCKS, c++) {
-                Slot &sl = slots[(size_t)(c % RING)];
+                StreamRing::Slot &sl = ring->at(c);
                 if (sl.busy) retire(sl);                                   // chunk c - RING, the oldest in flight: writes stay in file order
                 const int64_t nb = std::min(CHUNK_BLOCKS, nblk - b0);
-                memcpy(sl.h_in, data + b0 * QK * es, (size_t)(nb * QK * es));
-                B200_CHECK(cudaMemcpyAsync(sl.d_in, sl.h_in, (size_t)(nb * QK * es), cudaMemcpyHostToDevice, sl.st));
-                quantize_blocks(target, p.info.type, sl.d_in, nb, sl.d_out, sl.d_hist, sl.st);
-                sl.out_bytes = (size_t)(nb * ggml_block_bytes(target));
-                B200_CHECK(cudaMemcpyAsync(sl.h_out, sl.d_out, sl.out_bytes, cudaMemcpyDeviceToHost, sl.st));
+                memcpy(sl.h, data + b0 * QK * es, (size_t)(nb * QK * es));
+                B200_CHECK(cudaMemcpyAsync(sl.d, sl.h, (size_t)(nb * QK * es), cudaMemcpyHostToDevice, sl.st));
+                quantize_blocks(target, p.info.type, sl.d, nb, sl.d + IN, d_hist + (c % RING) * 16, sl.st);
+                sl.bytes = (size_t)(nb * ggml_block_bytes(target));
+                B200_CHECK(cudaMemcpyAsync(sl.h + IN, sl.d + IN, sl.bytes, cudaMemcpyDeviceToHost, sl.st));
                 B200_CHECK(cudaEventRecord(sl.done, sl.st));
                 sl.busy = true;
             }
             for (int k = 0; k < RING; k++) {
-                Slot &sl = slots[(size_t)((c + k) % RING)];
+                StreamRing::Slot &sl = ring->at(c + k);
                 if (sl.busy) retire(sl);
             }
             unsigned long long h[RING * 16];

@@ -610,6 +610,44 @@ int b200_session_read_kv(b200_session *s, int32_t which, void *host_out, size_t 
     return s ? s->read_kv(which, host_out, nbytes) : B200_ERR_BAD_ARG;
 }
 
+// ---- snapshots (snapshot.cu): the reference sizes LLaMA's cache by n_embd and uses n_embd_gqa of it per position, V by channel as here ------------
+static RefKvLayout ref_layout(const b200_model *m) { return RefKvLayout{m->hp.n_layer, m->gqa, m->hp.n_embd, false}; }
+
+int b200_session_get_snapshot(b200_session *s, b200_snapshot *snap) {
+    if (!s || s->m->tp_world > 1) return B200_ERR_BAD_ARG;
+    return s->get_snapshot(ref_layout(s->m), s->logits.get(), snap);
+}
+
+int b200_session_write_snapshot(b200_session *s, const char *path) {
+    if (!s || s->m->tp_world > 1) return B200_ERR_BAD_ARG;
+    return s->write_snapshot(ref_layout(s->m), s->logits.get(), path);
+}
+
+static b200_session *session_from(b200_model *m, const b200_snapshot *snap, const char *path, int32_t flags, int *err) {
+    if (!m || m->tp_world > 1 || (flags & ~(B200_SESSION_NO_GRAPH | B200_SESSION_UNFUSED | B200_SESSION_FAST | B200_SESSION_KV_F32))) {
+        if (err) *err = B200_ERR_BAD_ARG;
+        return nullptr;
+    }
+    return session_from_snapshot<b200_session>(snap, path, m->hp.context_size, m->hp.n_vocab, ref_layout(m), err,
+        [m, flags](int n_batch, bool kv32, float *&logits) -> b200_session * {
+            if ((flags & B200_SESSION_KV_F32) && !kv32) return nullptr;            // the cache type is the snapshot's
+            const b200_session_config cfg{n_batch, flags | (kv32 ? B200_SESSION_KV_F32 : 0)};
+            b200_session *s = b200_model_start_session(m, &cfg);
+            if (s) logits = s->logits.get();
+            return s;
+        },
+        [](b200_session *s) { b200_session_free(s); });
+}
+
+b200_session *b200_model_session_from_snapshot(b200_model *m, const b200_snapshot *snap, int32_t flags, int *err) {
+    return session_from(m, snap, nullptr, flags, err);
+}
+
+b200_session *b200_model_session_read_snapshot(b200_model *m, const char *path, int32_t flags, int *err) {
+    if (!path) { if (err) *err = B200_ERR_BAD_ARG; return nullptr; }
+    return session_from(m, nullptr, path, flags, err);
+}
+
 int b200_session_set_tap(b200_session *s, int32_t layer, int32_t stage) {
     if (!s || s->m->tp_world > 1) return B200_ERR_BAD_ARG;
     s->tap_layer = layer; s->tap_stage = stage; s->tap_count = 0;

@@ -12,7 +12,8 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .session import ContextFull, LoraAdapters, ModelKVMemoryType, _check, _Generation, _Native, _perplexity, _vocab_id, ggml_dims, kv_array, kv_flags
+from .session import (ContextFull, InferenceSnapshot, LoraAdapters, ModelKVMemoryType, _check, _Generation, _Native, _perplexity, _ref_cache_bytes,
+                      _Snapshots, _vocab_id, ggml_dims, kv_array, kv_flags)
 
 
 class NeoxHparams(C.Structure):
@@ -50,6 +51,12 @@ def _bind(L):
     L.b200_neox_read_tokens.argtypes = [vp, vp, i32]
     L.b200_neox_last_logits.argtypes = [vp, vp]
     L.b200_neox_session_free.argtypes = [vp]
+    L.b200_neox_get_snapshot.argtypes = [vp, C.POINTER(_lib.Snapshot)]
+    L.b200_neox_write_snapshot.argtypes = [vp, C.c_char_p]
+    L.b200_neox_session_from_snapshot.restype = vp
+    L.b200_neox_session_from_snapshot.argtypes = [vp, C.POINTER(_lib.Snapshot), C.POINTER(C.c_int)]
+    L.b200_neox_session_read_snapshot.restype = vp
+    L.b200_neox_session_read_snapshot.argtypes = [vp, C.c_char_p, C.POINTER(C.c_int)]
     L._neox_ready = True
     return L
 
@@ -164,19 +171,44 @@ class GptJ(GptNeoX):
     ARCH = 4
 
 
-class NeoxSession(_Generation, _Native):
+class NeoxSession(_Generation, _Snapshots, _Native):
     _HANDLE, _FREE = "_s", "b200_neox_session_free"
     _INFER, _TOKENS, _LAST = "b200_neox_infer_next_token", "b200_neox_read_tokens", "b200_neox_last_logits"
+    _GET_SNAP, _WRITE_SNAP = "b200_neox_get_snapshot", "b200_neox_write_snapshot"
+    _FROM_SNAP, _READ_SNAP = "b200_neox_session_from_snapshot", "b200_neox_session_read_snapshot"
 
-    def __init__(self, model: GptNeoX, n_batch: int, flags: int = 0):
+    def __init__(self, model: GptNeoX, n_batch: int, flags: int = 0, _handle=None):
         self.model, self.L = model, model.L
         self.kv_f32 = flags != 0
         self.n_batch = n_batch
-        self._s = self.L.b200_neox_start_session_flags(model._m, n_batch, flags)
+        self._s = _handle or self.L.b200_neox_start_session_flags(model._m, n_batch, flags)
         if not self._s:
             raise RuntimeError("b200_neox_start_session failed (all tensors loaded?)")
         self.n_vocab = int(model.hyperparameters["n_vocab"])
-        self._last_logits = np.zeros(self.n_vocab, np.float32)
+        self._last_logits = None if _handle else np.zeros(self.n_vocab, np.float32)
+
+    @classmethod
+    def from_snapshot(cls, snapshot: InferenceSnapshot, model: GptNeoX) -> "NeoxSession":
+        """InferenceSession::from_snapshot for every architecture of this runtime (see InferenceSession.from_snapshot)"""
+        return cls._from(snapshot, model, 0)
+
+    @classmethod
+    def read_snapshot(cls, path: str, model: GptNeoX) -> "NeoxSession":
+        """from_snapshot of a session file, streamed into HBM"""
+        return cls._read(path, model, 0)
+
+    @staticmethod
+    def _start_args(flags):
+        return ()
+
+    @staticmethod
+    def _cache_bytes(model, variant):
+        hp = model.hyperparameters
+        return _ref_cache_bytes(hp["n_layer"], model.context_size, hp["n_embd"], variant)
+
+    @classmethod
+    def _adopt(cls, model, handle, config):
+        return cls(model, config.n_batch, 8 if config.memory_k_type == ModelKVMemoryType.Float32 else 0, _handle=handle)
 
     @property
     def n_past(self) -> int:

@@ -9,6 +9,8 @@ Names follow the reference so that the parity tests read like its own integratio
   InferenceError::ContextFull      crates/llm-base/src/inference_session.rs:311-313
   infer_next_token / infer         crates/llm-base/src/inference_session.rs:381-512, InferenceRequest / InferenceStats / InferenceFeedback
   InferenceParameters / Sampler    crates/llm-base/src/inference_session.rs, samplers.rs:97-211 (the default chain, run on the device)
+  get_snapshot / from_snapshot     crates/llm-base/src/inference_session.rs:591-646, InferenceSnapshot / SnapshotError :733-792; session files as
+                                   the CLI's --save-session / --load-session (binaries/llm-cli/src/snapshot.rs)
 """
 import ctypes as C
 import enum
@@ -36,6 +38,18 @@ class EndOfText(Exception):
 
 class SamplerFailure(Exception):
     """InferenceError::SamplerFailure: the last logits row holds a NaN.  n_past, tokens() and last_logits are as they were before the call."""
+
+
+class SnapshotError(Exception):
+    """SnapshotError, and a session file this library cannot read (B200_ERR_SNAPSHOT_FORMAT: see b200_snapshot in include/llm_b200.h)"""
+
+
+class MemorySizeMismatch(SnapshotError):
+    """SnapshotError::MemorySizeMismatch: the snapshot's memory_k (or, when that fits, memory_v) is not the size of this model's cache"""
+
+    def __init__(self, self_size: int, input_size: int):
+        super().__init__(f"memory size mismatch: session {self_size} bytes, snapshot {input_size} bytes")
+        self.self_size, self.input_size = self_size, input_size
 
 
 @dataclass
@@ -68,6 +82,7 @@ class InferenceRequest:
     prompt: Sequence[int] = ()                      # token ids (tokenization is the caller's)
     parameters: InferenceParameters = field(default_factory=InferenceParameters)
     maximum_token_count: Optional[int] = None       # None: until end of text (or ContextFull)
+    play_back_previous_tokens: bool = False         # infer first calls callback(id) for every id of tokens() (a restored session's history)
 
 
 @dataclass
@@ -113,6 +128,12 @@ def kv_array(raw: np.ndarray, kv_f32: bool) -> np.ndarray:
     return raw.view(np.float32) if kv_f32 else raw.view(np.uint16)
 
 
+# ModelKVMemoryType as the snapshot encodes it: bincode's enum variant index (Float16 = 0, Float32 = 1), neither enum ggml_type nor .value above
+KV_VARIANT = {ModelKVMemoryType.Float16: 0, ModelKVMemoryType.Float32: 1}
+KV_FROM_VARIANT = {v: k for k, v in KV_VARIANT.items()}
+SNAPSHOT_SIZE_MISMATCH, SNAPSHOT_FORMAT = -18, -19
+
+
 @dataclass
 class InferenceSessionConfig:
     n_batch: int = 8                  # inference_session.rs:837
@@ -154,6 +175,112 @@ def _check(rc, what):
         raise SamplerFailure(what)
     if rc != 0:
         raise RuntimeError(f"{what} failed with code {rc}")
+
+
+@dataclass
+class InferenceSnapshot:
+    """InferenceSnapshot: the session at npast, with memory_k / memory_v as the reference's bytes (include/llm_b200.h: b200_snapshot)"""
+    npast: int
+    config: InferenceSessionConfig                  # n_batch and the KV types
+    n_threads: int
+    tokens: np.ndarray                              # np.uint32, the ids at positions [0, npast)
+    last_logits: np.ndarray                         # np.float32, n_vocab
+    memory_k: np.ndarray                            # np.uint8
+    memory_v: np.ndarray
+
+
+def _snapshot_struct(snap: InferenceSnapshot):
+    """the b200_snapshot of `snap`, and the arrays it points into (to be kept alive for the call)"""
+    kt, vt = KV_VARIANT[snap.config.memory_k_type], KV_VARIANT[snap.config.memory_v_type]
+    arrs = [np.ascontiguousarray(snap.tokens, np.uint32), np.ascontiguousarray(snap.last_logits, np.float32),
+            np.ascontiguousarray(snap.memory_k, np.uint8).ravel(), np.ascontiguousarray(snap.memory_v, np.uint8).ravel()]
+    c = _lib.Snapshot(npast=snap.npast, memory_k_type=kt, memory_v_type=vt, n_batch=snap.config.n_batch, n_threads=snap.n_threads,
+                      n_tokens=arrs[0].size, tokens=arrs[0].ctypes.data, n_logits=arrs[1].size, last_logits=arrs[1].ctypes.data,
+                      memory_k_bytes=arrs[2].nbytes, memory_v_bytes=arrs[3].nbytes, memory_k=arrs[2].ctypes.data, memory_v=arrs[3].ctypes.data)
+    return c, arrs
+
+
+def _snapshot_refused(rc: int, what: str, self_bytes, k_bytes: int, v_bytes: int):
+    """the exception of a from_snapshot refusal: self_bytes(variant) is the model's cache size for a KV type"""
+    if rc == SNAPSHOT_SIZE_MISMATCH:
+        raise MemorySizeMismatch(self_bytes, k_bytes if k_bytes != self_bytes else v_bytes)
+    if rc == SNAPSHOT_FORMAT:
+        raise SnapshotError(f"{what}: not a session file this library reads (code {rc})")
+    _check(rc, what)
+    raise RuntimeError(f"{what} failed")
+
+
+def _snapshot_file_header(L, path: str) -> "_lib.Snapshot":
+    h = _lib.Snapshot()
+    rc = L.b200_snapshot_read_header(str(path).encode(), C.byref(h))
+    if rc != 0:
+        _snapshot_refused(rc, f"read_snapshot({path})", 0, 0, 0)
+    return h
+
+
+def _ref_cache_bytes(n_layer: int, context_size: int, n_embd: int, variant: int) -> int:
+    """the reference's memory_k / memory_v size: n_layer x context_size x n_embd values (also with grouped-query attention)"""
+    return n_layer * context_size * n_embd * (4 if variant == 1 else 2)
+
+
+class _Snapshots:
+    """get_snapshot / write_snapshot and the from_snapshot / read_snapshot constructors of a native session: `_GET_SNAP`, `_WRITE_SNAP`,
+    `_FROM_SNAP`, `_READ_SNAP` name the library's entry points; `_adopt(model, handle, config)` wraps a session handle, `_start_args(flags)` are
+    the extra arguments of the constructors, `_cache_bytes(model, variant)` the size a snapshot's memory must have."""
+    _GET_SNAP = _WRITE_SNAP = _FROM_SNAP = _READ_SNAP = ""
+
+    def get_snapshot(self) -> InferenceSnapshot:
+        """InferenceSession::get_snapshot: a copy of the session, the cache in the reference's layout (after the work queued so far)"""
+        get = getattr(self.L, self._GET_SNAP)
+        h = _lib.Snapshot()
+        _check(get(self._s, C.byref(h)), "get_snapshot")
+        tok, lg = np.empty(h.n_tokens, np.uint32), np.empty(h.n_logits, np.float32)
+        mk, mv = np.empty(h.memory_k_bytes, np.uint8), np.empty(h.memory_v_bytes, np.uint8)
+        h.tokens, h.last_logits, h.memory_k, h.memory_v = tok.ctypes.data, lg.ctypes.data, mk.ctypes.data, mv.ctypes.data
+        _check(get(self._s, C.byref(h)), "get_snapshot")
+        cfg = InferenceSessionConfig(n_batch=h.n_batch, memory_k_type=KV_FROM_VARIANT[h.memory_k_type], memory_v_type=KV_FROM_VARIANT[h.memory_v_type])
+        return InferenceSnapshot(npast=h.npast, config=cfg, n_threads=h.n_threads, tokens=tok, last_logits=lg, memory_k=mk, memory_v=mv)
+
+    def write_snapshot(self, path: str):
+        """the snapshot as the CLI's session file (bincode in a zstd frame of raw blocks), streamed from HBM"""
+        _check(getattr(self.L, self._WRITE_SNAP)(self._s, str(path).encode()), f"write_snapshot({path})")
+
+    @classmethod
+    def _restore(cls, model, entry, source, flags, sizes, config):
+        err = C.c_int(0)
+        h = entry(model._m, source, *cls._start_args(flags), C.byref(err))
+        if not h:
+            kt, kb, vb = sizes()
+            _snapshot_refused(err.value, "from_snapshot", cls._cache_bytes(model, kt), kb, vb)
+        return cls._adopt(model, h, config())
+
+    @classmethod
+    def _from(cls, snapshot: InferenceSnapshot, model, flags: int):
+        c, keep = _snapshot_struct(snapshot)
+        return cls._restore(model, getattr(model.L, cls._FROM_SNAP), C.byref(c), flags,
+                            lambda: (KV_VARIANT[snapshot.config.memory_k_type], keep[2].nbytes, keep[3].nbytes),
+                            lambda: InferenceSessionConfig(n_batch=snapshot.config.n_batch, flags=flags, memory_k_type=snapshot.config.memory_k_type,
+                                                           memory_v_type=snapshot.config.memory_v_type))
+
+    @classmethod
+    def _read(cls, path: str, model, flags: int):
+        hdr = {}
+
+        def header():
+            if not hdr:
+                hdr["h"] = _snapshot_file_header(model.L, path)
+            return hdr["h"]
+
+        def sizes():
+            h = header()
+            return h.memory_k_type, h.memory_k_bytes, h.memory_v_bytes
+
+        def config():
+            h = header()
+            kv = KV_FROM_VARIANT[h.memory_k_type]
+            return InferenceSessionConfig(n_batch=h.n_batch, flags=flags, memory_k_type=kv, memory_v_type=kv)
+
+        return cls._restore(model, getattr(model.L, cls._READ_SNAP), str(path).encode(), flags, sizes, config)
 
 
 def _perplexity(entry, handle, tokens, bos: int, context_size: int, callback, return_terms: bool):
@@ -239,6 +366,9 @@ class _Generation:
         reference returns it."""
         stats = InferenceStats()
         t0 = time.perf_counter()
+        if request.play_back_previous_tokens and callback is not None:
+            for tok in self.tokens():               # inference_session.rs:443-457: the feedback is ignored, as for SnapshotToken
+                callback(int(tok))
         if len(request.prompt):
             self.feed_prompt(request.prompt)
         stats.feed_prompt_duration = time.perf_counter() - t0
@@ -386,19 +516,45 @@ class Llama(_Native):
         return 2 if eot is None else eot
 
 
-class InferenceSession(_Generation, _Native):
+class InferenceSession(_Generation, _Snapshots, _Native):
     _HANDLE, _FREE = "_s", "b200_session_free"
     _INFER, _TOKENS, _LAST = "b200_session_infer_next_token", "b200_session_read_tokens", "b200_session_last_logits"
+    _GET_SNAP, _WRITE_SNAP = "b200_session_get_snapshot", "b200_session_write_snapshot"
+    _FROM_SNAP, _READ_SNAP = "b200_model_session_from_snapshot", "b200_model_session_read_snapshot"
 
-    def __init__(self, model: Llama, config: InferenceSessionConfig):
+    def __init__(self, model: Llama, config: InferenceSessionConfig, _handle=None):
         self.model, self.config, self.L = model, config, model.L
         self.kv_f32 = kv_flags(config.memory_k_type, config.memory_v_type) != 0
         cfg = _lib.SessionConfig(n_batch=config.n_batch, flags=config.flags | (SESSION_KV_F32 if self.kv_f32 else 0))
-        self._s = self.L.b200_model_start_session(model._m, C.byref(cfg))
+        self._s = _handle or self.L.b200_model_start_session(model._m, C.byref(cfg))
         if not self._s:
             raise RuntimeError("b200_model_start_session failed (all tensors loaded?)")
         self.n_vocab = int(model.hyperparameters["n_vocab"])
-        self._last_logits = np.zeros(self.n_vocab, np.float32)
+        self._last_logits = None if _handle else np.zeros(self.n_vocab, np.float32)
+
+    @classmethod
+    def from_snapshot(cls, snapshot: InferenceSnapshot, model: Llama, flags: int = 0) -> "InferenceSession":
+        """InferenceSession::from_snapshot: a session of `model` with the snapshot's n_batch and KV types, cache, history and last row.  flags may
+        add B200_SESSION_NO_GRAPH / UNFUSED / FAST.  Raises MemorySizeMismatch for another geometry, context size or KV type."""
+        return cls._from(snapshot, model, flags)
+
+    @classmethod
+    def read_snapshot(cls, path: str, model: Llama, flags: int = 0) -> "InferenceSession":
+        """from_snapshot of a session file (the CLI's --load-session), streamed into HBM; SnapshotError if the file cannot be read"""
+        return cls._read(path, model, flags)
+
+    @staticmethod
+    def _start_args(flags):
+        return (flags,)
+
+    @staticmethod
+    def _cache_bytes(model, variant):
+        hp = model.hyperparameters
+        return _ref_cache_bytes(hp["n_layer"], model.params.context_size, hp["n_embd"], variant)
+
+    @classmethod
+    def _adopt(cls, model, handle, config):
+        return cls(model, config, _handle=handle)
 
     @property
     def n_past(self) -> int:
