@@ -212,6 +212,17 @@ int  b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, fl
  * sampler, penalty off) */
 int  b200_session_top_k(b200_session *s, int32_t k, int32_t *ids_out, float *logits_out);
 int  b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out);
+/* Model::evaluate with OutputRequest::embeddings (crates/llm-base/src/model/mod.rs:257-266, model/common.rs:40-59): b200_session_evaluate, and when
+ * embeddings_out (HOST, nullable) is set, the n_embd f32 of row n - 1 of the final norm's output -- rms_norm, then * norm.weight (llama lib.rs:343-348),
+ * the tensor the lm_head reads -- bit-identical to the reference's CPU graph (B200_SESSION_FAST sessions: from their own order-free numbers).
+ * The request changes nothing else: logits, both caches, n_past, the history, last_logits and last_launches are the same with and without it.
+ * Every session form serves it (NO_GRAPH, UNFUSED, FAST, both KV types, F16 weights, LoRA-patched models); a tensor-parallel session returns
+ * B200_ERR_BAD_ARG when embeddings_out is set.  b200_session_evaluate is this with embeddings_out NULL. */
+int  b200_session_evaluate_output(b200_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits, float *embeddings_out);
+/* InferenceSession::feed_prompt with an OutputRequest (inference_session.rs:299-350): every chunk is evaluated with the request, so embeddings_out
+ * (nullable) receives the last row of the last chunk; an empty prompt (n = 0) leaves it untouched.  Refusals as b200_session_evaluate_output.
+ * b200_session_feed_prompt is this with embeddings_out NULL. */
+int  b200_session_feed_prompt_output(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out, float *embeddings_out);
 /* InferenceSession::infer_next_token (inference_session.rs:381-419): sample a token from the last evaluated row with the chain of b200_sampler
  * (history window: the session's tokens), append it to the history and evaluate it as a one-token step.  The id is returned as soon as the
  * sampler has run, while the step is still on the device; only the id crosses PCIe, and the next call queues behind the step.  End of text is
@@ -313,6 +324,10 @@ b200_neox_session *b200_neox_start_session(b200_neox_model *m, int32_t n_batch);
 /* flags: 0 (f16 KV cache) or B200_SESSION_KV_F32 (f32 cache, bit-exact with the reference's F32 memory_k / memory_v); NULL for any other flag */
 b200_neox_session *b200_neox_start_session_flags(b200_neox_model *m, int32_t n_batch, int32_t flags);
 int  b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits);
+/* b200_session_evaluate_output for every architecture of this runtime: embeddings_out (nullable) receives row n - 1 of the final LayerNorm's output,
+ * norm * gain + bias -- GPT-NeoX ln_f (gptneox lib.rs:333-337), GPT-2 ln_f (gpt2 :311-317), BLOOM output_norm (bloom :317-324), GPT-J ln_f
+ * (gptj :286-289) -- or norm * gain with no add node for MPT's norm_f (mpt :236-239, so a -0 stays -0).  b200_neox_evaluate is this with NULL. */
+int  b200_neox_evaluate_output(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits, float *embeddings_out);
 int  b200_neox_evaluate_device(b200_neox_session *s, int32_t n);       /* tokens of the last evaluate stay in HBM, logits stay in HBM */
 int32_t b200_neox_n_past(const b200_neox_session *s);
 int  b200_neox_set_n_past(b200_neox_session *s, int32_t n_past);

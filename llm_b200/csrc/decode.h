@@ -31,6 +31,7 @@ struct DecodeParams {
     const int32_t *token;
     int *n_past;                        // device copy of InferenceSession::n_past; the step's last kernel increments it
     float *x, *q, *kq, *ff, *logits;
+    float *normed;                      // single GPU: the final norm's f32 row [e], stored by every step (OutputRequest::embeddings); else null
     int4 *xpack_d, *xpack_f;            // activation records of wo's input (written by the attention kernel) and of w2's input (the w13 epilogue)
     // tensor-parallel decode (tp.cuh): dims above are THIS RANK's (n_head, n_head_kv, gqa = local heads / cache width; f = local n_ff / G;
     // n_vocab = local rows of the lm_head) except e = the full n_embd; e_loc = n_embd / G (q rows, rows of wo / w2 owned here)
@@ -64,6 +65,7 @@ struct NeoxParams {
     const uint16_t *lut_gelu, *lut_exp;
     const int32_t *token; int *n_past;
     float *x, *qkv, *q, *attn_out, *logits;     // residual stream [e], raw qkv [3e], roped q [e], attention branch output [e]
+    float *normed;                              // the final LayerNorm's f32 row [e], stored by every step (OutputRequest::embeddings)
     int4 *xpack_a, *xpack_d, *xpack_f;          // records: layer-norm output (K = e), attention rows (K = e), gelu output (K = 4e)
     // MPT / BLOOM (crates/models/{mpt,bloom}): the GPT-2 row layout (no wpe) plus ALiBi; MPT leaves every bias pointer null
     const float *alibi = nullptr;               // per-head ALiBi slopes [n_head] (alibi_slopes), else nullptr

@@ -76,10 +76,12 @@ __device__ __forceinline__ float kv_load(__half v) { return __half2float(v); }
 __device__ __forceinline__ float kv_load(float v) { return v; }
 
 // ---- 1 / 6: rms_norm * gain -> records.  grid = e/128 CTAs of 256 threads; every CTA reduces the whole row (16 KB from L2) and
-//      quantizes its own 4 blocks per warp pass. ------------------------------------------------------------------------------------
-template <bool TP>
+//      quantizes its own 4 blocks per warp pass.  STORE (the token's final norm only): each CTA also stores its own float4s of the f32 row to
+//      `normed` -- rms_norm, then the separately rounded * gain: the embeddings of OutputRequest (llama lib.rs:343-348). ----------------------
+template <bool TP, bool STORE = false>
 __device__ __forceinline__ void norm_pack_body(const float *__restrict__ x, const float *__restrict__ gain, int4 *__restrict__ pack,
-                                               int e, float eps, int q81, int off, int scale16, unsigned long long *prof, const TpSync &S) {
+                                               int e, float eps, int q81, int off, int scale16, unsigned long long *prof, const TpSync &S,
+                                               float *__restrict__ normed = nullptr) {
     const TpCtx &T = c_tp;
     __shared__ double shd[8];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -136,6 +138,7 @@ __device__ __forceinline__ void norm_pack_body(const float *__restrict__ x, cons
     float4 v;
     v.x = __fmul_rn(__fmul_rn(xv.x, scale), gv.x); v.y = __fmul_rn(__fmul_rn(xv.y, scale), gv.y);
     v.z = __fmul_rn(__fmul_rn(xv.z, scale), gv.z); v.w = __fmul_rn(__fmul_rn(xv.w, scale), gv.w);
+    if constexpr (STORE) if (active) ((float4 *)normed)[mine] = v;
     pack_quad(v, pack + (active ? mine >> 3 : 0) * 4, lane, active, q81, off, scale16);
     prof_end(prof);
 }
@@ -148,6 +151,12 @@ __global__ void __launch_bounds__(256) norm_pack_kernel(const float *__restrict_
 __global__ void __launch_bounds__(256) norm_pack_tp_kernel(const float *__restrict__ x, const float *__restrict__ gain, int4 *__restrict__ pack,
                                                            int e, float eps, int q81, int off, int scale16, unsigned long long *prof, const TpSync S) {
     norm_pack_body<true>(x, gain, pack, e, eps, q81, off, scale16, prof, S);
+}
+// the final norm of a single-GPU token: norm_pack_kernel's records, and the f32 row in `normed` (8 more bytes: the block is still one 64-byte line)
+__global__ void __launch_bounds__(256) norm_pack_store_kernel(const float *__restrict__ x, const float *__restrict__ gain, int4 *__restrict__ pack,
+                                                              int e, float eps, int q81, int off, int scale16, unsigned long long *prof,
+                                                              float *__restrict__ normed) {
+    norm_pack_body<false, true>(x, gain, pack, e, eps, q81, off, scale16, prof, TpSync{}, normed);
 }
 
 // ---- mat-vec with fused epilogues --------------------------------------------------------------------------------------------------
@@ -917,9 +926,11 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     };
     int n = 0;
     auto pr = [&]() -> unsigned long long * { return P.prof && n < B200_PROF_SLOTS ? P.prof + n : nullptr; };   // timeline slot of the next launch
-    auto launch_norm = [&](const float *x, const float *gain, const TpSync &S) {               // rms_norm * gain -> records of the next mat-vec
+    // rms_norm * gain -> records of the next mat-vec; with `normed` (the final norm of a single-GPU token) also the f32 row
+    auto launch_norm = [&](const float *x, const float *gain, const TpSync &S, float *normed = nullptr) {
         const dim3 grid((e / QK + 31) / 32), block(256);
         if constexpr (TP) launch_k(norm_pack_tp_kernel, grid, block, 0, st, x, gain, xpack_a, e, P.eps, q81, off, s16, pr(), S);
+        else if (normed) launch_k(norm_pack_store_kernel, grid, block, 0, st, x, gain, xpack_a, e, P.eps, q81, off, s16, pr(), normed);
         else { (void)S; launch_k(norm_pack_kernel, grid, block, 0, st, x, gain, xpack_a, e, P.eps, q81, off, s16, pr()); }
         n++;
     };
@@ -978,7 +989,7 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         D.ts = ts(TPB_XF, v, TPB_FF, v, TPB_X, v); D.row0 = tp ? P.row0_e : 0;
         D.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.w2, D, p_w2, st); n++;
     }
-    launch_norm(P.x, P.norm, ts(TPB_X, (unsigned)P.n_layer, -1, 0, -1, 0));
+    launch_norm(P.x, P.norm, ts(TPB_X, (unsigned)P.n_layer, -1, 0, -1, 0), P.normed);
     MmvArgs Z{}; Z.xpack = xpack_a; Z.dst = P.logits; Z.addend = nullptr; Z.n_past_inc = P.n_past;
     Z.ts = ts(-1, 0, -1, 0, TPB_LOGITS, 0); Z.row0 = tp ? P.row0_v : 0;
     Z.prof = pr(); launch_mmv<TYPE, EPI_LOGITS, TP>(P.output, Z, p_out, st); n++;
@@ -995,9 +1006,10 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
 // LayerNorm (ggml_compute_forward_norm_f32, LC/ggml.c:10063-10111) * gain + bias -> Q8 records.  Same shape as norm_pack_kernel: every CTA reduces
 // the whole row from registers (two passes: mean, then the variance of the centred values) and packs its own 32 blocks.
 // BIAS false (MPT): norm * gain only -- no add node, so a -0 stays -0.
-template <bool BIAS>
+// STORE (the token's final norm only): each CTA also stores its own float4s of the f32 row to `normed`, the embeddings of OutputRequest.
+template <bool BIAS, bool STORE = false>
 __device__ __forceinline__ void ln_pack_body(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
-                                             int e, int q81, int off, int scale16) {
+                                             int e, int q81, int off, int scale16, float *__restrict__ normed = nullptr) {
     __shared__ double shd[8];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     pdl_trigger();
@@ -1040,6 +1052,7 @@ __device__ __forceinline__ void ln_pack_body(const float *__restrict__ x, const 
         y.x = __fmul_rn(__fmul_rn(xv.x, scale), gv.x); y.y = __fmul_rn(__fmul_rn(xv.y, scale), gv.y);
         y.z = __fmul_rn(__fmul_rn(xv.z, scale), gv.z); y.w = __fmul_rn(__fmul_rn(xv.w, scale), gv.w);
     }
+    if constexpr (STORE) if (active) ((float4 *)normed)[mine] = y;
     pack_quad(y, pack + (active ? mine >> 3 : 0) * 4, lane, active, q81, off, scale16);
 }
 __global__ void __launch_bounds__(256) ln_pack_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
@@ -1049,6 +1062,15 @@ __global__ void __launch_bounds__(256) ln_pack_kernel(const float *__restrict__ 
 __global__ void __launch_bounds__(256) ln_pack_nobias_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
                                                              int e, int q81, int off, int scale16) {
     ln_pack_body<false>(x, gain, bias, pack, e, q81, off, scale16);
+}
+// the final LayerNorm of a token (gptneox lib.rs:333-337, gpt2 :311-317, mpt :236-239, bloom :317-324, gptj :286-289): the records, and the f32 row in `normed`
+__global__ void __launch_bounds__(256) ln_pack_store_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
+                                                            int e, int q81, int off, int scale16, float *__restrict__ normed) {
+    ln_pack_body<true, true>(x, gain, bias, pack, e, q81, off, scale16, normed);
+}
+__global__ void __launch_bounds__(256) ln_pack_nobias_store_kernel(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias,
+                                                                   int4 *__restrict__ pack, int e, int q81, int off, int scale16, float *__restrict__ normed) {
+    ln_pack_body<false, true>(x, gain, bias, pack, e, q81, off, scale16, normed);
 }
 
 // qkv [3e] (bias added) -> q [e], k -> f16 cache row n_past, v -> f16 cache column n_past.  GPT-NeoX (gptneox lib.rs:205-247): rows per head are q | k | v
@@ -1112,6 +1134,7 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
     // MPT has no biases: its norms take ln_pack_nobias_kernel and its up-projection the gelu epilogue without a bias node
     const bool biased = layers[0].ln1_b != nullptr, fc_bias = layers[0].bfc != nullptr;
     auto ln_kernel = biased ? ln_pack_kernel : ln_pack_nobias_kernel;
+    auto ln_final = biased ? ln_pack_store_kernel : ln_pack_nobias_store_kernel;     // + the f32 row (NeoxParams::normed)
     const CtaFootprint f_ln = footprint_of(ln_kernel, 256, 0);
     const CtaFootprint f_attn = attn_fused_footprint(false, P.hd, P.alibi != nullptr, P.kv_type, fa_smem);
     const CtaFootprint f_store = with_kv_type(P.kv_type, [](auto kt) { return footprint_of(neox_rope_store_kernel<decltype(kt)>, 256, 0); });
@@ -1145,7 +1168,7 @@ void neox_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         MmvArgs D{}; D.xpack = P.xpack_f; D.dst = P.x; D.bias = L.bproj; D.add1 = P.attn_out; D.add2 = P.parallel_residual ? P.x : nullptr;
         launch_mmv<TYPE, EPI_BIAS>(L.wproj, D, p_proj, st); n++;
     }
-    launch_k(ln_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16); n++;                          // :332-334
+    launch_k(ln_final, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16, P.normed); n++;                 // :332-334
     MmvArgs Z{}; Z.xpack = P.xpack_a; Z.dst = P.logits; Z.n_past_inc = P.n_past;
     launch_mmv<TYPE, EPI_BIAS>(P.lm_head, Z, p_head, st); n++;                                                                                        // :342
     B200_CHECK(cudaGetLastError());
@@ -1191,7 +1214,7 @@ void gptj_ops_t(const NeoxParams &P, const std::vector<NeoxLayer> &layers, int n
         MmvArgs D{}; D.xpack = P.xpack_f; D.dst = P.x; D.bias = L.bproj; D.add1 = P.attn_out; D.add2 = P.x;
         launch_mmv<TYPE, EPI_BIAS>(L.wproj, D, p_proj, st); n++;                                                                                       // :276-282
     }
-    launch_k(ln_pack_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16); n++;                          // :286-287
+    launch_k(ln_pack_store_kernel, ln_grid, dim3(256), 0, st, (const float *)P.x, P.lnf_g, P.lnf_b, P.xpack_a, e, q81, off, s16, P.normed); n++;         // :286-287
     MmvArgs Z{}; Z.xpack = P.xpack_a; Z.dst = P.logits; Z.bias = P.lm_head_b; Z.n_past_inc = P.n_past;
     launch_mmv<TYPE, EPI_BIAS>(P.lm_head, Z, p_head, st); n++;                                                                                        // :292-296
     B200_CHECK(cudaGetLastError());

@@ -269,6 +269,13 @@ void SessionCore::copy_logits(float *out, const float *logits, int n, bool all_r
     memcpy(out, h_logits.get(), rows * V * 4);
 }
 
+void SessionCore::copy_row(float *out, const float *row, int n) {
+    if (!out) return;
+    cudaStream_t st = rt().stream;
+    B200_CHECK(cudaMemcpyAsync(out, row, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+}
+
 int SessionCore::set_n_past(int v) {
     if (v < 0 || v > n_past) return B200_ERR_BAD_ARG;
     n_past = v;

@@ -167,6 +167,7 @@ struct SessionCore {
     int stage_tokens(const int32_t *tokens, int n);   // validates the ids and uploads them to d_tokens (and to the history at n_past)
     void record_tokens(int n);          // d_tokens[0, n) -> history at n_past (evaluate entry points whose ids are already in HBM)
     void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)
+    void copy_row(float *out, const float *row, int n);                        // n floats of a device row to out (if not null), after the queued work
     int set_n_past(int v);
     // InferenceSession::perplexity over tokens[0, n) with C = n_ctx: chunk i = [iC, (i+1)C) is evaluated from n_past 0 in batches of n_batch, its
     // first token replaced by bos; rows [min(512, C/2), C - 1) are scored on the device (ppl.cu).  forward(rows) runs one batch of the staged

@@ -426,6 +426,7 @@ b200_neox_session *b200_neox_start_session_flags(b200_neox_model *m, int32_t n_b
     P.kq_scale = m->kq_scale; P.rope_cs = m->rope ? m->rope->cs : nullptr; P.rope_half = m->rope ? m->rope->half : 0;
     P.lut_gelu = luts().gelu; P.lut_exp = luts().exp; P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
     P.x = s->x.get(); P.qkv = s->qkv.get(); P.q = s->qdec.get(); P.attn_out = s->attn.get(); P.logits = s->logits.get();
+    P.normed = s->cur.get();                                     // row 0 of cur: where forward()'s final LayerNorm leaves a one-token batch
     P.xpack_a = s->xpack_a.get(); P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
     B200_CHECK(cudaDeviceSynchronize());
     return s;
@@ -446,13 +447,19 @@ int b200_neox_evaluate_device(b200_neox_session *s, int32_t n) {
     return B200_OK;
 }
 
-int b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits) {
+// embeddings_out: row n - 1 of the final LayerNorm's output, which forward() leaves in cur (the graph step: its row 0)
+int b200_neox_evaluate_output(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits, float *embeddings_out) {
     if (!s || !tokens) return B200_ERR_BAD_ARG;
     if (const int rc = s->admit(n)) return rc;
     if (const int rc = s->stage_tokens(tokens, n)) return rc;
     forward(s, n, all_logits != 0);
     s->copy_logits(logits_out, s->logits.get(), n, all_logits != 0);
+    s->copy_row(embeddings_out, s->cur.get() + (size_t)(n - 1) * s->m->hp.n_embd, s->m->hp.n_embd);
     return B200_OK;
+}
+
+int b200_neox_evaluate(b200_neox_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits) {
+    return b200_neox_evaluate_output(s, tokens, n, logits_out, all_logits, nullptr);
 }
 
 int b200_neox_perplexity(b200_neox_session *s, const int32_t *tokens, int64_t n, int32_t bos, float *ppl_out, float *terms_out, int32_t *n_chunk_out) {

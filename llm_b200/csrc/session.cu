@@ -467,7 +467,7 @@ static b200_session *start_session_tp(b200_session *s) {
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
     P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = nullptr; P.ff = nullptr; P.logits = s->logits.get();
-    P.xpack_d = nullptr; P.xpack_f = nullptr;
+    P.xpack_d = nullptr; P.xpack_f = nullptr; P.normed = nullptr;        // embeddings are not offered on tensor-parallel sessions
     P.e_loc = m->e_loc; P.head0 = r * (hp.n_head / G); P.n_vocab_full = hp.n_vocab;
     P.row0_e = (int64_t)r * m->e_loc; P.row0_w13 = (int64_t)r * 2 * m->f_loc; P.row0_v = (int64_t)r * m->v_loc;
     P.prof = nullptr;
@@ -520,6 +520,7 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     P.lut_silu = luts().silu; P.lut_exp = luts().exp;
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
     P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = s->kq.get(); P.ff = s->ff.get(); P.logits = s->logits.get();
+    P.normed = s->cur.get();                                     // row 0 of cur: where forward()'s final rms_norm leaves a one-token batch
     s->xpack_d = device_alloc<int4>((e / QK) * 64);
     s->xpack_f = device_alloc<int4>((f / QK) * 64);
     P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
@@ -552,14 +553,15 @@ int b200_session_evaluate_device(b200_session *s, const int32_t *d_tokens, int32
 }
 const float *b200_session_device_logits(b200_session *s) { return s ? s->logits.get() : nullptr; }
 
-int b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits) {
-    if (!s || !tokens) return B200_ERR_BAD_ARG;
+// embeddings_out: row n - 1 of the final norm's output, which forward() leaves in cur (the graph step: its row 0)
+int b200_session_evaluate_output(b200_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits, float *embeddings_out) {
+    if (!s || !tokens || (embeddings_out && s->m->tp_world > 1)) return B200_ERR_BAD_ARG;
     if (const int rc = s->admit(n)) return rc;
     if (s->m->tp_world > 1 && n > 1) {                  // tensor-parallel sessions have the decode schedule only: a batch is fed token by token
         const size_t V = s->m->hp.n_vocab;
         for (int i = 0; i < n; i++) {
             float *out = !logits_out ? nullptr : all_logits ? logits_out + (size_t)i * V : (i == n - 1 ? logits_out : nullptr);
-            const int rc = b200_session_evaluate(s, tokens + i, 1, out, 0);
+            const int rc = b200_session_evaluate_output(s, tokens + i, 1, out, 0, nullptr);
             if (rc != B200_OK) return rc;
         }
         return B200_OK;
@@ -567,7 +569,12 @@ int b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, flo
     if (const int rc = s->stage_tokens(tokens, n)) return rc;
     forward(s, n, all_logits != 0);
     s->copy_logits(logits_out, s->logits.get(), n, all_logits != 0);
+    s->copy_row(embeddings_out, s->cur.get() + (size_t)(n - 1) * s->m->hp.n_embd, s->m->hp.n_embd);
     return B200_OK;
+}
+
+int b200_session_evaluate(b200_session *s, const int32_t *tokens, int32_t n, float *logits_out, int32_t all_logits) {
+    return b200_session_evaluate_output(s, tokens, n, logits_out, all_logits, nullptr);
 }
 
 // InferenceSession::perplexity (SessionCore::perplexity): tensor-parallel sessions are refused, FAST sessions run (their logits are not the reference's)
@@ -593,16 +600,21 @@ int b200_session_infer_next_token(b200_session *s, const b200_sampler *sampler, 
 int32_t b200_session_read_tokens(b200_session *s, int32_t *tokens_out, int32_t max) { return s ? s->read_tokens(tokens_out, max) : B200_ERR_BAD_ARG; }
 int b200_session_last_logits(b200_session *s, float *logits_out) { return s ? s->last_logits(s->logits.get(), logits_out) : B200_ERR_BAD_ARG; }
 
-int b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out) {
-    if (!s || !tokens || n < 0) return B200_ERR_BAD_ARG;
+// every chunk gets the same request in the reference (:317), so what it leaves behind is the last chunk's: only that one is copied out
+int b200_session_feed_prompt_output(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out, float *embeddings_out) {
+    if (!s || !tokens || n < 0 || (embeddings_out && s->m->tp_world > 1)) return B200_ERR_BAD_ARG;
     if (s->n_past + n > s->m->hp.context_size) return B200_ERR_CONTEXT_FULL;          // inference_session.rs:311-313
     for (int i = 0; i < n; i += s->cfg.n_batch) {                                     // :315-316 chunks(n_batch)
         const int c = (n - i) < s->cfg.n_batch ? (n - i) : s->cfg.n_batch;
         const bool last = i + c >= n;
-        const int rc = b200_session_evaluate(s, tokens + i, c, last ? last_logits_out : nullptr, 0);
+        const int rc = b200_session_evaluate_output(s, tokens + i, c, last ? last_logits_out : nullptr, 0, last ? embeddings_out : nullptr);
         if (rc != B200_OK) return rc;
     }
     return B200_OK;
+}
+
+int b200_session_feed_prompt(b200_session *s, const int32_t *tokens, int32_t n, float *last_logits_out) {
+    return b200_session_feed_prompt_output(s, tokens, n, last_logits_out, nullptr);
 }
 
 // n_layer x context_size x the cache width (tensor-parallel: this rank's heads) elements of the cache's type

@@ -12,8 +12,8 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .session import (ContextFull, InferenceSnapshot, LoraAdapters, ModelKVMemoryType, _check, _Generation, _Native, _perplexity, _ref_cache_bytes,
-                      _Snapshots, _vocab_id, ggml_dims, kv_array, kv_flags)
+from .session import (ContextFull, InferenceSnapshot, LoraAdapters, ModelKVMemoryType, OutputRequest, _check, _embeddings_buffer, _Generation, _Native,
+                      _perplexity, _ref_cache_bytes, _Snapshots, _vocab_id, ggml_dims, kv_array, kv_flags)
 
 
 class NeoxHparams(C.Structure):
@@ -39,6 +39,7 @@ def _bind(L):
     L.b200_neox_start_session_flags.restype = vp
     L.b200_neox_start_session_flags.argtypes = [vp, i32, i32]
     L.b200_neox_evaluate.argtypes = [vp, vp, i32, vp, i32]
+    L.b200_neox_evaluate_output.argtypes = [vp, vp, i32, vp, i32, vp]
     L.b200_neox_evaluate_device.argtypes = [vp, i32]
     L.b200_neox_n_past.argtypes = [vp]
     L.b200_neox_set_n_past.argtypes = [vp, i32]
@@ -218,23 +219,30 @@ class NeoxSession(_Generation, _Snapshots, _Native):
     def last_launches(self) -> int:
         return self.L.b200_neox_last_launches(self._s)
 
-    def evaluate(self, tokens, all_logits: bool = False) -> np.ndarray:
+    def evaluate(self, tokens, all_logits: bool = False, output_request: Optional[OutputRequest] = None) -> np.ndarray:
+        """Model::evaluate; output_request.embeddings, when not None, is replaced with the n_embd f32 of the last row of the final LayerNorm's output"""
         tokens = np.ascontiguousarray(tokens, np.int32)
         out = np.empty((tokens.size if all_logits else 1, self.n_vocab), np.float32)
-        _check(self.L.b200_neox_evaluate(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size, out.ctypes.data_as(C.c_void_p), 1 if all_logits else 0), "evaluate")
+        embd = _embeddings_buffer(output_request, self.model.hyperparameters["n_embd"])
+        _check(self.L.b200_neox_evaluate_output(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size, out.ctypes.data_as(C.c_void_p), 1 if all_logits else 0,
+                                                None if embd is None else embd.ctypes.data_as(C.c_void_p)), "evaluate")
+        if embd is not None:
+            output_request.embeddings = embd
         self._last_logits = out[-1].copy()
         return out if all_logits else out[0]
 
-    def feed_prompt(self, tokens) -> np.ndarray:
-        """InferenceSession::feed_prompt (inference_session.rs:299-350): the prompt in chunks of n_batch; returns last_logits.  ContextFull if
-        it does not fit (nothing is evaluated then); an empty prompt leaves last_logits untouched."""
+    def feed_prompt(self, tokens, output_request: Optional[OutputRequest] = None) -> np.ndarray:
+        """InferenceSession::feed_prompt (inference_session.rs:299-350): the prompt in chunks of n_batch, each evaluated with output_request (so its
+        embeddings are the last chunk's last row); returns last_logits.  ContextFull if it does not fit (nothing is evaluated then); an empty prompt
+        leaves last_logits and output_request untouched."""
         tokens = np.ascontiguousarray(tokens, np.int32).ravel()
         if tokens.size == 0:
             return self.last_logits
         if self.n_past + tokens.size > self.model.context_size:
             raise ContextFull("feed_prompt")
         for i in range(0, tokens.size, self.n_batch):
-            self.evaluate(tokens[i:i + self.n_batch])
+            last = i + self.n_batch >= tokens.size
+            self.evaluate(tokens[i:i + self.n_batch], output_request=output_request if last else None)
         return self.last_logits
 
     def perplexity(self, tokens, callback=None, bos: Optional[int] = None, return_terms: bool = False):

@@ -149,6 +149,14 @@ class InferenceSessionConfig:
 class OutputRequest:
     all_logits: Optional[np.ndarray] = None     # set to an empty array to request all rows (OutputRequest::all_logits)
     want_all_logits: bool = False
+    # OutputRequest::embeddings (model/common.rs:40-59): set to any array (an empty one will do) to request them; evaluate / feed_prompt replace it
+    # with the n_embd f32 of the last row of the final norm's output
+    embeddings: Optional[np.ndarray] = None
+
+
+def _embeddings_buffer(request: Optional[OutputRequest], n_embd: int) -> Optional[np.ndarray]:
+    """the host row an evaluate fills when `request` asks for embeddings, else None"""
+    return None if request is None or request.embeddings is None else np.empty(n_embd, np.float32)
 
 
 _HP_KEYS = ("n_vocab", "n_embd", "n_head", "n_head_kv", "n_layer", "n_rot", "n_ff")
@@ -566,24 +574,33 @@ class InferenceSession(_Generation, _Snapshots, _Native):
         _check(self.L.b200_session_top_k(self._s, k, ids.ctypes.data_as(C.c_void_p), vals.ctypes.data_as(C.c_void_p)), "top_k")
         return ids, vals
 
-    def evaluate(self, tokens, all_logits: bool = False) -> np.ndarray:
+    def evaluate(self, tokens, all_logits: bool = False, output_request: Optional[OutputRequest] = None) -> np.ndarray:
         """Model::evaluate: one forward pass over `tokens` (<= n_batch) appended at n_past; returns logits
-        ([n, n_vocab] when all_logits else the last row, which is also kept in self.last_logits)."""
+        ([n, n_vocab] when all_logits else the last row, which is also kept in self.last_logits).  output_request.embeddings, when not None,
+        is replaced with the n_embd f32 of the last row of the final norm's output (a tensor-parallel session refuses that request: RuntimeError)."""
         tokens = np.ascontiguousarray(tokens, np.int32)
         n = tokens.size
         out = np.empty((n if all_logits else 1, self.n_vocab), np.float32)
-        _check(self.L.b200_session_evaluate(self._s, tokens.ctypes.data_as(C.c_void_p), n, out.ctypes.data_as(C.c_void_p),
-                                            1 if all_logits else 0), "evaluate")
+        embd = _embeddings_buffer(output_request, self.model.hyperparameters["n_embd"])
+        _check(self.L.b200_session_evaluate_output(self._s, tokens.ctypes.data_as(C.c_void_p), n, out.ctypes.data_as(C.c_void_p),
+                                                   1 if all_logits else 0, None if embd is None else embd.ctypes.data_as(C.c_void_p)), "evaluate")
+        if embd is not None:
+            output_request.embeddings = embd
         self._last_logits = out[-1].copy()
         return out if all_logits else out[0]
 
-    def feed_prompt(self, tokens) -> np.ndarray:
+    def feed_prompt(self, tokens, output_request: Optional[OutputRequest] = None) -> np.ndarray:
+        """InferenceSession::feed_prompt: the prompt in chunks of n_batch, each evaluated with output_request (so its embeddings are the last
+        chunk's last row); returns last_logits."""
         tokens = np.ascontiguousarray(tokens, np.int32)
         if tokens.size == 0:                      # the reference leaves last_logits untouched for an empty prompt (inference_session.rs:299-350)
             return self.last_logits
         out = np.empty(self.n_vocab, np.float32)
-        _check(self.L.b200_session_feed_prompt(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size,
-                                               out.ctypes.data_as(C.c_void_p)), "feed_prompt")
+        embd = _embeddings_buffer(output_request, self.model.hyperparameters["n_embd"])
+        _check(self.L.b200_session_feed_prompt_output(self._s, tokens.ctypes.data_as(C.c_void_p), tokens.size, out.ctypes.data_as(C.c_void_p),
+                                                      None if embd is None else embd.ctypes.data_as(C.c_void_p)), "feed_prompt")
+        if embd is not None:
+            output_request.embeddings = embd
         self._last_logits = out
         return out
 
