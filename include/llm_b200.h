@@ -405,6 +405,9 @@ int  b200_op_quantize_blocks_device(int32_t target, int32_t src_type, const void
 /* the snapshot's transpose kernel on DEVICE buffers, enqueued on b200_stream() without a sync (for kernel timing): d_dst[c][r] = d_src[r][c] for
  * r < rows, c < cols, elements of elem_bytes (2 or 4) bytes, row strides src_ld / dst_ld elements; bit patterns are copied as they are */
 int  b200_op_transpose_device(int32_t elem_bytes, const void *d_src, int64_t src_ld, void *d_dst, int64_t dst_ld, int64_t rows, int64_t cols);
+/* the seam's row norms on DEVICE buffers, enqueued on b200_stream() without a sync (for kernel timing): op 1 = ggml_rms_norm (eps), op 2 = ggml_norm;
+ * rows rows of n f32 at d_x -> d_y */
+int  b200_op_norm_device(int32_t op, const float *d_x, float *d_y, int64_t n, int64_t rows, float eps);
 /* wtype: GGML_TYPE_F16 (1; K % 64 == 0, impl AUTO or EXACT = mul_mat_f16_exact), GGML_TYPE_Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 (2,3,6,7,8; K % 64 == 0), or the K-quants Q2_K..Q6_K (10..14; K % 256 == 0, impl AUTO or EXACT:
  * ggml_vec_dot_q{2,3,4,5,6}_K_q8_K of LC/k_quants.c:1240,1763,2492,3023,3592 on quantize_row_q8_K activations, bit-exact with the reference's AVX2 build) */
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);

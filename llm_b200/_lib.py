@@ -150,5 +150,6 @@ def lib():
     L.b200_model_session_read_snapshot.argtypes = [vp, C.c_char_p, i32, C.POINTER(C.c_int)]
     L.b200_snapshot_read_header.argtypes = [C.c_char_p, C.POINTER(Snapshot)]
     L.b200_op_transpose_device.argtypes = [i32, vp, i64, vp, i64, i64, i64]
+    L.b200_op_norm_device.argtypes = [i32, vp, vp, i64, i64, C.c_float]
     _lib = L
     return L

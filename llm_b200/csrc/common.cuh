@@ -85,6 +85,77 @@ __device__ __forceinline__ double warp_sum(double v) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
+// ---- the norms' row sums, bit for bit --------------------------------------------------------------------------------------------
+// ggml_compute_forward_norm_f32 / _rms_norm_f32 (LC/ggml.c:10063-10175) add a row's n terms in index order in a double (ggml_float) and keep
+// only the float (float)(sum / n).  The kernels add the same terms in a tree, T.  When every sum within a bound d of T gives the float T gives,
+// so does the reference's in-order sum Q: x -> (float)(x / n) is monotone.  row_sum_within checks that with both ends rounded outwards; it
+// fails for inf / NaN.  Otherwise the caller adds the row again in order (row_sum_in_order).
+__device__ __forceinline__ bool row_sum_within(double T, double d, int64_t n) {
+    const double nd = (double)n;
+    if (!(fabs(T) <= 0x1.fffffffffffffp+1023) || !(d <= 0x1.fffffffffffffp+1023)) return false;
+    return (float)(__dsub_rd(T, d) / nd) == (float)(__dadd_ru(T, d) / nd);
+}
+// Any order of adding the terms lies within gamma_{n-1} A of the exact sum (A = sum |term|, gamma_k = k u / (1 - k u), u = 2^-53), so
+// |Q - T| <= 2 gamma_{n-1} A.  Enough for sums of squares, where A = T.
+__device__ __forceinline__ bool row_sum_settled(double T, double A, int64_t n) {
+    return row_sum_within(T, __dmul_ru(__dmul_ru((double)n, 0x1.0001p-52), A), n);    // >= 2 gamma_{n-1} A, with room for A's own tree rounding
+}
+// A tighter bound for sums that cancel (norm's sum x over a row of mean ~0, where the one above fails for a few rows in a thousand): the in-order
+// sum's error is at most u / (1 - u) sum_k |Q_k| over its partial sums, |Q_k| <= |P_k| + 2 gamma_n A for prefix sums P_k computed in any
+// order (S = sum_k |P_k|, prefix_abs_sum), and T's own error is at most gamma_depth A, depth = the most additions on one path of its tree.
+__device__ __forceinline__ double row_sum_prefix_bound(double S, double A, int64_t n, int depth) {
+    const double nd = (double)n;
+    const double k = __dadd_ru((double)depth, __dmul_ru(__dmul_ru(4.0 * nd, nd), 0x1p-53));
+    return __dmul_ru(0x1.00001p-53, __dadd_ru(S, __dmul_ru(k, A)));
+}
+// sum_k |x_0 + ... + x_k| over the row, from a block scan of blockDim.x-element chunks (blockDim.x a multiple of 32, at most 1024).  Call from
+// all threads, on a block-uniform branch.  Out of line: it runs only where row_sum_settled fails.
+static __device__ __noinline__ double prefix_abs_sum(const float *x, int64_t n) {
+    __shared__ double wsum[32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    double carry = 0.0, acc = 0.0;
+    for (int64_t base = 0; base < n; base += blockDim.x) {
+        const int64_t i = base + threadIdx.x;
+        double v = i < n ? (double)__ldcg(x + i) : 0.0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const double t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+        __syncthreads();                                        // every thread has read wsum of the previous chunk
+        if (lane == 31) wsum[wid] = v;
+        __syncthreads();
+        double off = carry, tot = carry;
+        for (int w = 0; w < nw; w++) { if (w < wid) off += wsum[w]; tot += wsum[w]; }
+        if (i < n) acc += fabs(off + v);
+        carry = tot;
+    }
+    acc = warp_sum(acc);
+    __syncthreads();
+    if (lane == 0) wsum[wid] = acc;
+    __syncthreads();
+    double S = 0.0;
+    for (int w = 0; w < nw; w++) S += wsum[w];
+    __syncthreads();                                            // wsum is free again
+    return S;
+}
+// The reference's sum: term(0) + term(1) + ... + term(n-1), one after another in a double.  Out of line, so that the kernels' register
+// allocation is not sized by this rarely taken loop.
+template <typename Term>
+__device__ __noinline__ double add_in_order(int64_t n, Term term) {
+    double s = 0.0;
+#pragma unroll 8
+    for (int64_t i = 0; i < n; i++) s += term(i);
+    return s;
+}
+// add_in_order on thread 0, the result to every thread of the block.  Call from all threads, on a block-uniform branch.
+template <typename Term>
+__device__ __forceinline__ double row_sum_in_order(int64_t n, Term term) {
+    __shared__ double r;
+    if (threadIdx.x == 0) r = add_in_order(n, term);
+    __syncthreads();
+    const double v = r;
+    __syncthreads();                                            // r is free again for the next row sum
+    return v;
+}
+
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

@@ -132,7 +132,18 @@ __device__ __forceinline__ void norm_pack_body(const float *__restrict__ x, cons
     s = warp_sum(s);
     if (lane == 0) shd[warp] = s;
     __syncthreads();
-    const double tot = ((shd[0] + shd[1]) + (shd[2] + shd[3])) + ((shd[4] + shd[5]) + (shd[6] + shd[7]));
+    double tot = ((shd[0] + shd[1]) + (shd[2] + shd[3])) + ((shd[4] + shd[5]) + (shd[6] + shd[7]));
+    if (!row_sum_settled(tot, tot, e)) {                        // every CTA has the same tot, so every CTA takes this branch
+        tot = row_sum_in_order(e, [=](int64_t i) {
+            float v;
+            if constexpr (!TP) v = __ldcg(x + i);
+            else {                                              // units this CTA's first pass has seen tagged (before the barrier)
+                const uint4 u = tp_ld2(T, S.in_buf, i >> 1);
+                v = __uint_as_float(i & 1 ? u.z : u.x);
+            }
+            return (double)__fmul_rn(v, v);
+        });
+    }
     const float mean = (float)(tot / (double)e);
     const float scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, eps)));
     float4 v;
@@ -1010,7 +1021,7 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
 template <bool BIAS, bool STORE = false>
 __device__ __forceinline__ void ln_pack_body(const float *__restrict__ x, const float *__restrict__ gain, const float *__restrict__ bias, int4 *__restrict__ pack,
                                              int e, int q81, int off, int scale16, float *__restrict__ normed = nullptr) {
-    __shared__ double shd[8];
+    __shared__ double shd[16];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     pdl_trigger();
     pdl_wait();
@@ -1022,17 +1033,26 @@ __device__ __forceinline__ void ln_pack_body(const float *__restrict__ x, const 
     const bool active = mine < nv;
     const float4 gv = active ? __ldg((const float4 *)gain + mine) : make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 bv = BIAS && active ? __ldg((const float4 *)bias + mine) : make_float4(0.f, 0.f, 0.f, 0.f);
-    auto total = [&](double s) {
-        s = warp_sum(s);
-        __syncthreads();
-        if (lane == 0) shd[warp] = s;
-        __syncthreads();
-        return ((shd[0] + shd[1]) + (shd[2] + shd[3])) + ((shd[4] + shd[5]) + (shd[6] + shd[7]));
-    };
-    double s = 0.0;
+    auto tree = [&](int k) { return ((shd[k] + shd[k + 1]) + (shd[k + 2] + shd[k + 3])) + ((shd[k + 4] + shd[k + 5]) + (shd[k + 6] + shd[k + 7])); };
+    // the mean: sum x and, for row_sum_settled, sum |x|
+    double s = 0.0, a = 0.0;
 #pragma unroll
-    for (int k = 0; k < MAXV; k++) if (tid + k * 256 < nv) { s += (double)v[k].x; s += (double)v[k].y; s += (double)v[k].z; s += (double)v[k].w; }
-    const float mean = (float)(total(s) / (double)e);
+    for (int k = 0; k < MAXV; k++) if (tid + k * 256 < nv) {
+        s += (double)v[k].x; s += (double)v[k].y; s += (double)v[k].z; s += (double)v[k].w;
+        a += fabs((double)v[k].x); a += fabs((double)v[k].y); a += fabs((double)v[k].z); a += fabs((double)v[k].w);
+    }
+    s = warp_sum(s); a = warp_sum(a);
+    if (lane == 0) { shd[warp] = s; shd[8 + warp] = a; }
+    __syncthreads();
+    double sum = tree(0);
+    const double abs_sum = tree(8);                             // the same in every CTA, and so is each decision below
+    if (!row_sum_settled(sum, abs_sum, e)) {
+        if (!row_sum_within(sum, row_sum_prefix_bound(prefix_abs_sum(x, e), abs_sum, e, 4 * MAXV + 8), e))
+            sum = row_sum_in_order(e, [=](int64_t i) { return (double)__ldcg(x + i); });
+#pragma unroll                                                  // the row again: the calls above need not keep it in registers
+        for (int k = 0; k < MAXV; k++) { const int i = tid + k * 256; v[k] = i < nv ? __ldcg((const float4 *)x + i) : make_float4(0.f, 0.f, 0.f, 0.f); }
+    }
+    const float mean = (float)(sum / (double)e);
     double s2 = 0.0;
     float4 xv = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
@@ -1042,7 +1062,14 @@ __device__ __forceinline__ void ln_pack_body(const float *__restrict__ x, const 
         s2 += (double)__fmul_rn(c.x, c.x); s2 += (double)__fmul_rn(c.y, c.y); s2 += (double)__fmul_rn(c.z, c.z); s2 += (double)__fmul_rn(c.w, c.w);
         if (k == (int)blockIdx.x) xv = c;                       // float4 index tid + k * 256 == mine
     }
-    const float variance = (float)(total(s2) / (double)e);
+    s2 = warp_sum(s2);
+    __syncthreads();                                            // every thread has read shd
+    if (lane == 0) shd[warp] = s2;
+    __syncthreads();
+    double sum2 = tree(0);
+    if (!row_sum_settled(sum2, sum2, e))
+        sum2 = row_sum_in_order(e, [=](int64_t i) { const float c = __fsub_rn(__ldcg(x + i), mean); return (double)__fmul_rn(c, c); });
+    const float variance = (float)(sum2 / (double)e);
     const float scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(variance, 1e-5f)));
     float4 y;
     if (BIAS) {

@@ -49,6 +49,14 @@ int check_timeout(int32_t impl) {
 
 extern "C" {
 
+int b200_op_norm_device(int32_t op, const float *d_x, float *d_y, int64_t n, int64_t rows, float eps) {
+    if ((op != 1 && op != 2) || !d_x || !d_y || n <= 0 || rows < 0 || rows > INT32_MAX) return B200_ERR_BAD_ARG;
+    Runtime &R = rt(); R.ensure_init();
+    if (op == 1) rms_norm(d_x, d_y, nullptr, n, rows, eps, R.stream);
+    else layer_norm(d_x, d_y, nullptr, nullptr, n, rows, R.stream);
+    return B200_OK;
+}
+
 int b200_op_quantize_act(int32_t vdt, const float *x, int64_t K, int64_t B, int8_t *qs_out, float *d_out, float *aux_out) {
     if (!x || K % QK || (vdt != T_Q8_0 && vdt != T_Q8_1)) return B200_ERR_BAD_ARG;
     Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();

@@ -3,7 +3,9 @@
 //
 // All of them feed an activation quantizer further down the graph, and that quantizer is discontinuous, so every
 // kernel reproduces the reference's arithmetic operation for operation (SURVEY.md §7 "hard parts"):
-//   * row sums in double (ggml_float, LC/ggml.c:270) -- the only freedom taken is the order of the double additions;
+//   * row sums in double (ggml_float, LC/ggml.c:270), added in a tree.  The norms' sums are exact with respect to order: a tree sum whose float
+//     result the in-order one could differ from is added again in index order (row_sum_settled / row_sum_in_order, common.cuh).  Softmax's
+//     terms are fp16 table values in (0, 1], multiples of 2^-24, so every partial sum of up to 2^29 of them is exact in a double, in any order;
 //   * SiLU / GELU / exp through the 64 Ki-entry fp16 tables, built here on the HOST with the same libm formulas as
 //     ggml_init (LC/ggml.c:4313-4326) and uploaded once (3 x 128 KB, L2 resident);
 //   * RoPE angles from a host-built table that follows the reference's sequential f32 `theta *= theta_scale`
@@ -98,7 +100,8 @@ __global__ void rms_norm_kernel(const float *__restrict__ x, float *__restrict__
     float *yr = y + (int64_t)blockIdx.x * n;
     double s = 0.0;
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) { const float v = xr[i]; s += (double)__fmul_rn(v, v); }
-    const double sum = block_sum(s, shd);
+    double sum = block_sum(s, shd);
+    if (!row_sum_settled(sum, sum, n)) sum = row_sum_in_order(n, [=](int64_t i) { const float v = xr[i]; return (double)__fmul_rn(v, v); });
     const float mean = (float)(sum / (double)n);
     const float scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, eps)));
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
@@ -119,12 +122,20 @@ __global__ void layer_norm_kernel(const float *__restrict__ x, float *__restrict
     __shared__ double shd[32];
     const float *xr = x + (int64_t)blockIdx.x * n;
     float *yr = y + (int64_t)blockIdx.x * n;
-    double s = 0.0;
-    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) s += (double)xr[i];
-    const float mean = (float)(block_sum(s, shd) / (double)n);
+    double s = 0.0, a = 0.0;
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) { const double v = (double)xr[i]; s += v; a += fabs(v); }
+    double sum = block_sum(s, shd);
+    const double abs_sum = block_sum(a, shd);
+    const int depth = (int)((n + blockDim.x - 1) / blockDim.x) + 11;          // each thread's chain, then two warp_sum trees
+    if (!row_sum_settled(sum, abs_sum, n) && !row_sum_within(sum, row_sum_prefix_bound(prefix_abs_sum(xr, n), abs_sum, n, depth), n))
+        sum = row_sum_in_order(n, [=](int64_t i) { return (double)xr[i]; });
+    const float mean = (float)(sum / (double)n);
     double s2 = 0.0;
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) { const float v = __fsub_rn(xr[i], mean); s2 += (double)__fmul_rn(v, v); }
-    const float variance = (float)(block_sum(s2, shd) / (double)n);
+    double sum2 = block_sum(s2, shd);
+    if (!row_sum_settled(sum2, sum2, n))
+        sum2 = row_sum_in_order(n, [=](int64_t i) { const float v = __fsub_rn(xr[i], mean); return (double)__fmul_rn(v, v); });
+    const float variance = (float)(sum2 / (double)n);
     const float scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(variance, 1e-5f)));
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
         float v = __fmul_rn(__fsub_rn(xr[i], mean), scale);
