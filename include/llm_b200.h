@@ -411,6 +411,13 @@ int  b200_op_norm_device(int32_t op, const float *d_x, float *d_y, int64_t n, in
 /* wtype: GGML_TYPE_F16 (1; K % 64 == 0, impl AUTO or EXACT = mul_mat_f16_exact), GGML_TYPE_Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 (2,3,6,7,8; K % 64 == 0), or the K-quants Q2_K..Q6_K (10..14; K % 256 == 0, impl AUTO or EXACT:
  * ggml_vec_dot_q{2,3,4,5,6}_K_q8_K of LC/k_quants.c:1240,1763,2492,3023,3592 on quantize_row_q8_K activations, bit-exact with the reference's AVX2 build) */
 int  b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, const float *x, int64_t B, float *dst, int32_t impl);
+/* the attention mat-muls of the sessions (KQ on the K cache, KQV on the V cache) on host buffers: ggml_mul_mat(src0, src1) with src0 of
+ * src0_type GGML_TYPE_F16 (1: ggml_vec_dot_f16 on src1 rounded to fp16) or GGML_TYPE_F32 (0: ggml_vec_dot_f32), bit-exact with the reference's AVX2 build.
+ * dst[i2][i1][i0] = dot(src0[i2 / (ne12 / ne02)] row i0, src1[i2] row i1) over ne00 elements; every stride is in bytes (src0 rows nb01, matrices nb02;
+ * src1 f32 rows nb11, matrices nb12; dst f32 rows nbd1, matrices nbd2).  causal_past >= 0 skips i0 > causal_past + i1: those elements of dst keep
+ * the values the caller passed in.  ne12 % ne02 == 0, ne11 and ne12 at most 65535. */
+int  b200_op_mul_mat_kv(int32_t src0_type, const void *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12, float *dst, int64_t nbd1, int64_t nbd2, int32_t causal_past);
 /* quantize_row_q8_K (LC/k_quants.c:1133-1183) of B rows of K floats -> B * K/256 block_q8_K {f32 d; i8 qs[256]; i16 bsums[16]} (292 bytes each), bit-exact */
 int  b200_op_quantize_q8_K(const float *x, int64_t K, int64_t B, void *blocks_out);
 /* LoraAdapter::patch of one adapter on host buffers: w (N rows of K, F32 or Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 GGML blocks) += scaling * ba, ba[n][k] = dot(a row k,

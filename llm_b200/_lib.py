@@ -136,6 +136,7 @@ def lib():
     L.b200_op_quantize_weights.argtypes = [i32, vp, i64, i64, vp]
     L.b200_op_quantize_blocks_device.argtypes = [i32, i32, vp, i64, vp, vp]
     L.b200_op_mul_mat.argtypes = [i32, vp, i64, i64, vp, i64, vp, i32]
+    L.b200_op_mul_mat_kv.argtypes = [i32, vp, i64, i64, i64, i64, i64, vp, i64, i64, i64, i64, vp, i64, i64, i32]
     L.b200_op_quantize_q8_K.argtypes = [vp, i64, i64, vp]
     L.b200_op_lora_patch.argtypes = [i32, vp, i64, i64, i32, vp, vp, i64, C.c_float]
     L.b200_model_load_tensor_lora.argtypes = [vp, C.c_char_p, i32, i32, i64, i64, vp, sz, C.POINTER(vp), i32]

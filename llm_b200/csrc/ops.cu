@@ -164,6 +164,32 @@ int b200_op_mul_mat(int32_t wtype, const void *w_ggml, int64_t K, int64_t N, con
     return B200_OK;
 }
 
+// the sessions' KQ / KQV (exact.cu: mul_mat_f16_exact / mul_mat_f32_exact) on host buffers with ggml_mul_mat's shapes and byte strides.  dst is
+// uploaded too, so the outputs the causal skip leaves alone come back as the caller's values.
+int b200_op_mul_mat_kv(int32_t src0_type, const void *src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
+                       const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12, float *dst, int64_t nbd1, int64_t nbd2, int32_t causal_past) {
+    const int64_t es = src0_type == T_F16 ? 2 : 4;
+    if ((src0_type != T_F16 && src0_type != T_F32) || !src0 || !src1 || !dst || ne00 < 1 || ne01 < 1 || ne02 < 1 || ne11 < 1 || ne12 < 1 ||
+        ne12 % ne02 || ne11 > 65535 || ne12 > 65535 || nb01 < ne00 * es || nb02 < 0 || nb11 < ne00 * 4 || nb12 < 0 || nbd1 < ne01 * 4 || nbd2 < 0 ||
+        nb01 % es || nb02 % es || nb11 % 4 || nb12 % 4 || nbd1 % 4 || nbd2 % 4)
+        return B200_ERR_BAD_ARG;
+    const size_t b0 = (size_t)((ne02 - 1) * nb02 + (ne01 - 1) * nb01 + ne00 * es);          // one past the last byte each operand touches
+    const size_t b1 = (size_t)((ne12 - 1) * nb12 + (ne11 - 1) * nb11 + ne00 * 4);
+    const size_t bd = (size_t)((ne12 - 1) * nbd2 + (ne11 - 1) * nbd1 + ne01 * 4);
+    Runtime &R = rt(); R.ensure_init(); R.op_arena.reset();
+    cudaStream_t st = R.stream;
+    void *d0 = R.op_arena.get(b0, st);
+    float *d1 = (float *)R.op_arena.get(b1, st), *dd = (float *)R.op_arena.get(bd, st);
+    B200_CHECK(cudaMemcpyAsync(d0, src0, b0, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(d1, src1, b1, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(dd, dst, bd, cudaMemcpyHostToDevice, st));
+    if (src0_type == T_F16) mul_mat_f16_exact((const __half *)d0, ne00, ne01, ne02, nb01, nb02, d1, ne11, ne12, nb11, nb12, dd, nbd1, nbd2, causal_past, st);
+    else mul_mat_f32_exact((const float *)d0, ne00, ne01, ne02, nb01, nb02, d1, ne11, ne12, nb11, nb12, dd, nbd1, nbd2, causal_past, st);
+    B200_CHECK(cudaMemcpyAsync(dst, dd, bd, cudaMemcpyDeviceToHost, st));
+    B200_CHECK(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
 // ggml_quantize_q{4_0,4_1,5_0,5_1,8_0} on the GPU (crates/llm-base/src/quantize.rs:320-414 calls them per tensor): f32 rows in, GGML blocks out,
 // through the kernel of b200_quantize_file
 int b200_op_quantize_weights(int32_t wtype, const float *w_host, int64_t K, int64_t N, void *ggml_blocks_out) {
