@@ -36,7 +36,8 @@ typedef struct b200_session b200_session;
 
 typedef struct {
     int32_t n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff;
-    int32_t wtype;            /* enum ggml_type of the 2-D weights: 1 F16, 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0 */
+    int32_t wtype;            /* enum ggml_type of the 2-D weights: 1 F16, 2 Q4_0, 3 Q4_1, 6 Q5_0, 7 Q5_1, 8 Q8_0, 10..14 Q2_K..Q6_K
+                                 (b200_llama_new_typed: of the weights its table does not name) */
     int32_t context_size;     /* ModelParameters::context_size (default 2048) */
     float   rope_freq_base;   /* RoPEOverrides::frequency_base (10000) */
     float   rope_freq_scale;  /* RoPEOverrides::frequency_scale (1) */
@@ -107,6 +108,20 @@ int  b200_init(int device);                                   /* accelerator::in
 int  b200_device_info(int32_t *sm_count, size_t *free_bytes, size_t *total_bytes);
 
 b200_model *b200_llama_new(const b200_llama_hparams *hp);
+/* Per-tensor weight types (mixed-type files: the quantizer writes output.weight as Q6_K whenever both its dimensions are multiples of 256, and the
+ * K_M mixes give wv / w2 / wo other types than the rest).  Each entry names one 2-D weight -- tok_embeddings.weight, output.weight,
+ * layers.<i>.attention.w{q,k,v,o}.weight, layers.<i>.feed_forward.w{1,2,3}.weight -- and gives its enum ggml_type: F16, Q4_0..Q8_0 or Q2_K..Q6_K;
+ * weights the table does not name are of hp->wtype.  Refused with NULL and *err (nullable), before anything is allocated:
+ *   B200_ERR_UNKNOWN_TENSOR            a name that is not a 2-D weight of this model
+ *   B200_ERR_UNSUPPORTED_ELEMENT_TYPE  any other type (F32 2-D weights included), wk / w3 of another type than wq / w1 of the same layer, or F16
+ *                                      weights beside weights of other types (an F16 model is F16 throughout)
+ *   B200_ERR_INVARIANT_BROKEN          a K-quant tensor whose rows are not whole 256-element super-blocks (ne0 % 256 != 0)
+ *   B200_ERR_BAD_ARG                   hyperparameters b200_llama_new refuses
+ * K-quant matrices keep the file's super-blocks and run kquants.cu's kernels (bit-exact with ggml_vec_dot_q*_K_q8_K).  A model whose layer matrices
+ * are all of one classic type decodes through the decode graph, with a K-quant lm_head as two more launches in place of its mat-vec; layers with
+ * a K-quant or a wv of its own type decode per op.  K-quants are refused on tensor-parallel shards (b200_llama_new_tp). */
+typedef struct { const char *name; int32_t type; } b200_tensor_type;
+b200_model *b200_llama_new_typed(const b200_llama_hparams *hp, const b200_tensor_type *types, int32_t n, int *err);
 /* Tensor-parallel shard tp_rank of tp_world (one process per GPU, <= 8; the north star's "weight rows shard across the 8 GPUs"): every 2-D weight but
  * tok_embeddings holds only this rank's OUTPUT ROWS -- wq/wk/wv: its heads, w1/w3: rows [rank*n_ff/G, +n_ff/G), wo/w2: rows [rank*n_embd/G, +n_embd/G),
  * output: rows [rank*n_vocab/G, +n_vocab/G) -- and b200_model_load_tensor takes exactly those rows.  Contrast: LC/ggml-cuda.cu:3355-3583 (row split by
@@ -159,8 +174,9 @@ int     b200_ggml_write(const char *path, const int32_t *hparam_words, int32_t n
                         const float *token_score, const b200_ggml_tensor_info *tensors, const void *const *data, int64_t n_tensors);
 int     b200_ggml_write_llama(const char *path, const b200_llama_hparams *hp, int32_t n_mult, int32_t file_type, const uint8_t *const *token_bytes, const uint32_t *token_len,
                               const float *token_score, const b200_ggml_tensor_info *tensors, const void *const *data, int64_t n_tensors);
-/* llm::load::<Llama>(path, ModelParameters): parse + b200_llama_new + one b200_model_load_tensor per tensor, straight from the mapping;
- * context_size / rope_* <= 0 keep the defaults (2048, 10000, 1) */
+/* llm::load::<Llama>(path, ModelParameters): parse + b200_llama_new_typed with every 2-D tensor's type from the file + one b200_model_load_tensor per
+ * tensor, straight from the mapping; context_size / rope_* <= 0 keep the defaults (2048, 10000, 1).  Its refusals come before anything is uploaded;
+ * B200_ERR_UNSUPPORTED_ELEMENT_TYPE also for a LoRA adapter (the _lora form) that targets a K-quant tensor. */
 b200_model *b200_llama_load_file(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int *err);
 /* same with ModelParameters::n_gqa (grouped-query attention: n_head_kv = n_head / n_gqa, e.g. 8 for 70B files) */
 b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa, int *err);

@@ -19,6 +19,11 @@ class LlamaHparams(C.Structure):
                 ("context_size", C.c_int32), ("rope_freq_base", C.c_float), ("rope_freq_scale", C.c_float)]
 
 
+class TensorType(C.Structure):
+    """b200_tensor_type: one 2-D weight's enum ggml_type (b200_llama_new_typed)"""
+    _fields_ = [("name", C.c_char_p), ("type", C.c_int32)]
+
+
 class GgmlTensorInfo(C.Structure):
     """b200_ggml_tensor_info <- TensorLoadInfo, crates/ggml/src/format/loader.rs:72-86."""
     _fields_ = [("name", C.c_char * 96), ("type", C.c_int32), ("n_dims", C.c_int32), ("ne", C.c_int64 * 2), ("offset", C.c_uint64), ("nbytes", C.c_uint64)]
@@ -65,6 +70,8 @@ def lib():
     L.b200_stream.restype = vp
     L.b200_llama_new.restype = vp
     L.b200_llama_new.argtypes = [C.POINTER(LlamaHparams)]
+    L.b200_llama_new_typed.restype = vp
+    L.b200_llama_new_typed.argtypes = [C.POINTER(LlamaHparams), C.POINTER(TensorType), i32, C.POINTER(C.c_int)]
     L.b200_llama_new_tp.restype = vp
     L.b200_llama_new_tp.argtypes = [C.POINTER(LlamaHparams), i32, i32]
     L.b200_session_tp_handle.argtypes = [vp, vp]

@@ -33,6 +33,7 @@ struct DecodeParams {
     float *x, *q, *kq, *ff, *logits;
     float *normed;                      // single GPU: the final norm's f32 row [e], stored by every step (OutputRequest::embeddings); else null
     int4 *xpack_d, *xpack_f;            // activation records of wo's input (written by the attention kernel) and of w2's input (the w13 epilogue)
+    void *xq8k = nullptr;               // single GPU, K-quant lm_head: the Q8_K super-blocks of the final norm's row (q8k_bytes(e, 1))
     // tensor-parallel decode (tp.cuh): dims above are THIS RANK's (n_head, n_head_kv, gqa = local heads / cache width; f = local n_ff / G;
     // n_vocab = local rows of the lm_head) except e = the full n_embd; e_loc = n_embd / G (q rows, rows of wo / w2 owned here)
     TpCtx tp;

@@ -969,7 +969,8 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
     const MmvPlan &p_w2 = mmv_plan<TYPE, EPI_RES, TP>(layers[0].w2, f_norm + p_qkv.cta);
     const MmvPlan &p_w13 = mmv_plan<TYPE, EPI_SILU, TP>(layers[0].w13, p_w2.cta);
     const MmvPlan &p_wo = mmv_plan<TYPE, EPI_RES, TP>(layers[0].wo, f_norm + p_w13.cta);
-    const MmvPlan &p_out = mmv_plan<TYPE, EPI_LOGITS, TP>(P.output, CtaFootprint{});
+    const bool kq_out = !TP && is_kquant(P.output.type);       // a K-quant lm_head (per-tensor types): not a mat-vec of this schedule's TYPE
+    const MmvPlan *p_out = kq_out ? nullptr : &mmv_plan<TYPE, EPI_LOGITS, TP>(P.output, CtaFootprint{});
     for (int il = 0; il < P.n_layer; il++) {
         const DecodeLayer &L = layers[il];
         const unsigned v = (unsigned)il + 1;                     // flag value of this layer's exchanges (tp.cuh)
@@ -1001,9 +1002,15 @@ void decode_ops_t(const DecodeParams &P, const std::vector<DecodeLayer> &layers,
         D.prof = pr(); launch_mmv<TYPE, EPI_RES, TP>(L.w2, D, p_w2, st); n++;
     }
     launch_norm(P.x, P.norm, ts(TPB_X, (unsigned)P.n_layer, -1, 0, -1, 0), P.normed);
-    MmvArgs Z{}; Z.xpack = xpack_a; Z.dst = P.logits; Z.addend = nullptr; Z.n_past_inc = P.n_past;
-    Z.ts = ts(-1, 0, -1, 0, TPB_LOGITS, 0); Z.row0 = tp ? P.row0_v : 0;
-    Z.prof = pr(); launch_mmv<TYPE, EPI_LOGITS, TP>(P.output, Z, p_out, st); n++;
+    if (kq_out) {
+        // ggml_mul_mat(output, cur) on the f32 row the final norm stored: quantize_row_q8_K, then the K-quant mat-vec, whose launch also advances n_past
+        quantize_act_q8k(P.normed, P.e, P.xq8k, P.e, 1, st); n++;
+        mul_mat_kq_exact(P.output.type, P.output.qs, P.xq8k, P.logits, P.n_vocab, P.e, P.n_vocab, 1, nullptr, 0, st, P.n_past); n++;
+    } else {
+        MmvArgs Z{}; Z.xpack = xpack_a; Z.dst = P.logits; Z.addend = nullptr; Z.n_past_inc = P.n_past;
+        Z.ts = ts(-1, 0, -1, 0, TPB_LOGITS, 0); Z.row0 = tp ? P.row0_v : 0;
+        Z.prof = pr(); launch_mmv<TYPE, EPI_LOGITS, TP>(P.output, Z, *p_out, st); n++;
+    }
     if (tp) {                                                    // gathered logits -> the plain array the host reads; then the epoch moves on
         launch_k(tp_collect_kernel, dim3((P.n_vocab_full + 255) / 256), dim3(256), 0, st, P.logits, P.n_vocab_full); n++;
         launch_k(tp_bump_kernel, dim3(1), dim3(32), 0, st); n++;

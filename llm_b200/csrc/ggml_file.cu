@@ -260,7 +260,7 @@ int b200_ggml_llama_hparams(const b200_ggml_file *f, b200_llama_hparams *out, in
     bool any_quant = false;
     out->wtype = -1;                                                             // "not found" (F32 = 0 is a valid element type)
     for (const TensorInfo &t : f->tensors) {
-        any_quant |= b200::is_quant(t.type);
+        any_quant |= b200::is_quant(t.type) || b200::is_kquant(t.type);
         if (t.name == "layers.0.feed_forward.w1.weight") out->n_ff = (int32_t)t.ne[1];
         if (t.name == "layers.0.attention.wq.weight") out->wtype = t.type;
     }
@@ -312,24 +312,26 @@ static b200_model *load_file_impl(const char *path, int32_t context_size, float 
     b200_llama_hparams hp;
     *err = b200_ggml_llama_hparams(f, &hp, nullptr, nullptr, nullptr);
     if (*err != B200_OK) { b200_ggml_close(f); return nullptr; }
-    if (!b200::is_qweight_type(hp.wtype)) {     // F32 / K-quant files parse, but this backend streams F16 and the five 32-element block formats only
-        fprintf(stderr, "llm_b200: %s: layers.0.attention.wq.weight is %s; this backend loads F16/Q4_0/Q4_1/Q5_0/Q5_1/Q8_0 weights\n", path, type_name(hp.wtype));
-        *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; b200_ggml_close(f); return nullptr;
-    }
     if (context_size > 0) hp.context_size = context_size;
     if (rope_freq_base > 0.f) hp.rope_freq_base = rope_freq_base;
     if (rope_freq_scale > 0.f) hp.rope_freq_scale = rope_freq_scale;
     if (n_gqa > 1) { if (hp.n_head % n_gqa) { *err = B200_ERR_BAD_ARG; b200_ggml_close(f); return nullptr; } hp.n_head_kv = hp.n_head / n_gqa; }
-    b200_model *m = b200_llama_new(&hp);
-    if (!m) { *err = B200_ERR_BAD_ARG; b200_ggml_close(f); return nullptr; }
+    // every 2-D tensor's own type (the model checks them: b200_llama_new_typed); a LoRA patch of a K-quant tensor is refused before any upload
+    std::vector<b200_tensor_type> types;
+    for (const TensorInfo &t : f->tensors) {
+        if (t.n_dims != 2 || !b200::llama_matrix_name(t.name.c_str(), hp.n_layer)) continue;   // the loop below reports any other tensor
+        types.push_back(b200_tensor_type{t.name.c_str(), t.type});
+        if (b200::is_kquant(t.type))
+            for (int32_t a = 0; a < n_adapters; a++)
+                if (adapters[a] && b200::lora_in_patch_set(adapters[a], t.name.c_str())) {
+                    fprintf(stderr, "llm_b200: %s: a LoRA adapter patches %s, a %s tensor: adapters apply to F16 and Q4_0..Q8_0 weights\n", path, t.name.c_str(), type_name(t.type));
+                    *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; b200_ggml_close(f); return nullptr;
+                }
+    }
+    b200_model *m = b200_llama_new_typed(&hp, types.data(), (int32_t)types.size(), err);
+    if (!m) { b200_ggml_close(f); return nullptr; }
     for (size_t i = 0; i < f->tensors.size(); i++) {
         const TensorInfo &t = f->tensors[i];
-        const bool is_norm = t.n_dims == 1;
-        if (!is_norm && t.type != hp.wtype) {     // one weight type per model (QWeight planes are per matrix, the decode graph is instantiated per type)
-            fprintf(stderr, "llm_b200: %s: tensor %s is %s, the model's weight type is %s: mixed-type files are not supported by this backend\n", path, t.name.c_str(),
-                    type_name(t.type), type_name(hp.wtype));
-            *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; b200_model_free(m); b200_ggml_close(f); return nullptr;
-        }
         const int rc = b200_model_load_tensor_lora(m, t.name.c_str(), t.type, t.n_dims, t.ne[0], t.ne[1], f->map + t.offset, (size_t)t.nbytes, adapters, n_adapters);
         if (rc != B200_OK) { *err = rc; b200_model_free(m); b200_ggml_close(f); return nullptr; }
     }

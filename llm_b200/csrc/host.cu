@@ -43,7 +43,7 @@ static int lora_apply(const LoraTarget &t, int wtype, int64_t K, int64_t N, void
 QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows) {
     QWeight v = w;
     v.N = nrows;
-    v.qs = w.qs + (size_t)row0 * w.nb * (w.type == T_F16 ? 64 : qs_bytes(w.type));
+    v.qs = w.qs + (size_t)row0 * w.nb * (w.type == T_F16 || is_kquant(w.type) ? qweight_block_bytes(w.type) : qs_bytes(w.type));
     if (w.qh) v.qh = w.qh + (size_t)row0 * w.nb;
     if (w.dm) v.dm = (const uint8_t *)w.dm + (size_t)row0 * w.nb * (has_min(w.type) ? 4 : 2);
     v.base = nullptr;

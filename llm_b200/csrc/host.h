@@ -32,13 +32,14 @@ QWeight row_view(const QWeight &w, int64_t row0, int64_t nrows);   // rows [row0
 
 // ---- the weights of one model -------------------------------------------------------------------------------------------------
 // One pass over a model's tensors in slab order: the sizing pass (base == nullptr) only advances `off`, the placing pass also points each tensor
-// into the slab. Quantized matrices take qweight_layout's bytes, f32 vectors are padded to 256 bytes.
+// into the slab. Quantized matrices take qweight_layout's bytes, f32 vectors are padded to 256 bytes.  A matrix is of `wtype` unless the layout
+// passes its own type (a per-tensor type of the model file).
 struct SlabCarver {
     int wtype; char *base;
     size_t off = 0, streamed = 0;       // streamed: GGML bytes of every matrix carved
-    void q(QWeight &w, int64_t K, int64_t N) {
-        off += qweight_layout(w, wtype, K, N, base ? base + off : nullptr);
-        streamed += (size_t)N * (K / QK) * qweight_block_bytes(wtype);
+    void q(QWeight &w, int64_t K, int64_t N, int type = -1) {
+        off += qweight_layout(w, type < 0 ? wtype : type, K, N, base ? base + off : nullptr);
+        streamed += (size_t)N * w.nb * qweight_block_bytes(w.type);
     }
     void f(float *&p, int64_t n) { if (base) p = (float *)(base + off); off += ((size_t)n * 4 + 255) & ~(size_t)255; }
 };
@@ -97,6 +98,9 @@ struct LoraTarget { const char *name; int64_t ne0, ne1; const b200_ggml_file *co
 // names the tensor patches its bytes in file layout after the upload and before they are placed (lora.cu).
 int load_slot(const Slot &s, int32_t type, const void *host, size_t nbytes, const LoraTarget *lora = nullptr);
 int read_slot(const Slot &s, void *host, size_t nbytes);                       // the inverse: GGML blocks or f32 back to the host
+
+// a 2-D weight of a LLaMA model of n_layer layers: tok_embeddings / output / layers.<i>.attention.w[qkvo] / layers.<i>.feed_forward.w[123] (session.cu)
+bool llama_matrix_name(const char *name, int n_layer);
 
 // ---- adapter files (ggml_file.cu) ----
 int64_t ggml_find_tensor(const b200_ggml_file *f, const char *name);        // index in the tensor table, -1 if absent

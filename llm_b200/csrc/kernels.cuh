@@ -70,18 +70,22 @@ void f16_to_f32(const void *src, float *dst, int64_t n, cudaStream_t st);       
 // ---- mul_mat.cu : the bit-exact ggml_mul_mat of every front end -------------------------------------------------------------------------
 bool prefill_gemm_tc5();         // B200_PREFILL_GEMM != "mma" (the default)
 // activation buffers for B rows of K: xq [B][K] int8, xds [B][K/32], xpack (K/32) * 64 bytes, xh xh_bytes(K, B)
-struct ExactActs { int8_t *xq; float2 *xds; int4 *xpack; __half *xh; };
+// xq8k: q8k_bytes(K, B) of Q8_K super-blocks, needed for K-quant weights only
+struct ExactActs { int8_t *xq; float2 *xds; int4 *xpack; __half *xh; void *xq8k = nullptr; };
 // dst[b*ldd + n] (+ addend[b*lda + n]) for B rows of x (row stride ldx): quantizes x and runs the exact kernel for B -- the streaming mat-vec
 // (B == 1), the wgmma GEMM (B >= 96, prefill_gemm_tc5()), the mma.sync GEMM (B >= 16) or exact.cu.  An F16 weight rounds x to fp16 and runs
-// exact_f16.cu's mat-vec (B == 1) or GEMM.  Returns the number of launches (2).
+// exact_f16.cu's mat-vec (B == 1) or GEMM.  A K-quant weight quantizes x to Q8_K and runs kquants.cu.  Returns the number of launches (2).
 int mul_mat_exact_auto(const QWeight &w, const float *x, int64_t ldx, int64_t B, float *dst, int64_t ldd, const float *addend, int64_t lda,
                        const ExactActs &a, cudaStream_t st);
 
-// ---- kquants.cu : Q4_K / Q5_K / Q6_K weights x Q8_K activations, bit-exact with ggml_vec_dot_q*_K_q8_K (AVX2 build) -------------------------
+// ---- kquants.cu : Q2_K .. Q6_K weights x Q8_K activations, bit-exact with ggml_vec_dot_q*_K_q8_K (AVX2 build) -------------------------
 size_t q8k_bytes(int64_t K, int64_t B);
 void quantize_act_q8k(const float *x, int64_t ldx, void *y, int64_t K, int64_t B, cudaStream_t st);       // quantize_row_q8_K of every src1 row -> block_q8_K
+// w_raw: N rows of K/256 GGML super-blocks, as in the file; n_past_inc (nullable): a word the launch increments once (the decode graph's last node)
 void mul_mat_kq_exact(int type, const void *w_raw, const void *xq8k, float *dst, int64_t ldd, int64_t K, int64_t N, int64_t B, const float *addend, int64_t lda,
-                      cudaStream_t st);                                                                   // w_raw: N rows of K/256 GGML super-blocks, as in the file
+                      cudaStream_t st, int *n_past_inc = nullptr);
+// get_rows on a K-quant matrix in file layout: dequantize_row_q*_K of rows ids[0, n) (w_raw: N rows of K/256 super-blocks)
+void get_rows_kq(int type, const void *w_raw, int64_t K, const int32_t *ids, float *dst, int64_t n, cudaStream_t st);
 
 // ---- synth.cu : seeded synthetic tensors generated in HBM (bench / tests) ------------------------------------------------------------
 void synth_qweight(const QWeight &w, uint64_t seed, cudaStream_t st);

@@ -13,18 +13,17 @@
 //     hsum_float_8(acc) (LC/k_quants.c:1193-1199) plus the "mins" term: Q4_K keeps 4 f32 lanes acc_m[t] = fma(dmin, (float)prod[t], acc_m[t]) reduced as
 //     (m0+m2)+(m1+m3) (:2618-2620, :2652-2655); Q5_K a scalar summs = fma(dmin, (float)(prod0+..+prod3), summs) (:3157-3160; contracted, vfmadd231ss);
 //     Q2_K folds its mins into the SAME 8 lanes first: acc_L = fma(dmin, (float)(m[2L] bsums[2L] + m[2L+1] bsums[2L+1]), acc_L) (:1346-1350).
-// One warp per (weight row, src1 row): lane = 8*part + L owns byte column L of two of the eight 32-byte groups; the integer partials meet by shuffles,
-// every lane then carries the f32 chain of its L.  This is a correctness-first kernel (weights re-read per src1 row through L2): the fused decode schedule
-// and the tensor-core prefill GEMMs serve the five classic formats only.
-#include "kernels.cuh"
+// lane = 8*part + L owns byte column L of two of the eight 32-byte groups; the integer partials meet by shuffles, every lane then carries the f32
+// chain of its L (kq_lanes.cuh).  Two kernels, chosen by the batch size: below 32 tokens (decode included) one warp per (weight row, token); from
+// 32 tokens on a tiled GEMM that stages 8 weight rows' super-blocks and 32 tokens' Q8_K blocks in shared memory once per super-block index.
+#include "kq_lanes.cuh"
 
 namespace b200 {
 
 namespace {
 
-constexpr int QKK = 256;
-struct __align__(4) BlockQ8K { float d; int8_t qs[QKK]; int16_t bsums[QKK / 16]; };   // LC/k_quants.h:112-117
-static_assert(sizeof(BlockQ8K) == 292, "block_q8_K");
+using kq::QKK;
+using kq::BlockQ8K;
 
 __device__ __forceinline__ int nearest_int_fma(float a, float b) {        // nearest_int(a*b) of LC/k_quants.c:36-42 as compiled (see the header)
     const float val = __fmaf_rn(a, b, 12582912.f);
@@ -72,123 +71,136 @@ __global__ void __launch_bounds__(128) quantize_q8k_kernel(const float *__restri
     if (lane == 0) yb->d = d;
 }
 
-__device__ __forceinline__ uint32_t ld_u32_a2(const uint8_t *p) {        // 4 bytes from a 2-byte aligned address (block_q6_K is 210 bytes)
-    return (uint32_t)*(const uint16_t *)p | ((uint32_t)*(const uint16_t *)(p + 2) << 16);
-}
-__device__ __forceinline__ float h2f(const uint8_t *p) { return __half2float(*(const __half *)p); }
-
-// 6-bit scale / min j of block_q4_K / block_q5_K (the utmp shuffles of LC/k_quants.c:2604-2609 = get_scale_min_k4, :316-324)
-__device__ __forceinline__ int k4_scale(const uint8_t *q, int j) { return j < 4 ? (q[j] & 63) : ((q[j + 4] & 0xF) | ((q[j - 4] >> 6) << 4)); }
-__device__ __forceinline__ int k4_min(const uint8_t *q, int j) { return j < 4 ? (q[j + 4] & 63) : ((q[j + 4] >> 4) | ((q[j] >> 6) << 4)); }
-
-template <int TYPE> struct KQ;
-template <> struct KQ<T_Q2_K> { static constexpr int BYTES = 84, QS = 16, QH = 0; };      // scales[16] qs[64] d dmin   (LC/k_quants.h:34-39)
-template <> struct KQ<T_Q3_K> { static constexpr int BYTES = 110, QS = 32, QH = 0; };     // hmask[32] qs[64] scales[12] d (:52-57)
-template <> struct KQ<T_Q4_K> { static constexpr int BYTES = 144, QS = 16, QH = 0; };
-template <> struct KQ<T_Q5_K> { static constexpr int BYTES = 176, QS = 48, QH = 16; };
-template <> struct KQ<T_Q6_K> { static constexpr int BYTES = 210, QS = 0, QH = 128; };
-
+// ---- short batches (B < KQ_GEMM_MIN, decode included): one warp per (weight row, token) --------------------------------------------------------
+// The warp walks its row's super-blocks in order through kq_load / kq_step (kq_lanes.cuh).  With N / 4 x B CTAs in flight it keeps more loads
+// outstanding than a tile that reuses weights can at these batch sizes, and it is the faster kernel there (DESIGN.md §4 has the measurements).
+// n_past_inc (nullable): incremented once, for a decode graph whose last node this is.
 template <int TYPE>
-__global__ void __launch_bounds__(128) mul_mat_kq_exact_kernel(const uint8_t *__restrict__ W, const BlockQ8K *__restrict__ X, float *__restrict__ dst, int64_t ldd,
-                                                               int64_t N, int64_t nsb, const float *__restrict__ addend, int64_t lda) {
-    const int lane = threadIdx.x & 31, L = lane & 7, part = lane >> 3;
+__global__ void __launch_bounds__(128) mul_mat_kq_warp_kernel(const uint8_t *__restrict__ W, const kq::BlockQ8K *__restrict__ X, float *__restrict__ dst,
+                                                              int64_t ldd, int64_t N, int nsb, const float *__restrict__ addend, int64_t lda, int *n_past_inc) {
+    const int lane = threadIdx.x & 31;
+    if (n_past_inc && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *n_past_inc = *n_past_inc + 1;
     const int64_t n = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5), b = blockIdx.y;
     if (n >= N) return;
-    const uint8_t *wrow = W + n * nsb * KQ<TYPE>::BYTES;
-    const BlockQ8K *xrow = X + b * nsb;
+    constexpr int BB = kq::Bytes<TYPE>::N;
+    const uint8_t *wrow = W + n * nsb * BB;
+    const kq::BlockQ8K *xrow = X + b * nsb;
     float acc = 0.f, accm = 0.f;
-    for (int64_t i = 0; i < nsb; i++) {
-        const uint8_t *wb = wrow + i * KQ<TYPE>::BYTES;
-        const BlockQ8K *xb = xrow + i;
-        const float yd = xb->d;
-        int p;
-        if (TYPE == T_Q2_K || TYPE == T_Q3_K) {
-            // 2-bit planes: group (j, k) = bits 2k of qs[32j ..] against q8[128j + 32k ..]; sub-block scale index 8j + 2k + (L >= 4) (get_scale_shuffle_q3k)
-            const int j = part >> 1;
-            float d;
-            uint32_t w, hm = 0;
-            if (TYPE == T_Q2_K) {
-                d = __fmul_rn(yd, h2f(wb + 80));
-                const float dmin = __fmul_rn(-yd, h2f(wb + 82));
-                const int prod = (int)(wb[2 * L] >> 4) * (int)xb->bsums[2 * L] + (int)(wb[2 * L + 1] >> 4) * (int)xb->bsums[2 * L + 1];
-                acc = __fmaf_rn(dmin, (float)prod, acc);              // the mins go into the SAME accumulator, before the quants (:1350)
-                w = *(const uint32_t *)(wb + 16 + 32 * j + 4 * L);
-            } else {
-                d = __fmul_rn(yd, h2f(wb + 108));
-                hm = ld_u32_a2(wb + 4 * L);
-                w = ld_u32_a2(wb + 32 + 32 * j + 4 * L);
-            }
-            p = 0;
+    for (int i = 0; i < nsb; i++) kq::kq_step<TYPE>(kq::kq_load<TYPE>(wrow + (int64_t)i * BB, lane), xrow + i, lane, acc, accm);
+    const float v = kq::kq_finish<TYPE>(acc, accm);
+    if (lane == 0) dst[b * ldd + n] = addend ? __fadd_rn(v, addend[b * lda + n]) : v;
+}
+
+// ---- batches of KQ_GEMM_MIN tokens and more (prefill): the tiled GEMM ------------------------------------------------------------------------------------------------------
+// A CTA owns GROWS weight rows (one per warp) x GTOK token rows.  Per super-block index it stages the GROWS weight super-blocks and the GTOK Q8_K
+// super-blocks in shared memory once; each warp reads its weight super-block once (kq_load) and folds it into the chains of all GTOK tokens
+// (kq_step), so each weight byte serves GTOK tokens and each activation byte GROWS rows.  Every output is still one complete
+// ggml_vec_dot_q*_K_q8_K in the reference's order.  The CTAs of consecutive indices take the token tiles of the same rows, so a matrix larger
+// than L2 comes from HBM about once per call.
+constexpr int GROWS = 8, GTOK = 32;
+template <int TYPE> struct KqTile { static constexpr int PITCH = (kq::Bytes<TYPE>::N + 4 + 15) / 16 * 16; };
+
+template <int TYPE>
+__global__ void __launch_bounds__(32 * GROWS) mul_mat_kq_gemm_kernel(const uint8_t *__restrict__ W, const kq::BlockQ8K *__restrict__ X, float *__restrict__ dst,
+                                                                      int64_t ldd, int64_t N, int nsb, int64_t B, int64_t ntt,
+                                                                      const float *__restrict__ addend, int64_t lda) {
+    constexpr int BB = kq::Bytes<TYPE>::N, PITCH = KqTile<TYPE>::PITCH;
+    __shared__ __align__(16) uint8_t ws[GROWS * PITCH];
+    __shared__ kq::BlockQ8K xs[GTOK];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t tt = blockIdx.x % ntt, rt = blockIdx.x / ntt;
+    const int64_t n0 = rt * GROWS, b0 = tt * GTOK;
+    const int nr = N - n0 < GROWS ? (int)(N - n0) : GROWS, nt = B - b0 < GTOK ? (int)(B - b0) : GTOK;
+    const int64_t row_bytes = (int64_t)nsb * BB;
+    float acc[GTOK], accm[GTOK];
 #pragma unroll
-            for (int kk = 0; kk < 2; kk++) {
-                const int k = 2 * (part & 1) + kk, si = 8 * j + 2 * k + (L >= 4);
-                const uint32_t lo = (w >> (2 * k)) & 0x03030303u;
-                const int xw = *(const int *)(xb->qs + 128 * j + 32 * k + 4 * L);
-                if (TYPE == T_Q2_K) p += (int)(wb[si] & 0xF) * __dp4a((int)lo, xw, 0);
-                else {
-                    const uint32_t q3h = ((~(hm >> (4 * j + k))) & 0x01010101u) << 2;       // 4 where the high bit is NOT set (:1936-1948)
-                    const uint8_t *s = wb + 96;                                             // 6-bit scales, the aux[] shuffles of :1907-1913
-                    const int wd = si >> 2, c = si & 3;
-                    const int sc = (int)(((s[(wd & 1) * 4 + c] >> (4 * (wd >> 1))) & 0xF) | (((s[8 + c] >> (2 * wd)) & 3) << 4)) - 32;
-                    p += sc * (__dp4a((int)lo, xw, 0) - __dp4a((int)q3h, xw, 0));
-                }
-            }
-            p += __shfl_xor_sync(0xffffffffu, p, 8);
-            p += __shfl_xor_sync(0xffffffffu, p, 16);
-            acc = __fmaf_rn(d, (float)p, acc);
-        } else if (TYPE == T_Q6_K) {
-            const float d = __fmul_rn(yd, h2f(wb + 208));
-            const int j = part >> 1, hs = part & 1;
-            const uint32_t wl = ld_u32_a2(wb + 64 * j + 32 * hs + 4 * L), wh = ld_u32_a2(wb + 128 + 32 * j + 4 * L);
-            const int8_t *sc = (const int8_t *)(wb + 192);
-            p = 0;
+    for (int t = 0; t < GTOK; t++) { acc[t] = 0.f; accm[t] = 0.f; }
+    for (int i = 0; i < nsb; i++) {
+        __syncthreads();                                                  // the previous super-block's readers are done
+        // weights: row r's super-block at ws + r * PITCH + (address & 3), copied as 2-byte words (blocks are 2-byte aligned), so kq_load's 4-byte
+        // reads see the alignment they have in global memory
+        for (int k = threadIdx.x; k < nr * (BB / 2); k += 32 * GROWS) {
+            const int r = k / (BB / 2), h = k - r * (BB / 2);
+            const uint8_t *src = W + (n0 + r) * row_bytes + (int64_t)i * BB;
+            ((uint16_t *)(ws + r * PITCH + ((uintptr_t)src & 3)))[h] = ((const uint16_t *)src)[h];
+        }
+        for (int k = threadIdx.x; k < nt * 73; k += 32 * GROWS) {             // 73 words per block_q8_K
+            const int t = k / 73, h = k - t * 73;
+            ((uint32_t *)&xs[t])[h] = ((const uint32_t *)(X + (b0 + t) * nsb + i))[h];
+        }
+        __syncthreads();
+        if (warp < nr) {
+            const uint8_t *src = W + (n0 + warp) * row_bytes + (int64_t)i * BB;
+            const kq::Lane w = kq::kq_load<TYPE>(ws + warp * PITCH + ((uintptr_t)src & 3), lane);
 #pragma unroll
-            for (int kk = 0; kk < 2; kk++) {                              // groups k = hs and hs + 2 of this 128-element half share the ql bytes
-                const int k = hs + 2 * kk;
-                const uint32_t nib = (kk ? (wl >> 4) : wl) & 0x0F0F0F0Fu;
-                const uint32_t q = nib | (((wh >> (2 * k)) & 0x03030303u) << 4);
-                const int xw = *(const int *)(xb->qs + 128 * j + 32 * k + 4 * L);
-                const int dot = __dp4a((int)q, xw, 0) - 32 * __dp4a(0x01010101, xw, 0);
-                p += (int)sc[2 * (4 * j + k) + (L >= 4)] * dot;
-            }
-            p += __shfl_xor_sync(0xffffffffu, p, 8);
-            p += __shfl_xor_sync(0xffffffffu, p, 16);
-            acc = __fmaf_rn(d, (float)p, acc);
-        } else {
-            const float d = __fmul_rn(yd, h2f(wb)), dmin = __fmul_rn(-yd, h2f(wb + 2));
-            const uint8_t *scq = wb + 4;
-            const uint32_t w = *(const uint32_t *)(wb + KQ<TYPE>::QS + 32 * part + 4 * L);
-            uint32_t lo = w & 0x0F0F0F0Fu, hi = (w >> 4) & 0x0F0F0F0Fu;
-            if (TYPE == T_Q5_K) {
-                const uint32_t hb = *(const uint32_t *)(wb + KQ<TYPE>::QH + 4 * L);
-                lo |= ((hb >> (2 * part)) & 0x01010101u) << 4;
-                hi |= ((hb >> (2 * part + 1)) & 0x01010101u) << 4;
-            }
-            const int x0 = *(const int *)(xb->qs + 64 * part + 4 * L), x1 = *(const int *)(xb->qs + 64 * part + 32 + 4 * L);
-            p = k4_scale(scq, 2 * part) * __dp4a((int)lo, x0, 0) + k4_scale(scq, 2 * part + 1) * __dp4a((int)hi, x1, 0);
-            p += __shfl_xor_sync(0xffffffffu, p, 8);
-            p += __shfl_xor_sync(0xffffffffu, p, 16);
-            acc = __fmaf_rn(d, (float)p, acc);
-            const int t = lane & 3;                                       // prod[t] of :2614-2617 (every lane carries the copy of its t)
-            const int q8a = (int)(int16_t)(xb->bsums[4 * t] + xb->bsums[4 * t + 1]), q8b = (int)(int16_t)(xb->bsums[4 * t + 2] + xb->bsums[4 * t + 3]);
-            int prod = k4_min(scq, 2 * t) * q8a + k4_min(scq, 2 * t + 1) * q8b;
-            if (TYPE == T_Q5_K) {
-                prod += __shfl_xor_sync(0xffffffffu, prod, 1);
-                prod += __shfl_xor_sync(0xffffffffu, prod, 2);
-            }
-            accm = __fmaf_rn(dmin, (float)prod, accm);
+            for (int t = 0; t < GTOK; t++)
+                if (t < nt) kq::kq_step<TYPE>(w, &xs[t], lane, acc[t], accm[t]);
         }
     }
-    float v = acc;                                                        // hsum_float_8: ((a0+a4)+(a2+a6)) + ((a1+a5)+(a3+a7))
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 4));
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
-    if (TYPE == T_Q4_K) {                                                 // (m0+m2) + (m1+m3)
-        accm = __fadd_rn(accm, __shfl_xor_sync(0xffffffffu, accm, 2));
-        accm = __fadd_rn(accm, __shfl_xor_sync(0xffffffffu, accm, 1));
+    if (warp >= nr) return;
+    const int64_t n = n0 + warp;
+#pragma unroll
+    for (int t = 0; t < GTOK; t++) {
+        if (t >= nt) break;
+        const float v = kq::kq_finish<TYPE>(acc[t], accm[t]);
+        const int64_t b = b0 + t;
+        if (lane == 0) dst[b * ldd + n] = addend ? __fadd_rn(v, addend[b * lda + n]) : v;
     }
-    if (TYPE == T_Q4_K || TYPE == T_Q5_K) v = __fadd_rn(v, accm);
-    if (lane == 0) dst[b * ldd + n] = addend ? __fadd_rn(v, addend[b * lda + n]) : v;
+}
+
+constexpr int KQ_GEMM_MIN = 32;               // the tiled GEMM from this batch size on (one whole token tile), the warp kernel below it
+
+template <int TYPE>
+void launch_kq(const void *w_raw, const void *xq8k, float *dst, int64_t ldd, int64_t N, int64_t nsb, int64_t B, const float *addend, int64_t lda,
+               int *n_past_inc, cudaStream_t st) {
+    const uint8_t *w = (const uint8_t *)w_raw;
+    const kq::BlockQ8K *x = (const kq::BlockQ8K *)xq8k;
+    if (B < KQ_GEMM_MIN) {
+        B200_ASSERT((N + 3) / 4 <= 0x7fffffffLL);
+        mul_mat_kq_warp_kernel<TYPE><<<dim3((unsigned)((N + 3) / 4), (unsigned)B), 128, 0, st>>>(w, x, dst, ldd, N, (int)nsb, addend, lda, n_past_inc);
+        return;
+    }
+    B200_ASSERT(!n_past_inc);
+    const int64_t ntt = (B + GTOK - 1) / GTOK, nrt = (N + GROWS - 1) / GROWS;
+    B200_ASSERT(ntt * nrt <= 0x7fffffffLL);
+    mul_mat_kq_gemm_kernel<TYPE><<<(unsigned)(ntt * nrt), 32 * GROWS, 0, st>>>(w, x, dst, ldd, N, (int)nsb, B, ntt, addend, lda);
+}
+
+// ---- get_rows: dequantize_row_q{2,3,4,5,6}_K (LC/k_quants.c:352, :531, :733, :926, :1065), one thread per element --------------------------------
+// As the reference's x86 build computes them: the block scale times the sub-block scale rounded first, then Q2_K / Q4_K / Q5_K contract
+// `dl * q - ml` into one fused multiply-add (vfnmadd / vfmsub in the disassembly of oracle/_ref), Q3_K has no min, Q6_K rounds (d * sc) * q twice.
+template <int TYPE>
+__global__ void get_rows_kq_kernel(const uint8_t *__restrict__ W, int64_t nsb, const int32_t *__restrict__ ids, float *__restrict__ dst, int64_t total) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int64_t K = nsb * QKK, i = t / K, c = t - i * K;
+    const int e = (int)(c % QKK);
+    const uint8_t *b = W + ((int64_t)ids[i] * nsb + c / QKK) * kq::Bytes<TYPE>::N;
+    float y;
+    if (TYPE == T_Q2_K || TYPE == T_Q3_K) {
+        const int n = e >> 7, r = e & 127, j = r >> 5, l = r & 31, is = 8 * n + 2 * j + (l >> 4);
+        const int q = (b[(TYPE == T_Q2_K ? 16 : 32) + 32 * n + l] >> (2 * j)) & 3;
+        if (TYPE == T_Q2_K) {
+            const float dl = __fmul_rn(kq::h2f(b + 80), (float)(b[is] & 0xF)), ml = __fmul_rn(kq::h2f(b + 82), (float)(b[is] >> 4));
+            y = __fmaf_rn(dl, (float)q, -ml);
+        } else {
+            const float dl = __fmul_rn(kq::h2f(b + 108), (float)kq::k3_scale(b + 96, is));
+            y = __fmul_rn(dl, (float)(q - ((b[l] >> (4 * n + j)) & 1 ? 0 : 4)));
+        }
+    } else if (TYPE == T_Q6_K) {
+        const int n = e >> 7, r = e & 127, g = r >> 5, l = r & 31;
+        const int lo = (b[64 * n + l + 32 * (g & 1)] >> (4 * (g >> 1))) & 0xF;
+        const int q = (lo | (((b[128 + 32 * n + l] >> (2 * g)) & 3) << 4)) - 32;
+        const int sc = ((const int8_t *)(b + 192))[8 * n + (l >> 4) + 2 * g];
+        y = __fmul_rn(__fmul_rn(kq::h2f(b + 208), (float)sc), (float)q);
+    } else {
+        const int j = e >> 6, hi = (e >> 5) & 1, l = e & 31, is = 2 * j + hi;
+        int q = (b[kq::Bytes<TYPE>::QS + 32 * j + l] >> (4 * hi)) & 0xF;
+        if (TYPE == T_Q5_K) q += (b[16 + l] >> is) & 1 ? 16 : 0;
+        const float d1 = __fmul_rn(kq::h2f(b), (float)kq::k4_scale(b + 4, is)), m1 = __fmul_rn(kq::h2f(b + 2), (float)kq::k4_min(b + 4, is));
+        y = __fmaf_rn(d1, (float)q, -m1);
+    }
+    dst[t] = y;
 }
 
 }  // namespace
@@ -204,19 +216,34 @@ void quantize_act_q8k(const float *x, int64_t ldx, void *y, int64_t K, int64_t B
 }
 
 void mul_mat_kq_exact(int type, const void *w_raw, const void *xq8k, float *dst, int64_t ldd, int64_t K, int64_t N, int64_t B, const float *addend, int64_t lda,
-                      cudaStream_t st) {
+                      cudaStream_t st, int *n_past_inc) {
     B200_ASSERT(is_kquant(type) && K % QKK == 0);
     if (!N || !B) return;
-    B200_ASSERT(B <= 65535);
-    const dim3 grid((unsigned)((N + 3) / 4), (unsigned)B);
     const int64_t nsb = K / QKK;
     switch (type) {
-        case T_Q2_K: mul_mat_kq_exact_kernel<T_Q2_K><<<grid, 128, 0, st>>>((const uint8_t *)w_raw, (const BlockQ8K *)xq8k, dst, ldd, N, nsb, addend, lda); break;
-        case T_Q3_K: mul_mat_kq_exact_kernel<T_Q3_K><<<grid, 128, 0, st>>>((const uint8_t *)w_raw, (const BlockQ8K *)xq8k, dst, ldd, N, nsb, addend, lda); break;
-        case T_Q4_K: mul_mat_kq_exact_kernel<T_Q4_K><<<grid, 128, 0, st>>>((const uint8_t *)w_raw, (const BlockQ8K *)xq8k, dst, ldd, N, nsb, addend, lda); break;
-        case T_Q5_K: mul_mat_kq_exact_kernel<T_Q5_K><<<grid, 128, 0, st>>>((const uint8_t *)w_raw, (const BlockQ8K *)xq8k, dst, ldd, N, nsb, addend, lda); break;
-        case T_Q6_K: mul_mat_kq_exact_kernel<T_Q6_K><<<grid, 128, 0, st>>>((const uint8_t *)w_raw, (const BlockQ8K *)xq8k, dst, ldd, N, nsb, addend, lda); break;
+        case T_Q2_K: launch_kq<T_Q2_K>(w_raw, xq8k, dst, ldd, N, nsb, B, addend, lda, n_past_inc, st); break;
+        case T_Q3_K: launch_kq<T_Q3_K>(w_raw, xq8k, dst, ldd, N, nsb, B, addend, lda, n_past_inc, st); break;
+        case T_Q4_K: launch_kq<T_Q4_K>(w_raw, xq8k, dst, ldd, N, nsb, B, addend, lda, n_past_inc, st); break;
+        case T_Q5_K: launch_kq<T_Q5_K>(w_raw, xq8k, dst, ldd, N, nsb, B, addend, lda, n_past_inc, st); break;
+        case T_Q6_K: launch_kq<T_Q6_K>(w_raw, xq8k, dst, ldd, N, nsb, B, addend, lda, n_past_inc, st); break;
         default: B200_ASSERT(!"mul_mat_kq_exact: type");
+    }
+    B200_CHECK(cudaGetLastError());
+}
+
+void get_rows_kq(int type, const void *w_raw, int64_t K, const int32_t *ids, float *dst, int64_t n, cudaStream_t st) {
+    B200_ASSERT(is_kquant(type) && K % QKK == 0);
+    const int64_t total = n * K, nsb = K / QKK;
+    if (!total) return;
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    const uint8_t *w = (const uint8_t *)w_raw;
+    switch (type) {
+        case T_Q2_K: get_rows_kq_kernel<T_Q2_K><<<grid, 256, 0, st>>>(w, nsb, ids, dst, total); break;
+        case T_Q3_K: get_rows_kq_kernel<T_Q3_K><<<grid, 256, 0, st>>>(w, nsb, ids, dst, total); break;
+        case T_Q4_K: get_rows_kq_kernel<T_Q4_K><<<grid, 256, 0, st>>>(w, nsb, ids, dst, total); break;
+        case T_Q5_K: get_rows_kq_kernel<T_Q5_K><<<grid, 256, 0, st>>>(w, nsb, ids, dst, total); break;
+        case T_Q6_K: get_rows_kq_kernel<T_Q6_K><<<grid, 256, 0, st>>>(w, nsb, ids, dst, total); break;
+        default: B200_ASSERT(!"get_rows_kq: type");
     }
     B200_CHECK(cudaGetLastError());
 }

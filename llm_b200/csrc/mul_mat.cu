@@ -22,6 +22,11 @@ int mul_mat_exact_auto(const QWeight &w, const float *x, int64_t ldx, int64_t B,
         else mul_mat_f16_gemm(w, a.xh, dst, ldd, B, addend, lda, st);
         return 2;
     }
+    if (is_kquant(w.type)) {                                 // quantize_row_q8_K, then ggml_vec_dot_q*_K_q8_K per output (kquants.cu)
+        quantize_act_q8k(x, ldx, a.xq8k, w.K, B, st);
+        mul_mat_kq_exact(w.type, w.qs, a.xq8k, dst, ldd, w.K, w.N, B, addend, lda, st);
+        return 2;
+    }
     const int vdt = vec_dot_type(w.type);
     if (B == 1 && mmv_exact_stream_supported(w)) {          // decode: TMA bulk-copy ring at HBM speed (exact_stream.cu)
         quantize_act_pack(w.type, x, a.xpack, w.K, st);

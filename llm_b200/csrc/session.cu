@@ -22,6 +22,7 @@ namespace {
 struct Layer {
     float *attention_norm = nullptr, *ffn_norm = nullptr;
     QWeight wqkv, wo, w13, w2;          // wqkv rows: [wq | wk | wv]; w13 rows: [w1 | w3]
+    QWeight wv;                         // wv of a type other than wq's: then wqkv rows are [wq | wk] and wv is this matrix (wv.N == 0 otherwise)
 };
 
 }  // namespace
@@ -35,6 +36,8 @@ struct b200_model : Weights {
     QWeight wte, output;
     float *norm = nullptr;
     std::vector<Layer> layers;
+    bool any_kquant = false, any_f16 = false;       // some 2-D weight is a K-quant / F16
+    bool uniform_layers = true;                     // every layer matrix is of hp.wtype (the layout and decode graph of a one-type file)
 
     bool lookup(const char *name, Slot &s, int &slot_id);
     int n_slots() const { return 3 + 9 * hp.n_layer; }
@@ -46,6 +49,7 @@ struct b200_session : SessionCore {     // memory_k [n_layer][n_ctx][gqa], memor
     // activations (sized for n_batch rows)
     DeviceBuf<float> x, cur, ff, qkv, kq, h13, hmul, logits;
     DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh;
+    DeviceBuf<char> xq8k;               // Q8_K activations of K-quant weights (models with one)
     // the graph decode schedule (decode_ops.cu)
     DeviceBuf<unsigned long long> d_prof;
     DeviceBuf<float> qbuf; DeviceBuf<int4> xpack_d, xpack_f;
@@ -79,11 +83,22 @@ bool b200_model::lookup(const char *name, Slot &s, int &slot_id) {
     s.is_q = true;
     if (!strcmp(sub, "attention.wq.weight")) { s.q = row_view(L.wqkv, 0, eq); slot_id = base + 2; return true; }
     if (!strcmp(sub, "attention.wk.weight")) { s.q = row_view(L.wqkv, eq, gqa); slot_id = base + 3; return true; }
-    if (!strcmp(sub, "attention.wv.weight")) { s.q = row_view(L.wqkv, eq + gqa, gqa); slot_id = base + 4; return true; }
+    if (!strcmp(sub, "attention.wv.weight")) { s.q = L.wv.N ? L.wv : row_view(L.wqkv, eq + gqa, gqa); slot_id = base + 4; return true; }
     if (!strcmp(sub, "attention.wo.weight")) { s.q = L.wo; slot_id = base + 5; return true; }
     if (!strcmp(sub, "feed_forward.w1.weight")) { s.q = L.w13; s.chunk = 32; s.row0 = 0;  s.stride = 64; s.rows = f; slot_id = base + 6; return true; }
     if (!strcmp(sub, "feed_forward.w3.weight")) { s.q = L.w13; s.chunk = 32; s.row0 = 32; s.stride = 64; s.rows = f; slot_id = base + 7; return true; }
     if (!strcmp(sub, "feed_forward.w2.weight")) { s.q = L.w2; slot_id = base + 8; return true; }
+    return false;
+}
+
+// the 2-D weights a LLaMA model holds: tok_embeddings, output, and layers.<il>.{attention.w[qkvo], feed_forward.w[123]}.weight
+bool b200::llama_matrix_name(const char *name, int n_layer) {
+    if (!strcmp(name, "tok_embeddings.weight") || !strcmp(name, "output.weight")) return true;
+    int il = -1, used = 0; char sub[64];
+    if (sscanf(name, "layers.%d.%63s%n", &il, sub, &used) != 2 || il < 0 || il >= n_layer || name[used]) return false;
+    static const char *const mats[] = {"attention.wq.weight", "attention.wk.weight", "attention.wv.weight", "attention.wo.weight",
+                                       "feed_forward.w1.weight", "feed_forward.w2.weight", "feed_forward.w3.weight"};
+    for (const char *m : mats) if (!strcmp(sub, m)) return true;
     return false;
 }
 
@@ -98,7 +113,8 @@ namespace {
 // ggml_mul_mat(w, x): quantize the f32 activation rows (the INIT phase of ggml_compute_forward_mul_mat) and multiply; returns the launches
 int matmul(b200_session *s, const QWeight &w, const float *x, float *dst, int64_t ldd, int64_t B, const float *addend, int64_t lda,
            cudaStream_t st, bool fast) {
-    if (!fast) return mul_mat_exact_auto(w, x, w.K, B, dst, ldd, addend, lda, {s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()}, st);
+    if (!fast || is_kquant(w.type))      // the order-free kernels take the five block formats: K-quants run their exact kernels in FAST sessions too
+        return mul_mat_exact_auto(w, x, w.K, B, dst, ldd, addend, lda, {s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get(), s->xq8k.get()}, st);
     quantize_act(vec_dot_type(w.type), x, w.K, s->xq.get(), s->xds.get(), w.K, B, st);
     if (B == 1)      mul_mat_vec_q(w, s->xq.get(), s->xds.get(), dst, addend, st);
     else if (B < 16) mul_mat_q_simple(w, s->xq.get(), s->xds.get(), dst, ldd, B, addend, lda, st);
@@ -148,6 +164,7 @@ void forward(b200_session *s, int n, bool all_rows = true) {
         rms_norm(s->x.get(), s->cur.get(), ly.attention_norm, e, n, 5e-6f, st); L++;                    // :183,186
         TAP(1, s->cur.get(), (size_t)n * e);
         L += matmul(s, ly.wqkv, s->cur.get(), s->qkv.get(), qkv_ld, n, nullptr, 0, st, fast);                // :194,208,223
+        if (ly.wv.N) L += matmul(s, ly.wv, s->cur.get(), s->qkv.get() + e + gqa, qkv_ld, n, nullptr, 0, st, fast);   // wv of its own type, into the same rows
         TAP(2, s->qkv.get(), (size_t)n * qkv_ld);
         // RoPE on Q and K heads in place: [hd, n_head + n_head_kv, n] with row stride qkv_ld    :190-217
         rope_f32(s->qkv.get(), s->qkv.get(), hd, n_head + n_head_kv, n, hd, qkv_ld, hd, qkv_ld, n_past, rope, st); L++;
@@ -272,9 +289,12 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
     // a valid quantized activation row for both K = n_embd and K = n_ff
     const bool fast = (s->cfg.flags & B200_SESSION_FAST) != 0;
     B200_CHECK(cudaMemsetAsync(s->hmul.get(), 0, (size_t)f * 4, st));
-    quantize_act(vec_dot_type(m->hp.wtype), s->hmul.get(), f, s->xq.get(), s->xds.get(), f, 1, st);
-    quantize_act_pack(m->hp.wtype, s->hmul.get(), s->xpack.get(), f, st);
+    if (!is_kquant(m->hp.wtype)) {
+        quantize_act(vec_dot_type(m->hp.wtype), s->hmul.get(), f, s->xq.get(), s->xds.get(), f, 1, st);
+        quantize_act_pack(m->hp.wtype, s->hmul.get(), s->xpack.get(), f, st);
+    }
     cvt_act_f16(s->hmul.get(), f, s->xh.get(), f, 1, st);
+    if (m->any_kquant) quantize_act_q8k(s->hmul.get(), f, s->xq8k.get(), f / 256 * 256, 1, st);
     (void)e;
     int64_t n = 0;
     auto mv = [&](const QWeight &w, float *out) {
@@ -282,13 +302,18 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
             if (mmv_f16_supported(w)) mul_mat_vec_f16(w, s->xh.get(), out, nullptr, st);
             else mul_mat_f16_gemm(w, s->xh.get(), out, w.N, 1, nullptr, 0, st);
         }
+        else if (is_kquant(w.type)) mul_mat_kq_exact(w.type, w.qs, s->xq8k.get(), out, w.N, w.K, w.N, 1, nullptr, 0, st);
         else if (fast) mul_mat_vec_q(w, s->xq.get(), s->xds.get(), out, nullptr, st);
         else if (mmv_exact_stream_supported(w)) mul_mat_vec_q_exact_stream(w, s->xpack.get(), out, nullptr, st);
         else mul_mat_q_exact(w, s->xq.get(), s->xds.get(), out, w.N, 1, nullptr, 0, st);
         n++;
     };
     auto pass = [&]() {
-        for (auto &L : m->layers) { mv(L.wqkv, s->qkv.get()); mv(L.wo, s->ff.get()); mv(L.w13, s->h13.get()); mv(L.w2, s->cur.get()); }
+        for (auto &L : m->layers) {
+            mv(L.wqkv, s->qkv.get());
+            if (L.wv.N) mv(L.wv, s->qkv.get());
+            mv(L.wo, s->ff.get()); mv(L.w13, s->h13.get()); mv(L.w2, s->cur.get());
+        }
         mv(m->output, s->logits.get());
     };
     pass();                      // warm-up (also first-touch of every page)
@@ -301,12 +326,63 @@ float b200_session_probe_matvec(b200_session *s, int32_t reps, int64_t *launches
     return ms;
 }
 
-static b200_model *llama_new_impl(const b200_llama_hparams *hp, int tp_rank, int tp_world) {
-    if (!hp || !is_qweight_type(hp->wtype) || hp->n_embd % 64 || hp->n_ff % 64 || hp->n_head <= 0 || hp->n_head_kv <= 0 ||
-        hp->n_head % hp->n_head_kv || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0) return nullptr;
+// the element type of each 2-D weight of one layer (wq and wk share one, w1 and w3 share one)
+struct LayerTypes { int qk, v, o, ff13, w2; };
+
+static b200_model *llama_new_impl(const b200_llama_hparams *hp, int tp_rank, int tp_world, const b200_tensor_type *types = nullptr, int32_t n_types = 0,
+                                  int *err = nullptr) {
+    int dummy; if (!err) err = &dummy;
+    *err = B200_ERR_BAD_ARG;
+    if (!hp || hp->n_embd % 64 || hp->n_ff % 64 || hp->n_head <= 0 || hp->n_head_kv <= 0 ||
+        hp->n_head % hp->n_head_kv || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0 || n_types < 0 || (n_types && !types)) return nullptr;
+    if (!is_qweight_type(hp->wtype) && !is_kquant(hp->wtype)) { *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; return nullptr; }
     const int G = tp_world;
     if (G < 1 || G > TP_MAX || tp_rank < 0 || tp_rank >= G) return nullptr;
     if (G > 1 && hp->wtype == T_F16) return nullptr;      // shards decode through the fused schedule only, which is built on Q8 activation records
+    // every 2-D weight's type: the table's entry, else hp->wtype; refused before anything is allocated
+    auto type_of = [&](const char *name) { int t = hp->wtype; for (int32_t i = 0; i < n_types; i++) if (types[i].name && !strcmp(types[i].name, name)) t = types[i].type; return t; };
+    for (int32_t i = 0; i < n_types; i++) {
+        if (!types[i].name) return nullptr;
+        if (!llama_matrix_name(types[i].name, hp->n_layer)) { *err = B200_ERR_UNKNOWN_TENSOR; return nullptr; }
+    }
+    auto check = [&](const char *name, int t, int64_t ne0) -> int {
+        if (!is_qweight_type(t) && !is_kquant(t)) {
+            fprintf(stderr, "llm_b200: %s is element type %d; 2-D weights are F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 or Q2_K..Q6_K\n", name, t);
+            return B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+        }
+        if (is_kquant(t) && ne0 % 256) { fprintf(stderr, "llm_b200: %s: a K-quant row of %lld elements is not whole super-blocks of 256\n", name, (long long)ne0); return B200_ERR_INVARIANT_BROKEN; }
+        if (is_kquant(t) && G > 1) { fprintf(stderr, "llm_b200: %s: K-quant weights are not offered on tensor-parallel shards\n", name); return B200_ERR_BAD_ARG; }
+        return B200_OK;
+    };
+    const int t_wte = type_of("tok_embeddings.weight"), t_out = type_of("output.weight");
+    if ((*err = check("tok_embeddings.weight", t_wte, hp->n_embd)) != B200_OK || (*err = check("output.weight", t_out, hp->n_embd)) != B200_OK) return nullptr;
+    std::vector<LayerTypes> lt((size_t)hp->n_layer);
+    for (int il = 0; il < hp->n_layer; il++) {
+        char nm[7][64];
+        static const char *const sfx[7] = {"attention.wq", "attention.wk", "attention.wv", "attention.wo", "feed_forward.w1", "feed_forward.w3", "feed_forward.w2"};
+        int t[7];
+        for (int k = 0; k < 7; k++) {
+            snprintf(nm[k], sizeof(nm[k]), "layers.%d.%s.weight", il, sfx[k]);
+            t[k] = type_of(nm[k]);
+            if ((*err = check(nm[k], t[k], k == 6 ? hp->n_ff : hp->n_embd)) != B200_OK) return nullptr;
+        }
+        // [wq | wk] and [w1 | w3] are one matrix each: no quantizer the reference ships writes their halves in different types
+        if (t[1] != t[0] || t[5] != t[4]) {
+            fprintf(stderr, "llm_b200: %s is of another element type than %s\n", t[1] != t[0] ? nm[1] : nm[5], t[1] != t[0] ? nm[0] : nm[4]);
+            *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+            return nullptr;
+        }
+        lt[il] = LayerTypes{t[0], t[2], t[3], t[4], t[6]};
+    }
+    // F16 weights come as whole F16 files: an F16 matrix beside block-format ones is refused (as before per-tensor types)
+    bool f16 = t_wte == T_F16 || t_out == T_F16, other = t_wte != T_F16 || t_out != T_F16;
+    for (const LayerTypes &x : lt)
+        for (int y : {x.qk, x.v, x.o, x.ff13, x.w2}) { f16 |= y == T_F16; other |= y != T_F16; }
+    if (f16 && other) {
+        fprintf(stderr, "llm_b200: F16 weights beside weights of other element types: F16 models are F16 throughout\n");
+        *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+        return nullptr;
+    }
     const int gqa_full = hp->n_embd / (hp->n_head / hp->n_head_kv);
     // row split: whole heads per rank, 32-row pieces of w1|w3 and of the lm_head, 32-element blocks of wo / w2's output slices
     if (G > 1 && (hp->n_head % G || hp->n_head_kv % G || (hp->n_ff / G) % 32 || hp->n_ff % G || (hp->n_embd / G) % 32 || hp->n_vocab % G || (hp->n_vocab / G) % 32)) return nullptr;
@@ -321,18 +397,34 @@ static b200_model *llama_new_impl(const b200_llama_hparams *hp, int tp_rank, int
     m->tp_rank = tp_rank; m->tp_world = G;
     m->e_loc = e / G; m->gqa_loc = gqa_full / G; m->f_loc = hp->n_ff / G; m->v_loc = v / G;
     m->layers.resize(hp->n_layer);
-    m->carve(t, m->n_slots(), [m, hp, e, v](SlabCarver &c) {
-        c.q(m->wte, e, v); c.q(m->output, e, m->v_loc); c.f(m->norm, e);
-        for (auto &L : m->layers) {
+    for (const LayerTypes &x : lt) m->uniform_layers &= x.qk == t && x.v == t && x.o == t && x.ff13 == t && x.w2 == t;
+    // with one type for every weight this is the layout of a one-type model: same matrices, same order, same bytes
+    m->carve(t, m->n_slots(), [m, hp, e, v, &lt, t_wte, t_out](SlabCarver &c) {
+        c.q(m->wte, e, v, t_wte); c.q(m->output, e, m->v_loc, t_out); c.f(m->norm, e);
+        for (int il = 0; il < hp->n_layer; il++) {
+            Layer &L = m->layers[il];
+            const LayerTypes &y = lt[il];
             c.f(L.attention_norm, e); c.f(L.ffn_norm, e);
-            c.q(L.wqkv, e, m->e_loc + 2 * m->gqa_loc); c.q(L.wo, e, m->e_loc); c.q(L.w13, e, 2 * m->f_loc); c.q(L.w2, hp->n_ff, m->e_loc);
+            if (y.v == y.qk) c.q(L.wqkv, e, m->e_loc + 2 * m->gqa_loc, y.qk);
+            else { c.q(L.wqkv, e, m->e_loc + m->gqa_loc, y.qk); c.q(L.wv, e, m->gqa_loc, y.v); }
+            c.q(L.wo, e, m->e_loc, y.o); c.q(L.w13, e, 2 * m->f_loc, y.ff13); c.q(L.w2, hp->n_ff, m->e_loc, y.w2);
         }
     });
-    m->weight_bytes -= (size_t)v * (e / QK) * qweight_block_bytes(t);   // tok_embeddings is only gathered from, never streamed
+    auto note = [m](const QWeight &w) { m->any_kquant |= is_kquant(w.type); m->any_f16 |= w.type == T_F16; };
+    note(m->wte); note(m->output);
+    for (const Layer &L : m->layers) { note(L.wqkv); note(L.wo); note(L.w13); note(L.w2); if (L.wv.N) note(L.wv); }
+    m->weight_bytes -= (size_t)v * m->wte.nb * qweight_block_bytes(m->wte.type);   // tok_embeddings is only gathered from, never streamed
+    *err = B200_OK;
     return m;
 }
 
 b200_model *b200_llama_new(const b200_llama_hparams *hp) { return llama_new_impl(hp, 0, 1); }
+
+// A model whose 2-D weights each have their own element type: types[0, n) name tensors (tok_embeddings.weight, output.weight,
+// layers.<i>.attention.w{q,k,v,o}.weight, layers.<i>.feed_forward.w{1,2,3}.weight); the others are of hp->wtype.
+b200_model *b200_llama_new_typed(const b200_llama_hparams *hp, const b200_tensor_type *types, int32_t n, int *err) {
+    return llama_new_impl(hp, 0, 1, types, n, err);
+}
 
 // Tensor-parallel shard `tp_rank` of `tp_world` (one process per GPU): the model's tensors keep their names, but every 2-D weight except
 // tok_embeddings holds only this rank's rows -- wq / wk / wv: its heads; w1 / w3: rows [rank * n_ff/G, +n_ff/G); wo / w2: rows
@@ -392,7 +484,11 @@ int b200_model_synthesize(b200_model *m, uint64_t seed) {
     const int64_t e = m->hp.n_embd;
     m->synthesize(seed, [m, e](SeedSeq &r) {
         r.q(m->wte); r.gain(m->norm, e); r.q(m->output);
-        for (auto &L : m->layers) { r.gain(L.attention_norm, e); r.gain(L.ffn_norm, e); r.q(L.wqkv); r.q(L.wo); r.q(L.w13); r.q(L.w2); }
+        for (auto &L : m->layers) {
+            r.gain(L.attention_norm, e); r.gain(L.ffn_norm, e); r.q(L.wqkv);
+            if (L.wv.N) r.q(L.wv);
+            r.q(L.wo); r.q(L.w13); r.q(L.w2);
+        }
     });
     return B200_OK;
 }
@@ -489,7 +585,7 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     s->m = m; s->cfg = *cfg;
     if (m->tp_world > 1) return start_session_tp(s);
     const b200_llama_hparams &hp = m->hp;
-    if (hp.wtype == T_F16 && (cfg->flags & B200_SESSION_FAST)) {   // the order-free kernels take the five block formats only
+    if (m->any_f16 && (cfg->flags & B200_SESSION_FAST)) {   // the order-free kernels take the five block formats only (K-quants run exact)
         fprintf(stderr, "llm_b200: start_session: B200_SESSION_FAST has no kernels for F16 weights\n");
         b200_session_free(s);
         return nullptr;
@@ -509,6 +605,7 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     s->xds = device_alloc<float2>(B * (kmax / QK) * sizeof(float2));
     s->xpack = device_alloc<int4>((kmax / QK) * 64);
     s->xh = device_alloc<__half>(xh_bytes(kmax, B));
+    if (m->any_kquant) s->xq8k = device_alloc<char>(q8k_bytes(kmax / 256 * 256, B));
     const RopeTable &rt_ = rope_table(hp.n_rot, 0, hp.rope_freq_base, hp.rope_freq_scale, m->hd, (int)n_ctx);
     // decode kernel parameters
     s->h_layers = decode_layers(s);
@@ -521,6 +618,7 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     P.token = s->d_tokens.get(); P.n_past = s->decode.d_n_past;
     P.x = s->x.get(); P.q = s->qbuf.get(); P.kq = s->kq.get(); P.ff = s->ff.get(); P.logits = s->logits.get();
     P.normed = s->cur.get();                                     // row 0 of cur: where forward()'s final rms_norm leaves a one-token batch
+    P.xq8k = s->xq8k.get();                                      // a K-quant lm_head's activation row
     s->xpack_d = device_alloc<int4>((e / QK) * 64);
     s->xpack_f = device_alloc<int4>((f / QK) * 64);
     P.xpack_d = s->xpack_d.get(); P.xpack_f = s->xpack_f.get();
@@ -531,9 +629,12 @@ b200_session *b200_model_start_session(b200_model *m, const b200_session_config 
     QWeight probe; probe.nb = (int64_t)e / QK;
     QWeight probe2; probe2.nb = (int64_t)f / QK;
     // F16 weights decode through the per-op path (exact_f16.cu's mat-vec): the fused schedule is built on Q8 activation records.  So does an f32
-    // cache whose context is longer than its two-kernel attention holds (the schedule's attention past 1664 positions).
+    // cache whose context is longer than its two-kernel attention holds (the schedule's attention past 1664 positions).  Per-tensor types: every
+    // layer matrix must be of the model's classic type; the lm_head may also be a K-quant (the quantizer's Q6_K output.weight), which the graph
+    // runs as quantize_row_q8_K + the K-quant mat-vec.  Layers with a K-quant or another type decode per op.
     s->graph_ok = hp.n_rot == m->hd && (m->hd == 64 || m->hd == 128) && mmv_exact_stream_supported(probe) && mmv_exact_stream_supported(probe2) &&
-                  e <= 6144 && n_ctx % 128 == 0 && hp.wtype != T_F16 && (s->kv_type != T_F32 || (int)n_ctx <= attn_sv_f32_max_ctx());
+                  e <= 6144 && n_ctx % 128 == 0 && hp.wtype != T_F16 && (s->kv_type != T_F32 || (int)n_ctx <= attn_sv_f32_max_ctx()) &&
+                  !is_kquant(hp.wtype) && m->uniform_layers && (m->output.type == hp.wtype || is_kquant(m->output.type));
     B200_CHECK(cudaDeviceSynchronize());   // the memsets / copies above ran on the legacy stream: order them before anything on the backend's non-blocking stream
     return s;
 }

@@ -51,6 +51,20 @@ __global__ void synth_f16_kernel(__half *w, int64_t n, uint64_t seed, float sigm
     if (i < n) w[i] = __float2half_rn(gauss(seed, (uint64_t)i) * sigma);
 }
 
+// K-quant weights (for timing): uniform random super-block bytes, then fp16 d (and dmin) ~ U[0.5, 1.5] / (16 sqrt(K)) in the block's fields
+__global__ void synth_kq_kernel(uint8_t *w, int type, int64_t nsb, uint64_t seed, float scale) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nsb) return;
+    const int bytes = kquant_block_bytes(type);
+    uint8_t *b = w + i * bytes;
+    for (int k = 0; k < bytes; k += 2) *(uint16_t *)(b + k) = (uint16_t)splitmix64(seed ^ ((uint64_t)i * 256 + k));
+    const uint64_t u = splitmix64(~seed ^ (uint64_t)i);
+    const __half d = __float2half_rn(scale * (0.5f + (float)(u & 0xFFFF) / 65536.f)), m = __float2half_rn(scale * (0.5f + (float)((u >> 16) & 0xFFFF) / 65536.f));
+    const int d_off = type == T_Q2_K ? 80 : type == T_Q3_K ? 108 : type == T_Q6_K ? 208 : 0;
+    *(__half *)(b + d_off) = d;
+    if (type == T_Q2_K || type == T_Q4_K || type == T_Q5_K) *(__half *)(b + d_off + 2) = m;
+}
+
 __global__ void synth_gain_kernel(float *g, int64_t n, uint64_t seed) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) g[i] = 1.0f + 0.1f * gauss(seed, (uint64_t)i);
@@ -62,6 +76,11 @@ void synth_qweight(const QWeight &w, uint64_t seed, cudaStream_t st) {
     if (w.type == T_F16) {
         const int64_t n = w.N * w.K;
         synth_f16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((__half *)w.qs, n, seed, 1.0f / sqrtf((float)w.K));
+        B200_CHECK(cudaGetLastError());
+        return;
+    }
+    if (is_kquant(w.type)) {
+        synth_kq_kernel<<<(unsigned)((nblk + 255) / 256), 256, 0, st>>>((uint8_t *)w.qs, w.type, nblk, seed, 1.0f / (16.0f * sqrtf((float)w.K)));
         B200_CHECK(cudaGetLastError());
         return;
     }

@@ -114,12 +114,17 @@ class GgmlFile:
 
 
 def write_llama(path: str, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray], shapes: Dict[str, Tuple[int, ...]],
-                vocabulary: Optional[Sequence[Tuple[bytes, float]]] = None, n_mult: int = 256, quantization_version: int = 2):
+                vocabulary: Optional[Sequence[Tuple[bytes, float]]] = None, n_mult: int = 256, quantization_version: int = 2,
+                tensor_types: Optional[Dict[str, int]] = None, llama_ftype: Optional[int] = None):
     """ggml::format::save for LLaMA (GGJT v3).  `tensors`: name -> GGML-layout bytes (uint8 block rows) or f32 arrays; `shapes`: name ->
-    (rows, cols) / (n,) as in oracle.synth.tensor_shapes (ggml order is reversed: ne0 = cols)."""
+    (rows, cols) / (n,) as in oracle.synth.tensor_shapes (ggml order is reversed: ne0 = cols).  `tensor_types`: {name: enum ggml_type} of the
+    block tensors that are not of hyperparameters["wtype"] (a quantizer's mix); `llama_ftype`: the header's file type (default: that of an
+    all-<wtype> file)."""
     L = _lib.lib()
     wtype = int(hyperparameters["wtype"])
-    llama_ftype = {0: 0, 1: 1, 2: 2, 3: 3, 8: 7, 6: 8, 7: 9}[wtype]               # llama_ftype of an all-<wtype> file (LC/llama.h)
+    tensor_types = tensor_types or {}
+    if llama_ftype is None:                                                       # llama_ftype of an all-<wtype> file (LC/llama.h)
+        llama_ftype = {0: 0, 1: 1, 2: 2, 3: 3, 8: 7, 6: 8, 7: 9, 10: 10, 11: 11, 12: 14, 13: 16, 14: 18}[wtype]
     hp = _lib.LlamaHparams(**{k: int(hyperparameters[k]) for k in ("n_vocab", "n_embd", "n_head", "n_head_kv", "n_layer", "n_rot", "n_ff")}, wtype=wtype)
     infos = (_lib.GgmlTensorInfo * len(tensors))()
     datas = (C.c_void_p * len(tensors))()
@@ -129,7 +134,7 @@ def write_llama(path: str, hyperparameters: Dict[str, int], tensors: Dict[str, n
         keep.append(a)
         shp = shapes[name]
         infos[i].name = name.encode()
-        infos[i].type = 0 if a.dtype == np.float32 else wtype
+        infos[i].type = 0 if a.dtype == np.float32 else 1 if a.dtype == np.float16 else int(tensor_types.get(name, wtype))
         infos[i].n_dims = len(shp)
         infos[i].ne[0] = shp[-1]
         infos[i].ne[1] = shp[0] if len(shp) == 2 else 1

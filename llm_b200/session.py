@@ -433,22 +433,29 @@ class LoraAdapters:
         self.close()
 
 
+KQUANT_BLOCK_BYTES = {10: 84, 11: 110, 12: 144, 13: 176, 14: 210}      # Q2_K .. Q6_K super-block bytes (LC/k_quants.h)
+
+
 def ggml_dims(arr: np.ndarray, wtype: int):
     """(n_dims, ne0, ne1) of a tensor given as GGML-layout block rows (uint8 [rows][row bytes]) or f32 ([n] or [rows][cols])"""
     if arr.dtype == np.float32:
         return (1, arr.shape[0], 1) if arr.ndim == 1 else (2, arr.shape[-1], arr.size // arr.shape[-1])
     if arr.dtype == np.float16:                  # F16 weights: [rows][cols] halves
         return 2, arr.shape[-1], arr.size // arr.shape[-1]
+    if wtype in KQUANT_BLOCK_BYTES:              # K-quants: 256-element super-blocks
+        return 2, arr.shape[-1] // KQUANT_BLOCK_BYTES[wtype] * 256, arr.size // arr.shape[-1]
     block = {2: 18, 3: 20, 6: 22, 7: 24, 8: 34}[wtype]
     return 2, arr.shape[-1] // block * 32, arr.size // arr.shape[-1]
 
 
 class Llama(_Native):
-    """KnownModel for LLaMA.  `hyperparameters` is a dict with n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff, wtype."""
+    """KnownModel for LLaMA.  `hyperparameters` is a dict with n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff, wtype.
+    `tensor_types`: {name: enum ggml_type} of 2-D weights whose type is not `wtype` (mixed-type files, b200_llama_new_typed)."""
     _HANDLE, _FREE = "_m", "b200_model_free"
+    tensor_types: Dict[str, int] = {}           # models loaded from a file or cut into shards: their types are in the C model
 
     def __init__(self, hyperparameters: Dict[str, int], params: ModelParameters = None, tensors: Dict[str, np.ndarray] = None,
-                 device: int = 0, vocabulary: Optional[Sequence] = None):
+                 device: int = 0, vocabulary: Optional[Sequence] = None, tensor_types: Optional[Dict[str, int]] = None):
         """vocabulary: the model file's tokens ((bytes, score) pairs, or bytes), consulted by eot_token_id()"""
         params = params or ModelParameters()
         self.vocabulary = [t[0] if isinstance(t, tuple) else bytes(t) for t in vocabulary] if vocabulary is not None else None
@@ -461,7 +468,17 @@ class Llama(_Native):
         hp = _lib.LlamaHparams(**{k: int(hyperparameters[k]) for k in _HP_KEYS}, wtype=int(hyperparameters["wtype"]),
                                context_size=params.context_size, rope_freq_base=params.rope_freq_base,
                                rope_freq_scale=params.rope_freq_scale)
-        self._m = self.L.b200_llama_new(C.byref(hp))
+        self.tensor_types = dict(tensor_types or {})
+        if self.tensor_types:
+            names = [n.encode() for n in self.tensor_types]
+            table = (_lib.TensorType * len(names))(*[_lib.TensorType(n, int(t)) for n, t in zip(names, self.tensor_types.values())])
+            err = C.c_int(0)
+            self._m = self.L.b200_llama_new_typed(C.byref(hp), table, len(names), C.byref(err))
+            if not self._m:
+                from .loader import LoadError
+                raise LoadError(err.value, "b200_llama_new_typed")
+        else:
+            self._m = self.L.b200_llama_new(C.byref(hp))
         if not self._m:
             raise ValueError(f"b200_llama_new rejected hyperparameters {hyperparameters}")
         if tensors is not None and params.lora_adapters:
@@ -477,7 +494,7 @@ class Llama(_Native):
     def load_tensor(self, name: str, arr: np.ndarray, adapters: "LoraAdapters" = None, shape: tuple = None):
         """`adapters`: patch the tensor with them (LoraAdapter::patch); `shape` is then its (rows, cols) / (n,) as in llama_tensor_shapes"""
         arr = np.ascontiguousarray(arr)
-        typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.hyperparameters["wtype"])
+        typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.tensor_types.get(name, self.hyperparameters["wtype"]))
         if adapters is None:
             _check(self.L.b200_model_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes),
                    f"load_tensor({name})")
