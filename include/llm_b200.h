@@ -329,6 +329,35 @@ b200_neox_model *b200_neox_new(const b200_neox_hparams *hp);
  * n_rot, use_parallel_residual and has_lm_head are ignored.  NULL for any other arch (and b200_neox_new returns NULL for 2 and 3).  Every other
  * b200_neox_* entry point serves these models unchanged. */
 b200_neox_model *b200_neox_new_alibi(const b200_neox_hparams *hp, float alibi_bias_max);
+/* Any of the five architectures (hp->arch 0 .. 4) with a per-tensor element type for its 2-D weights: types[0, n) name matrices by the model's
+ * tensor names (GPT-J: attn.q_proj / k_proj / v_proj), the others are of hp->wtype.  Types: F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 and Q2_K..Q6_K (K-quant
+ * matrices keep the file's 256-element super-blocks).  A tied output (GPT-2 without model/lm_head, MPT) streams wte in wte's type.  GPT-J's q_proj and
+ * k_proj share a type; a v_proj of another type becomes its own matrix writing the same qkv rows.  alibi_bias_max: MPT / BLOOM (ignored by the
+ * others); rope_freq_base / rope_freq_scale (<= 0: 10000 / 1): ModelParameters::rope_overrides of GPT-NeoX and GPT-J (ignored by the others).
+ * Refused before anything is allocated, with *err: B200_ERR_UNSUPPORTED_ELEMENT_TYPE for F32 2-D weights, F16 weights beside other types, GPT-J
+ * q_proj and k_proj of different types; B200_ERR_INVARIANT_BROKEN for a K-quant row that is not whole super-blocks; B200_ERR_UNKNOWN_TENSOR for a
+ * name the model does not hold; B200_ERR_BAD_ARG for hyperparameters the untyped forms refuse.  A model whose matrices all share one classic type
+ * has the untyped form's layout and decode graph; a model with a K-quant matrix or with mixed types decodes per op.  b200_neox_new and
+ * b200_neox_new_alibi are this with no table and the default RoPE. */
+b200_neox_model *b200_neox_new_typed(const b200_neox_hparams *hp, float alibi_bias_max, float rope_freq_base, float rope_freq_scale,
+                                     const b200_tensor_type *types, int32_t n, int *err);
+int  b200_neox_is_loaded(b200_neox_model *m);                          /* every tensor of the model has been loaded */
+/* llm::load_dynamic for the GPT-NeoX-family architectures: arch B200_ARCH_GPT2 / GPTNEOX / MPT / BLOOM / GPTJ.  The header maps to
+ * b200_neox_hparams as the reference's KnownModel::new reads it (b200_ggml_neox_hparams), every 2-D weight's type comes from the file
+ * (b200_neox_new_typed), and each tensor is uploaded from the mapping through b200_neox_load_tensor_lora with the adapters lora_paths[0, n_lora).
+ * context_size <= 0: 2048 (ModelParameters::default); GPT-2's context is the header's n_ctx whatever is asked, as its learned positions (model/wpe)
+ * have that many rows.  rope_freq_base / rope_freq_scale <= 0: 10000 / 1.  The quantization-version rule of the LLaMA loader applies; an adapter that
+ * targets a K-quant tensor is B200_ERR_UNSUPPORTED_ELEMENT_TYPE, before the model is created; a missing tensor is B200_ERR_NOT_LOADED. */
+b200_neox_model *b200_neox_load_file(const char *path, int32_t arch, int32_t context_size, float rope_freq_base, float rope_freq_scale,
+                                     const char *const *lora_paths, int32_t n_lora, int *err);
+/* the GPT-NeoX-family view of a header (a file opened as B200_ARCH_GPT2 .. B200_ARCH_GPTJ): n_vocab, n_embd, n_head, n_layer, n_rot (GPT-NeoX, GPT-J),
+ * use_parallel_residual (GPT-NeoX), arch (0 GPT-NeoX, 1 GPT-2, 2 MPT, 3 BLOOM, 4 GPT-J), has_lm_head (GPT-2: model/lm_head present), wtype (the type
+ * of the file's first 2-D weight), context_size (GPT-2: the header's n_ctx; the others 2048, the default the loader starts from); *alibi_bias_max:
+ * MPT's header float, 8 for BLOOM, 0 otherwise; the quantization version and its rule (B200_ERR_QUANTIZATION_VERSION) as b200_ggml_llama_hparams */
+int     b200_ggml_neox_hparams(const b200_ggml_file *f, b200_neox_hparams *out, float *alibi_bias_max, int32_t *quantization_version);
+/* the type table the loaders build: every 2-D weight of the file that a model of the file's architecture and n_layer holds, in file order.
+ * The names point into the file handle (valid until b200_ggml_close).  Returns the count (at most max entries are written), or a negative error. */
+int64_t b200_ggml_weight_types(const b200_ggml_file *f, b200_tensor_type *out, int64_t max);
 int  b200_neox_load_tensor(b200_neox_model *m, const char *name, int32_t type, const void *host_data, size_t nbytes);
 /* shaped load (2-D: ne0 = row length, ne1 = rows; 1-D: ne1 = 1) with the LoRA adapters of b200_model_load_tensor_lora */
 int  b200_neox_load_tensor_lora(b200_neox_model *m, const char *name, int32_t type, int32_t n_dims, int64_t ne0, int64_t ne1, const void *host_data, size_t nbytes,

@@ -15,8 +15,9 @@
 //   FileType                     crates/llm-base/src/loader.rs:32-50        file_type = quantization_version * 1000 + llama_ftype
 //   quantization version rule    crates/llm-base/src/loader.rs:459-484      0 is read as 1 (GGJT v2) / 2 (GGJT v3); quantized tensors require 2
 //   ggml::format::save           crates/ggml/src/format/saver.rs:86-160     the writer (GGJT v3)
-// The parser is plain host code (mmap, no CUDA): the CPU test-suite exercises it without a GPU.  b200_llama_load_file() then feeds every tensor
-// to b200_model_load_tensor straight from the mapping (TensorLoader::load + transfer_to(Backend::Gpu)).
+// The parser is plain host code (mmap, no CUDA): the CPU test-suite exercises it without a GPU.  b200_llama_load_file() and b200_neox_load_file()
+// (llm::load_dynamic's other architectures) then feed every tensor to the model straight from the mapping (TensorLoader::load +
+// transfer_to(Backend::Gpu)), through one shared loop (load_tensors).
 #include <fcntl.h>
 #include <stdio.h>
 #include <string.h>
@@ -73,6 +74,85 @@ struct b200_ggml_file {
     std::vector<float> scores;
     std::vector<TensorInfo> tensors;
 };
+
+namespace {
+
+// the header words of each architecture (B200_ARCH_LLAMA .. B200_ARCH_GPTJ) that the loaders read: file_type (FileType, loader.rs:32-50) and n_layer
+int file_type_word(int32_t arch) { static const int w[] = {6, 5, 7, 7, 5, 6}; return w[arch]; }
+int n_layer_word(int32_t arch) { return arch == B200_ARCH_MPT ? 3 : 4; }
+// b200_neox_hparams.arch of a file's architecture, -1 for LLaMA and LoRA
+int neox_arch(int32_t arch) {
+    switch (arch) { case B200_ARCH_GPTNEOX: return 0; case B200_ARCH_GPT2: return 1; case B200_ARCH_MPT: return 2; case B200_ARCH_BLOOM: return 3; case B200_ARCH_GPTJ: return 4; }
+    return -1;
+}
+
+// a 2-D weight that a model of the file's architecture and n_layer holds
+bool holds_matrix(const b200_ggml_file *f, const TensorInfo &t) {
+    if (t.n_dims != 2 || f->arch == B200_ARCH_LORA) return false;
+    const int n_layer = f->hp[n_layer_word(f->arch)];
+    return f->arch == B200_ARCH_LLAMA ? b200::llama_matrix_name(t.name.c_str(), n_layer) : b200::neox_matrix_name(neox_arch(f->arch), t.name.c_str(), n_layer);
+}
+
+// the quantization-version rule of crates/llm-base/src/loader.rs:459-484, for every architecture: the file type's version, 0 read as 1 (GGJT v2) /
+// 2 (GGJT v3); quantized tensors require 2
+int quantization_version(const b200_ggml_file *f, int32_t *qv_out) {
+    int32_t qv = (int32_t)((uint32_t)f->hp[file_type_word(f->arch)] / 1000u);
+    if (qv == 0 && f->magic == MAGIC_GGJT) qv = f->version == 2 ? 1 : f->version == 3 ? 2 : 0;
+    if (qv_out) *qv_out = qv;
+    for (const TensorInfo &t : f->tensors)
+        if ((b200::is_quant(t.type) || b200::is_kquant(t.type)) && qv != 2) return B200_ERR_QUANTIZATION_VERSION;
+    return B200_OK;
+}
+
+// ModelParameters::lora_adapters: every adapter is opened (ggml::format::load with LoraParameters) and stays open while the model's tensors load
+struct Adapters {
+    std::vector<b200_ggml_file *> files;
+    Adapters() = default;
+    Adapters(const Adapters &) = delete;
+    ~Adapters() { for (b200_ggml_file *a : files) b200_ggml_close(a); }
+    int open(const char *const *paths, int32_t n) {
+        if (n < 0 || (n > 0 && !paths)) return B200_ERR_BAD_ARG;
+        for (int32_t i = 0; i < n; i++) {
+            int err = B200_OK;
+            b200_ggml_file *a = b200_ggml_open_arch(paths[i], B200_ARCH_LORA, &err);
+            if (!a) return err;
+            files.push_back(a);
+        }
+        return B200_OK;
+    }
+};
+
+// What every model file load shares (llm::load, crates/llm-base/src/loader.rs:419-567): the type of each 2-D weight the model holds, in file order;
+// adapters checked against K-quant targets before anything is created; the model for that table (make); every tensor uploaded from the mapping
+// (MmapCompatibleLoader::load, loader.rs:661-669); the loaded check.  The caller closes the file.
+template <class M, class Make>
+M *load_tensors(const b200_ggml_file *f, const char *path, const b200_ggml_file *const *adapters, int32_t n_adapters, int *err, Make &&make,
+                int (*load)(M *, const char *, int32_t, int32_t, int64_t, int64_t, const void *, size_t, const b200_ggml_file *const *, int32_t),
+                int (*loaded)(M *), void (*release)(M *)) {
+    std::vector<b200_tensor_type> types;
+    for (const TensorInfo &t : f->tensors) {
+        if (!holds_matrix(f, t)) continue;                  // the upload below reports any other tensor
+        types.push_back(b200_tensor_type{t.name.c_str(), t.type});
+        if (b200::is_kquant(t.type))
+            for (int32_t a = 0; a < n_adapters; a++)
+                if (adapters[a] && b200::lora_in_patch_set(adapters[a], t.name.c_str())) {
+                    fprintf(stderr, "llm_b200: %s: a LoRA adapter patches %s, a %s tensor: adapters apply to F16 and Q4_0..Q8_0 weights\n", path, t.name.c_str(), type_name(t.type));
+                    *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+                    return nullptr;
+                }
+    }
+    M *m = make(types, err);
+    if (!m) return nullptr;
+    for (const TensorInfo &t : f->tensors) {
+        const int rc = load(m, t.name.c_str(), t.type, t.n_dims, t.ne[0], t.ne[1], f->map + t.offset, (size_t)t.nbytes, adapters, n_adapters);
+        if (rc != B200_OK) { *err = rc; release(m); return nullptr; }
+    }
+    if (!loaded(m)) { *err = B200_ERR_NOT_LOADED; release(m); return nullptr; }
+    *err = B200_OK;
+    return m;
+}
+
+}  // namespace
 
 // ---- the LoRA hook's view of an adapter file (host.h) ----
 int64_t b200::ggml_find_tensor(const b200_ggml_file *f, const char *name) {
@@ -252,21 +332,49 @@ int b200_ggml_llama_hparams(const b200_ggml_file *f, b200_llama_hparams *out, in
     memset(out, 0, sizeof(*out));
     out->n_vocab = f->hp[0]; out->n_embd = f->hp[1]; out->n_head = f->hp[3]; out->n_head_kv = f->hp[3]; out->n_layer = f->hp[4]; out->n_rot = f->hp[5];
     out->context_size = 2048; out->rope_freq_base = 10000.0f; out->rope_freq_scale = 1.0f;
-    int32_t qv = (int32_t)((uint32_t)f->hp[6] / 1000u);
-    if (qv == 0 && f->magic == MAGIC_GGJT) qv = f->version == 2 ? 1 : f->version == 3 ? 2 : 0;
+    const int qrc = ::quantization_version(f, quantization_version);
     if (n_mult) *n_mult = f->hp[2];
     if (llama_ftype) *llama_ftype = (int32_t)((uint32_t)f->hp[6] % 1000u);
-    if (quantization_version) *quantization_version = qv;
-    bool any_quant = false;
     out->wtype = -1;                                                             // "not found" (F32 = 0 is a valid element type)
     for (const TensorInfo &t : f->tensors) {
-        any_quant |= b200::is_quant(t.type) || b200::is_kquant(t.type);
         if (t.name == "layers.0.feed_forward.w1.weight") out->n_ff = (int32_t)t.ne[1];
         if (t.name == "layers.0.attention.wq.weight") out->wtype = t.type;
     }
-    if (any_quant && qv != 2) return B200_ERR_QUANTIZATION_VERSION;
+    if (qrc != B200_OK) return qrc;
     if (out->n_ff == 0 || out->wtype < 0) return B200_ERR_UNKNOWN_TENSOR;
     return B200_OK;
+}
+
+// GPT-NeoX-family view of the header, as each KnownModel::new reads it: gptneox lib.rs:36-140 (n_rot, use_parallel_residual), gpt2 lib.rs:43-136
+// (has_lm_head from model/lm_head, lib.rs:67-70; context = n_ctx, the rows of model/wpe), mpt lib.rs (alibi_bias_max), bloom lib.rs:240 (ALiBi bias 8),
+// gptj lib.rs:47-122 (n_rot)
+int b200_ggml_neox_hparams(const b200_ggml_file *f, b200_neox_hparams *out, float *alibi_bias_max, int32_t *quantization_version) {
+    if (!f || !out || neox_arch(f->arch) < 0) return B200_ERR_BAD_ARG;
+    memset(out, 0, sizeof(*out));
+    const int32_t *w = f->hp;
+    out->arch = neox_arch(f->arch);
+    out->context_size = 2048;
+    float bias = 0.f;
+    switch (f->arch) {
+        case B200_ARCH_GPTNEOX: out->n_vocab = w[0]; out->n_embd = w[2]; out->n_head = w[3]; out->n_layer = w[4]; out->n_rot = w[5]; out->use_parallel_residual = w[6]; break;
+        case B200_ARCH_GPT2:    out->n_vocab = w[0]; out->context_size = w[1]; out->n_embd = w[2]; out->n_head = w[3]; out->n_layer = w[4];
+                                out->has_lm_head = b200::ggml_find_tensor(f, "model/lm_head") >= 0; break;
+        case B200_ARCH_MPT:     out->n_embd = w[0]; out->n_head = w[2]; out->n_layer = w[3]; out->n_vocab = w[4]; memcpy(&bias, &w[5], 4); break;
+        case B200_ARCH_BLOOM:   out->n_vocab = w[0]; out->n_embd = w[1]; out->n_head = w[3]; out->n_layer = w[4]; bias = 8.0f; break;
+        case B200_ARCH_GPTJ:    out->n_vocab = w[0]; out->n_embd = w[2]; out->n_head = w[3]; out->n_layer = w[4]; out->n_rot = w[5]; break;
+    }
+    if (alibi_bias_max) *alibi_bias_max = bias;
+    out->wtype = b200::T_F16;
+    for (const TensorInfo &t : f->tensors) if (holds_matrix(f, t)) { out->wtype = t.type; break; }
+    return ::quantization_version(f, quantization_version);
+}
+
+int64_t b200_ggml_weight_types(const b200_ggml_file *f, b200_tensor_type *out, int64_t max) {
+    if (!f || max < 0 || (max > 0 && !out)) return B200_ERR_BAD_ARG;
+    int64_t n = 0;
+    for (const TensorInfo &t : f->tensors)
+        if (holds_matrix(f, t)) { if (n < max) out[n] = b200_tensor_type{t.name.c_str(), t.type}; n++; }
+    return n;
 }
 
 // ggml::format::save: GGJT v3, the architecture's hyperparameter words verbatim, tensor data 32-byte aligned.  tensors = n_tensors x {name, type, n_dims, ne,
@@ -316,28 +424,10 @@ static b200_model *load_file_impl(const char *path, int32_t context_size, float 
     if (rope_freq_base > 0.f) hp.rope_freq_base = rope_freq_base;
     if (rope_freq_scale > 0.f) hp.rope_freq_scale = rope_freq_scale;
     if (n_gqa > 1) { if (hp.n_head % n_gqa) { *err = B200_ERR_BAD_ARG; b200_ggml_close(f); return nullptr; } hp.n_head_kv = hp.n_head / n_gqa; }
-    // every 2-D tensor's own type (the model checks them: b200_llama_new_typed); a LoRA patch of a K-quant tensor is refused before any upload
-    std::vector<b200_tensor_type> types;
-    for (const TensorInfo &t : f->tensors) {
-        if (t.n_dims != 2 || !b200::llama_matrix_name(t.name.c_str(), hp.n_layer)) continue;   // the loop below reports any other tensor
-        types.push_back(b200_tensor_type{t.name.c_str(), t.type});
-        if (b200::is_kquant(t.type))
-            for (int32_t a = 0; a < n_adapters; a++)
-                if (adapters[a] && b200::lora_in_patch_set(adapters[a], t.name.c_str())) {
-                    fprintf(stderr, "llm_b200: %s: a LoRA adapter patches %s, a %s tensor: adapters apply to F16 and Q4_0..Q8_0 weights\n", path, t.name.c_str(), type_name(t.type));
-                    *err = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; b200_ggml_close(f); return nullptr;
-                }
-    }
-    b200_model *m = b200_llama_new_typed(&hp, types.data(), (int32_t)types.size(), err);
-    if (!m) { b200_ggml_close(f); return nullptr; }
-    for (size_t i = 0; i < f->tensors.size(); i++) {
-        const TensorInfo &t = f->tensors[i];
-        const int rc = b200_model_load_tensor_lora(m, t.name.c_str(), t.type, t.n_dims, t.ne[0], t.ne[1], f->map + t.offset, (size_t)t.nbytes, adapters, n_adapters);
-        if (rc != B200_OK) { *err = rc; b200_model_free(m); b200_ggml_close(f); return nullptr; }
-    }
-    if (!b200_model_is_loaded(m)) { *err = B200_ERR_NOT_LOADED; b200_model_free(m); b200_ggml_close(f); return nullptr; }
+    b200_model *m = load_tensors<b200_model>(f, path, adapters, n_adapters, err,
+        [&hp](const std::vector<b200_tensor_type> &types, int *e) { return b200_llama_new_typed(&hp, types.data(), (int32_t)types.size(), e); },
+        b200_model_load_tensor_lora, b200_model_is_loaded, b200_model_free);
     b200_ggml_close(f);
-    *err = B200_OK;
     return m;
 }
 b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa, int *err) {
@@ -345,20 +435,34 @@ b200_model *b200_llama_load_file_gqa(const char *path, int32_t context_size, flo
     return load_file_impl(path, context_size, rope_freq_base, rope_freq_scale, n_gqa, nullptr, 0, err);
 }
 
-// ModelParameters::lora_adapters: every adapter is opened (ggml::format::load with LoraParameters) and stays open while the model's tensors load
 b200_model *b200_llama_load_file_lora(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int32_t n_gqa,
                                       const char *const *lora_paths, int32_t n_lora, int *err) {
     int dummy; if (!err) err = &dummy;
-    if (n_lora < 0 || (n_lora > 0 && !lora_paths)) { *err = B200_ERR_BAD_ARG; return nullptr; }
-    std::vector<b200_ggml_file *> ad;
-    auto close_all = [&]() { for (b200_ggml_file *a : ad) b200_ggml_close(a); };
-    for (int32_t i = 0; i < n_lora; i++) {
-        b200_ggml_file *a = b200_ggml_open_arch(lora_paths[i], B200_ARCH_LORA, err);
-        if (!a) { close_all(); return nullptr; }
-        ad.push_back(a);
-    }
-    b200_model *m = load_file_impl(path, context_size, rope_freq_base, rope_freq_scale, n_gqa, ad.data(), n_lora, err);
-    close_all();
+    Adapters ad;
+    if ((*err = ad.open(lora_paths, n_lora)) != B200_OK) return nullptr;
+    return load_file_impl(path, context_size, rope_freq_base, rope_freq_scale, n_gqa, ad.files.data(), n_lora, err);
+}
+
+// llm::load_dynamic for the GPT-NeoX-family architectures (crates/llm/src/lib.rs:214): the same steps as the LLaMA loader, on b200_neox_new_typed
+b200_neox_model *b200_neox_load_file(const char *path, int32_t arch, int32_t context_size, float rope_freq_base, float rope_freq_scale,
+                                     const char *const *lora_paths, int32_t n_lora, int *err) {
+    int dummy; if (!err) err = &dummy;
+    if (!path || neox_arch(arch) < 0) { *err = B200_ERR_BAD_ARG; return nullptr; }
+    Adapters ad;
+    if ((*err = ad.open(lora_paths, n_lora)) != B200_OK) return nullptr;
+    b200_ggml_file *f = b200_ggml_open_arch(path, arch, err);
+    if (!f) return nullptr;
+    b200_neox_hparams hp;
+    float alibi_bias_max = 0.f;
+    *err = b200_ggml_neox_hparams(f, &hp, &alibi_bias_max, nullptr);
+    if (*err != B200_OK) { b200_ggml_close(f); return nullptr; }
+    if (context_size > 0 && arch != B200_ARCH_GPT2) hp.context_size = context_size;    // GPT-2: the rows of model/wpe
+    b200_neox_model *m = load_tensors<b200_neox_model>(f, path, ad.files.data(), n_lora, err,
+        [&](const std::vector<b200_tensor_type> &types, int *e) {
+            return b200_neox_new_typed(&hp, alibi_bias_max, rope_freq_base, rope_freq_scale, types.data(), (int32_t)types.size(), e);
+        },
+        b200_neox_load_tensor_lora, b200_neox_is_loaded, b200_neox_free);
+    b200_ggml_close(f);
     return m;
 }
 b200_model *b200_llama_load_file(const char *path, int32_t context_size, float rope_freq_base, float rope_freq_scale, int *err) {

@@ -101,6 +101,8 @@ int read_slot(const Slot &s, void *host, size_t nbytes);                       /
 
 // a 2-D weight of a LLaMA model of n_layer layers: tok_embeddings / output / layers.<i>.attention.w[qkvo] / layers.<i>.feed_forward.w[123] (session.cu)
 bool llama_matrix_name(const char *name, int n_layer);
+// a 2-D weight of a GPT-NeoX-family model (b200_neox_hparams.arch) of n_layer layers: a matrix, or one of GPT-J's q_proj / k_proj / v_proj (neox.cu)
+bool neox_matrix_name(int arch, const char *name, int n_layer);
 
 // ---- adapter files (ggml_file.cu) ----
 int64_t ggml_find_tensor(const b200_ggml_file *f, const char *name);        // index in the tensor table, -1 if absent

@@ -63,12 +63,15 @@ struct b200_neox_model : Weights {
     QkvLayout qkv_layout;
     bool parallel = false;                                        // GPT-NeoX with use_parallel_residual: attention and MLP both read inpL
     float kq_scale = 0.0f;
+    bool any_kquant = false;                                      // some matrix is a K-quant (the sessions hold a Q8_K activation buffer)
+    bool uniform = true;                                          // every matrix is of hp.wtype, as one fused qkv per layer: the decode graph's layout
     bool neox() const { return hp.arch == 0; }
     bool mpt() const { return hp.arch == 2; }
     bool bloom() const { return hp.arch == 3; }
     bool gptj() const { return hp.arch == 4; }
-    // MPT: every bias null; GPT-J: ln2_*, bqkv and bdense null (one LayerNorm per layer, no attention biases)
-    struct Layer { QWeight wqkv, wdense, wfc, wproj; float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj; };
+    // MPT: every bias null; GPT-J: ln2_*, bqkv and bdense null (one LayerNorm per layer, no attention biases).  wv: GPT-J's v_proj of another
+    // type than q_proj: then wqkv holds [q_proj | k_proj] and wv is its own matrix writing the same qkv rows (wv.N == 0 otherwise)
+    struct Layer { QWeight wqkv, wdense, wfc, wproj; float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bdense, *bfc, *bproj; QWeight wv; };
     std::vector<Layer> layers;
     template <class F> void each_tensor(F &&f);
     int64_t dim(Dim d) const;
@@ -81,6 +84,7 @@ struct b200_neox_session : SessionCore {   // memory_k [n_layer][n_ctx][e], memo
     DeviceBuf<float> qdec;
     DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh;
     DeviceBuf<int4> xpack_a, xpack_d, xpack_f;
+    DeviceBuf<char> xq8k;                                         // Q8_K activations of K-quant weights (models with one)
     std::vector<NeoxLayer> dl;
     NeoxParams dp;
 };
@@ -177,7 +181,11 @@ bool b200_neox_model::lookup(const char *name, Slot &s, int &id) {
         if (l < 0 ? !strcmp(name, d.name) : l == il && !strcmp(sub, d.name)) {
             s = Slot();
             if (d.kind == MAT) { s.q = o.*d.q; s.is_q = true; }
-            else if (d.kind == ROWS) { s.q = row_view(o.*d.q, d.at * (int64_t)hp.n_embd, hp.n_embd); s.is_q = true; }
+            else if (d.kind == ROWS) {     // rows past the fused matrix's own: GPT-J's v_proj of its own type
+                const QWeight &q = o.*d.q;
+                s.q = (d.at + 1) * (int64_t)hp.n_embd > q.N ? layers[l].wv : row_view(q, d.at * (int64_t)hp.n_embd, hp.n_embd);
+                s.is_q = true;
+            }
             else { s.f = o.*d.f; s.n = dim(d.K); }
             id = slot;
             found = true;
@@ -198,8 +206,9 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     int L = 0;
     // the graph schedule's attention keeps the whole bucket in shared memory: steps in buckets past 3264 positions run per op below, and the
     // graph cache re-uploads the device n_past when graph steps resume (after a rewind)
-    // F16 weights decode per op (exact_f16.cu's mat-vec): the graph schedule is built on Q8 activation records
-    if (n == 1 && hp.wtype != T_F16 && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {   // f32 cache: up to 1664 positions
+    // F16 weights decode per op (exact_f16.cu's mat-vec): the graph schedule is built on Q8 activation records.  So do models with a K-quant
+    // matrix or with matrices of more than one type: the graph takes one classic type throughout.
+    if (n == 1 && hp.wtype != T_F16 && m->uniform && !m->any_kquant && neox_decode_fits(s->dp, DecodeGraphCache::bucket(n_kv, n_ctx))) {   // f32 cache: up to 1664 positions
         s->last_launches = s->decode.run(n_kv, n_ctx, true, [s, &hp](int bucket, cudaStream_t st, int *nodes) {
             neox_decode_enqueue(s->dp, s->dl, hp.wtype, bucket, st, nodes);
         }, st);
@@ -207,7 +216,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         s->last_n = 1;
         return;
     }
-    const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get()};
+    const ExactActs acts{s->xq.get(), s->xds.get(), s->xpack.get(), s->xh.get(), s->xq8k.get()};
     const bool kv32 = s->kv_type == T_F32;
     const int64_t ke = (int64_t)s->kv_elem_bytes();
     const bool gptj = m->gptj(), parallel = m->parallel;
@@ -226,6 +235,7 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
         void *Kl = s->kv_at(0, (size_t)il * n_ctx * e), *Vl = s->kv_at(1, (size_t)il * n_ctx * e);
         layer_norm(s->x.get(), s->cur.get(), ly.ln1_g, ly.ln1_b, e, n, st); L++;                                                  // :192-196
         L += mul_mat_exact_auto(ly.wqkv, s->cur.get(), e, n, s->qkv.get(), ld3, nullptr, 0, acts, st);                                // :199
+        if (ly.wv.N) L += mul_mat_exact_auto(ly.wv, s->cur.get(), e, n, s->qkv.get() + voff, ld3, nullptr, 0, acts, st);               // GPT-J v_proj of its own type
         if (ly.bqkv) { add_f32(s->qkv.get(), ly.bqkv, s->qkv.get(), (int64_t)n * ld3, ld3, st); L++; }                            // :200 (MPT: no bias)
         if (rope) {   // RoPE in place on q and k: mode 2 (GPT-NeoX :205-228), mode 0 (GPT-J :178-201)
             rope_f32(s->qkv.get(), s->qkv.get(), hd, n_head, n, hs, ld3, hs, ld3, n_past, *rope, st); L++;
@@ -292,44 +302,121 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     s->n_past += n;
 }
 
-// hp->arch 0 / 1 / 4 (b200_neox_new) or 2 / 3 (b200_neox_new_alibi, alibi_bias_max: the ALiBi bias of MPT's header, 8 for BLOOM).
-// GPT-NeoX and GPT-J rotate: n_rot even, positive and at most the head size (the asserts of ggml_rope, LC/ggml.c:11807-11808)
-b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max) {
-    if (!hp || !is_qweight_type(hp->wtype) || hp->n_embd % 64 || hp->n_head <= 0 || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0 ||
-        ((hp->arch == 0 || hp->arch == 4) && (hp->n_rot <= 0 || hp->n_rot % 2 || hp->n_rot > hp->n_embd / hp->n_head))) return nullptr;
-    rt().ensure_init();
+// a tensor's whole name: the model's own, or the layer prefix of layer il (layer_fmt up to its "%95s") followed by the suffix
+std::string full_name(const ArchTensors &a, const char *name, int il) {
+    if (il < 0) return name;
+    const std::string pre(a.layer_fmt, strstr(a.layer_fmt, "%95s") - a.layer_fmt);
+    char buf[64];
+    snprintf(buf, sizeof(buf), pre.c_str(), il);
+    return std::string(buf) + name;
+}
+
+// hp->arch 0 .. 4; alibi_bias_max: MPT's header float, 8 for BLOOM (ignored by the others); rope_freq_base / scale <= 0: 10000 / 1.
+// GPT-NeoX and GPT-J rotate: n_rot even, positive and at most the head size (the asserts of ggml_rope, LC/ggml.c:11807-11808).
+// Every matrix is of hp->wtype unless types[0, n_types) names it (the model file's per-tensor types); every refusal comes before any allocation.
+b200_neox_model *neox_new(const b200_neox_hparams *hp, float alibi_bias_max, float rope_freq_base, float rope_freq_scale, const b200_tensor_type *types,
+                          int32_t n_types, int *err) {
+    int dummy; if (!err) err = &dummy;
+    *err = B200_ERR_BAD_ARG;
+    if (!hp || hp->arch < 0 || hp->arch > 4 || hp->n_embd % 64 || hp->n_head <= 0 || hp->n_embd % hp->n_head || hp->n_layer <= 0 || hp->context_size <= 0 ||
+        ((hp->arch == 0 || hp->arch == 4) && (hp->n_rot <= 0 || hp->n_rot % 2 || hp->n_rot > hp->n_embd / hp->n_head)) || n_types < 0 || (n_types && !types)) return nullptr;
+    for (int32_t i = 0; i < n_types; i++) if (!types[i].name) return nullptr;
     b200_neox_model *m = new b200_neox_model();
     m->hp = *hp;
-    const int e = hp->n_embd, v = hp->n_vocab, t = hp->wtype, hd = e / hp->n_head;
+    const int e = hp->n_embd, hd = e / hp->n_head;
     m->hd = hd;
     m->layers.resize(hp->n_layer);
+    // the type of every matrix in slab order (mt), and each layer's separate v_proj type (vt, -1: v_proj is the last third of the fused qkv)
+    const ArchTensors &arch = arch_tensors(hp->arch);
+    std::vector<uint8_t> used((size_t)n_types, 0);
+    auto type_of = [&](const std::string &name) {
+        int t = hp->wtype;
+        for (int32_t i = 0; i < n_types; i++) if (!strcmp(types[i].name, name.c_str())) { t = types[i].type; used[(size_t)i] = 1; }
+        return t;
+    };
+    std::vector<int> mt, vt((size_t)hp->n_layer, -1);
+    bool f16 = false, other = false;
+    int rc = B200_OK;
+    size_t fused = 0;                                   // mt's entry of the layer's nameless fused matrix (GPT-J's wqkv)
+    m->each_tensor([&](const auto &d, auto &, int il) {
+        if (rc != B200_OK || (d.kind != MAT && d.kind != ROWS)) return;
+        if (!d.name) { fused = mt.size(); mt.push_back(-1); return; }      // typed by its rows
+        const std::string name = full_name(arch, d.name, il);
+        const int t = type_of(name);
+        if (!is_qweight_type(t) && !is_kquant(t)) {
+            fprintf(stderr, "llm_b200: %s is element type %d; 2-D weights are F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0 or Q2_K..Q6_K\n", name.c_str(), t);
+            rc = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; return;
+        }
+        const int64_t ne0 = d.kind == ROWS ? e : m->dim(d.K);
+        if (is_kquant(t) && ne0 % 256) {
+            fprintf(stderr, "llm_b200: %s: a K-quant row of %lld elements is not whole super-blocks of 256\n", name.c_str(), (long long)ne0);
+            rc = B200_ERR_INVARIANT_BROKEN; return;
+        }
+        (t == T_F16 ? f16 : other) = true;
+        if (d.kind == MAT) { mt.push_back(t); return; }
+        if (d.at == 0) mt[fused] = t;                   // q_proj types the fused matrix
+        else if (d.at == 1 && t != mt[fused]) {         // [q_proj | k_proj] is one matrix: no quantizer the reference ships writes them in two types
+            fprintf(stderr, "llm_b200: %s is of another element type than the layer's q_proj\n", name.c_str());
+            rc = B200_ERR_UNSUPPORTED_ELEMENT_TYPE;
+        } else if (d.at == 2 && t != mt[fused]) vt[(size_t)il] = t;
+    });
+    for (int32_t i = 0; i < n_types && rc == B200_OK; i++)
+        if (!used[(size_t)i]) { fprintf(stderr, "llm_b200: %s is not a matrix of this model\n", types[i].name); rc = B200_ERR_UNKNOWN_TENSOR; }
+    // F16 weights come as whole F16 files: an F16 matrix beside block-format ones is refused (as for LLaMA)
+    if (rc == B200_OK && f16 && other) { fprintf(stderr, "llm_b200: F16 weights beside weights of other element types: F16 models are F16 throughout\n"); rc = B200_ERR_UNSUPPORTED_ELEMENT_TYPE; }
+    if (rc != B200_OK) { *err = rc; delete m; return nullptr; }
+    for (int t : mt) { m->uniform &= t == hp->wtype; m->any_kquant |= is_kquant(t); }
+    for (int t : vt) { m->uniform &= t < 0; m->any_kquant |= is_kquant(t); }
+    rt().ensure_init();
     int n_slots = 0;
     m->each_tensor([&n_slots](const auto &d, auto &, int) { n_slots += d.name != nullptr; });
-    m->carve(t, n_slots, [m](SlabCarver &c) {
-        m->each_tensor([&](const auto &d, auto &o, int) {
-            if (d.kind == MAT) c.q(o.*d.q, m->dim(d.K), m->dim(d.N));
+    // with one type for every matrix this is the layout of a one-type model: same matrices, same order, same bytes
+    m->carve(hp->wtype, n_slots, [m, &mt, &vt, e](SlabCarver &c) {
+        size_t k = 0;
+        m->each_tensor([&](const auto &d, auto &o, int il) {
+            if (d.kind == MAT) {
+                const bool split = !d.name && vt[(size_t)il] >= 0;
+                c.q(o.*d.q, m->dim(d.K), split ? 2 * (int64_t)e : m->dim(d.N), mt[k++]);
+                if (split) c.q(m->layers[il].wv, e, e, vt[(size_t)il]);
+            }
             else if (d.kind != ROWS) c.f(o.*d.f, m->dim(d.K));
         });
     });
     // no output matrix (GPT-2 without model/lm_head, gpt2 lib.rs:319-320; MPT): the output projection is tied to wte, which is streamed as the lm_head
+    // in wte's type
     if (!m->lm_head.qs) m->lm_head = m->wte;
-    else m->weight_bytes -= (size_t)v * (e / QK) * qweight_block_bytes(t);  // the embedding table is gathered from, not streamed
+    else m->weight_bytes -= (size_t)hp->n_vocab * m->wte.nb * qweight_block_bytes(m->wte.type);  // the embedding table is gathered from, not streamed
     if (m->mpt() || m->bloom()) {
         const std::vector<float> slopes = alibi_slopes(hp->n_head, alibi_bias_max);
         m->alibi = device_alloc<float>(slopes.size() * 4);
         B200_CHECK(cudaMemcpy(m->alibi.get(), slopes.data(), slopes.size() * 4, cudaMemcpyHostToDevice));
     }
     // GPT-NeoX: mode 2 on n_rot of every head; GPT-J: mode 0 over ALL hd elements of the head with theta_scale base^(-2/n_rot) (gptj lib.rs:178-201,
-    // LC/ggml.c:11859-11874 walks ne0, not n_dims)
-    if (m->neox() || m->gptj()) m->rope = &rope_table(hp->n_rot, m->neox() ? 2 : 0, 10000.0f, 1.0f, hd, hp->context_size);
+    // LC/ggml.c:11859-11874 walks ne0, not n_dims).  ModelParameters::rope_overrides: ggml_rope_custom_inplace's base and scale (context.rs:558-590)
+    if (m->neox() || m->gptj())
+        m->rope = &rope_table(hp->n_rot, m->neox() ? 2 : 0, rope_freq_base > 0.f ? rope_freq_base : 10000.0f, rope_freq_scale > 0.f ? rope_freq_scale : 1.0f,
+                              hd, hp->context_size);
     // where q / k / v of head h live inside a row of the fused projection: GPT-NeoX per head [q | k | v], the others the three thirds of the row
     m->qkv_layout = m->neox() ? QkvLayout{3 * hd, hd, 2 * hd} : QkvLayout{hd, e, 2 * e};
     m->parallel = m->neox() && hp->use_parallel_residual;
     m->kq_scale = 1.0f / sqrtf((float)e / (float)hp->n_head);                                                                   // gptneox lib.rs:270-273
+    *err = B200_OK;
     return m;
 }
 
 }  // namespace
+
+// a 2-D weight a model of architecture `arch` (b200_neox_hparams.arch) and n_layer layers holds: a MAT or ROWS entry of its tensor table
+bool b200::neox_matrix_name(int arch, const char *name, int n_layer) {
+    if (arch < 0 || arch > 4) return false;
+    const ArchTensors &a = arch_tensors(arch);
+    auto matrix = [](const auto &d, const char *n) { return d.name && (d.kind == MAT || d.kind == ROWS) && !strcmp(n, d.name); };
+    for (const TensorDef<Model> &d : a.globals) if (matrix(d, name)) return true;
+    int il = -1, used = 0; char sub[96];
+    if (sscanf(name, (std::string(a.layer_fmt) + "%n").c_str(), &il, sub, &used) != 2 || il < 0 || il >= n_layer || name[used]) return false;
+    for (const TensorDef<Layer> &d : a.layer) if (matrix(d, sub)) return true;
+    return false;
+}
 
 // ggml_compute_forward_alibi_f32 (LC/ggml.c:11570-11588), the slope of head k.  libm powf on the host, as the reference's CPU build calls it:
 // the same glibc gives the same bits, which CUDA's powf does not promise.
@@ -344,11 +431,21 @@ std::vector<float> b200::alibi_slopes(int n_head, float max_bias) {
 
 extern "C" {
 
-b200_neox_model *b200_neox_new(const b200_neox_hparams *hp) { return hp && (hp->arch == 0 || hp->arch == 1 || hp->arch == 4) ? neox_new(hp, 0.0f) : nullptr; }
-
-b200_neox_model *b200_neox_new_alibi(const b200_neox_hparams *hp, float alibi_bias_max) {
-    return hp && (hp->arch == 2 || hp->arch == 3) ? neox_new(hp, alibi_bias_max) : nullptr;   // MPT, BLOOM
+// the untyped forms: one classic or F16 type for every matrix, the default RoPE
+b200_neox_model *b200_neox_new(const b200_neox_hparams *hp) {
+    return hp && (hp->arch == 0 || hp->arch == 1 || hp->arch == 4) && is_qweight_type(hp->wtype) ? neox_new(hp, 0.0f, 0.0f, 0.0f, nullptr, 0, nullptr) : nullptr;
 }
+
+b200_neox_model *b200_neox_new_alibi(const b200_neox_hparams *hp, float alibi_bias_max) {   // MPT, BLOOM
+    return hp && (hp->arch == 2 || hp->arch == 3) && is_qweight_type(hp->wtype) ? neox_new(hp, alibi_bias_max, 0.0f, 0.0f, nullptr, 0, nullptr) : nullptr;
+}
+
+b200_neox_model *b200_neox_new_typed(const b200_neox_hparams *hp, float alibi_bias_max, float rope_freq_base, float rope_freq_scale,
+                                     const b200_tensor_type *types, int32_t n, int *err) {
+    return neox_new(hp, alibi_bias_max, rope_freq_base, rope_freq_scale, types, n, err);
+}
+
+int b200_neox_is_loaded(b200_neox_model *m) { return m && m->all_loaded(); }
 
 size_t b200_neox_weight_bytes(b200_neox_model *m) { return m ? m->weight_bytes : 0; }
 
@@ -379,8 +476,8 @@ int b200_neox_load_tensor_lora(b200_neox_model *m, const char *name, int32_t typ
 int b200_neox_synthesize(b200_neox_model *m, uint64_t seed) {
     if (!m) return B200_ERR_BAD_ARG;
     m->synthesize(seed, [m](SeedSeq &r) {
-        m->each_tensor([&](const auto &d, auto &o, int) {
-            if (d.kind == MAT) r.q(o.*d.q);
+        m->each_tensor([&](const auto &d, auto &o, int il) {
+            if (d.kind == MAT) { r.q(o.*d.q); if (!d.name && m->layers[il].wv.N) r.q(m->layers[il].wv); }
             else if (d.kind == GAIN) r.gain(o.*d.f, m->dim(d.K));
             else if (d.kind == BIAS) r.bias(o.*d.f, m->dim(d.K));
         });
@@ -411,6 +508,7 @@ b200_neox_session *b200_neox_start_session_flags(b200_neox_model *m, int32_t n_b
     s->xq = device_alloc<int8_t>(B * 4 * e); s->xds = device_alloc<float2>(B * (4 * e / QK) * sizeof(float2));
     s->xpack = device_alloc<int4>((4 * e / QK) * 64); s->xh = device_alloc<__half>(xh_bytes(4 * e, B));
     s->qdec = device_alloc<float>(e * 4);
+    if (m->any_kquant) s->xq8k = device_alloc<char>(q8k_bytes(4 * e, B));           // the widest K: fc_out's 4 n_embd
     s->xpack_a = device_alloc<int4>((e / QK) * 64); s->xpack_d = device_alloc<int4>((e / QK) * 64); s->xpack_f = device_alloc<int4>((4 * e / QK) * 64);
     s->dl.resize(hp.n_layer);
     for (int il = 0; il < hp.n_layer; il++) {

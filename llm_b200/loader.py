@@ -4,6 +4,7 @@ Mirrors the reference's loading surface:
   ggml::format::load / TensorLoadInfo     crates/ggml/src/format/loader.rs:160-281          -> GgmlFile
   ggml::format::save                       crates/ggml/src/format/saver.rs:86-160            -> write_llama
   llm::load::<Llama>(path, params)         crates/llm-base/src/loader.rs:419-567             -> load
+  llm::load_dynamic(architecture, ...)     crates/llm/src/lib.rs:214                          -> load_dynamic
   LoadError variants                       crates/ggml/src/format/loader.rs:38-70            -> LoadError.kind
 The parser runs without a GPU; `load` needs one (the tensors go straight from the file mapping to HBM).
 """
@@ -155,9 +156,11 @@ def write_llama(path: str, hyperparameters: Dict[str, int], tensors: Dict[str, n
 
 
 def write_model(path: str, arch: str, header: Dict[str, int], tensors: Dict[str, np.ndarray], shapes: Dict[str, Tuple[int, ...]], wtype: int,
-                vocabulary: Optional[Sequence[Tuple[bytes, float]]] = None):
-    """ggml::format::save for any of the architectures: `header` holds the words of HPARAM_NAMES[arch] (FLOAT_WORDS as floats)."""
+                vocabulary: Optional[Sequence[Tuple[bytes, float]]] = None, tensor_types: Optional[Dict[str, int]] = None):
+    """ggml::format::save for any of the architectures: `header` holds the words of HPARAM_NAMES[arch] (FLOAT_WORDS as floats).  Tensors that are
+    not f32 are of `wtype`, or of tensor_types[name] (enum ggml_type) when it names them."""
     L = _lib.lib()
+    tensor_types = tensor_types or {}
     words = [_f32_bits(header[k]) if k in FLOAT_WORDS else int(header["n_vocab"]) if k == "n_vocab_again" else int(header[k]) for k in HPARAM_NAMES[arch]]
     infos = (_lib.GgmlTensorInfo * len(tensors))()
     datas = (C.c_void_p * len(tensors))()
@@ -167,7 +170,7 @@ def write_model(path: str, arch: str, header: Dict[str, int], tensors: Dict[str,
         keep.append(a)
         shp = shapes[name]
         infos[i].name = name.encode()
-        infos[i].type = 0 if a.dtype == np.float32 else wtype
+        infos[i].type = 0 if a.dtype == np.float32 else int(tensor_types.get(name, wtype))
         infos[i].n_dims = len(shp)
         infos[i].ne[0] = shp[-1]
         infos[i].ne[1] = shp[0] if len(shp) == 2 else 1
@@ -213,4 +216,68 @@ def load(path: str, params: ModelParameters = None, device: int = 0) -> Llama:
     model = Llama.__new__(Llama)
     model.L, model.hyperparameters, model.params, model._m = L, hp, params, m
     model.vocabulary = vocabulary                                  # eot_token_id()
+    return model
+
+
+def neox_hyperparameters(f: GgmlFile) -> Dict[str, int]:
+    """The GPT-NeoX-family view of a file's header (b200_ggml_neox_hparams): the hyperparameters the architecture's class takes, the type of the
+    file's first 2-D weight as wtype, has_lm_head (GPT-2), alibi_bias_max (MPT's header float, 8 for BLOOM) and the quantization version."""
+    from . import neox
+    L = neox._bind(f.L)
+    hp, bias, qv = neox.NeoxHparams(), C.c_float(), C.c_int32()
+    rc = L.b200_ggml_neox_hparams(f._f, C.byref(hp), C.byref(bias), C.byref(qv))
+    if rc != 0:
+        raise LoadError(rc, f"hyperparameters of {f.path}")
+    out = {k: getattr(hp, k) for k in ("n_vocab", "n_embd", "n_head", "n_layer", "n_rot", "use_parallel_residual", "wtype", "arch", "has_lm_head")}
+    out.update(n_ctx=hp.context_size, alibi_bias_max=bias.value, quantization_version=qv.value)
+    return out
+
+
+def weight_types(f: GgmlFile) -> Dict[str, int]:
+    """{name: enum ggml_type} of every 2-D weight of the file that its architecture's model holds: the table the loaders build (b200_ggml_weight_types)"""
+    from . import neox
+    L = neox._bind(f.L)
+    n = L.b200_ggml_weight_types(f._f, None, 0)
+    if n < 0:
+        raise LoadError(n, f"weight types of {f.path}")
+    tab = (_lib.TensorType * max(1, n))()
+    L.b200_ggml_weight_types(f._f, tab, n)
+    return {tab[i].name.decode(): tab[i].type for i in range(n)}
+
+
+def load_dynamic(architecture: str, path: str, params: ModelParameters = None, device: int = 0):
+    """llm::load_dynamic: "llama" is `load`; "gptneox", "gpt2", "mpt", "bloom" and "gptj" parse the file, create the model for its header with every
+    2-D weight's type from the file, and upload every tensor from the mapping to HBM, patched by params.lora_adapters (in order) where they name it.
+    params.context_size (GPT-2: the header's n_ctx, the rows of model/wpe), rope_freq_base and rope_freq_scale (GPT-NeoX, GPT-J) are honoured.
+    Returns a Llama, GptNeoX, Gpt2, Mpt, Bloom or GptJ with the file's vocabulary."""
+    if architecture == "llama":
+        return load(path, params, device)
+    from . import neox
+    classes = {"gptneox": neox.GptNeoX, "gpt2": neox.Gpt2, "mpt": neox.Mpt, "bloom": neox.Bloom, "gptj": neox.GptJ}
+    if architecture not in classes:
+        raise ValueError(f"unknown architecture {architecture!r}: one of llama, {', '.join(classes)}")
+    params = params or ModelParameters()
+    if not params.use_gpu:
+        raise ValueError("llm_b200 has no CPU path: ModelParameters.use_gpu must be True")
+    L = neox._bind(_lib.lib())
+    rc = L.b200_init(device)
+    if rc != 0:
+        raise RuntimeError(f"b200_init failed with code {rc}")
+    f = GgmlFile(path, architecture)
+    hp = neox_hyperparameters(f)
+    vocabulary = [t for t, _ in f.vocabulary()]
+    f.close()
+    err = C.c_int(0)
+    adapters = params.lora_adapters or []
+    paths = (C.c_char_p * max(1, len(adapters)))(*[p.encode() for p in adapters])
+    m = L.b200_neox_load_file(path.encode(), ARCH[architecture], params.context_size, params.rope_freq_base, params.rope_freq_scale, paths,
+                              len(adapters), C.byref(err))
+    if not m:
+        raise LoadError(err.value, f"load {path}")
+    cls = classes[architecture]
+    model = cls.__new__(cls)
+    model.L, model._m, model.vocabulary = L, m, vocabulary
+    model.hyperparameters = hp
+    model.context_size = hp["n_ctx"] if architecture == "gpt2" or params.context_size <= 0 else params.context_size
+    model.rope = (params.rope_freq_base, params.rope_freq_scale)
     return model

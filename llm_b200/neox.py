@@ -28,6 +28,14 @@ def _bind(L):
     L.b200_neox_new.argtypes = [C.POINTER(NeoxHparams)]
     L.b200_neox_new_alibi.restype = vp
     L.b200_neox_new_alibi.argtypes = [C.POINTER(NeoxHparams), C.c_float]
+    L.b200_neox_new_typed.restype = vp
+    L.b200_neox_new_typed.argtypes = [C.POINTER(NeoxHparams), C.c_float, C.c_float, C.c_float, C.POINTER(_lib.TensorType), i32, C.POINTER(C.c_int)]
+    L.b200_neox_is_loaded.argtypes = [vp]
+    L.b200_neox_load_file.restype = vp
+    L.b200_neox_load_file.argtypes = [C.c_char_p, i32, i32, C.c_float, C.c_float, C.POINTER(C.c_char_p), i32, C.POINTER(C.c_int)]
+    L.b200_ggml_neox_hparams.argtypes = [vp, C.POINTER(NeoxHparams), C.POINTER(C.c_float), C.POINTER(i32)]
+    L.b200_ggml_weight_types.restype = C.c_int64
+    L.b200_ggml_weight_types.argtypes = [vp, C.POINTER(_lib.TensorType), C.c_int64]
     L.b200_neox_load_tensor.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
     L.b200_neox_load_tensor_lora.argtypes = [vp, C.c_char_p, i32, i32, C.c_int64, C.c_int64, vp, C.c_size_t, C.POINTER(vp), i32]
     L.b200_neox_synthesize.argtypes = [vp, C.c_uint64]
@@ -64,7 +72,8 @@ def _bind(L):
 
 class GptNeoX(_Native):
     """hyperparameters: n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype.  lora_adapters: LoRA adapter files applied in
-    order to every tensor they name (ModelParameters::lora_adapters)."""
+    order to every tensor they name (ModelParameters::lora_adapters).  tensor_types: {name: enum ggml_type} of 2-D weights whose type is not wtype
+    (mixed-type and K-quant files, b200_neox_new_typed).  rope_freq_base / rope_freq_scale: ModelParameters::rope_overrides (GPT-NeoX and GPT-J)."""
 
     ARCH = 0
     _HANDLE, _FREE = "_m", "b200_neox_free"
@@ -72,12 +81,17 @@ class GptNeoX(_Native):
     BOT_TOKEN: Optional[bytes] = None       # the vocabulary entry bot_token_id() names (MPT, BLOOM); None: the model has no BOS token
     EOT_TOKEN: bytes = b"<|endoftext|>"     # the entry eot_token_id() names (gptneox lib.rs:376-378, gpt2 :353-355, gptj :329-331, mpt :277-279)
 
+    tensor_types: Dict[str, int] = {}           # models loaded from a file: their types are in the C model
+
     def __init__(self, hyperparameters: Dict[str, int], tensors: Dict[str, np.ndarray] = None, context_size: int = None, device: int = 0,
-                 lora_adapters: Optional[List[str]] = None, vocabulary: Optional[Sequence] = None):
+                 lora_adapters: Optional[List[str]] = None, vocabulary: Optional[Sequence] = None, tensor_types: Optional[Dict[str, int]] = None,
+                 rope_freq_base: float = 10000.0, rope_freq_scale: float = 1.0):
         """vocabulary: the model file's tokens (GgmlFile.vocabulary(): (bytes, score) pairs, or bytes), consulted by bot_token_id()"""
         self.L = _bind(_lib.lib())
         _check(self.L.b200_init(device), "b200_init")
         self.hyperparameters = dict(hyperparameters)
+        self.tensor_types = dict(tensor_types or {})
+        self.rope = (float(rope_freq_base), float(rope_freq_scale))
         self.vocabulary = [t[0] if isinstance(t, tuple) else bytes(t) for t in vocabulary] if vocabulary is not None else None
         self.context_size = context_size or hyperparameters["n_ctx"]
         hp = NeoxHparams(n_vocab=hyperparameters["n_vocab"], n_embd=hyperparameters["n_embd"], n_head=hyperparameters["n_head"], n_layer=hyperparameters["n_layer"],
@@ -93,11 +107,11 @@ class GptNeoX(_Native):
             return
         for name, arr in (tensors or {}).items():
             arr = np.ascontiguousarray(arr)
-            typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(hyperparameters["wtype"])
+            typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.tensor_types.get(name, hyperparameters["wtype"]))
             _check(self.L.b200_neox_load_tensor(self._m, name.encode(), typ, arr.ctypes.data_as(C.c_void_p), arr.nbytes), f"load_tensor({name})")
 
     def _load_lora(self, name, arr, ad):
-        typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.hyperparameters["wtype"])
+        typ = 0 if arr.dtype == np.float32 else 1 if arr.dtype == np.float16 else int(self.tensor_types.get(name, self.hyperparameters["wtype"]))
         nd, ne0, ne1 = ggml_dims(arr, typ)
         rc = self.L.b200_neox_load_tensor_lora(self._m, name.encode(), typ, nd, ne0, ne1, arr.ctypes.data_as(C.c_void_p), arr.nbytes, ad.handles, ad.n)
         if rc != 0:
@@ -105,7 +119,17 @@ class GptNeoX(_Native):
             raise LoadError(rc, f"load_tensor({name})")
 
     def _new(self, hp):
-        return self.L.b200_neox_new(C.byref(hp))
+        names = [n.encode() for n in self.tensor_types]
+        table = (_lib.TensorType * max(1, len(names)))(*[_lib.TensorType(n, int(t)) for n, t in zip(names, self.tensor_types.values())])
+        err = C.c_int(0)
+        m = self.L.b200_neox_new_typed(C.byref(hp), self._alibi_bias_max(), self.rope[0], self.rope[1], table, len(names), C.byref(err))
+        if not m and err.value != -2:               # B200_ERR_BAD_ARG: hyperparameters the untyped forms refuse too (ValueError below)
+            from .loader import LoadError
+            raise LoadError(err.value, "b200_neox_new_typed")
+        return m
+
+    def _alibi_bias_max(self):
+        return 0.0
 
     def synthesize(self, seed: int = 0x4E580000):
         _check(self.L.b200_neox_synthesize(self._m, seed), "synthesize")
@@ -148,9 +172,6 @@ class Mpt(GptNeoX):
 
     def _alibi_bias_max(self):
         return float(self.hyperparameters["alibi_bias_max"])
-
-    def _new(self, hp):
-        return self.L.b200_neox_new_alibi(C.byref(hp), self._alibi_bias_max())
 
 
 class Bloom(Mpt):
