@@ -82,10 +82,11 @@ def make_llama_mixed(hp, mix, ref, seed=0x5EED0000, overrides=None):
 
 
 class RefKq(B.RefLib):
-    """the reference ggml + a copy of ref_harness.c whose LLaMA model takes a type per 2-D weight"""
+    """the reference ggml + a copy of ref_harness.c whose LLaMA model takes a type per 2-D weight; kv32=True: the same copy with an F32 KV cache
+    (oracle/kquant_kv32.mk's _ref/libggml_ref_kq_kv32.so; read its caches with oracle.kv32.kv_f32)"""
 
-    def __init__(self):
-        super().__init__("ref_kq")
+    def __init__(self, kv32=False):
+        super().__init__("ref_kq_kv32" if kv32 else "ref_kq")
         self.lib.rk_set_types.argtypes = [C.c_void_p, C.c_int]
 
     def llama_typed(self, hp, tensors, types, n_threads=8, n_batch=512):
@@ -102,5 +103,5 @@ class RefKq(B.RefLib):
             self.lib.rk_set_types(None, 0)
 
 
-def have_ref_kq():
-    return os.path.exists(os.path.join(HERE, "_ref", "libggml_ref_kq.so"))
+def have_ref_kq(kv32=False):
+    return os.path.exists(os.path.join(HERE, "_ref", "libggml_ref_kq_kv32.so" if kv32 else "libggml_ref_kq.so"))

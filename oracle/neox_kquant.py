@@ -4,7 +4,8 @@ without ModelParameters::rope_overrides -- TEST INFRASTRUCTURE.
 make_typed(arch, hp, types, ref) draws the architecture's synthetic model (oracle.synth / alibi / gptj, the same draws as their one-type makers) and
 quantizes each 2-D weight with its own type through the reference's own quantizers (kquant.quantize_as).  ref_typed(arch, hp, tensors, types, rope)
 runs the reference graph of the architecture on it: oracle/neox_kquant.mk's libraries, copies of ref_gpt2.c / ref_alibi.c / ref_gptj.c whose 2-D
-weights take their types from kquant_types.inc and whose RoPE nodes take the overrides of rope_custom.inc.
+weights take their types from kquant_types.inc and whose RoPE nodes take the overrides of rope_custom.inc.  kv32=True: the same graphs on an F32
+KV cache (oracle/kquant_kv32.mk's _ref/*_kq_kv32.so; read their caches with oracle.kv32.kv_f32).
 """
 import ctypes as C
 import os
@@ -14,12 +15,16 @@ import numpy as np
 from . import alibi, gptj, kquant, kv32, synth
 from .bindings import HERE, RefGpt2, RefLib
 
-LIBS = {k: os.path.join(HERE, "_ref", f"libggml_{k}.so") for k in ("ref_nxkq", "alibi_kq", "gptj_kq")}
+LIBS = {k + s: os.path.join(HERE, "_ref", f"libggml_{k}{s}.so") for k in ("ref_nxkq", "alibi_kq", "gptj_kq") for s in ("", "_kv32")}
 ARCHS = ("gptneox", "gpt2", "mpt", "bloom", "gptj")
 
 
-def have_ref():
-    return all(os.path.exists(p) for p in LIBS.values())
+def _kv(kv32):
+    return "_kv32" if kv32 else ""
+
+
+def have_ref(kv32=False):
+    return all(os.path.exists(p) for k, p in LIBS.items() if k.endswith("_kv32") == kv32)
 
 
 def tensor_shapes(arch, hp, lm_head=False):
@@ -61,14 +66,16 @@ def make_typed(arch, hp, base, ref, types=None, lm_head=False, seed=None):
 _libs = {}
 
 
-def ref_lib():
-    """RefLib over _ref/libggml_ref_nxkq.so: the reference's quantizers and the GPT-2 / GPT-NeoX graphs of the typed copy"""
-    if "ref_nxkq" not in _libs:
-        r = RefLib("ref_nxkq")
+def ref_lib(kv32=False):
+    """RefLib over _ref/libggml_ref_nxkq.so (kv32: _ref/libggml_ref_nxkq_kv32.so): the reference's quantizers and the GPT-2 / GPT-NeoX graphs of
+    the typed copy"""
+    key = "ref_nxkq" + _kv(kv32)
+    if key not in _libs:
+        r = RefLib(key)
         r.lib.rk_set_types.argtypes = [C.c_void_p, C.c_int]
         r.lib.rk_set_rope.argtypes = [C.c_float, C.c_float]
-        _libs["ref_nxkq"] = r
-    return _libs["ref_nxkq"]
+        _libs[key] = r
+    return _libs[key]
 
 
 def _lib(key, prefix, params):
@@ -94,8 +101,8 @@ def _lib(key, prefix, params):
 
 
 class _Alibi(alibi.RefAlibi):
-    def __init__(self, hp, tensors, arch, n_threads=8, n_batch=512):
-        self.L, self.hp, self.arch = _lib("alibi_kq", "ra_", alibi.RaParams), dict(hp), arch
+    def __init__(self, hp, tensors, arch, n_threads=8, n_batch=512, f32_cache=False):
+        self.L, self.hp, self.arch = _lib("alibi_kq" + _kv(f32_cache), "ra_", alibi.RaParams), dict(hp), arch
         bias_max = float(hp.get("alibi_bias_max", 8.0)) if arch == alibi.MPT else 8.0
         p = alibi.RaParams(n_threads=n_threads, n_batch=n_batch, arch=arch, alibi_bias_max=bias_max,
                            **{k: int(hp[k]) for k in ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "wtype")})
@@ -103,32 +110,32 @@ class _Alibi(alibi.RefAlibi):
 
 
 class _GptJ(gptj.RefGptJ):
-    def __init__(self, hp, tensors, n_threads=8, n_batch=512):
-        self.L, self.hp = _lib("gptj_kq", "rj_", gptj.RjParams), dict(hp)
+    def __init__(self, hp, tensors, n_threads=8, n_batch=512, f32_cache=False):
+        self.L, self.hp = _lib("gptj_kq" + _kv(f32_cache), "rj_", gptj.RjParams), dict(hp)
         p = gptj.RjParams(n_threads=n_threads, n_batch=n_batch, **{k: int(hp[k]) for k in ("n_vocab", "n_ctx", "n_embd", "n_head", "n_layer", "n_rot", "wtype")})
         kv32._load_tensors(self, self.L.rj_new, self.L.rj_tensor, self.L.rj_finalize, p, tensors)
 
 
 class RefTyped:
     """the reference graph of `arch` on a typed model; rope = (base, scale): the RoPE nodes are ggml_rope_custom_inplace with them (GPT-NeoX, GPT-J).
-    eval / reset / kv / close as the one-type reference models."""
+    kv32: the graph on an F32 KV cache.  eval / reset / kv / close as the one-type reference models."""
 
-    def __init__(self, arch, hp, tensors, types, rope=None, n_threads=8, n_batch=512):
+    def __init__(self, arch, hp, tensors, types, rope=None, n_threads=8, n_batch=512, kv32=False):
         self.arch, self.rope = arch, rope if arch in ("gptneox", "gptj") else None      # the others have no RoPE
         lm_head = "model/lm_head" in tensors
         tab = np.array([types.get(n, hp["wtype"]) for n in matrices(arch, hp, lm_head)], np.int32)
         if arch in ("gpt2", "gptneox"):
-            self.L = ref_lib().lib
+            self.L = ref_lib(kv32).lib
         else:
-            self.L = _lib("gptj_kq", "rj_", gptj.RjParams) if arch == "gptj" else _lib("alibi_kq", "ra_", alibi.RaParams)
+            self.L = _lib("gptj_kq" + _kv(kv32), "rj_", gptj.RjParams) if arch == "gptj" else _lib("alibi_kq" + _kv(kv32), "ra_", alibi.RaParams)
         self.L.rk_set_types(tab.ctypes.data, tab.size)
         try:
             if arch in ("gpt2", "gptneox"):
-                self.m = RefGpt2(ref_lib(), hp, tensors, 0, n_threads, n_batch, arch=1 if arch == "gptneox" else 0)
+                self.m = RefGpt2(ref_lib(kv32), hp, tensors, 0, n_threads, n_batch, arch=1 if arch == "gptneox" else 0)
             elif arch == "gptj":
-                self.m = _GptJ(hp, tensors, n_threads, n_batch)
+                self.m = _GptJ(hp, tensors, n_threads, n_batch, kv32)
             else:
-                self.m = _Alibi(hp, tensors, alibi.MPT if arch == "mpt" else alibi.BLOOM, n_threads, n_batch)
+                self.m = _Alibi(hp, tensors, alibi.MPT if arch == "mpt" else alibi.BLOOM, n_threads, n_batch, kv32)
         finally:
             self.L.rk_set_types(None, 0)
 
