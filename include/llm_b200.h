@@ -247,6 +247,28 @@ int  b200_session_feed_prompt_output(b200_session *s, const int32_t *tokens, int
  * B200_ERR_SAMPLER_FAILURE on a NaN in the row: n_past, the history and the last row are restored; B200_ERR_BAD_ARG: no row evaluated yet,
  * top_k < 1, temperature <= 0, penalty <= 0, a negative last_n, null pointers, a tensor-parallel session.  B200_SESSION_FAST sessions run. */
 int  b200_session_infer_next_token(b200_session *s, const b200_sampler *sampler, int32_t *token_out);
+
+/* ---- batched decode: one step advances many sessions of one LLaMA model (KnownModel is Send + Sync: one model, many sessions) ----------------
+ * The weights are read once per step for all n sessions, and each session's own cache once.  Every session ends exactly as if it had run
+ * b200_session_evaluate(s, &tokens[i], 1, ..) alone: n_past + 1, the id appended to its history, its cache slot n_past written, its last row
+ * (row 0 of its logits, last_n 1) what last_logits, top_k, infer_next_token and get_snapshot read, bit for bit; last_launches is the batched
+ * step's launch count (the same for every n).  A later single-session step uploads the new n_past to its decode graphs.
+ * Refused as a whole, with nothing enqueued and no session changed:
+ *   B200_ERR_BAD_ARG        n < 1 or n > B200_MAX_SESSIONS; a null entry; a session of another model; the same session twice; a tensor-parallel
+ *                           model; a B200_SESSION_FAST session; sessions whose KV cache types differ; a token id outside [0, n_vocab) (evaluate);
+ *                           a sampler b200_session_infer_next_token refuses, or a session with no evaluated row (infer)
+ *   B200_ERR_CONTEXT_FULL   a session with no room, by the rule of the single-session call: n_past + 1 > context_size for evaluate,
+ *                           n_past + 1 >= context_size for infer */
+#define B200_MAX_SESSIONS 64
+/* One decode step for n sessions of model m: session i evaluates tokens[i] at its own n_past.  logits_out: n x n_vocab, nullable. */
+int  b200_model_evaluate_sessions(b200_model *m, b200_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out);
+/* InferenceSession::infer_next_token for n sessions at once: session i samples from its last row with samplers[i] (its own seed and draw), then
+ * one batched step evaluates the sampled ids.  tokens_out[i] (-1 on a failure) and status_out[i]: B200_OK, or B200_ERR_SAMPLER_FAILURE when
+ * session i's row holds a NaN -- that session is not stepped, so its n_past, history, last row and cache are as they were, while the others
+ * advance.  The call returns B200_OK then; end of text is the caller's test on tokens_out[i], as for b200_session_infer_next_token. */
+int  b200_model_infer_next_tokens(b200_model *m, b200_session *const *sessions, int32_t n, const b200_sampler *samplers,
+                                  int32_t *tokens_out, int32_t *status_out);
+
 /* the token ids at positions [0, n_past) -- what every evaluate fed and infer_next_token sampled (InferenceSession::tokens); a rewind truncates
  * them.  Copies min(n_past, max) ids and returns n_past, or a negative error code. */
 int32_t b200_session_read_tokens(b200_session *s, int32_t *tokens_out, int32_t max);

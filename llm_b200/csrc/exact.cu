@@ -144,11 +144,12 @@ constexpr int F16X_WARPS = 8;
 template <bool F32>
 __device__ __forceinline__ void mul_mat_attn_warp(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                                                   const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
-                                                  char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+                                                  char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past,
+                                                  unsigned bx, unsigned by, unsigned bz) {   // the output block (the grid's, or a batched row's)
     using T0 = typename AttnSrc0<F32>::T;
     const int lane = threadIdx.x & 31;
-    const int64_t i0 = (int64_t)blockIdx.x * F16X_WARPS + (threadIdx.x >> 5);
-    const int64_t i1 = blockIdx.y, i2 = blockIdx.z;
+    const int64_t i0 = (int64_t)bx * F16X_WARPS + (threadIdx.x >> 5);
+    const int64_t i1 = by, i2 = bz;
     if (i0 >= ne01) return;
     if (causal_past >= 0 && i0 > causal_past + i1) return;
     const int64_t i02 = i2 / (ne12 / ne02);
@@ -179,12 +180,14 @@ __device__ __forceinline__ void mul_mat_attn_warp(const char *__restrict__ src0,
 __global__ void __launch_bounds__(F16X_WARPS * 32) mul_mat_f16_exact_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                                                                             const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                                                                             char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
-    mul_mat_attn_warp<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+    mul_mat_attn_warp<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past,
+                              blockIdx.x, blockIdx.y, blockIdx.z);
 }
 __global__ void __launch_bounds__(F16X_WARPS * 32) mul_mat_f32_exact_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                                                                             const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                                                                             char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
-    mul_mat_attn_warp<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+    mul_mat_attn_warp<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past,
+                              blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // ---- batched version: shared-memory tiles, 4 threads per dot, 8 dots per thread --------------------------------------------------------
@@ -351,6 +354,50 @@ void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne
                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                        float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st) {
     mul_mat_attn<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past, st);
+}
+
+// ---- the same two mat-muls for a batched decode step: row (session) blockIdx.z of n, each on its own cache and position ---------------------
+// One output per warp, as mul_mat_f16_exact_kernel / mul_mat_f32_exact_kernel with one src1 row: the same dot, chains, tree and leftovers.
+// KQ: grid (max_n_kv / 8, n_head, n); outputs past the row's n_kv exit at once.
+template <bool F32>
+__global__ void __launch_bounds__(F16X_WARPS * 32) attn_kq_rows_kernel(const BatchRow *__restrict__ rows, size_t layer_off, const float *__restrict__ q, int64_t q_ld,
+                                                                       int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ kq) {
+    constexpr int64_t es = F32 ? 4 : 2;
+    const int64_t gqa = (int64_t)n_head_kv * hd;
+    const int z = blockIdx.z, n_past = rows[z].n_past;
+    const char *K = (const char *)rows[z].K + layer_off * es;
+    mul_mat_attn_warp<F32>(K, hd, n_past + 1, n_head_kv, gqa * es, hd * es, (const char *)(q + z * q_ld), 1, n_head, 0, hd * 4,
+                           (char *)(kq + (int64_t)z * n_head * n_ctx), 0, (int64_t)n_ctx * 4, n_past,
+                           blockIdx.x, 0, blockIdx.y);
+}
+// KQV: grid (hd / 8, n_head, n); out row z holds the merged heads [n_head][hd]
+template <bool F32>
+__global__ void __launch_bounds__(F16X_WARPS * 32) attn_kqv_rows_kernel(const BatchRow *__restrict__ rows, size_t layer_off, const float *__restrict__ kq,
+                                                                        int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ out, int64_t ld_out) {
+    constexpr int64_t es = F32 ? 4 : 2;
+    const int z = blockIdx.z;
+    const char *V = (const char *)rows[z].V + layer_off * es;
+    mul_mat_attn_warp<F32>(V, rows[z].n_past + 1, hd, n_head_kv, (int64_t)n_ctx * es, (int64_t)n_ctx * hd * es, (const char *)(kq + (int64_t)z * n_head * n_ctx),
+                           1, n_head, 0, (int64_t)n_ctx * 4, (char *)(out + z * ld_out), 0, (int64_t)hd * 4, -1,
+                           blockIdx.x, 0, blockIdx.y);
+}
+
+void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int hd, int n_head, int n_head_kv,
+                  int n_ctx, float *kq, cudaStream_t st) {
+    B200_ASSERT(n >= 1 && n <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
+    const dim3 grid((unsigned)((max_n_kv + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)n);
+    (kv_type == T_F32 ? attn_kq_rows_kernel<true> : attn_kq_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(rows, layer_off, q, q_ld, hd, n_head, n_head_kv,
+                                                                                                                 n_ctx, kq);
+    B200_CHECK(cudaGetLastError());
+}
+
+void attn_kqv_rows(int kv_type, const BatchRow *rows, int n, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx,
+                   float *out, int64_t ld_out, cudaStream_t st) {
+    B200_ASSERT(n >= 1 && n <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
+    const dim3 grid((unsigned)((hd + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)n);
+    (kv_type == T_F32 ? attn_kqv_rows_kernel<true> : attn_kqv_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(rows, layer_off, kq, hd, n_head, n_head_kv,
+                                                                                                                   n_ctx, out, ld_out);
+    B200_CHECK(cudaGetLastError());
 }
 
 }  // namespace b200

@@ -276,6 +276,13 @@ void SessionCore::copy_row(float *out, const float *row, int n) {
     B200_CHECK(cudaStreamSynchronize(st));
 }
 
+void SessionCore::commit_step(int launches) {
+    n_past += 1;
+    last_n = 1;
+    last_launches = launches;
+    decode.dev_n_past = -1;                     // the next graph step uploads n_past
+}
+
 int SessionCore::set_n_past(int v) {
     if (v < 0 || v > n_past) return B200_ERR_BAD_ARG;
     n_past = v;

@@ -175,6 +175,9 @@ struct SessionCore {
     void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)
     void copy_row(float *out, const float *row, int n);                        // n floats of a device row to out (if not null), after the queued work
     int set_n_past(int v);
+    // the host half of committing a step of a batched decode to this session (its device half, history[n_past] and row 0 of the logits, is the
+    // step's commit kernel): n_past + 1, last_n 1, the step's launches, and the decode graphs' device n_past stale
+    void commit_step(int launches);
     // InferenceSession::perplexity over tokens[0, n) with C = n_ctx: chunk i = [iC, (i+1)C) is evaluated from n_past 0 in batches of n_batch, its
     // first token replaced by bos; rows [min(512, C/2), C - 1) are scored on the device (ppl.cu).  forward(rows) runs one batch of the staged
     // tokens at n_past and leaves every row's logits in `logits`.  Each batch's terms are computed on the stream before the next batch overwrites

@@ -177,4 +177,34 @@ void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne
                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                        float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st);
 
+// ---- batched decode over many sessions of one model (session.cu: b200_model_evaluate_sessions) -------------------------------------------
+// Row i of a batched step belongs to its own session: the session's whole memory_k / memory_v ([n_layer][n_ctx][gqa] and [n_layer][gqa][n_ctx],
+// of the step's one cache type), its position n_past (the row's token goes to slot n_past), its logits buffer and history.  Uploaded once per step.
+struct BatchRow { void *K, *V; float *logits; int32_t *hist; int n_past; };
+// rowops.cu: RoPE mode 0 on the n_head + n_head_kv heads of row i of qkv ([n][qkv_ld]: q | k | v) at position rows[i].n_past, in place, and
+// K (roped) / V of the row stored into its session's cache at that slot (layer_off: elements to this layer's slice) -- rope_f32 + cpy_strided
+// of forward() on each row.  One launch.
+void rope_store_rows(float *qkv, int64_t qkv_ld, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off, int n_ctx,
+                     int kv_type, const RopeTable &tab, cudaStream_t st);
+// rowops.cu: kq[i][h][0, n_past_i + 1) = soft_max(scale * kq[i][h][.]) (the row stride is n_ctx), soft_max's arithmetic per row.  One launch.
+void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, cudaStream_t st);
+// exact.cu: KQ and KQV of forward() on each row's own cache, in mul_mat_f16_exact / mul_mat_f32_exact's arithmetic (kv_type T_F16 / T_F32):
+//   kq[i][h][j] = K_i[j][hk] . Q[i][h] for j <= n_past_i (q rows of stride q_ld; kq rows of stride n_ctx, [n][n_head]);
+//   out[i][h * hd + c] = V_i[hk][c][:] . kq[i][h][:]  (out rows of stride ld_out).  max_n_kv: the largest n_past_i + 1.  One launch each.
+void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int hd, int n_head, int n_head_kv,
+                  int n_ctx, float *kq, cudaStream_t st);
+void attn_kqv_rows(int kv_type, const BatchRow *rows, int n, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx,
+                   float *out, int64_t ld_out, cudaStream_t st);
+// sample.cu: sample_row for n sessions in one chain of launches (select, merges, tail), session i taken from the grid.  Each job is one session's
+// row, history window, arguments and buffers; its id, n_kept and result are sample_row's.  jobs: device table of n (the caller uploads it).
+struct SampleJob {
+    const float *row; const int32_t *hist; int n_vocab, n_past;
+    SampleArgs a; SampleBufs b;
+    int32_t *tok_dst, *hist_dst; SampleResult *res;
+};
+// the launches for n jobs of which the widest (most merge levels) has n_vocab ids and top_k candidates; returns the number of launches
+int sample_rows(const SampleJob *jobs, int n, int max_n_vocab, int max_kk, cudaStream_t st);
+// the candidates the chain keeps for top_k: min(top_k, n_vocab, 1024)
+__host__ __device__ inline int sample_kk(int top_k, int n_vocab) { return top_k < n_vocab ? (top_k < 1024 ? top_k : 1024) : (n_vocab < 1024 ? n_vocab : 1024); }
+
 }  // namespace b200

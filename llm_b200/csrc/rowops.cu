@@ -156,11 +156,11 @@ void layer_norm(const float *x, float *y, const float *gain, const float *bias, 
 // multiply-add as the reference's x86 build compiles it)
 template <bool ALIBI>
 __device__ __forceinline__ void soft_max_body(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int do_scale,
-                                              int n_past, int do_mask, int do_softmax, const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi) {
+                                              int n_past, int do_mask, int do_softmax, const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi,
+                                              int64_t r) {
     extern __shared__ float row[];
     __shared__ double shd[32];
     __shared__ float shf[32];
-    const int64_t r = blockIdx.x;
     const int64_t j = r % nr;                       // row index inside its [nc, nr] matrix: mask col > n_past + j
     const float *xr = x + r * nc;
     float *yr = y + r * nc;
@@ -193,11 +193,11 @@ __device__ __forceinline__ void soft_max_body(const float *__restrict__ x, float
 }
 __global__ void soft_max_kernel(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int do_scale,
                                 int n_past, int do_mask, int do_softmax, const uint16_t *__restrict__ t_exp) {
-    soft_max_body<false>(x, y, nc, nr, scale, do_scale, n_past, do_mask, do_softmax, t_exp, nullptr);
+    soft_max_body<false>(x, y, nc, nr, scale, do_scale, n_past, do_mask, do_softmax, t_exp, nullptr, blockIdx.x);
 }
 __global__ void soft_max_alibi_kernel(const float *__restrict__ x, float *__restrict__ y, int64_t nc, int64_t nr, float scale, int n_past,
                                       const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi) {
-    soft_max_body<true>(x, y, nc, nr, scale, 1, n_past, 1, 1, t_exp, alibi);
+    soft_max_body<true>(x, y, nc, nr, scale, 1, n_past, 1, 1, t_exp, alibi, blockIdx.x);
 }
 void soft_max_alibi(const float *x, float *y, int64_t nc, int64_t rows, int64_t nr, float scale, int n_past, const float *alibi, cudaStream_t st) {
     if (rows == 0 || nc == 0) return;
@@ -305,6 +305,12 @@ const RopeTable &rope_table(int n_dims, int mode, float freq_base, float freq_sc
     return cache[key];
 }
 
+// the pair (x0, x1) rotated by c = {cos, sin}:
+// gcc contracts `x0*c - x1*s` to fma(x0, c, -(x1*s)) and `x0*s + x1*c` to fma(x0, s, x1*c) in the reference build
+__device__ __forceinline__ float2 rope_pair(float x0, float x1, float2 c) {
+    return make_float2(__fmaf_rn(x0, c.x, -__fmul_rn(x1, c.y)), __fmaf_rn(x0, c.y, __fmul_rn(x1, c.x)));
+}
+
 // one thread per rotated pair
 __global__ void rope_kernel(const float *x, float *y, int64_t ne0, int64_t ne1, int64_t ne2, int64_t s1, int64_t s2,
                             int64_t ds1, int64_t ds2, int n_past, const float2 *__restrict__ cs, int half, int n_dims, int neox) {
@@ -319,10 +325,9 @@ __global__ void rope_kernel(const float *x, float *y, int64_t ne0, int64_t ne1, 
     else { const int hb = n_dims / 2; const int ib = i / hb, ic = i % hb; e0 = (int64_t)ib * n_dims + ic; e1 = e0 + hb; }
     const float *src = x + i2 * s2 + i1 * s1;
     float *dst = y + i2 * ds2 + i1 * ds1;
-    const float x0 = src[e0], x1 = src[e1];
-    // gcc contracts `x0*c - x1*s` to fma(x0, c, -(x1*s)) and `x0*s + x1*c` to fma(x0, s, x1*c) in the reference build
-    dst[e0] = __fmaf_rn(x0, c.x, -__fmul_rn(x1, c.y));
-    dst[e1] = __fmaf_rn(x0, c.y, __fmul_rn(x1, c.x));
+    const float2 r = rope_pair(src[e0], src[e1], c);
+    dst[e0] = r.x;
+    dst[e1] = r.y;
 }
 void rope_f32(const float *x, float *y, int64_t ne0, int64_t ne1, int64_t ne2, int64_t s1, int64_t s2, int64_t ds1, int64_t ds2,
               int n_past, const RopeTable &tab, cudaStream_t st) {
@@ -354,6 +359,63 @@ void cpy_strided(const void *src, int src_type, const StridedDesc &s, void *dst,
     B200_ASSERT((src_type == T_F32 || src_type == T_F16) && (dst_type == T_F32 || dst_type == T_F16));
     if (n == 0) return;
     cpy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const char *)src, src_type, s, (char *)dst, dst_type, d, n);
+    B200_CHECK(cudaGetLastError());
+}
+
+// ---- batched decode rows (kernels.cuh: BatchRow) ------------------------------------------------------------------------------
+// soft_max of row (blockIdx.y, head blockIdx.x): soft_max_body on its n_past + 1 scores, scaled, one row per matrix (the mask keeps them all)
+__global__ void soft_max_rows_kernel(float *__restrict__ kq, const BatchRow *__restrict__ rows, int n_head, int n_ctx, float scale, const uint16_t *__restrict__ t_exp) {
+    const int n_past = rows[blockIdx.y].n_past;
+    float *x = kq + ((int64_t)blockIdx.y * n_head + blockIdx.x) * n_ctx;
+    soft_max_body<false>(x, x, n_past + 1, 1, scale, 1, n_past, 1, 1, t_exp, nullptr, 0);
+}
+void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, cudaStream_t st) {
+    const size_t smem = (size_t)n_ctx * sizeof(float);
+    static size_t smem_set = 48 * 1024;
+    if (smem > smem_set) {
+        B200_ASSERT(smem <= 200 * 1024);
+        B200_CHECK(cudaFuncSetAttribute(soft_max_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        smem_set = smem;
+    }
+    soft_max_rows_kernel<<<dim3((unsigned)n_head, (unsigned)n), 256, smem, st>>>(kq, rows, n_head, n_ctx, scale, luts().exp);
+    B200_CHECK(cudaGetLastError());
+}
+
+// thread t of row i: t < (n_head + n_head_kv) * half rotates one pair of a Q or K head (a K pair is also stored at slot n_past of the row's
+// memory_k); the next gqa threads store one V value each at slot n_past of the row's memory_v (transposed: [gqa][n_ctx])
+template <typename KT>
+__global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, int hd, int n_head, int n_head_kv, const BatchRow *__restrict__ rows,
+                                       size_t layer_off, int n_ctx, const float2 *__restrict__ cs, int half, int64_t per_row, int64_t total) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int64_t z = t / per_row, k = t - z * per_row;
+    const int n_past = rows[z].n_past;
+    const int64_t e = (int64_t)n_head * hd, gqa = (int64_t)n_head_kv * hd, n_pairs = (int64_t)(n_head + n_head_kv) * half;
+    float *row = qkv + z * qkv_ld;
+    if (k < n_pairs) {
+        const int i = (int)(k % half);
+        const int64_t head = k / half, e0 = head * hd + 2 * (int64_t)i;
+        const float2 r = rope_pair(row[e0], row[e0 + 1], __ldg(cs + (int64_t)n_past * half + i));
+        row[e0] = r.x;
+        row[e0 + 1] = r.y;
+        if (head >= n_head) {
+            KT *K = (KT *)rows[z].K + layer_off + (size_t)n_past * gqa + (e0 - e);
+            if constexpr (sizeof(KT) == 2) { K[0] = __float2half_rn(r.x); K[1] = __float2half_rn(r.y); } else { K[0] = r.x; K[1] = r.y; }
+        }
+    } else {
+        const int64_t c = k - n_pairs;
+        const float v = row[e + gqa + c];
+        KT *V = (KT *)rows[z].V + layer_off + (size_t)c * n_ctx + n_past;
+        if constexpr (sizeof(KT) == 2) *V = __float2half_rn(v); else *V = v;
+    }
+}
+void rope_store_rows(float *qkv, int64_t qkv_ld, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off, int n_ctx,
+                     int kv_type, const RopeTable &tab, cudaStream_t st) {
+    B200_ASSERT(tab.ne0 == hd && tab.mode == 0 && hd % 2 == 0 && n_ctx <= tab.n_pos);
+    const int64_t per_row = (int64_t)(n_head + n_head_kv) * tab.half + (int64_t)n_head_kv * hd, total = per_row * n;
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (kv_type == T_F32) rope_store_rows_kernel<float><<<grid, 256, 0, st>>>(qkv, qkv_ld, hd, n_head, n_head_kv, rows, layer_off, n_ctx, tab.cs, tab.half, per_row, total);
+    else rope_store_rows_kernel<__half><<<grid, 256, 0, st>>>(qkv, qkv_ld, hd, n_head, n_head_kv, rows, layer_off, n_ctx, tab.cs, tab.half, per_row, total);
     B200_CHECK(cudaGetLastError());
 }
 

@@ -46,11 +46,13 @@ __device__ __forceinline__ void sort_desc(uint64_t *s, int n = TILE) {
         }
 }
 
-__global__ void __launch_bounds__(THREADS) sample_select_kernel(const float *__restrict__ row, int n_vocab, const int32_t *__restrict__ hist, int lo, int hi,
-                                                                float penalty, int kk, uint64_t *__restrict__ out, int *fail) {
+// the kernels' bodies take their CTA's index `blk`: the single-row kernels pass blockIdx.x, the many-row ones (sample_rows) blockIdx.x of the
+// row blockIdx.y
+__device__ __forceinline__ void sample_select(const float *__restrict__ row, int n_vocab, const int32_t *__restrict__ hist, int lo, int hi,
+                                              float penalty, int kk, uint64_t *__restrict__ out, int *fail, unsigned blk) {
     __shared__ uint64_t s[TILE];
     __shared__ uint32_t mark[TILE / 32];          // ids of this slice in the penalty window
-    const int base = blockIdx.x * TILE, tid = threadIdx.x;
+    const int base = blk * TILE, tid = threadIdx.x;
     for (int t = tid; t < TILE / 32; t += THREADS) mark[t] = 0;
     __syncthreads();
     for (int j = lo + tid; j < hi; j += THREADS) {
@@ -72,16 +74,23 @@ __global__ void __launch_bounds__(THREADS) sample_select_kernel(const float *__r
     }
     if (__syncthreads_or(nan) && tid == 0) atomicOr(fail, 1);
     sort_desc(s);
-    for (int t = tid; t < kk; t += THREADS) out[(size_t)blockIdx.x * kk + t] = s[t];
+    for (int t = tid; t < kk; t += THREADS) out[(size_t)blk * kk + t] = s[t];
+}
+__global__ void __launch_bounds__(THREADS) sample_select_kernel(const float *__restrict__ row, int n_vocab, const int32_t *__restrict__ hist, int lo, int hi,
+                                                                float penalty, int kk, uint64_t *__restrict__ out, int *fail) {
+    sample_select(row, n_vocab, hist, lo, hi, penalty, kk, out, fail, blockIdx.x);
 }
 
-__global__ void __launch_bounds__(THREADS) sample_merge_kernel(const uint64_t *__restrict__ in, int n, int kk, uint64_t *__restrict__ out) {
+__device__ __forceinline__ void sample_merge(const uint64_t *__restrict__ in, int n, int kk, uint64_t *__restrict__ out, unsigned blk) {
     __shared__ uint64_t s[TILE];
-    const int base = blockIdx.x * TILE;
+    const int base = blk * TILE;
     for (int t = threadIdx.x; t < TILE; t += THREADS) s[t] = base + t < n ? in[base + t] : 0;
     __syncthreads();
     sort_desc(s);
-    for (int t = threadIdx.x; t < kk; t += THREADS) out[(size_t)blockIdx.x * kk + t] = s[t];
+    for (int t = threadIdx.x; t < kk; t += THREADS) out[(size_t)blk * kk + t] = s[t];
+}
+__global__ void __launch_bounds__(THREADS) sample_merge_kernel(const uint64_t *__restrict__ in, int n, int kk, uint64_t *__restrict__ out) {
+    sample_merge(in, n, kk, out, blockIdx.x);
 }
 
 struct TailArgs {
@@ -90,9 +99,9 @@ struct TailArgs {
     uint64_t seed, draw;
 };
 
-__global__ void __launch_bounds__(THREADS) sample_tail_kernel(const uint64_t *__restrict__ in, int n, TailArgs a, const float *__restrict__ row, int *fail,
-                                                              SampleResult *res, int32_t *tok_dst, int32_t *hist_dst, int32_t *cand_ids, float *cand_vals,
-                                                              float *cand_probs, float *backup) {
+__device__ __forceinline__ void sample_tail(const uint64_t *__restrict__ in, int n, const TailArgs &a, const float *__restrict__ row, int *fail,
+                                            SampleResult *res, int32_t *tok_dst, int32_t *hist_dst, int32_t *cand_ids, float *cand_vals,
+                                            float *cand_probs, float *backup) {
     __shared__ uint64_t s[TILE];
     __shared__ int failed, n_kept;
     __shared__ float S;
@@ -155,10 +164,62 @@ __global__ void __launch_bounds__(THREADS) sample_tail_kernel(const uint64_t *__
         }
     }
 }
+__global__ void __launch_bounds__(THREADS) sample_tail_kernel(const uint64_t *__restrict__ in, int n, TailArgs a, const float *__restrict__ row, int *fail,
+                                                              SampleResult *res, int32_t *tok_dst, int32_t *hist_dst, int32_t *cand_ids, float *cand_vals,
+                                                              float *cand_probs, float *backup) {
+    sample_tail(in, n, a, row, fail, res, tok_dst, hist_dst, cand_ids, cand_vals, cand_probs, backup);
+}
+
+// ---- many rows (sample_rows): job blockIdx.y, or blockIdx.x for the tail -----------------------------------------------------------
+// A job's chain: select over ceil(n_vocab / TILE) CTAs into keys[0], then merge levels while more than TILE candidates are left, each from
+// keys[l & 1] into keys[(l + 1) & 1], then the tail on keys[levels & 1] -- sample_row's launches, in the same buffers.
+__device__ __forceinline__ int job_lo(const SampleJob &j) {
+    return j.a.penalty == 1.0f || j.a.last_n <= 0 ? j.n_past : (j.n_past > j.a.last_n ? j.n_past - j.a.last_n : 0);
+}
+__global__ void __launch_bounds__(THREADS) sample_select_rows_kernel(const SampleJob *__restrict__ jobs) {
+    const SampleJob &j = jobs[blockIdx.y];
+    if ((int)blockIdx.x * TILE >= j.n_vocab) return;
+    sample_select(j.row, j.n_vocab, j.hist, job_lo(j), j.n_past, j.a.penalty, sample_kk(j.a.top_k, j.n_vocab), j.b.keys[0], j.b.fail, blockIdx.x);
+}
+// merge level `level` (0-based) of every job that has one
+__global__ void __launch_bounds__(THREADS) sample_merge_rows_kernel(const SampleJob *__restrict__ jobs, int level) {
+    const SampleJob &j = jobs[blockIdx.y];
+    const int kk = sample_kk(j.a.top_k, j.n_vocab);
+    int n = (j.n_vocab + TILE - 1) / TILE * kk;
+    for (int l = 0; l < level && n > TILE; l++) n = (n + TILE - 1) / TILE * kk;
+    if (n <= TILE || (int)blockIdx.x * TILE >= n) return;
+    sample_merge(j.b.keys[level & 1], n, kk, j.b.keys[(level + 1) & 1], blockIdx.x);
+}
+__global__ void __launch_bounds__(THREADS) sample_tail_rows_kernel(const SampleJob *__restrict__ jobs) {
+    const SampleJob &j = jobs[blockIdx.x];
+    const int kk = sample_kk(j.a.top_k, j.n_vocab);
+    int n = (j.n_vocab + TILE - 1) / TILE * kk, cur = 0;
+    while (n > TILE) { n = (n + TILE - 1) / TILE * kk; cur ^= 1; }
+    const TailArgs t{j.n_vocab, kk, j.a.top_p, j.a.temperature, j.a.seed, j.a.draw};
+    sample_tail(j.b.keys[cur], n, t, j.row, j.b.fail, j.res, j.tok_dst, j.hist_dst, nullptr, nullptr, nullptr, j.b.backup);
+}
 
 }  // namespace
 
 size_t sample_key_bytes(int n_vocab) { return (size_t)((n_vocab + TILE - 1) / TILE) * 1024 * sizeof(uint64_t); }
+
+int sample_rows(const SampleJob *jobs, int n, int max_n_vocab, int max_kk, cudaStream_t st) {
+    B200_ASSERT(n >= 1 && n <= 65535 && max_kk >= 1 && max_n_vocab >= 1);
+    int grid = (max_n_vocab + TILE - 1) / TILE, launches = 2;
+    sample_select_rows_kernel<<<dim3((unsigned)grid, (unsigned)n), THREADS, 0, st>>>(jobs);
+    B200_CHECK(cudaGetLastError());
+    // the most candidates any job has at each level: the widest row with the most candidates per CTA
+    for (int64_t m = (int64_t)grid * max_kk, level = 0; m > TILE; level++) {
+        grid = (int)((m + TILE - 1) / TILE);
+        sample_merge_rows_kernel<<<dim3((unsigned)grid, (unsigned)n), THREADS, 0, st>>>(jobs, (int)level);
+        B200_CHECK(cudaGetLastError());
+        m = (int64_t)grid * max_kk;
+        launches++;
+    }
+    sample_tail_rows_kernel<<<(unsigned)n, THREADS, 0, st>>>(jobs);
+    B200_CHECK(cudaGetLastError());
+    return launches;
+}
 
 void sample_row(const float *row, int n_vocab, const int32_t *hist, int n_past, const SampleArgs &a, const SampleBufs &b, int32_t *tok_dst, int32_t *hist_dst,
                 SampleResult *res, int32_t *cand_ids, float *cand_vals, float *cand_probs, cudaStream_t st) {

@@ -528,6 +528,59 @@ class Llama(_Native):
     def context_size(self) -> int:
         return self.params.context_size
 
+    MAX_SESSIONS = 64                           # B200_MAX_SESSIONS
+
+    def _session_handles(self, sessions):
+        return (C.c_void_p * max(1, len(sessions)))(*[s._s for s in sessions])
+
+    def evaluate_sessions(self, sessions: Sequence["InferenceSession"], tokens) -> np.ndarray:
+        """One decode step for several sessions of this model: session i evaluates tokens[i] at its own n_past, reading the weights once for
+        all of them.  Each session ends exactly as after session.evaluate([tokens[i]]) alone, bit for bit.  Returns the [n, n_vocab] logits.
+        Refused as a whole, nothing changed (RuntimeError, or ContextFull when a session has no room): 0 or more than 64 sessions, a session of
+        another model, the same session twice, FAST sessions, mixed KV cache types, an id outside the vocabulary.  See include/llm_b200.h."""
+        tokens = np.ascontiguousarray(tokens, np.int32).ravel()
+        n = len(sessions)
+        if tokens.size != n:
+            raise ValueError(f"{n} sessions, {tokens.size} tokens")
+        out = np.empty((max(n, 1), int(self.hyperparameters["n_vocab"])), np.float32)
+        _check(self.L.b200_model_evaluate_sessions(self._m, self._session_handles(sessions), n, tokens.ctypes.data_as(C.c_void_p),
+                                                   out.ctypes.data_as(C.c_void_p)), "evaluate_sessions")
+        for i, s in enumerate(sessions):
+            s._last_logits = None
+        return out[:n]
+
+    def infer_next_tokens(self, sessions: Sequence["InferenceSession"], params, rngs: Sequence[Rng]) -> List[int]:
+        """infer_next_token for several sessions at once: session i samples from its last row with its own parameters and rngs[i], then one
+        batched step evaluates every sampled id.  `params`: one InferenceParameters (or None) for all, or one per session.  Returns the ids; each
+        rngs[i].draw advances by one for every session that sampled.  End of text is NOT raised: the id is returned (and has been evaluated), and
+        the caller compares it with eot_token_id().  A session whose row holds a NaN is left as it was; once the others have advanced,
+        SamplerFailure is raised with `.sessions`, the failed indices, and `.tokens`, the ids (-1 at the failed ones)."""
+        n = len(sessions)
+        plist = list(params) if isinstance(params, (list, tuple)) else [params] * n
+        if len(plist) != n or len(rngs) != n:
+            raise ValueError(f"{n} sessions, {len(plist)} parameters, {len(rngs)} rngs")
+        table = (_lib.SamplerParams * max(n, 1))()
+        for i, (p, rng) in enumerate(zip(plist, rngs)):
+            sp = (p or InferenceParameters()).sampler
+            table[i] = _lib.SamplerParams(repetition_penalty=sp.repetition_penalty, repetition_last_n=sp.repetition_last_n, top_k=sp.top_k,
+                                          top_p=sp.top_p, temperature=sp.temperature, seed=rng.seed, draw=rng.draw)
+        toks, status = np.full(max(n, 1), -1, np.int32), np.zeros(max(n, 1), np.int32)
+        _check(self.L.b200_model_infer_next_tokens(self._m, self._session_handles(sessions), n, table, toks.ctypes.data_as(C.c_void_p),
+                                                   status.ctypes.data_as(C.c_void_p)), "infer_next_tokens")
+        failed = []
+        for i, (s, rng) in enumerate(zip(sessions, rngs)):
+            if status[i] == 0:
+                rng.draw += 1
+                s._last_logits = None
+            else:
+                failed.append(i)
+        ids = [int(t) for t in toks[:n]]
+        if failed:
+            err = SamplerFailure(f"infer_next_tokens: sampler failure in sessions {failed}")
+            err.sessions, err.tokens = failed, ids
+            raise err
+        return ids
+
     def bot_token_id(self) -> Optional[int]:
         """KnownModel::bot_token_id: LLaMA has none (llama lib.rs:382-384)"""
         return None
