@@ -411,6 +411,28 @@ int32_t b200_neox_read_tokens(b200_neox_session *s, int32_t *tokens_out, int32_t
 int  b200_neox_last_logits(b200_neox_session *s, float *logits_out);
 void b200_neox_session_free(b200_neox_session *s);
 
+/* ---- batched decode: one step advances many sessions of one GPT-NeoX, GPT-2, MPT, BLOOM or GPT-J model ------------------------------------
+ * The contract of b200_model_evaluate_sessions / b200_model_infer_next_tokens, for this runtime.  The weights are read once per step for all n
+ * sessions, and each session's own cache once.  Every session ends exactly as if it had run b200_neox_evaluate(s, &tokens[i], 1, ..) alone:
+ * n_past + 1, the id appended to its history, its cache slot n_past written, its last row (row 0 of its logits, last_n 1) what last_logits,
+ * infer_next_token and get_snapshot read, bit for bit; last_launches is the batched step's launch count (the same for every n).  A later
+ * single-session step uploads the new n_past to its decode graphs.
+ * Refused as a whole, with nothing enqueued and no session changed:
+ *   B200_ERR_BAD_ARG        n < 1 or n > B200_MAX_SESSIONS; a null entry; a session of another model; the same session twice; sessions whose KV
+ *                           cache types differ; a token id outside [0, n_vocab) (evaluate); a sampler b200_neox_infer_next_token refuses, or a
+ *                           session with no evaluated row (infer)
+ *   B200_ERR_CONTEXT_FULL   a session with no room, by the rule of the single-session call: n_past + 1 > context_size for evaluate,
+ *                           n_past + 1 >= context_size for infer
+ * This runtime has no FAST or tensor-parallel sessions (b200_neox_start_session_flags refuses both), so the LLaMA pair's refusals of those have
+ * no counterpart here.  The pointers are not checked for their runtime: pass sessions of this runtime only. */
+/* One decode step for n sessions of model m: session i evaluates tokens[i] at its own n_past.  logits_out: n x n_vocab, nullable. */
+int  b200_neox_evaluate_sessions(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out);
+/* b200_neox_infer_next_token for n sessions at once: session i samples from its last row with samplers[i], then one batched step evaluates the
+ * sampled ids.  tokens_out[i] (-1 on a failure) and status_out[i]: B200_OK, or B200_ERR_SAMPLER_FAILURE when session i's row holds a NaN -- that
+ * session is not stepped, so its n_past, history, last row and cache are as they were, while the others advance.  The call returns B200_OK then. */
+int  b200_neox_infer_next_tokens(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const b200_sampler *samplers,
+                                 int32_t *tokens_out, int32_t *status_out);
+
 /* ---- session snapshots: InferenceSession::get_snapshot / from_snapshot (crates/llm-base/src/inference_session.rs:591-646, types :733-792) and the
  * CLI's session files (--save-session / --load-session / --persist-session, binaries/llm-cli/src/snapshot.rs) ------------------------------------
  * memory_k / memory_v are the reference's bytes: n_layer x context_size x n_embd values of the cache's type each (for LLaMA with grouped-query

@@ -50,9 +50,6 @@ struct NeoxLayer {
     void *K, *V;                        // [n_ctx][e] by position / [e][n_ctx] transposed, as the reference lays out memory_k / memory_v (:233-247),
                                         // of NeoxParams::kv_type
 };
-// where q / k / v of head h start inside a row of the fused qkv projection: h * head_stride, + k_off, + v_off.  GPT-NeoX: per head [q | k | v]
-// (3 hd, hd, 2 hd); GPT-2, MPT, BLOOM, GPT-J: the three thirds of the row (hd, e, 2 e)
-struct QkvLayout { int head_stride, k_off, v_off; };
 struct NeoxParams {
     int n_layer, e, hd, n_head, n_ctx, n_vocab, parallel_residual;
     int kv_type;                                // the KV cache's element type: T_F16 or T_F32

@@ -361,12 +361,12 @@ void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne
 // KQ: grid (max_n_kv / 8, n_head, n); outputs past the row's n_kv exit at once.
 template <bool F32>
 __global__ void __launch_bounds__(F16X_WARPS * 32) attn_kq_rows_kernel(const BatchRow *__restrict__ rows, size_t layer_off, const float *__restrict__ q, int64_t q_ld,
-                                                                       int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ kq) {
+                                                                       int64_t q_hs, int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ kq) {
     constexpr int64_t es = F32 ? 4 : 2;
     const int64_t gqa = (int64_t)n_head_kv * hd;
     const int z = blockIdx.z, n_past = rows[z].n_past;
     const char *K = (const char *)rows[z].K + layer_off * es;
-    mul_mat_attn_warp<F32>(K, hd, n_past + 1, n_head_kv, gqa * es, hd * es, (const char *)(q + z * q_ld), 1, n_head, 0, hd * 4,
+    mul_mat_attn_warp<F32>(K, hd, n_past + 1, n_head_kv, gqa * es, hd * es, (const char *)(q + z * q_ld), 1, n_head, 0, q_hs * 4,
                            (char *)(kq + (int64_t)z * n_head * n_ctx), 0, (int64_t)n_ctx * 4, n_past,
                            blockIdx.x, 0, blockIdx.y);
 }
@@ -382,11 +382,11 @@ __global__ void __launch_bounds__(F16X_WARPS * 32) attn_kqv_rows_kernel(const Ba
                            blockIdx.x, 0, blockIdx.y);
 }
 
-void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int hd, int n_head, int n_head_kv,
-                  int n_ctx, float *kq, cudaStream_t st) {
+void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int64_t q_hs, int hd, int n_head,
+                  int n_head_kv, int n_ctx, float *kq, cudaStream_t st) {
     B200_ASSERT(n >= 1 && n <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
     const dim3 grid((unsigned)((max_n_kv + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)n);
-    (kv_type == T_F32 ? attn_kq_rows_kernel<true> : attn_kq_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(rows, layer_off, q, q_ld, hd, n_head, n_head_kv,
+    (kv_type == T_F32 ? attn_kq_rows_kernel<true> : attn_kq_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(rows, layer_off, q, q_ld, q_hs, hd, n_head, n_head_kv,
                                                                                                                  n_ctx, kq);
     B200_CHECK(cudaGetLastError());
 }

@@ -1,6 +1,7 @@
 // llm_b200/csrc/host.cu -- tensor slots and session state shared by the LLaMA and GPT-NeoX / GPT-2 runtimes (host.h)
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -281,6 +282,98 @@ void SessionCore::commit_step(int launches) {
     last_n = 1;
     last_launches = launches;
     decode.dev_n_past = -1;                     // the next graph step uploads n_past
+}
+
+// ---- batched decode (host.h: BatchCore) ------------------------------------------------------------------------------------------------
+// the device half of committing a batched step: row i's id to its session's history at n_past, its logits to row 0 of the session's logits
+__global__ void commit_rows_kernel(const BatchRow *__restrict__ rows, const int32_t *__restrict__ ids, const float *__restrict__ logits, int n_vocab) {
+    const BatchRow &r = rows[blockIdx.y];
+    const float *src = logits + (size_t)blockIdx.y * n_vocab;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_vocab; i += gridDim.x * blockDim.x) r.logits[i] = src[i];
+    if (blockIdx.x == 0 && threadIdx.x == 0) r.hist[r.n_past] = ids[blockIdx.y];
+}
+
+void BatchCore::reserve(int n, int n_vocab, const BatchFront &f) {
+    if (n <= cap) return;
+    B200_CHECK(cudaStreamSynchronize(rt().stream));                  // the buffers being replaced may still be in use
+    const size_t B = n;
+    f.reserve(B);
+    logits = device_alloc<float>(B * (size_t)n_vocab * 4);
+    rows = device_alloc<BatchRow>(B * sizeof(BatchRow)); h_rows = pinned_alloc<BatchRow>(B * sizeof(BatchRow));
+    jobs = device_alloc<SampleJob>(B * sizeof(SampleJob)); h_jobs = pinned_alloc<SampleJob>(B * sizeof(SampleJob));
+    ids = device_alloc<int32_t>(B * 4); h_ids = pinned_alloc<int32_t>(B * 4);
+    if (!staged) { cudaEvent_t ev; B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); staged.reset(ev); }
+    cap = n;
+}
+
+// one batched step of sessions ss[0, n) on tokens[0, n) (checked by the caller): stage the row table and the ids, run forward_rows, commit
+// every row.  logits_out (nullable): the n rows.
+void BatchCore::step(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f) {
+    cudaStream_t st = rt().stream;
+    const int V = ss[0].s->n_vocab;
+    reserve(n, V, f);
+    B200_CHECK(cudaEventSynchronize(staged.get()));
+    int max_n_kv = 0;
+    for (int i = 0; i < n; i++) {
+        SessionCore *s = ss[i].s;
+        h_rows.get()[i] = BatchRow{s->memory_k.get(), s->memory_v.get(), ss[i].logits, s->history.get(), s->n_past};
+        h_ids.get()[i] = tokens[i];
+        max_n_kv = std::max(max_n_kv, s->n_past + 1);
+    }
+    B200_CHECK(cudaMemcpyAsync(rows.get(), h_rows.get(), (size_t)n * sizeof(BatchRow), cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(ids.get(), h_ids.get(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaEventRecord(staged.get(), st));
+    int L = f.forward_rows(n, ss[0].s->kv_type, max_n_kv);
+    commit_rows_kernel<<<dim3((unsigned)std::min((V + 255) / 256, 64), (unsigned)n), 256, 0, st>>>(rows.get(), ids.get(), logits.get(), V); L++;
+    B200_CHECK(cudaGetLastError());
+    for (int i = 0; i < n; i++) ss[i].s->commit_step(L);
+    if (logits_out) {
+        B200_CHECK(cudaMemcpyAsync(logits_out, logits.get(), (size_t)n * V * 4, cudaMemcpyDeviceToHost, st));
+        B200_CHECK(cudaStreamSynchronize(st));
+    }
+}
+
+int BatchCore::evaluate(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f) {
+    if (!tokens) return B200_ERR_BAD_ARG;
+    for (int i = 0; i < n; i++) if (tokens[i] < 0 || tokens[i] >= ss[i].s->n_vocab) return B200_ERR_BAD_ARG;
+    for (int i = 0; i < n; i++) if (const int rc = ss[i].s->admit(1)) return rc;           // the single-session evaluate's rule
+    step(ss, n, tokens, logits_out, f);
+    return B200_OK;
+}
+
+// infer_next_token for n sessions: the batched sampler on each session's last row, then (once its results are in) one batched step over the
+// sessions whose sampler succeeded.  A failed session is not stepped at all, so its state is what it was.
+int BatchCore::infer(const BatchSession *ss, int n, const b200_sampler *samplers, int32_t *tokens_out, int32_t *status_out, const BatchFront &f) {
+    if (!samplers || !tokens_out || !status_out) return B200_ERR_BAD_ARG;
+    SampleArgs a[B200_MAX_SESSIONS];
+    for (int i = 0; i < n; i++) if (!sampler_args(&samplers[i], a[i]) || ss[i].s->last_n < 1) return B200_ERR_BAD_ARG;
+    for (int i = 0; i < n; i++) if (ss[i].s->n_past + 1 >= ss[i].s->n_ctx) return B200_ERR_CONTEXT_FULL;   // the single-session infer's rule
+    cudaStream_t st = rt().stream;
+    const int V = ss[0].s->n_vocab;
+    reserve(n, V, f);
+    B200_CHECK(cudaEventSynchronize(staged.get()));
+    int max_kk = 1;
+    for (int i = 0; i < n; i++) {
+        SessionCore *s = ss[i].s;
+        const SampleBufs b{{s->sample_keys.get(), s->sample_keys.get() + sample_key_bytes(V) / 8}, s->sample_fail.get(), nullptr};
+        h_jobs.get()[i] = SampleJob{ss[i].logits + (size_t)(s->last_n - 1) * V, s->history.get(), V, s->n_past, a[i], b, nullptr, nullptr, s->d_sample};
+        max_kk = std::max(max_kk, sample_kk(a[i].top_k, V));
+    }
+    B200_CHECK(cudaMemcpyAsync(jobs.get(), h_jobs.get(), (size_t)n * sizeof(SampleJob), cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaEventRecord(staged.get(), st));
+    sample_rows(jobs.get(), n, V, max_kk, st);
+    B200_CHECK(cudaStreamSynchronize(st));
+    BatchSession ok[B200_MAX_SESSIONS];
+    int32_t ids_ok[B200_MAX_SESSIONS];
+    int k = 0;
+    for (int i = 0; i < n; i++) {
+        const volatile SampleResult *r = ss[i].s->h_sample.get();
+        if (r->status != 0) { status_out[i] = B200_ERR_SAMPLER_FAILURE; tokens_out[i] = -1; continue; }
+        status_out[i] = B200_OK; tokens_out[i] = r->id;
+        ok[k] = ss[i]; ids_ok[k++] = r->id;
+    }
+    if (k) step(ok, k, ids_ok, nullptr, f);
+    return B200_OK;
 }
 
 int SessionCore::set_n_past(int v) {

@@ -242,4 +242,45 @@ Sess *session_from_snapshot(const b200_snapshot *snap, const char *path, int n_c
 // a b200_sampler as the kernels take it; false if it is out of range (top_k < 1, temperature or penalty <= 0 or NaN, last_n < 0, top_p NaN)
 bool sampler_args(const b200_sampler *s, SampleArgs &a);
 
+// ---- batched decode: one step for n sessions of one model (b200_model_evaluate_sessions, b200_neox_evaluate_sessions) -------------------
+// One session of a batched call: its core and its logits buffer (row 0 takes the step's row).
+struct BatchSession { SessionCore *s; float *logits; };
+// The refusals of a batched call that depend only on its sessions (B200_ERR_BAD_ARG or B200_OK): n outside [1, B200_MAX_SESSIONS], a null
+// entry, a session whose model is not m, the same session twice, sessions whose KV cache types differ.  Fills out[0, n) when it accepts.
+template <class M, class S> int batch_sessions(const M *m, S *const *ss, int n, BatchSession *out) {
+    if (!m || !ss || n < 1 || n > B200_MAX_SESSIONS) return B200_ERR_BAD_ARG;
+    for (int i = 0; i < n; i++) {
+        S *s = ss[i];
+        if (!s || s->m != m || s->kv_type != ss[0]->kv_type) return B200_ERR_BAD_ARG;
+        for (int j = 0; j < i; j++) if (ss[j] == s) return B200_ERR_BAD_ARG;
+        out[i] = BatchSession{s, s->logits.get()};
+    }
+    return B200_OK;
+}
+// The front end's half of a batched step.  reserve(n): grow its activations to n rows (the stream is idle when it is called).
+// forward_rows(n, kv_type, max_n_kv): enqueue the forward pass of the n staged rows (BatchCore::rows, ::ids) into BatchCore::logits, every row's
+// arithmetic that of the single-session forward on that row alone, and return its launches (the same for every n).
+struct BatchFront {
+    std::function<void(size_t n)> reserve;
+    std::function<int(int n, int kv_type, int max_n_kv)> forward_rows;
+};
+// What a model keeps for its batched steps: the row table, the ids, the sampler jobs, their pinned staging and the logits of n rows, grown on
+// demand to the largest n seen and freed with the model.
+struct BatchCore {
+    int cap = 0;
+    DeviceBuf<float> logits;
+    DeviceBuf<BatchRow> rows; DeviceBuf<SampleJob> jobs; DeviceBuf<int32_t> ids;
+    PinnedBuf<BatchRow> h_rows; PinnedBuf<SampleJob> h_jobs; PinnedBuf<int32_t> h_ids;
+    Event staged;                       // recorded after the uploads: the pinned tables are not rewritten before they have been read
+
+    // b200_model_evaluate_sessions over sessions ss[0, n) that batch_sessions accepted: the ids and the context checked, then one step
+    int evaluate(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f);
+    // b200_model_infer_next_tokens over accepted sessions: the samplers checked, every row sampled, then one step of the sessions that sampled
+    int infer(const BatchSession *ss, int n, const b200_sampler *samplers, int32_t *tokens_out, int32_t *status_out, const BatchFront &f);
+
+private:
+    void reserve(int n, int n_vocab, const BatchFront &f);
+    void step(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f);
+};
+
 }  // namespace b200

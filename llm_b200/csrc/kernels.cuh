@@ -177,22 +177,31 @@ void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne
                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                        float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st);
 
-// ---- batched decode over many sessions of one model (session.cu: b200_model_evaluate_sessions) -------------------------------------------
+// ---- batched decode over many sessions of one model (b200_model_evaluate_sessions, b200_neox_evaluate_sessions; host.h: BatchCore) -------
 // Row i of a batched step belongs to its own session: the session's whole memory_k / memory_v ([n_layer][n_ctx][gqa] and [n_layer][gqa][n_ctx],
 // of the step's one cache type), its position n_past (the row's token goes to slot n_past), its logits buffer and history.  Uploaded once per step.
 struct BatchRow { void *K, *V; float *logits; int32_t *hist; int n_past; };
-// rowops.cu: RoPE mode 0 on the n_head + n_head_kv heads of row i of qkv ([n][qkv_ld]: q | k | v) at position rows[i].n_past, in place, and
-// K (roped) / V of the row stored into its session's cache at that slot (layer_off: elements to this layer's slice) -- rope_f32 + cpy_strided
-// of forward() on each row.  One launch.
-void rope_store_rows(float *qkv, int64_t qkv_ld, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off, int n_ctx,
-                     int kv_type, const RopeTable &tab, cudaStream_t st);
+// where q / k / v of head h start inside a row of the fused qkv projection: h * head_stride, + k_off, + v_off.  LLaMA: (hd, e, e + gqa);
+// GPT-NeoX: per head [q | k | v] (3 hd, hd, 2 hd); GPT-2, MPT, BLOOM, GPT-J: the three thirds of the row (hd, e, 2 e)
+struct QkvLayout { int head_stride, k_off, v_off; };
+// rowops.cu: RoPE on the n_head q and n_head_kv k heads of row i of qkv ([n][qkv_ld], laid out by `lay`) at position rows[i].n_past, in place,
+// and the row's K (all hd elements of each head, roped or not) / V stored into its session's cache at that slot (layer_off: elements to this
+// layer's slice; V transposed, by channel) -- rope_f32 + cpy_strided of forward() on each row.  tab: mode 0 (adjacent pairs, LLaMA and GPT-J)
+// or mode 2 (rope_f32's NeoX pairing on chunks of n_dims, GPT-NeoX) over the head's hd elements; nullptr: no rotation (GPT-2, MPT, BLOOM).
+// One launch.
+void rope_store_rows(float *qkv, int64_t qkv_ld, QkvLayout lay, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off,
+                     int n_ctx, int kv_type, const RopeTable *tab, cudaStream_t st);
 // rowops.cu: kq[i][h][0, n_past_i + 1) = soft_max(scale * kq[i][h][.]) (the row stride is n_ctx), soft_max's arithmetic per row.  One launch.
 void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, cudaStream_t st);
+// rowops.cu: the same with head h's ALiBi term, soft_max_alibi's arithmetic per row (alibi: device slopes [n_head]).  One launch.
+void soft_max_alibi_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, const float *alibi, cudaStream_t st);
+// rowops.cu: x[i][c] += wpe[n_past_i][c] for c < e -- GPT-2's learned position of each row, add_f32's rounding.  One launch.
+void add_pos_rows(float *x, const float *wpe, const BatchRow *rows, int n, int e, cudaStream_t st);
 // exact.cu: KQ and KQV of forward() on each row's own cache, in mul_mat_f16_exact / mul_mat_f32_exact's arithmetic (kv_type T_F16 / T_F32):
-//   kq[i][h][j] = K_i[j][hk] . Q[i][h] for j <= n_past_i (q rows of stride q_ld; kq rows of stride n_ctx, [n][n_head]);
+//   kq[i][h][j] = K_i[j][hk] . Q[i][h] for j <= n_past_i (q rows of stride q_ld, head h at h * q_hs; kq rows of stride n_ctx, [n][n_head]);
 //   out[i][h * hd + c] = V_i[hk][c][:] . kq[i][h][:]  (out rows of stride ld_out).  max_n_kv: the largest n_past_i + 1.  One launch each.
-void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int hd, int n_head, int n_head_kv,
-                  int n_ctx, float *kq, cudaStream_t st);
+void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int64_t q_hs, int hd, int n_head,
+                  int n_head_kv, int n_ctx, float *kq, cudaStream_t st);
 void attn_kqv_rows(int kv_type, const BatchRow *rows, int n, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx,
                    float *out, int64_t ld_out, cudaStream_t st);
 // sample.cu: sample_row for n sessions in one chain of launches (select, merges, tail), session i taken from the grid.  Each job is one session's

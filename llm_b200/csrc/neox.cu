@@ -49,6 +49,14 @@ template <class O> constexpr TensorDef<O> bias(const char *n, FRef<O> f, Dim K =
 template <class O> constexpr TensorDef<O> rows(const char *n, QRef<O> q, uint8_t at) { return {n, ROWS, q, nullptr, E, E, at}; }
 template <class O> constexpr TensorDef<O> if_lm_head(TensorDef<O> d) { d.if_lm_head = true; return d; }
 
+// The activations of a batched decode step (b200_neox_evaluate_sessions): rows of n sessions, grown on demand to the largest n seen, freed with
+// the model.
+struct NeoxBatch {
+    BatchCore core;                     // the row table, the ids, the sampler jobs and the logits (host.h)
+    DeviceBuf<float> x, cur, qkv, kq, attn, h4, hact, t;
+    DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh; DeviceBuf<char> xq8k;
+};
+
 }  // namespace
 
 struct b200_neox_model : Weights {
@@ -65,6 +73,7 @@ struct b200_neox_model : Weights {
     float kq_scale = 0.0f;
     bool any_kquant = false;                                      // some matrix is a K-quant (the sessions hold a Q8_K activation buffer)
     bool uniform = true;                                          // every matrix is of hp.wtype, as one fused qkv per layer: the decode graph's layout
+    NeoxBatch batch;
     bool neox() const { return hp.arch == 0; }
     bool mpt() const { return hp.arch == 2; }
     bool bloom() const { return hp.arch == 3; }
@@ -300,6 +309,91 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     s->last_launches = L;
     s->last_n = n;
     s->n_past += n;
+}
+
+// ---- batched decode: one step for n sessions of one model (b200_neox_evaluate_sessions) -------------------------------------------------
+// forward() with n rows that belong to n sessions: the weight mat-muls and the row-wise nodes over all n rows; the learned positions, RoPE, the
+// cache stores and the attention per row on its own session's cache and position (the row table).  Each row's arithmetic is forward()'s on that
+// row alone.  Returns the launches; the same for every n.
+int forward_rows(b200_neox_model *m, int n, int kv_type, int max_n_kv, cudaStream_t st) {
+    const b200_neox_hparams &hp = m->hp;
+    NeoxBatch &w = m->batch;
+    const int e = hp.n_embd, hd = m->hd, n_head = hp.n_head, n_ctx = hp.context_size, V = hp.n_vocab;
+    const int64_t ld3 = 3 * (int64_t)e, e4 = 4 * (int64_t)e, ne = (int64_t)n * e;
+    const QkvLayout lay = m->qkv_layout;
+    const BatchRow *rows = w.core.rows.get();
+    const ExactActs acts{w.xq.get(), w.xds.get(), w.xpack.get(), w.xh.get(), w.xq8k.get()};
+    auto mm = [&](const QWeight &W, const float *x, float *dst, int64_t ldd) { return mul_mat_exact_auto(W, x, W.K, n, dst, ldd, nullptr, 0, acts, st); };
+    float *x = w.x.get(), *cur = w.cur.get(), *qkv = w.qkv.get(), *kq = w.kq.get(), *attn = w.attn.get(), *h4 = w.h4.get(), *hact = w.hact.get(),
+          *t = w.t.get(), *logits = w.core.logits.get();
+    int L = 0;
+    if (m->emb_g) {
+        get_rows_q(m->wte, w.core.ids.get(), t, n, st); L++;
+        layer_norm(t, x, m->emb_g, m->emb_b, e, n, st); L++;
+    } else {
+        get_rows_q(m->wte, w.core.ids.get(), x, n, st); L++;
+    }
+    if (m->wpe) { add_pos_rows(x, m->wpe, rows, n, e, st); L++; }
+    for (int il = 0; il < hp.n_layer; il++) {
+        const b200_neox_model::Layer &ly = m->layers[il];
+        const size_t layer_off = (size_t)il * n_ctx * e;
+        layer_norm(x, cur, ly.ln1_g, ly.ln1_b, e, n, st); L++;
+        L += mm(ly.wqkv, cur, qkv, ld3);
+        if (ly.wv.N) L += mm(ly.wv, cur, qkv + lay.v_off, ld3);
+        if (ly.bqkv) { add_f32(qkv, ly.bqkv, qkv, n * ld3, ld3, st); L++; }
+        rope_store_rows(qkv, ld3, lay, hd, n_head, n_head, rows, n, layer_off, n_ctx, kv_type, m->rope, st); L++;
+        attn_kq_rows(kv_type, rows, n, max_n_kv, layer_off, qkv, ld3, lay.head_stride, hd, n_head, n_head, n_ctx, kq, st); L++;
+        if (m->alibi) soft_max_alibi_rows(kq, rows, n, n_head, n_ctx, m->kq_scale, m->alibi.get(), st);
+        else soft_max_rows(kq, rows, n, n_head, n_ctx, m->kq_scale, st);
+        L++;
+        float *kqv = m->gptj() ? t : cur;                     // GPT-J: cur still feeds fc_in
+        attn_kqv_rows(kv_type, rows, n, layer_off, kq, hd, n_head, n_head, n_ctx, kqv, e, st); L++;
+        L += mm(ly.wdense, kqv, attn, e);
+        if (m->gptj()) {
+            L += mm(ly.wfc, cur, h4, e4);
+            add_f32(h4, ly.bfc, h4, n * e4, e4, st); L++;
+            unary_lut(UNARY_GELU, h4, hact, n * e4, st); L++;
+            L += mm(ly.wproj, hact, t, e);
+            add_f32(t, ly.bproj, t, ne, e, st); L++;
+            add_f32(t, attn, t, ne, ne, st); L++;
+            add_f32(t, x, x, ne, ne, st); L++;
+            continue;
+        }
+        if (ly.bdense) { add_f32(attn, ly.bdense, attn, ne, e, st); L++; }
+        const float *ff_in = x;
+        if (!m->parallel) { add_f32(attn, x, attn, ne, ne, st); L++; ff_in = attn; }
+        layer_norm(ff_in, cur, ly.ln2_g, ly.ln2_b, e, n, st); L++;
+        L += mm(ly.wfc, cur, h4, e4);
+        if (ly.bfc) { add_f32(h4, ly.bfc, h4, n * e4, e4, st); L++; }
+        unary_lut(UNARY_GELU, h4, hact, n * e4, st); L++;
+        L += mm(ly.wproj, hact, t, e);
+        if (ly.bproj) { add_f32(t, ly.bproj, t, ne, e, st); L++; }
+        add_f32(t, attn, t, ne, ne, st); L++;
+        if (m->parallel) { add_f32(t, x, x, ne, ne, st); L++; }
+        else { B200_CHECK(cudaMemcpyAsync(x, t, (size_t)ne * 4, cudaMemcpyDeviceToDevice, st)); }
+    }
+    layer_norm(x, cur, m->lnf_g, m->lnf_b, e, n, st); L++;
+    L += mm(m->lm_head, cur, logits, V);
+    if (m->lm_head_b) { add_f32(logits, m->lm_head_b, logits, (int64_t)n * V, V, st); L++; }
+    return L;
+}
+
+// the batched step's activations for B rows (BatchCore::reserve, with the stream idle): b200_neox_start_session's buffers
+void batch_reserve(b200_neox_model *m, size_t B) {
+    NeoxBatch &w = m->batch;
+    const b200_neox_hparams &hp = m->hp;
+    const size_t e = hp.n_embd, n_ctx = hp.context_size;
+    w.x = device_alloc<float>(B * e * 4); w.cur = device_alloc<float>(B * e * 4); w.qkv = device_alloc<float>(B * 3 * e * 4);
+    w.kq = device_alloc<float>((size_t)hp.n_head * B * n_ctx * 4); w.attn = device_alloc<float>(B * e * 4);
+    w.h4 = device_alloc<float>(B * 4 * e * 4); w.hact = device_alloc<float>(B * 4 * e * 4); w.t = device_alloc<float>(B * e * 4);
+    w.xq = device_alloc<int8_t>(B * 4 * e); w.xds = device_alloc<float2>(B * (4 * e / QK) * sizeof(float2));
+    w.xpack = device_alloc<int4>((4 * e / QK) * 64); w.xh = device_alloc<__half>(xh_bytes(4 * e, B));
+    if (m->any_kquant) w.xq8k = device_alloc<char>(q8k_bytes(4 * e, B));          // the widest K: fc_out's 4 n_embd
+}
+
+BatchFront batch_front(b200_neox_model *m) {
+    return BatchFront{[m](size_t B) { batch_reserve(m, B); },
+                      [m](int n, int kv_type, int max_n_kv) { return forward_rows(m, n, kv_type, max_n_kv, rt().stream); }};
 }
 
 // a tensor's whole name: the model's own, or the layer prefix of layer il (layer_fmt up to its "%95s") followed by the suffix
@@ -569,6 +663,20 @@ int b200_neox_infer_next_token(b200_neox_session *s, const b200_sampler *sampler
     SampleArgs a;
     if (!s || !sampler_args(sampler, a)) return B200_ERR_BAD_ARG;
     return s->infer_next_token(a, s->logits.get(), [s]() { forward(s, 1, true); }, token_out);
+}
+
+// ---- batched decode over sessions of one model (include/llm_b200.h) -------------------------------------------------------------------------
+int b200_neox_evaluate_sessions(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out) {
+    BatchSession ss[B200_MAX_SESSIONS];
+    if (const int rc = batch_sessions(m, sessions, n, ss)) return rc;
+    return m->batch.core.evaluate(ss, n, tokens, logits_out, batch_front(m));
+}
+
+int b200_neox_infer_next_tokens(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const b200_sampler *samplers, int32_t *tokens_out,
+                                int32_t *status_out) {
+    BatchSession ss[B200_MAX_SESSIONS];
+    if (const int rc = batch_sessions(m, sessions, n, ss)) return rc;
+    return m->batch.core.infer(ss, n, samplers, tokens_out, status_out, batch_front(m));
 }
 
 int32_t b200_neox_read_tokens(b200_neox_session *s, int32_t *tokens_out, int32_t max) { return s ? s->read_tokens(tokens_out, max) : B200_ERR_BAD_ARG; }

@@ -381,41 +381,88 @@ void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx
     B200_CHECK(cudaGetLastError());
 }
 
-// thread t of row i: t < (n_head + n_head_kv) * half rotates one pair of a Q or K head (a K pair is also stored at slot n_past of the row's
-// memory_k); the next gqa threads store one V value each at slot n_past of the row's memory_v (transposed: [gqa][n_ctx])
+// soft_max_alibi of row (blockIdx.y, head blockIdx.x): soft_max_body<true> on its n_past + 1 scores with the head's slope (alibi + head and r = 0:
+// alibi[r / nr] is that slope, and column i's term fma(i, slope, v) depends on the key position alone)
+__global__ void soft_max_alibi_rows_kernel(float *__restrict__ kq, const BatchRow *__restrict__ rows, int n_head, int n_ctx, float scale,
+                                           const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi) {
+    const int n_past = rows[blockIdx.y].n_past;
+    float *x = kq + ((int64_t)blockIdx.y * n_head + blockIdx.x) * n_ctx;
+    soft_max_body<true>(x, x, n_past + 1, 1, scale, 1, n_past, 1, 1, t_exp, alibi + blockIdx.x, 0);
+}
+void soft_max_alibi_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, const float *alibi, cudaStream_t st) {
+    const size_t smem = (size_t)n_ctx * sizeof(float);
+    static size_t smem_set = 48 * 1024;
+    if (smem > smem_set) {
+        B200_ASSERT(smem <= 200 * 1024);
+        B200_CHECK(cudaFuncSetAttribute(soft_max_alibi_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        smem_set = smem;
+    }
+    soft_max_alibi_rows_kernel<<<dim3((unsigned)n_head, (unsigned)n), 256, smem, st>>>(kq, rows, n_head, n_ctx, scale, luts().exp, alibi);
+    B200_CHECK(cudaGetLastError());
+}
+
+__global__ void add_pos_rows_kernel(float *__restrict__ x, const float *__restrict__ wpe, const BatchRow *__restrict__ rows, int e, int64_t total) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int64_t z = t / e, c = t - z * e;
+    x[t] = __fadd_rn(x[t], wpe[(int64_t)rows[z].n_past * e + c]);
+}
+void add_pos_rows(float *x, const float *wpe, const BatchRow *rows, int n, int e, cudaStream_t st) {
+    const int64_t total = (int64_t)n * e;
+    add_pos_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, wpe, rows, e, total);
+    B200_CHECK(cudaGetLastError());
+}
+
+// one element into a KV cache of type KT (fp16: round to nearest, as cpy_strided)
 template <typename KT>
-__global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, int hd, int n_head, int n_head_kv, const BatchRow *__restrict__ rows,
-                                       size_t layer_off, int n_ctx, const float2 *__restrict__ cs, int half, int64_t per_row, int64_t total) {
+__device__ __forceinline__ void kv_store(KT *p, float v) { if constexpr (sizeof(KT) == 2) *p = __float2half_rn(v); else *p = v; }
+
+// thread t of row i, in three ranges:
+//   t < (n_head + n_head_kv) * half: rotates one pair of a q or k head, rope_kernel's pairing (mode 0: adjacent; mode 2: n_dims / 2 apart inside
+//     chunks of n_dims); a k pair is also stored at slot n_past of the row's memory_k;
+//   the next n_head_kv * (hd - 2 half): stores one k element no pair covers (every element when nothing rotates, half = 0);
+//   the next gqa: stores one v value at slot n_past of the row's memory_v (transposed: [gqa][n_ctx]).
+template <typename KT>
+__global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, QkvLayout lay, int hd, int n_head, int n_head_kv,
+                                       const BatchRow *__restrict__ rows, size_t layer_off, int n_ctx, const float2 *__restrict__ cs, int half,
+                                       int n_dims, int neox, int64_t per_row, int64_t total) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= total) return;
     const int64_t z = t / per_row, k = t - z * per_row;
     const int n_past = rows[z].n_past;
-    const int64_t e = (int64_t)n_head * hd, gqa = (int64_t)n_head_kv * hd, n_pairs = (int64_t)(n_head + n_head_kv) * half;
+    const int64_t gqa = (int64_t)n_head_kv * hd, n_pairs = (int64_t)(n_head + n_head_kv) * half, plain = hd - 2 * half;
+    const int64_t n_plain = n_head_kv * plain;
     float *row = qkv + z * qkv_ld;
+    KT *K = (KT *)rows[z].K + layer_off + (size_t)n_past * gqa;
     if (k < n_pairs) {
         const int i = (int)(k % half);
-        const int64_t head = k / half, e0 = head * hd + 2 * (int64_t)i;
-        const float2 r = rope_pair(row[e0], row[e0 + 1], __ldg(cs + (int64_t)n_past * half + i));
-        row[e0] = r.x;
-        row[e0 + 1] = r.y;
-        if (head >= n_head) {
-            KT *K = (KT *)rows[z].K + layer_off + (size_t)n_past * gqa + (e0 - e);
-            if constexpr (sizeof(KT) == 2) { K[0] = __float2half_rn(r.x); K[1] = __float2half_rn(r.y); } else { K[0] = r.x; K[1] = r.y; }
-        }
+        const int64_t head = k / half;
+        int64_t e0, e1;
+        if (!neox) { e0 = 2 * (int64_t)i; e1 = e0 + 1; }
+        else { const int hb = n_dims / 2; const int ib = i / hb, ic = i % hb; e0 = (int64_t)ib * n_dims + ic; e1 = e0 + hb; }
+        const int64_t hk = head - n_head, base = hk < 0 ? head * lay.head_stride : lay.k_off + hk * lay.head_stride;
+        const float2 r = rope_pair(row[base + e0], row[base + e1], __ldg(cs + (int64_t)n_past * half + i));
+        row[base + e0] = r.x;
+        row[base + e1] = r.y;
+        if (hk >= 0) { kv_store(K + hk * hd + e0, r.x); kv_store(K + hk * hd + e1, r.y); }
+    } else if (k < n_pairs + n_plain) {
+        const int64_t c = k - n_pairs, hk = c / plain, d = 2 * half + c % plain;
+        kv_store(K + hk * hd + d, row[lay.k_off + hk * lay.head_stride + d]);
     } else {
-        const int64_t c = k - n_pairs;
-        const float v = row[e + gqa + c];
-        KT *V = (KT *)rows[z].V + layer_off + (size_t)c * n_ctx + n_past;
-        if constexpr (sizeof(KT) == 2) *V = __float2half_rn(v); else *V = v;
+        const int64_t c = k - n_pairs - n_plain, hk = c / hd, d = c % hd;
+        kv_store((KT *)rows[z].V + layer_off + (size_t)c * n_ctx + n_past, row[lay.v_off + hk * lay.head_stride + d]);
     }
 }
-void rope_store_rows(float *qkv, int64_t qkv_ld, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off, int n_ctx,
-                     int kv_type, const RopeTable &tab, cudaStream_t st) {
-    B200_ASSERT(tab.ne0 == hd && tab.mode == 0 && hd % 2 == 0 && n_ctx <= tab.n_pos);
-    const int64_t per_row = (int64_t)(n_head + n_head_kv) * tab.half + (int64_t)n_head_kv * hd, total = per_row * n;
+void rope_store_rows(float *qkv, int64_t qkv_ld, QkvLayout lay, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off,
+                     int n_ctx, int kv_type, const RopeTable *tab, cudaStream_t st) {
+    B200_ASSERT(!tab || (tab->ne0 == hd && hd % 2 == 0 && n_ctx <= tab->n_pos));
+    const int half = tab ? tab->half : 0;
+    const int64_t per_row = (int64_t)(n_head + n_head_kv) * half + (int64_t)n_head_kv * (hd - 2 * half) + (int64_t)n_head_kv * hd, total = per_row * n;
     const unsigned grid = (unsigned)((total + 255) / 256);
-    if (kv_type == T_F32) rope_store_rows_kernel<float><<<grid, 256, 0, st>>>(qkv, qkv_ld, hd, n_head, n_head_kv, rows, layer_off, n_ctx, tab.cs, tab.half, per_row, total);
-    else rope_store_rows_kernel<__half><<<grid, 256, 0, st>>>(qkv, qkv_ld, hd, n_head, n_head_kv, rows, layer_off, n_ctx, tab.cs, tab.half, per_row, total);
+    const float2 *cs = tab ? tab->cs : nullptr;
+    const int n_dims = tab ? tab->n_dims : 0, neox = tab ? tab->mode : 0;
+    if (kv_type == T_F32) rope_store_rows_kernel<float><<<grid, 256, 0, st>>>(qkv, qkv_ld, lay, hd, n_head, n_head_kv, rows, layer_off, n_ctx, cs, half, n_dims, neox, per_row, total);
+    else rope_store_rows_kernel<__half><<<grid, 256, 0, st>>>(qkv, qkv_ld, lay, hd, n_head, n_head_kv, rows, layer_off, n_ctx, cs, half, n_dims, neox, per_row, total);
     B200_CHECK(cudaGetLastError());
 }
 

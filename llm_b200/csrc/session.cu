@@ -9,7 +9,6 @@
 // so one activation quantization and one mat-mul launch serve them.
 #include <string.h>
 
-#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -27,14 +26,11 @@ struct Layer {
 };
 
 // The activations of a batched decode step (b200_model_evaluate_sessions): rows of n sessions, grown on demand to the largest n seen, freed with the
-// model.  The row table and the ids are staged in pinned memory and uploaded once per step.
+// model.
 struct BatchWs {
-    int cap = 0;
-    DeviceBuf<float> x, cur, ff, qkv, kq, h13, hmul, logits;
+    BatchCore core;                     // the row table, the ids, the sampler jobs and the logits (host.h)
+    DeviceBuf<float> x, cur, ff, qkv, kq, h13, hmul;
     DeviceBuf<int8_t> xq; DeviceBuf<float2> xds; DeviceBuf<int4> xpack; DeviceBuf<__half> xh; DeviceBuf<char> xq8k;
-    DeviceBuf<BatchRow> rows; DeviceBuf<SampleJob> jobs; DeviceBuf<int32_t> ids;
-    PinnedBuf<BatchRow> h_rows; PinnedBuf<SampleJob> h_jobs; PinnedBuf<int32_t> h_ids;
-    Event staged;                       // recorded after the uploads: the pinned tables are not rewritten before they have been read
 };
 
 }  // namespace
@@ -251,22 +247,23 @@ int forward_rows(b200_model *m, int n, int kv_type, int max_n_kv, cudaStream_t s
     const int qkv_ld = e + 2 * gqa;
     const float kq_scale = 1.0f / sqrtf((float)e / (float)n_head);                           // llama lib.rs:268-270
     const RopeTable &rope = rope_table(hp.n_rot, 0, hp.rope_freq_base, hp.rope_freq_scale, hd, n_ctx);
+    const BatchRow *rows = w.core.rows.get();
     const ExactActs acts{w.xq.get(), w.xds.get(), w.xpack.get(), w.xh.get(), w.xq8k.get()};
     auto mm = [&](const QWeight &W, const float *x, float *dst, int64_t ldd, const float *addend) {
         return mul_mat_exact_auto(W, x, W.K, n, dst, ldd, addend, addend ? ldd : 0, acts, st);
     };
     int L = 0;
-    get_rows_q(m->wte, w.ids.get(), w.x.get(), n, st); L++;
+    get_rows_q(m->wte, w.core.ids.get(), w.x.get(), n, st); L++;
     for (int il = 0; il < hp.n_layer; il++) {
         const Layer &ly = m->layers[il];
         const size_t layer_off = (size_t)il * n_ctx * gqa;
         rms_norm(w.x.get(), w.cur.get(), ly.attention_norm, e, n, 5e-6f, st); L++;
         L += mm(ly.wqkv, w.cur.get(), w.qkv.get(), qkv_ld, nullptr);
         if (ly.wv.N) L += mm(ly.wv, w.cur.get(), w.qkv.get() + e + gqa, qkv_ld, nullptr);
-        rope_store_rows(w.qkv.get(), qkv_ld, hd, n_head, n_head_kv, w.rows.get(), n, layer_off, n_ctx, kv_type, rope, st); L++;
-        attn_kq_rows(kv_type, w.rows.get(), n, max_n_kv, layer_off, w.qkv.get(), qkv_ld, hd, n_head, n_head_kv, n_ctx, w.kq.get(), st); L++;
-        soft_max_rows(w.kq.get(), w.rows.get(), n, n_head, n_ctx, kq_scale, st); L++;
-        attn_kqv_rows(kv_type, w.rows.get(), n, layer_off, w.kq.get(), hd, n_head, n_head_kv, n_ctx, w.cur.get(), e, st); L++;
+        rope_store_rows(w.qkv.get(), qkv_ld, QkvLayout{hd, e, e + gqa}, hd, n_head, n_head_kv, rows, n, layer_off, n_ctx, kv_type, &rope, st); L++;
+        attn_kq_rows(kv_type, rows, n, max_n_kv, layer_off, w.qkv.get(), qkv_ld, hd, hd, n_head, n_head_kv, n_ctx, w.kq.get(), st); L++;
+        soft_max_rows(w.kq.get(), rows, n, n_head, n_ctx, kq_scale, st); L++;
+        attn_kqv_rows(kv_type, rows, n, layer_off, w.kq.get(), hd, n_head, n_head_kv, n_ctx, w.cur.get(), e, st); L++;
         L += mm(ly.wo, w.cur.get(), w.ff.get(), e, w.x.get());                                   // inpFF = wo.cur + inpSA
         rms_norm(w.ff.get(), w.cur.get(), ly.ffn_norm, e, n, 5e-6f, st); L++;
         L += mm(ly.w13, w.cur.get(), w.h13.get(), 2 * f, nullptr);
@@ -274,24 +271,15 @@ int forward_rows(b200_model *m, int n, int kv_type, int max_n_kv, cudaStream_t s
         L += mm(ly.w2, w.hmul.get(), w.x.get(), e, w.ff.get());
     }
     rms_norm(w.x.get(), w.cur.get(), m->norm, e, n, 5e-6f, st); L++;
-    L += mm(m->output, w.cur.get(), w.logits.get(), hp.n_vocab, nullptr);
+    L += mm(m->output, w.cur.get(), w.core.logits.get(), hp.n_vocab, nullptr);
     return L;
 }
 
-// the device half of committing a batched step: row i's id to its session's history at n_past, its logits to row 0 of the session's logits
-__global__ void commit_rows_kernel(const BatchRow *__restrict__ rows, const int32_t *__restrict__ ids, const float *__restrict__ logits, int n_vocab) {
-    const BatchRow &r = rows[blockIdx.y];
-    const float *src = logits + (size_t)blockIdx.y * n_vocab;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_vocab; i += gridDim.x * blockDim.x) r.logits[i] = src[i];
-    if (blockIdx.x == 0 && threadIdx.x == 0) r.hist[r.n_past] = ids[blockIdx.y];
-}
-
-void batch_reserve(b200_model *m, int n) {
+// the batched step's activations: n rows, grown to the largest n seen (BatchCore::reserve, with the stream idle)
+void batch_reserve(b200_model *m, size_t B) {
     BatchWs &w = m->batch;
-    if (n <= w.cap) return;
-    B200_CHECK(cudaStreamSynchronize(rt().stream));                  // the buffers being replaced may still be in use
     const b200_llama_hparams &hp = m->hp;
-    const size_t e = hp.n_embd, f = hp.n_ff, B = n, n_ctx = hp.context_size, gqa = m->gqa, kmax = e > f ? e : f;
+    const size_t e = hp.n_embd, f = hp.n_ff, n_ctx = hp.context_size, gqa = m->gqa, kmax = e > f ? e : f;
     w.x = device_alloc<float>(B * e * 4);
     w.cur = device_alloc<float>(B * e * 4);
     w.ff = device_alloc<float>(B * e * 4);
@@ -299,56 +287,24 @@ void batch_reserve(b200_model *m, int n) {
     w.kq = device_alloc<float>((size_t)hp.n_head * B * n_ctx * 4);
     w.h13 = device_alloc<float>(B * 2 * f * 4);
     w.hmul = device_alloc<float>(B * f * 4);
-    w.logits = device_alloc<float>(B * (size_t)hp.n_vocab * 4);
     w.xq = device_alloc<int8_t>(B * kmax);
     w.xds = device_alloc<float2>(B * (kmax / QK) * sizeof(float2));
     w.xpack = device_alloc<int4>((kmax / QK) * 64);
     w.xh = device_alloc<__half>(xh_bytes(kmax, B));
     if (m->any_kquant) w.xq8k = device_alloc<char>(q8k_bytes(kmax / 256 * 256, B));
-    w.rows = device_alloc<BatchRow>(B * sizeof(BatchRow)); w.h_rows = pinned_alloc<BatchRow>(B * sizeof(BatchRow));
-    w.jobs = device_alloc<SampleJob>(B * sizeof(SampleJob)); w.h_jobs = pinned_alloc<SampleJob>(B * sizeof(SampleJob));
-    w.ids = device_alloc<int32_t>(B * 4); w.h_ids = pinned_alloc<int32_t>(B * 4);
-    if (!w.staged) { cudaEvent_t ev; B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); w.staged.reset(ev); }
-    w.cap = n;
 }
 
-// every refusal of a batched call that does not depend on its tokens or samplers: B200_ERR_BAD_ARG or B200_OK
-int batch_check(const b200_model *m, b200_session *const *ss, int n) {
-    if (!m || !ss || n < 1 || n > B200_MAX_SESSIONS || m->tp_world > 1) return B200_ERR_BAD_ARG;
-    for (int i = 0; i < n; i++) {
-        const b200_session *s = ss[i];
-        if (!s || s->m != m || (s->cfg.flags & B200_SESSION_FAST) || s->kv_type != ss[0]->kv_type) return B200_ERR_BAD_ARG;
-        for (int j = 0; j < i; j++) if (ss[j] == s) return B200_ERR_BAD_ARG;
-    }
+// the sessions of a batched call (host.h: batch_sessions), and the two refusals only LLaMA has: a tensor-parallel model, a FAST session
+int batch_check(const b200_model *m, b200_session *const *ss, int n, BatchSession *out) {
+    if (const int rc = batch_sessions(m, ss, n, out)) return rc;
+    if (m->tp_world > 1) return B200_ERR_BAD_ARG;
+    for (int i = 0; i < n; i++) if (ss[i]->cfg.flags & B200_SESSION_FAST) return B200_ERR_BAD_ARG;
     return B200_OK;
 }
 
-// one batched step of sessions ss[0, n) on tokens[0, n) (checked by the caller): stage the row table and the ids, run forward_rows, commit
-// every row.  logits_out (nullable): the n rows.
-void batch_step(b200_model *m, b200_session *const *ss, int n, const int32_t *tokens, float *logits_out) {
-    cudaStream_t st = rt().stream;
-    batch_reserve(m, n);
-    BatchWs &w = m->batch;
-    B200_CHECK(cudaEventSynchronize(w.staged.get()));
-    int max_n_kv = 0;
-    for (int i = 0; i < n; i++) {
-        b200_session *s = ss[i];
-        w.h_rows.get()[i] = BatchRow{s->memory_k.get(), s->memory_v.get(), s->logits.get(), s->history.get(), s->n_past};
-        w.h_ids.get()[i] = tokens[i];
-        max_n_kv = std::max(max_n_kv, s->n_past + 1);
-    }
-    B200_CHECK(cudaMemcpyAsync(w.rows.get(), w.h_rows.get(), (size_t)n * sizeof(BatchRow), cudaMemcpyHostToDevice, st));
-    B200_CHECK(cudaMemcpyAsync(w.ids.get(), w.h_ids.get(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    B200_CHECK(cudaEventRecord(w.staged.get(), st));
-    const int V = m->hp.n_vocab;
-    int L = forward_rows(m, n, ss[0]->kv_type, max_n_kv, st);
-    commit_rows_kernel<<<dim3((unsigned)std::min((V + 255) / 256, 64), (unsigned)n), 256, 0, st>>>(w.rows.get(), w.ids.get(), w.logits.get(), V); L++;
-    B200_CHECK(cudaGetLastError());
-    for (int i = 0; i < n; i++) ss[i]->commit_step(L);
-    if (logits_out) {
-        B200_CHECK(cudaMemcpyAsync(logits_out, w.logits.get(), (size_t)n * V * 4, cudaMemcpyDeviceToHost, st));
-        B200_CHECK(cudaStreamSynchronize(st));
-    }
+BatchFront batch_front(b200_model *m) {
+    return BatchFront{[m](size_t B) { batch_reserve(m, B); },
+                      [m](int n, int kv_type, int max_n_kv) { return forward_rows(m, n, kv_type, max_n_kv, rt().stream); }};
 }
 
 }  // namespace
@@ -825,50 +781,16 @@ int b200_session_infer_next_token(b200_session *s, const b200_sampler *sampler, 
 
 // ---- batched decode over sessions of one model (include/llm_b200.h) -------------------------------------------------------------------------
 int b200_model_evaluate_sessions(b200_model *m, b200_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out) {
-    if (const int rc = batch_check(m, sessions, n)) return rc;
-    if (!tokens) return B200_ERR_BAD_ARG;
-    for (int i = 0; i < n; i++) if (tokens[i] < 0 || tokens[i] >= m->hp.n_vocab) return B200_ERR_BAD_ARG;
-    for (int i = 0; i < n; i++) if (const int rc = sessions[i]->admit(1)) return rc;       // b200_session_evaluate's rule
-    batch_step(m, sessions, n, tokens, logits_out);
-    return B200_OK;
+    BatchSession ss[B200_MAX_SESSIONS];
+    if (const int rc = batch_check(m, sessions, n, ss)) return rc;
+    return m->batch.core.evaluate(ss, n, tokens, logits_out, batch_front(m));
 }
 
-// infer_next_token for n sessions: the batched sampler on each session's last row, then (once its results are in) one batched step over the
-// sessions whose sampler succeeded.  A failed session is not stepped at all, so its state is what it was.
 int b200_model_infer_next_tokens(b200_model *m, b200_session *const *sessions, int32_t n, const b200_sampler *samplers, int32_t *tokens_out,
                                  int32_t *status_out) {
-    if (const int rc = batch_check(m, sessions, n)) return rc;
-    if (!samplers || !tokens_out || !status_out) return B200_ERR_BAD_ARG;
-    SampleArgs a[B200_MAX_SESSIONS];
-    for (int i = 0; i < n; i++) if (!sampler_args(&samplers[i], a[i]) || sessions[i]->last_n < 1) return B200_ERR_BAD_ARG;
-    for (int i = 0; i < n; i++) if (sessions[i]->n_past + 1 >= sessions[i]->n_ctx) return B200_ERR_CONTEXT_FULL;   // b200_session_infer_next_token's rule
-    cudaStream_t st = rt().stream;
-    batch_reserve(m, n);
-    BatchWs &w = m->batch;
-    B200_CHECK(cudaEventSynchronize(w.staged.get()));
-    const int V = m->hp.n_vocab;
-    int max_kk = 1;
-    for (int i = 0; i < n; i++) {
-        b200_session *s = sessions[i];
-        const SampleBufs b{{s->sample_keys.get(), s->sample_keys.get() + sample_key_bytes(V) / 8}, s->sample_fail.get(), nullptr};
-        w.h_jobs.get()[i] = SampleJob{s->logits.get() + (size_t)(s->last_n - 1) * V, s->history.get(), V, s->n_past, a[i], b, nullptr, nullptr, s->d_sample};
-        max_kk = std::max(max_kk, sample_kk(a[i].top_k, V));
-    }
-    B200_CHECK(cudaMemcpyAsync(w.jobs.get(), w.h_jobs.get(), (size_t)n * sizeof(SampleJob), cudaMemcpyHostToDevice, st));
-    B200_CHECK(cudaEventRecord(w.staged.get(), st));
-    sample_rows(w.jobs.get(), n, V, max_kk, st);
-    B200_CHECK(cudaStreamSynchronize(st));
-    b200_session *ok[B200_MAX_SESSIONS];
-    int32_t ids[B200_MAX_SESSIONS];
-    int k = 0;
-    for (int i = 0; i < n; i++) {
-        const volatile SampleResult *r = sessions[i]->h_sample.get();
-        if (r->status != 0) { status_out[i] = B200_ERR_SAMPLER_FAILURE; tokens_out[i] = -1; continue; }
-        status_out[i] = B200_OK; tokens_out[i] = r->id;
-        ok[k] = sessions[i]; ids[k++] = r->id;
-    }
-    if (k) batch_step(m, ok, k, ids, nullptr);
-    return B200_OK;
+    BatchSession ss[B200_MAX_SESSIONS];
+    if (const int rc = batch_check(m, sessions, n, ss)) return rc;
+    return m->batch.core.infer(ss, n, samplers, tokens_out, status_out, batch_front(m));
 }
 
 int32_t b200_session_read_tokens(b200_session *s, int32_t *tokens_out, int32_t max) { return s ? s->read_tokens(tokens_out, max) : B200_ERR_BAD_ARG; }

@@ -12,8 +12,8 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .session import (ContextFull, InferenceSnapshot, LoraAdapters, ModelKVMemoryType, OutputRequest, _check, _embeddings_buffer, _Generation, _Native,
-                      _perplexity, _ref_cache_bytes, _Snapshots, _vocab_id, ggml_dims, kv_array, kv_flags)
+from .session import (ContextFull, InferenceSnapshot, LoraAdapters, ModelKVMemoryType, OutputRequest, _BatchedSessions, _check, _embeddings_buffer,
+                      _Generation, _Native, _perplexity, _ref_cache_bytes, _Snapshots, _vocab_id, ggml_dims, kv_array, kv_flags)
 
 
 class NeoxHparams(C.Structure):
@@ -56,6 +56,8 @@ def _bind(L):
     L.b200_neox_sync.argtypes = [vp]
     L.b200_neox_perplexity.argtypes = [vp, vp, C.c_int64, i32, vp, vp, C.POINTER(i32)]
     L.b200_neox_infer_next_token.argtypes = [vp, C.POINTER(_lib.SamplerParams), C.POINTER(i32)]
+    L.b200_neox_evaluate_sessions.argtypes = [vp, C.POINTER(vp), i32, vp, vp]
+    L.b200_neox_infer_next_tokens.argtypes = [vp, C.POINTER(vp), i32, C.POINTER(_lib.SamplerParams), vp, vp]
     L.b200_neox_read_tokens.restype = i32
     L.b200_neox_read_tokens.argtypes = [vp, vp, i32]
     L.b200_neox_last_logits.argtypes = [vp, vp]
@@ -70,13 +72,14 @@ def _bind(L):
     return L
 
 
-class GptNeoX(_Native):
+class GptNeoX(_BatchedSessions, _Native):
     """hyperparameters: n_vocab, n_ctx, n_embd, n_head, n_layer, n_rot, use_parallel_residual, wtype.  lora_adapters: LoRA adapter files applied in
     order to every tensor they name (ModelParameters::lora_adapters).  tensor_types: {name: enum ggml_type} of 2-D weights whose type is not wtype
     (mixed-type and K-quant files, b200_neox_new_typed).  rope_freq_base / rope_freq_scale: ModelParameters::rope_overrides (GPT-NeoX and GPT-J)."""
 
     ARCH = 0
     _HANDLE, _FREE = "_m", "b200_neox_free"
+    _EVAL_SESSIONS, _INFER_SESSIONS = "b200_neox_evaluate_sessions", "b200_neox_infer_next_tokens"
 
     BOT_TOKEN: Optional[bytes] = None       # the vocabulary entry bot_token_id() names (MPT, BLOOM); None: the model has no BOS token
     EOT_TOKEN: bytes = b"<|endoftext|>"     # the entry eot_token_id() names (gptneox lib.rs:376-378, gpt2 :353-355, gptj :329-331, mpt :277-279)
@@ -285,3 +288,6 @@ class NeoxSession(_Generation, _Snapshots, _Native):
 
     def sync(self):
         self.L.b200_neox_sync(self._s)
+
+
+GptNeoX._SESSION = NeoxSession

@@ -396,6 +396,77 @@ class _Generation:
         return stats
 
 
+class _BatchedSessions:
+    """Batched decode over the sessions of one model (include/llm_b200.h: b200_model_evaluate_sessions / b200_neox_evaluate_sessions):
+    `_EVAL_SESSIONS` and `_INFER_SESSIONS` name the library's entry points, `_SESSION` the model's session class; the model keeps `L`, `_m` and
+    `hyperparameters`."""
+    _EVAL_SESSIONS, _INFER_SESSIONS = "", ""
+    _SESSION: type = type(None)
+    MAX_SESSIONS = 64                           # B200_MAX_SESSIONS
+
+    def _session_handles(self, sessions):
+        return (C.c_void_p * max(1, len(sessions)))(*[s._s for s in sessions])
+
+    def _own(self, sessions, what):
+        """the library cannot tell one runtime's session handle from another's, nor check a handle it was not given by this model's runtime"""
+        for s in sessions:
+            if not isinstance(s, self._SESSION):
+                raise TypeError(f"{what}: {type(s).__name__} is not a {self._SESSION.__name__}")
+            if s.model is not self:
+                raise RuntimeError(f"{what}: a session of another model")
+
+    def evaluate_sessions(self, sessions: Sequence["InferenceSession"], tokens) -> np.ndarray:
+        """One decode step for several sessions of this model: session i evaluates tokens[i] at its own n_past, reading the weights once for
+        all of them.  Each session ends exactly as after session.evaluate([tokens[i]]) alone, bit for bit.  Returns the [n, n_vocab] logits.
+        Refused as a whole, nothing changed (RuntimeError, or ContextFull when a session has no room): 0 or more than 64 sessions, a session of
+        another model, the same session twice, FAST sessions (LLaMA), mixed KV cache types, an id outside the vocabulary; TypeError for a session that
+        is not of this model's runtime.  See include/llm_b200.h."""
+        tokens = np.ascontiguousarray(tokens, np.int32).ravel()
+        n = len(sessions)
+        if tokens.size != n:
+            raise ValueError(f"{n} sessions, {tokens.size} tokens")
+        self._own(sessions, "evaluate_sessions")
+        out = np.empty((max(n, 1), int(self.hyperparameters["n_vocab"])), np.float32)
+        _check(getattr(self.L, self._EVAL_SESSIONS)(self._m, self._session_handles(sessions), n, tokens.ctypes.data_as(C.c_void_p),
+                                                   out.ctypes.data_as(C.c_void_p)), "evaluate_sessions")
+        for i, s in enumerate(sessions):
+            s._last_logits = None
+        return out[:n]
+
+    def infer_next_tokens(self, sessions: Sequence["InferenceSession"], params, rngs: Sequence[Rng]) -> List[int]:
+        """infer_next_token for several sessions at once: session i samples from its last row with its own parameters and rngs[i], then one
+        batched step evaluates every sampled id.  `params`: one InferenceParameters (or None) for all, or one per session.  Returns the ids; each
+        rngs[i].draw advances by one for every session that sampled.  End of text is NOT raised: the id is returned (and has been evaluated), and
+        the caller compares it with eot_token_id().  A session whose row holds a NaN is left as it was; once the others have advanced,
+        SamplerFailure is raised with `.sessions`, the failed indices, and `.tokens`, the ids (-1 at the failed ones)."""
+        n = len(sessions)
+        plist = list(params) if isinstance(params, (list, tuple)) else [params] * n
+        if len(plist) != n or len(rngs) != n:
+            raise ValueError(f"{n} sessions, {len(plist)} parameters, {len(rngs)} rngs")
+        table = (_lib.SamplerParams * max(n, 1))()
+        for i, (p, rng) in enumerate(zip(plist, rngs)):
+            sp = (p or InferenceParameters()).sampler
+            table[i] = _lib.SamplerParams(repetition_penalty=sp.repetition_penalty, repetition_last_n=sp.repetition_last_n, top_k=sp.top_k,
+                                          top_p=sp.top_p, temperature=sp.temperature, seed=rng.seed, draw=rng.draw)
+        self._own(sessions, "infer_next_tokens")
+        toks, status = np.full(max(n, 1), -1, np.int32), np.zeros(max(n, 1), np.int32)
+        _check(getattr(self.L, self._INFER_SESSIONS)(self._m, self._session_handles(sessions), n, table, toks.ctypes.data_as(C.c_void_p),
+                                                   status.ctypes.data_as(C.c_void_p)), "infer_next_tokens")
+        failed = []
+        for i, (s, rng) in enumerate(zip(sessions, rngs)):
+            if status[i] == 0:
+                rng.draw += 1
+                s._last_logits = None
+            else:
+                failed.append(i)
+        ids = [int(t) for t in toks[:n]]
+        if failed:
+            err = SamplerFailure(f"infer_next_tokens: sampler failure in sessions {failed}")
+            err.sessions, err.tokens = failed, ids
+            raise err
+        return ids
+
+
 def _vocab_id(vocabulary, token: bytes) -> Optional[int]:
     try:
         return vocabulary.index(token)
@@ -448,10 +519,11 @@ def ggml_dims(arr: np.ndarray, wtype: int):
     return 2, arr.shape[-1] // block * 32, arr.size // arr.shape[-1]
 
 
-class Llama(_Native):
+class Llama(_BatchedSessions, _Native):
     """KnownModel for LLaMA.  `hyperparameters` is a dict with n_vocab, n_embd, n_head, n_head_kv, n_layer, n_rot, n_ff, wtype.
     `tensor_types`: {name: enum ggml_type} of 2-D weights whose type is not `wtype` (mixed-type files, b200_llama_new_typed)."""
     _HANDLE, _FREE = "_m", "b200_model_free"
+    _EVAL_SESSIONS, _INFER_SESSIONS = "b200_model_evaluate_sessions", "b200_model_infer_next_tokens"
     tensor_types: Dict[str, int] = {}           # models loaded from a file or cut into shards: their types are in the C model
 
     def __init__(self, hyperparameters: Dict[str, int], params: ModelParameters = None, tensors: Dict[str, np.ndarray] = None,
@@ -527,59 +599,6 @@ class Llama(_Native):
 
     def context_size(self) -> int:
         return self.params.context_size
-
-    MAX_SESSIONS = 64                           # B200_MAX_SESSIONS
-
-    def _session_handles(self, sessions):
-        return (C.c_void_p * max(1, len(sessions)))(*[s._s for s in sessions])
-
-    def evaluate_sessions(self, sessions: Sequence["InferenceSession"], tokens) -> np.ndarray:
-        """One decode step for several sessions of this model: session i evaluates tokens[i] at its own n_past, reading the weights once for
-        all of them.  Each session ends exactly as after session.evaluate([tokens[i]]) alone, bit for bit.  Returns the [n, n_vocab] logits.
-        Refused as a whole, nothing changed (RuntimeError, or ContextFull when a session has no room): 0 or more than 64 sessions, a session of
-        another model, the same session twice, FAST sessions, mixed KV cache types, an id outside the vocabulary.  See include/llm_b200.h."""
-        tokens = np.ascontiguousarray(tokens, np.int32).ravel()
-        n = len(sessions)
-        if tokens.size != n:
-            raise ValueError(f"{n} sessions, {tokens.size} tokens")
-        out = np.empty((max(n, 1), int(self.hyperparameters["n_vocab"])), np.float32)
-        _check(self.L.b200_model_evaluate_sessions(self._m, self._session_handles(sessions), n, tokens.ctypes.data_as(C.c_void_p),
-                                                   out.ctypes.data_as(C.c_void_p)), "evaluate_sessions")
-        for i, s in enumerate(sessions):
-            s._last_logits = None
-        return out[:n]
-
-    def infer_next_tokens(self, sessions: Sequence["InferenceSession"], params, rngs: Sequence[Rng]) -> List[int]:
-        """infer_next_token for several sessions at once: session i samples from its last row with its own parameters and rngs[i], then one
-        batched step evaluates every sampled id.  `params`: one InferenceParameters (or None) for all, or one per session.  Returns the ids; each
-        rngs[i].draw advances by one for every session that sampled.  End of text is NOT raised: the id is returned (and has been evaluated), and
-        the caller compares it with eot_token_id().  A session whose row holds a NaN is left as it was; once the others have advanced,
-        SamplerFailure is raised with `.sessions`, the failed indices, and `.tokens`, the ids (-1 at the failed ones)."""
-        n = len(sessions)
-        plist = list(params) if isinstance(params, (list, tuple)) else [params] * n
-        if len(plist) != n or len(rngs) != n:
-            raise ValueError(f"{n} sessions, {len(plist)} parameters, {len(rngs)} rngs")
-        table = (_lib.SamplerParams * max(n, 1))()
-        for i, (p, rng) in enumerate(zip(plist, rngs)):
-            sp = (p or InferenceParameters()).sampler
-            table[i] = _lib.SamplerParams(repetition_penalty=sp.repetition_penalty, repetition_last_n=sp.repetition_last_n, top_k=sp.top_k,
-                                          top_p=sp.top_p, temperature=sp.temperature, seed=rng.seed, draw=rng.draw)
-        toks, status = np.full(max(n, 1), -1, np.int32), np.zeros(max(n, 1), np.int32)
-        _check(self.L.b200_model_infer_next_tokens(self._m, self._session_handles(sessions), n, table, toks.ctypes.data_as(C.c_void_p),
-                                                   status.ctypes.data_as(C.c_void_p)), "infer_next_tokens")
-        failed = []
-        for i, (s, rng) in enumerate(zip(sessions, rngs)):
-            if status[i] == 0:
-                rng.draw += 1
-                s._last_logits = None
-            else:
-                failed.append(i)
-        ids = [int(t) for t in toks[:n]]
-        if failed:
-            err = SamplerFailure(f"infer_next_tokens: sampler failure in sessions {failed}")
-            err.sessions, err.tokens = failed, ids
-            raise err
-        return ids
 
     def bot_token_id(self) -> Optional[int]:
         """KnownModel::bot_token_id: LLaMA has none (llama lib.rs:382-384)"""
@@ -702,3 +721,6 @@ class InferenceSession(_Generation, _Snapshots, _Native):
     @property
     def last_launches(self) -> int:
         return self.L.b200_session_last_launches(self._s)
+
+
+Llama._SESSION = InferenceSession
