@@ -269,6 +269,23 @@ int  b200_model_evaluate_sessions(b200_model *m, b200_session *const *sessions, 
 int  b200_model_infer_next_tokens(b200_model *m, b200_session *const *sessions, int32_t n, const b200_sampler *samplers,
                                   int32_t *tokens_out, int32_t *status_out);
 
+/* ---- ragged batched evaluation: one step feeds many sessions of one LLaMA model a chunk of tokens each -----------------------------------
+ * Session i evaluates counts[i] >= 1 tokens, taken in order from tokens[] (the chunks back to back, session 0's first), at its own n_past; the
+ * weights are read once for all sum(counts) rows.  New sessions prefill their prompts in the same pass as others decode (continuous batching).
+ * Every session ends exactly as after b200_session_evaluate(s_i, its chunk, counts[i], .., all_logits) alone, bit for bit: n_past + counts[i],
+ * its chunk appended to its history, its cache slots [n_past, n_past + counts[i]) written, last_n = counts[i], and the last row (and with
+ * all_logits every row of the chunk) what last_logits, top_k, infer_next_token and get_snapshot read; last_launches is the step's launch count.
+ * A later single-session step uploads the new n_past to its decode graphs.  b200_model_evaluate_sessions and b200_model_infer_next_tokens are
+ * this step with every count 1.
+ * logits_out (nullable): all_logits ? sum(counts) rows in token order : n rows, session i's last row.
+ * Refused as a whole, with nothing enqueued and no session changed:
+ *   B200_ERR_BAD_ARG        every refusal of b200_model_evaluate_sessions; null counts or tokens; counts[i] < 1 or above the session's n_batch (the
+ *                           single evaluate's rule); sum(counts) > B200_MAX_BATCH_ROWS; a token id outside [0, n_vocab)
+ *   B200_ERR_CONTEXT_FULL   n_past + counts[i] > context_size for some session, the single evaluate's rule */
+#define B200_MAX_BATCH_ROWS 4096   /* sum of counts[] in one ragged step */
+int  b200_model_evaluate_ragged(b200_model *m, b200_session *const *sessions, int32_t n, const int32_t *counts, const int32_t *tokens,
+                                float *logits_out, int32_t all_logits);
+
 /* the token ids at positions [0, n_past) -- what every evaluate fed and infer_next_token sampled (InferenceSession::tokens); a rewind truncates
  * them.  Copies min(n_past, max) ids and returns n_past, or a negative error code. */
 int32_t b200_session_read_tokens(b200_session *s, int32_t *tokens_out, int32_t max);
@@ -432,6 +449,11 @@ int  b200_neox_evaluate_sessions(b200_neox_model *m, b200_neox_session *const *s
  * session is not stepped, so its n_past, history, last row and cache are as they were, while the others advance.  The call returns B200_OK then. */
 int  b200_neox_infer_next_tokens(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const b200_sampler *samplers,
                                  int32_t *tokens_out, int32_t *status_out);
+/* b200_model_evaluate_ragged for this runtime, with b200_neox_evaluate as the single call: session i evaluates counts[i] tokens of tokens[]
+ * at its own n_past, bit-identical to evaluating its chunk alone; the same refusals (no FAST or tensor-parallel sessions exist here), and
+ * b200_neox_evaluate_sessions / b200_neox_infer_next_tokens are this step with every count 1. */
+int  b200_neox_evaluate_ragged(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const int32_t *counts, const int32_t *tokens,
+                               float *logits_out, int32_t all_logits);
 
 /* ---- session snapshots: InferenceSession::get_snapshot / from_snapshot (crates/llm-base/src/inference_session.rs:591-646, types :733-792) and the
  * CLI's session files (--save-session / --load-session / --persist-session, binaries/llm-cli/src/snapshot.rs) ------------------------------------

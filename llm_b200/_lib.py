@@ -99,6 +99,7 @@ def lib():
     L.b200_session_infer_next_token.argtypes = [vp, C.POINTER(SamplerParams), C.POINTER(i32)]
     L.b200_model_evaluate_sessions.argtypes = [vp, C.POINTER(vp), i32, vp, vp]
     L.b200_model_infer_next_tokens.argtypes = [vp, C.POINTER(vp), i32, C.POINTER(SamplerParams), vp, vp]
+    L.b200_model_evaluate_ragged.argtypes = [vp, C.POINTER(vp), i32, vp, vp, vp, i32]
     L.b200_session_read_tokens.restype = i32
     L.b200_session_read_tokens.argtypes = [vp, vp, i32]
     L.b200_session_last_logits.argtypes = [vp, vp]

@@ -198,17 +198,19 @@ __global__ void __launch_bounds__(F16X_WARPS * 32) mul_mat_f32_exact_kernel(cons
 // hadds) is: in-thread, quad shuffle 2, quad shuffle 1, in-thread -- the reference's association exactly.  Inner loop per thread and 32-element
 // step: 12 LDS.128 + 64 FFMA.
 constexpr int FT_A = 16, FT_B = 32, FT_K = 64, FT_STRIDE = FT_K + 4, FT_THREADS = 256;      // stride 68 floats: quads of a quarter-warp hit disjoint banks
+static_assert(FT_B == ATTN_TILE_ROWS, "a ragged step's tile table counts query tiles of FT_B rows");
 
 template <bool F32>
 __device__ __forceinline__ void mul_mat_attn_tiled(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                                                    const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
-                                                   char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
+                                                   char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past,
+                                                   unsigned bx, unsigned by, unsigned bz) {   // the output tile (the grid's, or a ragged step's)
     using T0 = typename AttnSrc0<F32>::T;
     using RA = typename std::conditional<F32, float4, uint2>::type;                   // one thread's 4 src0 elements
     __shared__ __align__(16) float sa[2][FT_A][FT_STRIDE];
     __shared__ __align__(16) float sb[2][FT_B][FT_STRIDE];
     const int tid = threadIdx.x, u = tid & 3, bq = (tid >> 2) & 7, ap = tid >> 5;        // quad (ap, bq): src0 rows 2ap, 2ap+1 x src1 rows 4bq..4bq+3
-    const int64_t a0 = (int64_t)blockIdx.x * FT_A, b0 = (int64_t)blockIdx.y * FT_B, i2 = blockIdx.z;
+    const int64_t a0 = (int64_t)bx * FT_A, b0 = (int64_t)by * FT_B, i2 = bz;
     if (causal_past >= 0 && a0 > causal_past + (b0 + FT_B - 1 < ne11 - 1 ? b0 + FT_B - 1 : ne11 - 1)) return;      // whole tile above the diagonal
     const int64_t i02 = i2 / (ne12 / ne02);
     const char *A = src0 + i02 * nb02, *Bm = src1 + i2 * nb12;
@@ -313,13 +315,15 @@ __device__ __forceinline__ void mul_mat_attn_tiled(const char *__restrict__ src0
 __global__ void __launch_bounds__(FT_THREADS) mul_mat_f16_tiled_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                                                                        const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                                                                        char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
-    mul_mat_attn_tiled<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+    mul_mat_attn_tiled<false>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past,
+                              blockIdx.x, blockIdx.y, blockIdx.z);
 }
 // (FT_THREADS, 1): without the one-CTA hint ptxas caps the f32 form at 128 registers and spills 24 bytes inside the main loop; it needs 145
 __global__ void __launch_bounds__(FT_THREADS, 1) mul_mat_f32_tiled_kernel(const char *__restrict__ src0, int64_t ne00, int64_t ne01, int64_t ne02, int64_t nb01, int64_t nb02,
                                                                        const char *__restrict__ src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                                                                        char *__restrict__ dst, int64_t nbd1, int64_t nbd2, int causal_past) {
-    mul_mat_attn_tiled<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past);
+    mul_mat_attn_tiled<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past,
+                              blockIdx.x, blockIdx.y, blockIdx.z);
 }
 
 // the tiled kernel wants src0 rows aligned to its 4-element loads (8 bytes f16, 16 bytes f32) and 16-byte aligned src1 rows; a handful of src1
@@ -356,48 +360,131 @@ void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne
     mul_mat_attn<true>(src0, ne00, ne01, ne02, nb01, nb02, src1, ne11, ne12, nb11, nb12, dst, nbd1, nbd2, causal_past, st);
 }
 
-// ---- the same two mat-muls for a batched decode step: row (session) blockIdx.z of n, each on its own cache and position ---------------------
-// One output per warp, as mul_mat_f16_exact_kernel / mul_mat_f32_exact_kernel with one src1 row: the same dot, chains, tree and leftovers.
-// KQ: grid (max_n_kv / 8, n_head, n); outputs past the row's n_kv exit at once.
+// ---- the same two mat-muls for a batched step: each chunk on its own cache and positions (kernels.cuh: BatchStep) ----------------------------
+// Warp form: row warp[blockIdx.z] of the step, one output per warp, as mul_mat_f16_exact_kernel / mul_mat_f32_exact_kernel with one src1 row:
+// the same dot, chains, tree and leftovers.  KQ: grid (max_n_kv / 8, n_head, n_warp); outputs past the row's pos exit at once.
 template <bool F32>
-__global__ void __launch_bounds__(F16X_WARPS * 32) attn_kq_rows_kernel(const BatchRow *__restrict__ rows, size_t layer_off, const float *__restrict__ q, int64_t q_ld,
-                                                                       int64_t q_hs, int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ kq) {
+__global__ void __launch_bounds__(F16X_WARPS * 32) attn_kq_rows_kernel(const BatchRow *__restrict__ rows, const int32_t *__restrict__ warp, size_t layer_off,
+                                                                       const float *__restrict__ q, int64_t q_ld, int64_t q_hs, int hd, int n_head, int n_head_kv,
+                                                                       int n_ctx, float *__restrict__ kq) {
     constexpr int64_t es = F32 ? 4 : 2;
     const int64_t gqa = (int64_t)n_head_kv * hd;
-    const int z = blockIdx.z, n_past = rows[z].n_past;
-    const char *K = (const char *)rows[z].K + layer_off * es;
-    mul_mat_attn_warp<F32>(K, hd, n_past + 1, n_head_kv, gqa * es, hd * es, (const char *)(q + z * q_ld), 1, n_head, 0, q_hs * 4,
-                           (char *)(kq + (int64_t)z * n_head * n_ctx), 0, (int64_t)n_ctx * 4, n_past,
+    const int z = warp[blockIdx.z];
+    const BatchRow &r = rows[z];
+    const char *K = (const char *)r.K + layer_off * es;
+    mul_mat_attn_warp<F32>(K, hd, r.n_kv, n_head_kv, gqa * es, hd * es, (const char *)(q + z * q_ld), 1, n_head, 0, q_hs * 4,
+                           (char *)(kq + (int64_t)z * n_head * n_ctx), 0, (int64_t)n_ctx * 4, r.pos,
                            blockIdx.x, 0, blockIdx.y);
 }
-// KQV: grid (hd / 8, n_head, n); out row z holds the merged heads [n_head][hd]
+// KQV: grid (hd / 8, n_head, n_warp); out row z holds the merged heads [n_head][hd]
 template <bool F32>
-__global__ void __launch_bounds__(F16X_WARPS * 32) attn_kqv_rows_kernel(const BatchRow *__restrict__ rows, size_t layer_off, const float *__restrict__ kq,
-                                                                        int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ out, int64_t ld_out) {
+__global__ void __launch_bounds__(F16X_WARPS * 32) attn_kqv_rows_kernel(const BatchRow *__restrict__ rows, const int32_t *__restrict__ warp, size_t layer_off,
+                                                                        const float *__restrict__ kq, int hd, int n_head, int n_head_kv, int n_ctx,
+                                                                        float *__restrict__ out, int64_t ld_out) {
     constexpr int64_t es = F32 ? 4 : 2;
-    const int z = blockIdx.z;
-    const char *V = (const char *)rows[z].V + layer_off * es;
-    mul_mat_attn_warp<F32>(V, rows[z].n_past + 1, hd, n_head_kv, (int64_t)n_ctx * es, (int64_t)n_ctx * hd * es, (const char *)(kq + (int64_t)z * n_head * n_ctx),
+    const int z = warp[blockIdx.z];
+    const BatchRow &r = rows[z];
+    const char *V = (const char *)r.V + layer_off * es;
+    mul_mat_attn_warp<F32>(V, r.n_kv, hd, n_head_kv, (int64_t)n_ctx * es, (int64_t)n_ctx * hd * es, (const char *)(kq + (int64_t)z * n_head * n_ctx),
                            1, n_head, 0, (int64_t)n_ctx * 4, (char *)(out + z * ld_out), 0, (int64_t)hd * 4, -1,
                            blockIdx.x, 0, blockIdx.y);
 }
 
-void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int64_t q_hs, int hd, int n_head,
-                  int n_head_kv, int n_ctx, float *kq, cudaStream_t st) {
-    B200_ASSERT(n >= 1 && n <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
-    const dim3 grid((unsigned)((max_n_kv + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)n);
-    (kv_type == T_F32 ? attn_kq_rows_kernel<true> : attn_kq_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(rows, layer_off, q, q_ld, q_hs, hd, n_head, n_head_kv,
-                                                                                                                 n_ctx, kq);
-    B200_CHECK(cudaGetLastError());
+// Tiled form: tile {chunk, query tile} = tiles[blockIdx.y], each chunk addressed as its single evaluate addresses its own buffers -- its cache at
+// layer_off, its q rows inside the step's qkv rows, its kq rows n_head * n_ctx apart, causal_past = n_past -- with the step's kq layout
+// [rows][n_head][n_ctx] and merged output rows.  KQ: grid (max_n_kv / 16, n_tiles, n_head); tiles past the chunk's n_kv exit at once, as do
+// whole tiles above the diagonal.
+template <bool F32>
+__device__ __forceinline__ void attn_kq_tile(const BatchChunk *__restrict__ chunks, const int2 *__restrict__ tiles, size_t layer_off, const float *__restrict__ q,
+                                             int64_t q_ld, int64_t q_hs, int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ kq) {
+    constexpr int64_t es = F32 ? 4 : 2;
+    const int2 t = tiles[blockIdx.y];
+    const BatchChunk c = chunks[t.x];
+    const int64_t n_kv = (int64_t)c.n_past + c.n, gqa = (int64_t)n_head_kv * hd;
+    if ((int64_t)blockIdx.x * FT_A >= n_kv) return;                      // the whole CTA: before the tile's first barrier
+    mul_mat_attn_tiled<F32>((const char *)c.K + layer_off * es, hd, n_kv, n_head_kv, gqa * es, hd * es,
+                            (const char *)(q + (int64_t)c.row0 * q_ld), c.n, n_head, q_ld * 4, q_hs * 4,
+                            (char *)(kq + (int64_t)c.row0 * n_head * n_ctx), (int64_t)n_head * n_ctx * 4, (int64_t)n_ctx * 4, c.n_past,
+                            blockIdx.x, (unsigned)t.y, blockIdx.z);
+}
+// KQV: grid (hd / 16, n_tiles, n_head); the dot runs over the chunk's n_kv columns
+template <bool F32>
+__device__ __forceinline__ void attn_kqv_tile(const BatchChunk *__restrict__ chunks, const int2 *__restrict__ tiles, size_t layer_off, const float *__restrict__ kq,
+                                              int hd, int n_head, int n_head_kv, int n_ctx, float *__restrict__ out, int64_t ld_out) {
+    constexpr int64_t es = F32 ? 4 : 2;
+    const int2 t = tiles[blockIdx.y];
+    const BatchChunk c = chunks[t.x];
+    mul_mat_attn_tiled<F32>((const char *)c.V + layer_off * es, (int64_t)c.n_past + c.n, hd, n_head_kv, (int64_t)n_ctx * es, (int64_t)n_ctx * hd * es,
+                            (const char *)(kq + (int64_t)c.row0 * n_head * n_ctx), c.n, n_head, (int64_t)n_head * n_ctx * 4, (int64_t)n_ctx * 4,
+                            (char *)(out + (int64_t)c.row0 * ld_out), ld_out * 4, (int64_t)hd * 4, -1,
+                            blockIdx.x, (unsigned)t.y, blockIdx.z);
+}
+// the launch bounds of mul_mat_f16_tiled_kernel / mul_mat_f32_tiled_kernel (the f32 form needs the one-CTA hint not to spill)
+__global__ void __launch_bounds__(FT_THREADS) attn_kq_tiles_f16_kernel(const BatchChunk *__restrict__ chunks, const int2 *__restrict__ tiles, size_t layer_off,
+                                                                       const float *__restrict__ q, int64_t q_ld, int64_t q_hs, int hd, int n_head, int n_head_kv,
+                                                                       int n_ctx, float *__restrict__ kq) {
+    attn_kq_tile<false>(chunks, tiles, layer_off, q, q_ld, q_hs, hd, n_head, n_head_kv, n_ctx, kq);
+}
+__global__ void __launch_bounds__(FT_THREADS, 1) attn_kq_tiles_f32_kernel(const BatchChunk *__restrict__ chunks, const int2 *__restrict__ tiles, size_t layer_off,
+                                                                          const float *__restrict__ q, int64_t q_ld, int64_t q_hs, int hd, int n_head, int n_head_kv,
+                                                                          int n_ctx, float *__restrict__ kq) {
+    attn_kq_tile<true>(chunks, tiles, layer_off, q, q_ld, q_hs, hd, n_head, n_head_kv, n_ctx, kq);
+}
+__global__ void __launch_bounds__(FT_THREADS) attn_kqv_tiles_f16_kernel(const BatchChunk *__restrict__ chunks, const int2 *__restrict__ tiles, size_t layer_off,
+                                                                        const float *__restrict__ kq, int hd, int n_head, int n_head_kv, int n_ctx,
+                                                                        float *__restrict__ out, int64_t ld_out) {
+    attn_kqv_tile<false>(chunks, tiles, layer_off, kq, hd, n_head, n_head_kv, n_ctx, out, ld_out);
+}
+__global__ void __launch_bounds__(FT_THREADS, 1) attn_kqv_tiles_f32_kernel(const BatchChunk *__restrict__ chunks, const int2 *__restrict__ tiles, size_t layer_off,
+                                                                           const float *__restrict__ kq, int hd, int n_head, int n_head_kv, int n_ctx,
+                                                                           float *__restrict__ out, int64_t ld_out) {
+    attn_kqv_tile<true>(chunks, tiles, layer_off, kq, hd, n_head, n_head_kv, n_ctx, out, ld_out);
 }
 
-void attn_kqv_rows(int kv_type, const BatchRow *rows, int n, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx,
-                   float *out, int64_t ld_out, cudaStream_t st) {
-    B200_ASSERT(n >= 1 && n <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
-    const dim3 grid((unsigned)((hd + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)n);
-    (kv_type == T_F32 ? attn_kqv_rows_kernel<true> : attn_kqv_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(rows, layer_off, kq, hd, n_head, n_head_kv,
-                                                                                                                   n_ctx, out, ld_out);
-    B200_CHECK(cudaGetLastError());
+// mul_mat_attn's alignment test on a chunk's KQ (K rows gqa apart, q rows q_ld apart, heads hd / q_hs apart) and KQV (V rows n_ctx apart, kq rows
+// n_head * n_ctx apart, heads n_ctx apart), for both cache types and every chunk's first row: the buffers themselves are cudaMalloc'd
+bool attn_tiles_aligned(int hd, int64_t q_ld, int64_t q_hs, int n_ctx) {
+    return hd % 4 == 0 && q_ld % 4 == 0 && q_hs % 4 == 0 && n_ctx % 4 == 0;
+}
+
+int attn_kq_step(const BatchStep &p, size_t layer_off, const float *q, int64_t q_ld, int64_t q_hs, int hd, int n_head, int n_head_kv, int n_ctx,
+                 float *kq, cudaStream_t st) {
+    B200_ASSERT(p.n_warp <= 65535 && p.n_tiles <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
+    const bool f32 = p.kv_type == T_F32;
+    int L = 0;
+    if (p.n_warp) {
+        const dim3 grid((unsigned)((p.max_n_kv_warp + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)p.n_warp);
+        (f32 ? attn_kq_rows_kernel<true> : attn_kq_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(p.rows, p.warp, layer_off, q, q_ld, q_hs, hd, n_head,
+                                                                                                         n_head_kv, n_ctx, kq);
+        B200_CHECK(cudaGetLastError()); L++;
+    }
+    if (p.n_tiles) {
+        const dim3 grid((unsigned)((p.max_n_kv_tiles + FT_A - 1) / FT_A), (unsigned)p.n_tiles, (unsigned)n_head);
+        (f32 ? attn_kq_tiles_f32_kernel : attn_kq_tiles_f16_kernel)<<<grid, FT_THREADS, 0, st>>>(p.chunks, p.tiles, layer_off, q, q_ld, q_hs, hd, n_head, n_head_kv,
+                                                                                                n_ctx, kq);
+        B200_CHECK(cudaGetLastError()); L++;
+    }
+    return L;
+}
+
+int attn_kqv_step(const BatchStep &p, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx, float *out, int64_t ld_out,
+                  cudaStream_t st) {
+    B200_ASSERT(p.n_warp <= 65535 && p.n_tiles <= 65535 && n_head <= 65535 && n_head % n_head_kv == 0);
+    const bool f32 = p.kv_type == T_F32;
+    int L = 0;
+    if (p.n_warp) {
+        const dim3 grid((unsigned)((hd + F16X_WARPS - 1) / F16X_WARPS), (unsigned)n_head, (unsigned)p.n_warp);
+        (f32 ? attn_kqv_rows_kernel<true> : attn_kqv_rows_kernel<false>)<<<grid, F16X_WARPS * 32, 0, st>>>(p.rows, p.warp, layer_off, kq, hd, n_head, n_head_kv,
+                                                                                                           n_ctx, out, ld_out);
+        B200_CHECK(cudaGetLastError()); L++;
+    }
+    if (p.n_tiles) {
+        const dim3 grid((unsigned)((hd + FT_A - 1) / FT_A), (unsigned)p.n_tiles, (unsigned)n_head);
+        (f32 ? attn_kqv_tiles_f32_kernel : attn_kqv_tiles_f16_kernel)<<<grid, FT_THREADS, 0, st>>>(p.chunks, p.tiles, layer_off, kq, hd, n_head, n_head_kv, n_ctx,
+                                                                                                  out, ld_out);
+        B200_CHECK(cudaGetLastError()); L++;
+    }
+    return L;
 }
 
 }  // namespace b200

@@ -277,20 +277,36 @@ void SessionCore::copy_row(float *out, const float *row, int n) {
     B200_CHECK(cudaStreamSynchronize(st));
 }
 
-void SessionCore::commit_step(int launches) {
-    n_past += 1;
-    last_n = 1;
+void SessionCore::commit_step(int n, int launches) {
+    n_past += n;
+    last_n = n;
     last_launches = launches;
     decode.dev_n_past = -1;                     // the next graph step uploads n_past
 }
 
-// ---- batched decode (host.h: BatchCore) ------------------------------------------------------------------------------------------------
-// the device half of committing a batched step: row i's id to its session's history at n_past, its logits to row 0 of the session's logits
+// ---- batched steps (host.h: BatchCore) ---------------------------------------------------------------------------------------------------
+// the device half of committing a batched step: row r's id to its session's history at its position, and (when the step computed them) its
+// logits to its session's row
 __global__ void commit_rows_kernel(const BatchRow *__restrict__ rows, const int32_t *__restrict__ ids, const float *__restrict__ logits, int n_vocab) {
     const BatchRow &r = rows[blockIdx.y];
-    const float *src = logits + (size_t)blockIdx.y * n_vocab;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_vocab; i += gridDim.x * blockDim.x) r.logits[i] = src[i];
-    if (blockIdx.x == 0 && threadIdx.x == 0) r.hist[r.n_past] = ids[blockIdx.y];
+    if (r.logits) {
+        const float *src = logits + (size_t)r.lrow * n_vocab;
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_vocab; i += gridDim.x * blockDim.x) r.logits[i] = src[i];
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) r.hist[r.pos] = ids[blockIdx.y];
+}
+
+const int32_t *decode_counts() {
+    static const std::vector<int32_t> ones(B200_MAX_SESSIONS, 1);
+    return ones.data();
+}
+
+// the step's tables for `rows` rows, packed in this order, each 16-byte aligned: BatchRow rows, int32 ids, warp rows, out rows, int2 tiles (at
+// most one per row), then the chunks
+static size_t tab_bytes(int rows) {
+    auto a = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t R = rows;
+    return a(R * sizeof(BatchRow)) + 3 * a(R * 4) + a(R * sizeof(int2)) + a(B200_MAX_SESSIONS * sizeof(BatchChunk));
 }
 
 void BatchCore::reserve(int n, int n_vocab, const BatchFront &f) {
@@ -299,45 +315,84 @@ void BatchCore::reserve(int n, int n_vocab, const BatchFront &f) {
     const size_t B = n;
     f.reserve(B);
     logits = device_alloc<float>(B * (size_t)n_vocab * 4);
-    rows = device_alloc<BatchRow>(B * sizeof(BatchRow)); h_rows = pinned_alloc<BatchRow>(B * sizeof(BatchRow));
-    jobs = device_alloc<SampleJob>(B * sizeof(SampleJob)); h_jobs = pinned_alloc<SampleJob>(B * sizeof(SampleJob));
-    ids = device_alloc<int32_t>(B * 4); h_ids = pinned_alloc<int32_t>(B * 4);
+    tab = device_alloc<char>(tab_bytes(n)); h_tab = pinned_alloc<char>(tab_bytes(n));
+    if (!jobs) { jobs = device_alloc<SampleJob>(B200_MAX_SESSIONS * sizeof(SampleJob)); h_jobs = pinned_alloc<SampleJob>(B200_MAX_SESSIONS * sizeof(SampleJob)); }
     if (!staged) { cudaEvent_t ev; B200_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); staged.reset(ev); }
     cap = n;
 }
 
-// one batched step of sessions ss[0, n) on tokens[0, n) (checked by the caller): stage the row table and the ids, run forward_rows, commit
-// every row.  logits_out (nullable): the n rows.
-void BatchCore::step(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f) {
+// one batched step of sessions ss[0, n), session i on tokens [sum counts[0, i), + counts[i]) (checked by the caller): stage the tables, run
+// forward_rows, commit every row.  Only each chunk's last row reaches the final norm and the lm_head unless all_logits (as in the single
+// evaluate), through a gather when some chunk has more than one row.  logits_out (nullable): every row (all_logits), else each chunk's last.
+void BatchCore::step(const BatchSession *ss, int n, const int32_t *counts, const int32_t *tokens, float *logits_out, bool all_logits, const BatchFront &f) {
     cudaStream_t st = rt().stream;
     const int V = ss[0].s->n_vocab;
-    reserve(n, V, f);
+    int rows_n = 0;
+    bool ones = true;
+    for (int i = 0; i < n; i++) { rows_n += counts[i]; ones &= counts[i] == 1; }
+    reserve(rows_n, V, f);
     B200_CHECK(cudaEventSynchronize(staged.get()));
-    int max_n_kv = 0;
-    for (int i = 0; i < n; i++) {
+    size_t off = 0;
+    auto carve = [&](size_t bytes) { const size_t o = off; off += (bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_rows = carve(rows_n * sizeof(BatchRow)), o_ids = carve(rows_n * 4), o_warp = carve(rows_n * 4), o_out = carve(rows_n * 4),
+                 o_tiles = carve(rows_n * sizeof(int2)), o_chunks = carve(n * sizeof(BatchChunk));
+    char *h = h_tab.get();
+    BatchRow *hr = (BatchRow *)(h + o_rows);
+    int32_t *hid = (int32_t *)(h + o_ids), *hw = (int32_t *)(h + o_warp), *ho = (int32_t *)(h + o_out);
+    int2 *ht = (int2 *)(h + o_tiles);
+    BatchChunk *hc = (BatchChunk *)(h + o_chunks);
+    const bool gather = !all_logits && !ones;
+    int n_warp = 0, max_warp = 0, n_tiles = 0, max_tiles = 0, n_chunks = 0;
+    for (int i = 0, r = 0; i < n; i++) {
         SessionCore *s = ss[i].s;
-        h_rows.get()[i] = BatchRow{s->memory_k.get(), s->memory_v.get(), ss[i].logits, s->history.get(), s->n_past};
-        h_ids.get()[i] = tokens[i];
-        max_n_kv = std::max(max_n_kv, s->n_past + 1);
+        const int c = counts[i], n_kv = s->n_past + c;
+        const bool tiled = f.tiled && c >= ATTN_TILED_MIN_ROWS;                         // mul_mat_attn's choice for the chunk's single evaluate
+        if (tiled) {
+            hc[n_chunks] = BatchChunk{s->memory_k.get(), s->memory_v.get(), r, c, s->n_past};
+            for (int t = 0; t * ATTN_TILE_ROWS < c; t++) ht[n_tiles++] = make_int2(n_chunks, t);
+            n_chunks++;
+            max_tiles = std::max(max_tiles, n_kv);
+        } else {
+            max_warp = std::max(max_warp, n_kv);
+        }
+        for (int j = 0; j < c; j++, r++) {
+            const bool out = all_logits || j == c - 1;
+            hr[r] = BatchRow{s->memory_k.get(), s->memory_v.get(), out ? ss[i].logits + (size_t)j * V : nullptr, s->history.get(), s->n_past + j, n_kv,
+                             out ? (all_logits ? r : i) : -1};
+            hid[r] = tokens[r];
+            if (!tiled) hw[n_warp++] = r;
+            if (gather && j == c - 1) ho[i] = r;
+        }
     }
-    B200_CHECK(cudaMemcpyAsync(rows.get(), h_rows.get(), (size_t)n * sizeof(BatchRow), cudaMemcpyHostToDevice, st));
-    B200_CHECK(cudaMemcpyAsync(ids.get(), h_ids.get(), (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK(cudaMemcpyAsync(tab.get(), h, off, cudaMemcpyHostToDevice, st));
     B200_CHECK(cudaEventRecord(staged.get(), st));
-    int L = f.forward_rows(n, ss[0].s->kv_type, max_n_kv);
-    commit_rows_kernel<<<dim3((unsigned)std::min((V + 255) / 256, 64), (unsigned)n), 256, 0, st>>>(rows.get(), ids.get(), logits.get(), V); L++;
+    const char *d = tab.get();
+    const int n_out = all_logits ? rows_n : n;
+    const BatchStep p{rows_n, ss[0].s->kv_type, (const BatchRow *)(d + o_rows), (const int32_t *)(d + o_ids),
+                      (const int32_t *)(d + o_warp), n_warp, max_warp, (const BatchChunk *)(d + o_chunks), (const int2 *)(d + o_tiles), n_tiles, max_tiles,
+                      gather ? (const int32_t *)(d + o_out) : nullptr, n_out, logits.get()};
+    int L = f.forward_rows(p);
+    commit_rows_kernel<<<dim3((unsigned)std::min((V + 255) / 256, 64), (unsigned)rows_n), 256, 0, st>>>(p.rows, p.ids, logits.get(), V); L++;
     B200_CHECK(cudaGetLastError());
-    for (int i = 0; i < n; i++) ss[i].s->commit_step(L);
+    for (int i = 0; i < n; i++) ss[i].s->commit_step(counts[i], L);
     if (logits_out) {
-        B200_CHECK(cudaMemcpyAsync(logits_out, logits.get(), (size_t)n * V * 4, cudaMemcpyDeviceToHost, st));
+        B200_CHECK(cudaMemcpyAsync(logits_out, logits.get(), (size_t)n_out * V * 4, cudaMemcpyDeviceToHost, st));
         B200_CHECK(cudaStreamSynchronize(st));
     }
 }
 
-int BatchCore::evaluate(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f) {
-    if (!tokens) return B200_ERR_BAD_ARG;
-    for (int i = 0; i < n; i++) if (tokens[i] < 0 || tokens[i] >= ss[i].s->n_vocab) return B200_ERR_BAD_ARG;
-    for (int i = 0; i < n; i++) if (const int rc = ss[i].s->admit(1)) return rc;           // the single-session evaluate's rule
-    step(ss, n, tokens, logits_out, f);
+int BatchCore::evaluate(const BatchSession *ss, int n, const int32_t *counts, const int32_t *tokens, float *logits_out, bool all_logits,
+                        const BatchFront &f) {
+    if (!counts || !tokens) return B200_ERR_BAD_ARG;
+    int64_t rows = 0;
+    for (int i = 0; i < n; i++) {
+        if (counts[i] < 1 || counts[i] > ss[i].s->n_batch) return B200_ERR_BAD_ARG;          // the single-session evaluate's rule (admit)
+        rows += counts[i];
+    }
+    if (rows > B200_MAX_BATCH_ROWS) return B200_ERR_BAD_ARG;
+    for (int64_t r = 0; r < rows; r++) if (tokens[r] < 0 || tokens[r] >= ss[0].s->n_vocab) return B200_ERR_BAD_ARG;
+    for (int i = 0; i < n; i++) if (const int rc = ss[i].s->admit(counts[i])) return rc;
+    step(ss, n, counts, tokens, logits_out, all_logits, f);
     return B200_OK;
 }
 
@@ -372,7 +427,7 @@ int BatchCore::infer(const BatchSession *ss, int n, const b200_sampler *samplers
         status_out[i] = B200_OK; tokens_out[i] = r->id;
         ok[k] = ss[i]; ids_ok[k++] = r->id;
     }
-    if (k) step(ok, k, ids_ok, nullptr, f);
+    if (k) step(ok, k, decode_counts(), ids_ok, nullptr, false, f);
     return B200_OK;
 }
 

@@ -175,9 +175,9 @@ struct SessionCore {
     void copy_logits(float *out, const float *logits, int n, bool all_rows);   // rows [0, n) of logits, or only row n - 1, to out (if not null)
     void copy_row(float *out, const float *row, int n);                        // n floats of a device row to out (if not null), after the queued work
     int set_n_past(int v);
-    // the host half of committing a step of a batched decode to this session (its device half, history[n_past] and row 0 of the logits, is the
-    // step's commit kernel): n_past + 1, last_n 1, the step's launches, and the decode graphs' device n_past stale
-    void commit_step(int launches);
+    // the host half of committing a batched step of n tokens to this session (its device half, history[n_past, n_past + n) and the logits rows, is
+    // the step's commit kernel): n_past + n, last_n n, the step's launches, and the decode graphs' device n_past stale
+    void commit_step(int n, int launches);
     // InferenceSession::perplexity over tokens[0, n) with C = n_ctx: chunk i = [iC, (i+1)C) is evaluated from n_past 0 in batches of n_batch, its
     // first token replaced by bos; rows [min(512, C/2), C - 1) are scored on the device (ppl.cu).  forward(rows) runs one batch of the staged
     // tokens at n_past and leaves every row's logits in `logits`.  Each batch's terms are computed on the stream before the next batch overwrites
@@ -242,8 +242,9 @@ Sess *session_from_snapshot(const b200_snapshot *snap, const char *path, int n_c
 // a b200_sampler as the kernels take it; false if it is out of range (top_k < 1, temperature or penalty <= 0 or NaN, last_n < 0, top_p NaN)
 bool sampler_args(const b200_sampler *s, SampleArgs &a);
 
-// ---- batched decode: one step for n sessions of one model (b200_model_evaluate_sessions, b200_neox_evaluate_sessions) -------------------
-// One session of a batched call: its core and its logits buffer (row 0 takes the step's row).
+// ---- batched steps: one step for n sessions of one model, each evaluating a chunk of its own (b200_model_evaluate_ragged,
+// b200_neox_evaluate_ragged; the decode steps b200_*_evaluate_sessions / b200_*_infer_next_tokens are the steps whose chunks are one token) -----
+// One session of a batched call: its core and its logits buffer (row j takes the row of its chunk's token j).
 struct BatchSession { SessionCore *s; float *logits; };
 // The refusals of a batched call that depend only on its sessions (B200_ERR_BAD_ARG or B200_OK): n outside [1, B200_MAX_SESSIONS], a null
 // entry, a session whose model is not m, the same session twice, sessions whose KV cache types differ.  Fills out[0, n) when it accepts.
@@ -257,30 +258,33 @@ template <class M, class S> int batch_sessions(const M *m, S *const *ss, int n, 
     }
     return B200_OK;
 }
+// the counts of a decode step: B200_MAX_SESSIONS ones
+const int32_t *decode_counts();
 // The front end's half of a batched step.  reserve(n): grow its activations to n rows (the stream is idle when it is called).
-// forward_rows(n, kv_type, max_n_kv): enqueue the forward pass of the n staged rows (BatchCore::rows, ::ids) into BatchCore::logits, every row's
-// arithmetic that of the single-session forward on that row alone, and return its launches (the same for every n).
+// forward_rows(p): enqueue the forward pass of the step's p.n staged rows into p.logits, every row's arithmetic that of its chunk's single-session
+// forward, and return its launches.  tiled: the tiled attention takes the front end's strides (attn_tiles_aligned).
 struct BatchFront {
     std::function<void(size_t n)> reserve;
-    std::function<int(int n, int kv_type, int max_n_kv)> forward_rows;
+    std::function<int(const BatchStep &p)> forward_rows;
+    bool tiled;
 };
-// What a model keeps for its batched steps: the row table, the ids, the sampler jobs, their pinned staging and the logits of n rows, grown on
-// demand to the largest n seen and freed with the model.
+// What a model keeps for its batched steps: the step's tables (rows, ids, the attention plan, the logits rows) in one pinned and one device
+// buffer, the sampler jobs, and the logits of up to `cap` rows, grown on demand to the largest step seen and freed with the model.
 struct BatchCore {
     int cap = 0;
     DeviceBuf<float> logits;
-    DeviceBuf<BatchRow> rows; DeviceBuf<SampleJob> jobs; DeviceBuf<int32_t> ids;
-    PinnedBuf<BatchRow> h_rows; PinnedBuf<SampleJob> h_jobs; PinnedBuf<int32_t> h_ids;
+    DeviceBuf<char> tab; PinnedBuf<char> h_tab;
+    DeviceBuf<SampleJob> jobs; PinnedBuf<SampleJob> h_jobs;
     Event staged;                       // recorded after the uploads: the pinned tables are not rewritten before they have been read
 
-    // b200_model_evaluate_sessions over sessions ss[0, n) that batch_sessions accepted: the ids and the context checked, then one step
-    int evaluate(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f);
+    // b200_model_evaluate_ragged over sessions ss[0, n) that batch_sessions accepted: the counts, the ids and the context checked, then one step
+    int evaluate(const BatchSession *ss, int n, const int32_t *counts, const int32_t *tokens, float *logits_out, bool all_logits, const BatchFront &f);
     // b200_model_infer_next_tokens over accepted sessions: the samplers checked, every row sampled, then one step of the sessions that sampled
     int infer(const BatchSession *ss, int n, const b200_sampler *samplers, int32_t *tokens_out, int32_t *status_out, const BatchFront &f);
 
 private:
-    void reserve(int n, int n_vocab, const BatchFront &f);
-    void step(const BatchSession *ss, int n, const int32_t *tokens, float *logits_out, const BatchFront &f);
+    void reserve(int rows, int n_vocab, const BatchFront &f);
+    void step(const BatchSession *ss, int n, const int32_t *counts, const int32_t *tokens, float *logits_out, bool all_logits, const BatchFront &f);
 };
 
 }  // namespace b200

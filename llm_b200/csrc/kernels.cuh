@@ -177,33 +177,57 @@ void mul_mat_f32_exact(const float *src0, int64_t ne00, int64_t ne01, int64_t ne
                        const float *src1, int64_t ne11, int64_t ne12, int64_t nb11, int64_t nb12,
                        float *dst, int64_t nbd1, int64_t nbd2, int causal_past, cudaStream_t st);
 
-// ---- batched decode over many sessions of one model (b200_model_evaluate_sessions, b200_neox_evaluate_sessions; host.h: BatchCore) -------
-// Row i of a batched step belongs to its own session: the session's whole memory_k / memory_v ([n_layer][n_ctx][gqa] and [n_layer][gqa][n_ctx],
-// of the step's one cache type), its position n_past (the row's token goes to slot n_past), its logits buffer and history.  Uploaded once per step.
-struct BatchRow { void *K, *V; float *logits; int32_t *hist; int n_past; };
+// ---- batched steps over many sessions of one model (b200_model_evaluate_ragged, b200_neox_evaluate_ragged and the decode steps built on them;
+// host.h: BatchCore) ------------------------------------------------------------------------------------------------------------------------
+// Row r of a batched step is token j of its session's chunk of n_s tokens: the session's whole memory_k / memory_v ([n_layer][n_ctx][gqa] and
+// [n_layer][gqa][n_ctx], of the step's one cache type), the row's position pos = n_past_s + j (its token goes to slot pos), its chunk's
+// n_kv = n_past_s + n_s (the columns of its scores, as in the chunk's single evaluate), and its history.  logits: where the row's logits go (its
+// session's row j), from row lrow of the step's logits; nullptr when the step computes none for it.  Uploaded once per step.
+struct BatchRow { void *K, *V; float *logits; int32_t *hist; int pos, n_kv, lrow; };
+// a chunk of 8 rows or more, attended in the tiled form: its session's caches, its first row in the step, its rows and its session's n_past
+struct BatchChunk { void *K, *V; int row0, n, n_past; };
+// One batched step as the kernels see it: device tables and their host counts.  A chunk of fewer than 8 rows (every row of a decode step) is
+// attended one warp per dot, row by row (warp: its rows' indices); a chunk of 8 or more rows, given attn_tiles_aligned, through 32-row query
+// tiles (tiles: {chunk, query tile} pairs), as mul_mat_attn picks the form for the chunk's single evaluate.  out: the rows whose logits are
+// computed, in order (each chunk's last row), or nullptr when every row's are.
+constexpr int ATTN_TILE_ROWS = 32, ATTN_TILED_MIN_ROWS = 8;        // query rows per tile of the tiled form (exact.cu: FT_B); the fewest it takes
+struct BatchStep {
+    int n, kv_type;                                 // rows; the sessions' cache type
+    const BatchRow *rows; const int32_t *ids;
+    const int32_t *warp; int n_warp, max_n_kv_warp;
+    const BatchChunk *chunks; const int2 *tiles; int n_tiles, max_n_kv_tiles;
+    const int32_t *out; int n_out;
+    float *logits;                                  // n_out (out) or n rows of n_vocab
+};
 // where q / k / v of head h start inside a row of the fused qkv projection: h * head_stride, + k_off, + v_off.  LLaMA: (hd, e, e + gqa);
 // GPT-NeoX: per head [q | k | v] (3 hd, hd, 2 hd); GPT-2, MPT, BLOOM, GPT-J: the three thirds of the row (hd, e, 2 e)
 struct QkvLayout { int head_stride, k_off, v_off; };
-// rowops.cu: RoPE on the n_head q and n_head_kv k heads of row i of qkv ([n][qkv_ld], laid out by `lay`) at position rows[i].n_past, in place,
+// rowops.cu: RoPE on the n_head q and n_head_kv k heads of row i of qkv ([n][qkv_ld], laid out by `lay`) at position rows[i].pos, in place,
 // and the row's K (all hd elements of each head, roped or not) / V stored into its session's cache at that slot (layer_off: elements to this
 // layer's slice; V transposed, by channel) -- rope_f32 + cpy_strided of forward() on each row.  tab: mode 0 (adjacent pairs, LLaMA and GPT-J)
 // or mode 2 (rope_f32's NeoX pairing on chunks of n_dims, GPT-NeoX) over the head's hd elements; nullptr: no rotation (GPT-2, MPT, BLOOM).
 // One launch.
 void rope_store_rows(float *qkv, int64_t qkv_ld, QkvLayout lay, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off,
                      int n_ctx, int kv_type, const RopeTable *tab, cudaStream_t st);
-// rowops.cu: kq[i][h][0, n_past_i + 1) = soft_max(scale * kq[i][h][.]) (the row stride is n_ctx), soft_max's arithmetic per row.  One launch.
+// rowops.cu: kq[i][h][0, n_kv_i) = soft_max(scale * kq[i][h][.]) with the columns past pos_i masked (the row stride is n_ctx): soft_max's
+// arithmetic on row pos_i - n_past of its chunk's [n_kv] rows.  One launch.
 void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, cudaStream_t st);
 // rowops.cu: the same with head h's ALiBi term, soft_max_alibi's arithmetic per row (alibi: device slopes [n_head]).  One launch.
 void soft_max_alibi_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, const float *alibi, cudaStream_t st);
-// rowops.cu: x[i][c] += wpe[n_past_i][c] for c < e -- GPT-2's learned position of each row, add_f32's rounding.  One launch.
+// rowops.cu: x[i][c] += wpe[pos_i][c] for c < e -- GPT-2's learned position of each row, add_f32's rounding.  One launch.
 void add_pos_rows(float *x, const float *wpe, const BatchRow *rows, int n, int e, cudaStream_t st);
-// exact.cu: KQ and KQV of forward() on each row's own cache, in mul_mat_f16_exact / mul_mat_f32_exact's arithmetic (kv_type T_F16 / T_F32):
-//   kq[i][h][j] = K_i[j][hk] . Q[i][h] for j <= n_past_i (q rows of stride q_ld, head h at h * q_hs; kq rows of stride n_ctx, [n][n_head]);
-//   out[i][h * hd + c] = V_i[hk][c][:] . kq[i][h][:]  (out rows of stride ld_out).  max_n_kv: the largest n_past_i + 1.  One launch each.
-void attn_kq_rows(int kv_type, const BatchRow *rows, int n, int max_n_kv, size_t layer_off, const float *q, int64_t q_ld, int64_t q_hs, int hd, int n_head,
-                  int n_head_kv, int n_ctx, float *kq, cudaStream_t st);
-void attn_kqv_rows(int kv_type, const BatchRow *rows, int n, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx,
-                   float *out, int64_t ld_out, cudaStream_t st);
+// rowops.cu: dst[k][0, e) = x[idx[k]][0, e) for k < n (the last rows of a step's chunks, before the final norm).  One launch.
+void gather_rows(const float *x, int64_t e, const int32_t *idx, int n, float *dst, cudaStream_t st);
+// exact.cu: KQ and KQV of forward() on each chunk's own cache, in mul_mat_f16_exact / mul_mat_f32_exact's arithmetic (kv_type T_F16 / T_F32):
+//   kq[i][h][j] = K_i[j][hk] . Q[i][h] for j <= pos_i (q rows of stride q_ld, head h at h * q_hs; kq rows of stride n_ctx, [n][n_head]);
+//   out[i][h * hd + c] = V_i[hk][c][0, n_kv_i) . kq[i][h][0, n_kv_i)  (out rows of stride ld_out).
+// One launch per form the step holds (warp rows, tiles); returns the launches.
+int attn_kq_step(const BatchStep &p, size_t layer_off, const float *q, int64_t q_ld, int64_t q_hs, int hd, int n_head, int n_head_kv, int n_ctx,
+                 float *kq, cudaStream_t st);
+int attn_kqv_step(const BatchStep &p, size_t layer_off, const float *kq, int hd, int n_head, int n_head_kv, int n_ctx, float *out, int64_t ld_out,
+                  cudaStream_t st);
+// the tiled form's alignment (mul_mat_attn's test) for every chunk of a step: q rows of stride q_ld, heads q_hs apart, hd-wide heads, n_ctx slots
+bool attn_tiles_aligned(int hd, int64_t q_ld, int64_t q_hs, int n_ctx);
 // sample.cu: sample_row for n sessions in one chain of launches (select, merges, tail), session i taken from the grid.  Each job is one session's
 // row, history window, arguments and buffers; its id, n_kept and result are sample_row's.  jobs: device table of n (the caller uploads it).
 struct SampleJob {

@@ -49,8 +49,8 @@ template <class O> constexpr TensorDef<O> bias(const char *n, FRef<O> f, Dim K =
 template <class O> constexpr TensorDef<O> rows(const char *n, QRef<O> q, uint8_t at) { return {n, ROWS, q, nullptr, E, E, at}; }
 template <class O> constexpr TensorDef<O> if_lm_head(TensorDef<O> d) { d.if_lm_head = true; return d; }
 
-// The activations of a batched decode step (b200_neox_evaluate_sessions): rows of n sessions, grown on demand to the largest n seen, freed with
-// the model.
+// The activations of a batched step (b200_neox_evaluate_ragged, b200_neox_evaluate_sessions): the rows of n sessions' chunks, grown on demand to
+// the largest step seen, freed with the model.
 struct NeoxBatch {
     BatchCore core;                     // the row table, the ids, the sampler jobs and the logits (host.h)
     DeviceBuf<float> x, cur, qkv, kq, attn, h4, hact, t;
@@ -311,49 +311,51 @@ void forward(b200_neox_session *s, int n, bool all_rows) {
     s->n_past += n;
 }
 
-// ---- batched decode: one step for n sessions of one model (b200_neox_evaluate_sessions) -------------------------------------------------
-// forward() with n rows that belong to n sessions: the weight mat-muls and the row-wise nodes over all n rows; the learned positions, RoPE, the
-// cache stores and the attention per row on its own session's cache and position (the row table).  Each row's arithmetic is forward()'s on that
-// row alone.  Returns the launches; the same for every n.
-int forward_rows(b200_neox_model *m, int n, int kv_type, int max_n_kv, cudaStream_t st) {
+// ---- batched steps: one step for n sessions of one model, a chunk each (b200_neox_evaluate_ragged; decode: chunks of one token) ---------------
+// forward() over the rows of n sessions' chunks: the weight mat-muls and the row-wise nodes over all rows; the learned positions, RoPE, the cache
+// stores and the attention per row on its own session's cache, position and chunk (the step's tables).  Each row's arithmetic is forward()'s on its
+// chunk alone, including the final LayerNorm and the lm_head on each chunk's last row only (p.out) unless every row's logits are asked for.
+// Returns the launches: the same for every step of one-token chunks.
+int forward_rows(b200_neox_model *m, const BatchStep &p, cudaStream_t st) {
     const b200_neox_hparams &hp = m->hp;
     NeoxBatch &w = m->batch;
-    const int e = hp.n_embd, hd = m->hd, n_head = hp.n_head, n_ctx = hp.context_size, V = hp.n_vocab;
+    const int n = p.n, e = hp.n_embd, hd = m->hd, n_head = hp.n_head, n_ctx = hp.context_size, V = hp.n_vocab;
     const int64_t ld3 = 3 * (int64_t)e, e4 = 4 * (int64_t)e, ne = (int64_t)n * e;
     const QkvLayout lay = m->qkv_layout;
-    const BatchRow *rows = w.core.rows.get();
+    const BatchRow *rows = p.rows;
+    const int kv_type = p.kv_type;
     const ExactActs acts{w.xq.get(), w.xds.get(), w.xpack.get(), w.xh.get(), w.xq8k.get()};
-    auto mm = [&](const QWeight &W, const float *x, float *dst, int64_t ldd) { return mul_mat_exact_auto(W, x, W.K, n, dst, ldd, nullptr, 0, acts, st); };
+    auto mm = [&](const QWeight &W, const float *x, float *dst, int64_t ldd, int64_t B) { return mul_mat_exact_auto(W, x, W.K, B, dst, ldd, nullptr, 0, acts, st); };
     float *x = w.x.get(), *cur = w.cur.get(), *qkv = w.qkv.get(), *kq = w.kq.get(), *attn = w.attn.get(), *h4 = w.h4.get(), *hact = w.hact.get(),
-          *t = w.t.get(), *logits = w.core.logits.get();
+          *t = w.t.get(), *logits = p.logits;
     int L = 0;
     if (m->emb_g) {
-        get_rows_q(m->wte, w.core.ids.get(), t, n, st); L++;
+        get_rows_q(m->wte, p.ids, t, n, st); L++;
         layer_norm(t, x, m->emb_g, m->emb_b, e, n, st); L++;
     } else {
-        get_rows_q(m->wte, w.core.ids.get(), x, n, st); L++;
+        get_rows_q(m->wte, p.ids, x, n, st); L++;
     }
     if (m->wpe) { add_pos_rows(x, m->wpe, rows, n, e, st); L++; }
     for (int il = 0; il < hp.n_layer; il++) {
         const b200_neox_model::Layer &ly = m->layers[il];
         const size_t layer_off = (size_t)il * n_ctx * e;
         layer_norm(x, cur, ly.ln1_g, ly.ln1_b, e, n, st); L++;
-        L += mm(ly.wqkv, cur, qkv, ld3);
-        if (ly.wv.N) L += mm(ly.wv, cur, qkv + lay.v_off, ld3);
+        L += mm(ly.wqkv, cur, qkv, ld3, n);
+        if (ly.wv.N) L += mm(ly.wv, cur, qkv + lay.v_off, ld3, n);
         if (ly.bqkv) { add_f32(qkv, ly.bqkv, qkv, n * ld3, ld3, st); L++; }
         rope_store_rows(qkv, ld3, lay, hd, n_head, n_head, rows, n, layer_off, n_ctx, kv_type, m->rope, st); L++;
-        attn_kq_rows(kv_type, rows, n, max_n_kv, layer_off, qkv, ld3, lay.head_stride, hd, n_head, n_head, n_ctx, kq, st); L++;
+        L += attn_kq_step(p, layer_off, qkv, ld3, lay.head_stride, hd, n_head, n_head, n_ctx, kq, st);
         if (m->alibi) soft_max_alibi_rows(kq, rows, n, n_head, n_ctx, m->kq_scale, m->alibi.get(), st);
         else soft_max_rows(kq, rows, n, n_head, n_ctx, m->kq_scale, st);
         L++;
         float *kqv = m->gptj() ? t : cur;                     // GPT-J: cur still feeds fc_in
-        attn_kqv_rows(kv_type, rows, n, layer_off, kq, hd, n_head, n_head, n_ctx, kqv, e, st); L++;
-        L += mm(ly.wdense, kqv, attn, e);
+        L += attn_kqv_step(p, layer_off, kq, hd, n_head, n_head, n_ctx, kqv, e, st);
+        L += mm(ly.wdense, kqv, attn, e, n);
         if (m->gptj()) {
-            L += mm(ly.wfc, cur, h4, e4);
+            L += mm(ly.wfc, cur, h4, e4, n);
             add_f32(h4, ly.bfc, h4, n * e4, e4, st); L++;
             unary_lut(UNARY_GELU, h4, hact, n * e4, st); L++;
-            L += mm(ly.wproj, hact, t, e);
+            L += mm(ly.wproj, hact, t, e, n);
             add_f32(t, ly.bproj, t, ne, e, st); L++;
             add_f32(t, attn, t, ne, ne, st); L++;
             add_f32(t, x, x, ne, ne, st); L++;
@@ -363,22 +365,24 @@ int forward_rows(b200_neox_model *m, int n, int kv_type, int max_n_kv, cudaStrea
         const float *ff_in = x;
         if (!m->parallel) { add_f32(attn, x, attn, ne, ne, st); L++; ff_in = attn; }
         layer_norm(ff_in, cur, ly.ln2_g, ly.ln2_b, e, n, st); L++;
-        L += mm(ly.wfc, cur, h4, e4);
+        L += mm(ly.wfc, cur, h4, e4, n);
         if (ly.bfc) { add_f32(h4, ly.bfc, h4, n * e4, e4, st); L++; }
         unary_lut(UNARY_GELU, h4, hact, n * e4, st); L++;
-        L += mm(ly.wproj, hact, t, e);
+        L += mm(ly.wproj, hact, t, e, n);
         if (ly.bproj) { add_f32(t, ly.bproj, t, ne, e, st); L++; }
         add_f32(t, attn, t, ne, ne, st); L++;
         if (m->parallel) { add_f32(t, x, x, ne, ne, st); L++; }
         else { B200_CHECK(cudaMemcpyAsync(x, t, (size_t)ne * 4, cudaMemcpyDeviceToDevice, st)); }
     }
-    layer_norm(x, cur, m->lnf_g, m->lnf_b, e, n, st); L++;
-    L += mm(m->lm_head, cur, logits, V);
-    if (m->lm_head_b) { add_f32(logits, m->lm_head_b, logits, (int64_t)n * V, V, st); L++; }
+    const float *xl = x;
+    if (p.out) { gather_rows(x, e, p.out, p.n_out, attn, st); L++; xl = attn; }         // each chunk's last row (attn is free here)
+    layer_norm(xl, cur, m->lnf_g, m->lnf_b, e, p.n_out, st); L++;
+    L += mm(m->lm_head, cur, logits, V, p.n_out);
+    if (m->lm_head_b) { add_f32(logits, m->lm_head_b, logits, (int64_t)p.n_out * V, V, st); L++; }
     return L;
 }
 
-// the batched step's activations for B rows (BatchCore::reserve, with the stream idle): b200_neox_start_session's buffers
+// the batched step's activations for B rows (BatchCore::reserve, with the stream idle): b200_neox_start_session's buffers; kq is [B][n_head][n_ctx]
 void batch_reserve(b200_neox_model *m, size_t B) {
     NeoxBatch &w = m->batch;
     const b200_neox_hparams &hp = m->hp;
@@ -392,8 +396,8 @@ void batch_reserve(b200_neox_model *m, size_t B) {
 }
 
 BatchFront batch_front(b200_neox_model *m) {
-    return BatchFront{[m](size_t B) { batch_reserve(m, B); },
-                      [m](int n, int kv_type, int max_n_kv) { return forward_rows(m, n, kv_type, max_n_kv, rt().stream); }};
+    return BatchFront{[m](size_t B) { batch_reserve(m, B); }, [m](const BatchStep &p) { return forward_rows(m, p, rt().stream); },
+                      attn_tiles_aligned(m->hd, 3 * (int64_t)m->hp.n_embd, m->qkv_layout.head_stride, m->hp.context_size)};
 }
 
 // a tensor's whole name: the model's own, or the layer prefix of layer il (layer_fmt up to its "%95s") followed by the suffix
@@ -665,11 +669,16 @@ int b200_neox_infer_next_token(b200_neox_session *s, const b200_sampler *sampler
     return s->infer_next_token(a, s->logits.get(), [s]() { forward(s, 1, true); }, token_out);
 }
 
-// ---- batched decode over sessions of one model (include/llm_b200.h) -------------------------------------------------------------------------
-int b200_neox_evaluate_sessions(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out) {
+// ---- batched steps over sessions of one model (include/llm_b200.h) ---------------------------------------------------------------------------
+int b200_neox_evaluate_ragged(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const int32_t *counts, const int32_t *tokens,
+                              float *logits_out, int32_t all_logits) {
     BatchSession ss[B200_MAX_SESSIONS];
     if (const int rc = batch_sessions(m, sessions, n, ss)) return rc;
-    return m->batch.core.evaluate(ss, n, tokens, logits_out, batch_front(m));
+    return m->batch.core.evaluate(ss, n, counts, tokens, logits_out, all_logits != 0, batch_front(m));
+}
+
+int b200_neox_evaluate_sessions(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out) {
+    return b200_neox_evaluate_ragged(m, sessions, n, decode_counts(), tokens, logits_out, 0);
 }
 
 int b200_neox_infer_next_tokens(b200_neox_model *m, b200_neox_session *const *sessions, int32_t n, const b200_sampler *samplers, int32_t *tokens_out,

@@ -362,12 +362,13 @@ void cpy_strided(const void *src, int src_type, const StridedDesc &s, void *dst,
     B200_CHECK(cudaGetLastError());
 }
 
-// ---- batched decode rows (kernels.cuh: BatchRow) ------------------------------------------------------------------------------
-// soft_max of row (blockIdx.y, head blockIdx.x): soft_max_body on its n_past + 1 scores, scaled, one row per matrix (the mask keeps them all)
+// ---- batched step rows (kernels.cuh: BatchRow) ------------------------------------------------------------------------------
+// soft_max of row (blockIdx.y, head blockIdx.x): soft_max_body on its chunk's n_kv scores, scaled, the columns past its position masked -- soft_max
+// on the chunk's rows with this row's j = pos - n_past added to n_past (a decode row: n_kv = pos + 1, the mask keeps them all)
 __global__ void soft_max_rows_kernel(float *__restrict__ kq, const BatchRow *__restrict__ rows, int n_head, int n_ctx, float scale, const uint16_t *__restrict__ t_exp) {
-    const int n_past = rows[blockIdx.y].n_past;
+    const BatchRow &r = rows[blockIdx.y];
     float *x = kq + ((int64_t)blockIdx.y * n_head + blockIdx.x) * n_ctx;
-    soft_max_body<false>(x, x, n_past + 1, 1, scale, 1, n_past, 1, 1, t_exp, nullptr, 0);
+    soft_max_body<false>(x, x, r.n_kv, 1, scale, 1, r.pos, 1, 1, t_exp, nullptr, 0);
 }
 void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, cudaStream_t st) {
     const size_t smem = (size_t)n_ctx * sizeof(float);
@@ -381,13 +382,13 @@ void soft_max_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx
     B200_CHECK(cudaGetLastError());
 }
 
-// soft_max_alibi of row (blockIdx.y, head blockIdx.x): soft_max_body<true> on its n_past + 1 scores with the head's slope (alibi + head and r = 0:
-// alibi[r / nr] is that slope, and column i's term fma(i, slope, v) depends on the key position alone)
+// soft_max_alibi of row (blockIdx.y, head blockIdx.x): soft_max_body<true> on its chunk's n_kv scores, masked past its position, with the head's
+// slope (alibi + head and r = 0: alibi[r / nr] is that slope, and column i's term fma(i, slope, v) depends on the key position alone)
 __global__ void soft_max_alibi_rows_kernel(float *__restrict__ kq, const BatchRow *__restrict__ rows, int n_head, int n_ctx, float scale,
                                            const uint16_t *__restrict__ t_exp, const float *__restrict__ alibi) {
-    const int n_past = rows[blockIdx.y].n_past;
+    const BatchRow &r = rows[blockIdx.y];
     float *x = kq + ((int64_t)blockIdx.y * n_head + blockIdx.x) * n_ctx;
-    soft_max_body<true>(x, x, n_past + 1, 1, scale, 1, n_past, 1, 1, t_exp, alibi + blockIdx.x, 0);
+    soft_max_body<true>(x, x, r.n_kv, 1, scale, 1, r.pos, 1, 1, t_exp, alibi + blockIdx.x, 0);
 }
 void soft_max_alibi_rows(float *kq, const BatchRow *rows, int n, int n_head, int n_ctx, float scale, const float *alibi, cudaStream_t st) {
     const size_t smem = (size_t)n_ctx * sizeof(float);
@@ -405,11 +406,24 @@ __global__ void add_pos_rows_kernel(float *__restrict__ x, const float *__restri
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= total) return;
     const int64_t z = t / e, c = t - z * e;
-    x[t] = __fadd_rn(x[t], wpe[(int64_t)rows[z].n_past * e + c]);
+    x[t] = __fadd_rn(x[t], wpe[(int64_t)rows[z].pos * e + c]);
 }
 void add_pos_rows(float *x, const float *wpe, const BatchRow *rows, int n, int e, cudaStream_t st) {
     const int64_t total = (int64_t)n * e;
     add_pos_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, wpe, rows, e, total);
+    B200_CHECK(cudaGetLastError());
+}
+
+__global__ void gather_rows_kernel(const float *__restrict__ x, int64_t e, const int32_t *__restrict__ idx, float *__restrict__ dst, int64_t total) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int64_t k = t / e, c = t - k * e;
+    dst[t] = x[(int64_t)idx[k] * e + c];
+}
+void gather_rows(const float *x, int64_t e, const int32_t *idx, int n, float *dst, cudaStream_t st) {
+    const int64_t total = (int64_t)n * e;
+    if (total == 0) return;
+    gather_rows_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, e, idx, dst, total);
     B200_CHECK(cudaGetLastError());
 }
 
@@ -419,9 +433,9 @@ __device__ __forceinline__ void kv_store(KT *p, float v) { if constexpr (sizeof(
 
 // thread t of row i, in three ranges:
 //   t < (n_head + n_head_kv) * half: rotates one pair of a q or k head, rope_kernel's pairing (mode 0: adjacent; mode 2: n_dims / 2 apart inside
-//     chunks of n_dims); a k pair is also stored at slot n_past of the row's memory_k;
+//     chunks of n_dims); a k pair is also stored at slot pos of the row's memory_k;
 //   the next n_head_kv * (hd - 2 half): stores one k element no pair covers (every element when nothing rotates, half = 0);
-//   the next gqa: stores one v value at slot n_past of the row's memory_v (transposed: [gqa][n_ctx]).
+//   the next gqa: stores one v value at slot pos of the row's memory_v (transposed: [gqa][n_ctx]).
 template <typename KT>
 __global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, QkvLayout lay, int hd, int n_head, int n_head_kv,
                                        const BatchRow *__restrict__ rows, size_t layer_off, int n_ctx, const float2 *__restrict__ cs, int half,
@@ -429,11 +443,11 @@ __global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, 
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= total) return;
     const int64_t z = t / per_row, k = t - z * per_row;
-    const int n_past = rows[z].n_past;
+    const int pos = rows[z].pos;
     const int64_t gqa = (int64_t)n_head_kv * hd, n_pairs = (int64_t)(n_head + n_head_kv) * half, plain = hd - 2 * half;
     const int64_t n_plain = n_head_kv * plain;
     float *row = qkv + z * qkv_ld;
-    KT *K = (KT *)rows[z].K + layer_off + (size_t)n_past * gqa;
+    KT *K = (KT *)rows[z].K + layer_off + (size_t)pos * gqa;
     if (k < n_pairs) {
         const int i = (int)(k % half);
         const int64_t head = k / half;
@@ -441,7 +455,7 @@ __global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, 
         if (!neox) { e0 = 2 * (int64_t)i; e1 = e0 + 1; }
         else { const int hb = n_dims / 2; const int ib = i / hb, ic = i % hb; e0 = (int64_t)ib * n_dims + ic; e1 = e0 + hb; }
         const int64_t hk = head - n_head, base = hk < 0 ? head * lay.head_stride : lay.k_off + hk * lay.head_stride;
-        const float2 r = rope_pair(row[base + e0], row[base + e1], __ldg(cs + (int64_t)n_past * half + i));
+        const float2 r = rope_pair(row[base + e0], row[base + e1], __ldg(cs + (int64_t)pos * half + i));
         row[base + e0] = r.x;
         row[base + e1] = r.y;
         if (hk >= 0) { kv_store(K + hk * hd + e0, r.x); kv_store(K + hk * hd + e1, r.y); }
@@ -450,7 +464,7 @@ __global__ void rope_store_rows_kernel(float *__restrict__ qkv, int64_t qkv_ld, 
         kv_store(K + hk * hd + d, row[lay.k_off + hk * lay.head_stride + d]);
     } else {
         const int64_t c = k - n_pairs - n_plain, hk = c / hd, d = c % hd;
-        kv_store((KT *)rows[z].V + layer_off + (size_t)c * n_ctx + n_past, row[lay.v_off + hk * lay.head_stride + d]);
+        kv_store((KT *)rows[z].V + layer_off + (size_t)c * n_ctx + pos, row[lay.v_off + hk * lay.head_stride + d]);
     }
 }
 void rope_store_rows(float *qkv, int64_t qkv_ld, QkvLayout lay, int hd, int n_head, int n_head_kv, const BatchRow *rows, int n, size_t layer_off,

@@ -25,8 +25,8 @@ struct Layer {
     QWeight wv;                         // wv of a type other than wq's: then wqkv rows are [wq | wk] and wv is this matrix (wv.N == 0 otherwise)
 };
 
-// The activations of a batched decode step (b200_model_evaluate_sessions): rows of n sessions, grown on demand to the largest n seen, freed with the
-// model.
+// The activations of a batched step (b200_model_evaluate_ragged, b200_model_evaluate_sessions): the rows of n sessions' chunks, grown on demand to
+// the largest step seen, freed with the model.
 struct BatchWs {
     BatchCore core;                     // the row table, the ids, the sampler jobs and the logits (host.h)
     DeviceBuf<float> x, cur, ff, qkv, kq, h13, hmul;
@@ -236,46 +236,49 @@ void forward(b200_session *s, int n, bool all_rows = true) {
     s->n_past += n;                                                                           // inference_session.rs:288
 }
 
-// ---- batched decode: one step for n sessions of one model (b200_model_evaluate_sessions) ------------------------------------------------
-// forward() with n rows that belong to n sessions: the weight mat-muls and the row-wise nodes over all n rows, RoPE, the cache stores and the
-// attention per row on its own session's cache and position (the workspace's row table).  Each row's arithmetic is forward()'s on that row alone.
-// Returns the launches; the same for every n.
-int forward_rows(b200_model *m, int n, int kv_type, int max_n_kv, cudaStream_t st) {
+// ---- batched steps: one step for n sessions of one model, a chunk each (b200_model_evaluate_ragged; decode: chunks of one token) --------------
+// forward() over the rows of n sessions' chunks: the weight mat-muls and the row-wise nodes over all rows, RoPE, the cache stores and the
+// attention per row on its own session's cache, position and chunk (the step's tables).  Each row's arithmetic is forward()'s on its chunk alone,
+// including the final norm and the lm_head on each chunk's last row only (p.out) unless every row's logits are asked for.  Returns the launches:
+// the same for every step of one-token chunks.
+int forward_rows(b200_model *m, const BatchStep &p, cudaStream_t st) {
     const b200_llama_hparams &hp = m->hp;
     BatchWs &w = m->batch;
-    const int e = hp.n_embd, f = hp.n_ff, hd = m->hd, gqa = m->gqa, n_head = hp.n_head, n_head_kv = hp.n_head_kv, n_ctx = hp.context_size;
+    const int e = hp.n_embd, f = hp.n_ff, hd = m->hd, gqa = m->gqa, n_head = hp.n_head, n_head_kv = hp.n_head_kv, n_ctx = hp.context_size, n = p.n;
     const int qkv_ld = e + 2 * gqa;
     const float kq_scale = 1.0f / sqrtf((float)e / (float)n_head);                           // llama lib.rs:268-270
     const RopeTable &rope = rope_table(hp.n_rot, 0, hp.rope_freq_base, hp.rope_freq_scale, hd, n_ctx);
-    const BatchRow *rows = w.core.rows.get();
+    const BatchRow *rows = p.rows;
     const ExactActs acts{w.xq.get(), w.xds.get(), w.xpack.get(), w.xh.get(), w.xq8k.get()};
-    auto mm = [&](const QWeight &W, const float *x, float *dst, int64_t ldd, const float *addend) {
-        return mul_mat_exact_auto(W, x, W.K, n, dst, ldd, addend, addend ? ldd : 0, acts, st);
+    auto mm = [&](const QWeight &W, const float *x, float *dst, int64_t ldd, const float *addend, int64_t B) {
+        return mul_mat_exact_auto(W, x, W.K, B, dst, ldd, addend, addend ? ldd : 0, acts, st);
     };
     int L = 0;
-    get_rows_q(m->wte, w.core.ids.get(), w.x.get(), n, st); L++;
+    get_rows_q(m->wte, p.ids, w.x.get(), n, st); L++;
     for (int il = 0; il < hp.n_layer; il++) {
         const Layer &ly = m->layers[il];
         const size_t layer_off = (size_t)il * n_ctx * gqa;
         rms_norm(w.x.get(), w.cur.get(), ly.attention_norm, e, n, 5e-6f, st); L++;
-        L += mm(ly.wqkv, w.cur.get(), w.qkv.get(), qkv_ld, nullptr);
-        if (ly.wv.N) L += mm(ly.wv, w.cur.get(), w.qkv.get() + e + gqa, qkv_ld, nullptr);
-        rope_store_rows(w.qkv.get(), qkv_ld, QkvLayout{hd, e, e + gqa}, hd, n_head, n_head_kv, rows, n, layer_off, n_ctx, kv_type, &rope, st); L++;
-        attn_kq_rows(kv_type, rows, n, max_n_kv, layer_off, w.qkv.get(), qkv_ld, hd, hd, n_head, n_head_kv, n_ctx, w.kq.get(), st); L++;
+        L += mm(ly.wqkv, w.cur.get(), w.qkv.get(), qkv_ld, nullptr, n);
+        if (ly.wv.N) L += mm(ly.wv, w.cur.get(), w.qkv.get() + e + gqa, qkv_ld, nullptr, n);
+        rope_store_rows(w.qkv.get(), qkv_ld, QkvLayout{hd, e, e + gqa}, hd, n_head, n_head_kv, rows, n, layer_off, n_ctx, p.kv_type, &rope, st); L++;
+        L += attn_kq_step(p, layer_off, w.qkv.get(), qkv_ld, hd, hd, n_head, n_head_kv, n_ctx, w.kq.get(), st);
         soft_max_rows(w.kq.get(), rows, n, n_head, n_ctx, kq_scale, st); L++;
-        attn_kqv_rows(kv_type, rows, n, layer_off, w.kq.get(), hd, n_head, n_head_kv, n_ctx, w.cur.get(), e, st); L++;
-        L += mm(ly.wo, w.cur.get(), w.ff.get(), e, w.x.get());                                   // inpFF = wo.cur + inpSA
+        L += attn_kqv_step(p, layer_off, w.kq.get(), hd, n_head, n_head_kv, n_ctx, w.cur.get(), e, st);
+        L += mm(ly.wo, w.cur.get(), w.ff.get(), e, w.x.get(), n);                                // inpFF = wo.cur + inpSA
         rms_norm(w.ff.get(), w.cur.get(), ly.ffn_norm, e, n, 5e-6f, st); L++;
-        L += mm(ly.w13, w.cur.get(), w.h13.get(), 2 * f, nullptr);
+        L += mm(ly.w13, w.cur.get(), w.h13.get(), 2 * f, nullptr, n);
         silu_mul_rows(w.h13.get(), w.hmul.get(), f, n, st); L++;
-        L += mm(ly.w2, w.hmul.get(), w.x.get(), e, w.ff.get());
+        L += mm(ly.w2, w.hmul.get(), w.x.get(), e, w.ff.get(), n);
     }
-    rms_norm(w.x.get(), w.cur.get(), m->norm, e, n, 5e-6f, st); L++;
-    L += mm(m->output, w.cur.get(), w.core.logits.get(), hp.n_vocab, nullptr);
+    const float *xl = w.x.get();
+    if (p.out) { gather_rows(w.x.get(), e, p.out, p.n_out, w.ff.get(), st); L++; xl = w.ff.get(); }   // each chunk's last row (ff is free here)
+    rms_norm(xl, w.cur.get(), m->norm, e, p.n_out, 5e-6f, st); L++;
+    L += mm(m->output, w.cur.get(), p.logits, hp.n_vocab, nullptr, p.n_out);
     return L;
 }
 
-// the batched step's activations: n rows, grown to the largest n seen (BatchCore::reserve, with the stream idle)
+// the batched step's activations: B rows, grown to the largest step seen (BatchCore::reserve, with the stream idle); kq is [B][n_head][n_ctx]
 void batch_reserve(b200_model *m, size_t B) {
     BatchWs &w = m->batch;
     const b200_llama_hparams &hp = m->hp;
@@ -303,8 +306,9 @@ int batch_check(const b200_model *m, b200_session *const *ss, int n, BatchSessio
 }
 
 BatchFront batch_front(b200_model *m) {
-    return BatchFront{[m](size_t B) { batch_reserve(m, B); },
-                      [m](int n, int kv_type, int max_n_kv) { return forward_rows(m, n, kv_type, max_n_kv, rt().stream); }};
+    const int qkv_ld = m->hp.n_embd + 2 * m->gqa;
+    return BatchFront{[m](size_t B) { batch_reserve(m, B); }, [m](const BatchStep &p) { return forward_rows(m, p, rt().stream); },
+                      attn_tiles_aligned(m->hd, qkv_ld, m->hd, m->hp.context_size)};
 }
 
 }  // namespace
@@ -779,11 +783,16 @@ int b200_session_infer_next_token(b200_session *s, const b200_sampler *sampler, 
     return s->infer_next_token(a, s->logits.get(), [s]() { forward(s, 1); }, token_out);
 }
 
-// ---- batched decode over sessions of one model (include/llm_b200.h) -------------------------------------------------------------------------
-int b200_model_evaluate_sessions(b200_model *m, b200_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out) {
+// ---- batched steps over sessions of one model (include/llm_b200.h) ---------------------------------------------------------------------------
+int b200_model_evaluate_ragged(b200_model *m, b200_session *const *sessions, int32_t n, const int32_t *counts, const int32_t *tokens,
+                               float *logits_out, int32_t all_logits) {
     BatchSession ss[B200_MAX_SESSIONS];
     if (const int rc = batch_check(m, sessions, n, ss)) return rc;
-    return m->batch.core.evaluate(ss, n, tokens, logits_out, batch_front(m));
+    return m->batch.core.evaluate(ss, n, counts, tokens, logits_out, all_logits != 0, batch_front(m));
+}
+
+int b200_model_evaluate_sessions(b200_model *m, b200_session *const *sessions, int32_t n, const int32_t *tokens, float *logits_out) {
+    return b200_model_evaluate_ragged(m, sessions, n, decode_counts(), tokens, logits_out, 0);
 }
 
 int b200_model_infer_next_tokens(b200_model *m, b200_session *const *sessions, int32_t n, const b200_sampler *samplers, int32_t *tokens_out,

@@ -58,6 +58,7 @@ def _bind(L):
     L.b200_neox_infer_next_token.argtypes = [vp, C.POINTER(_lib.SamplerParams), C.POINTER(i32)]
     L.b200_neox_evaluate_sessions.argtypes = [vp, C.POINTER(vp), i32, vp, vp]
     L.b200_neox_infer_next_tokens.argtypes = [vp, C.POINTER(vp), i32, C.POINTER(_lib.SamplerParams), vp, vp]
+    L.b200_neox_evaluate_ragged.argtypes = [vp, C.POINTER(vp), i32, vp, vp, vp, i32]
     L.b200_neox_read_tokens.restype = i32
     L.b200_neox_read_tokens.argtypes = [vp, vp, i32]
     L.b200_neox_last_logits.argtypes = [vp, vp]
@@ -80,6 +81,7 @@ class GptNeoX(_BatchedSessions, _Native):
     ARCH = 0
     _HANDLE, _FREE = "_m", "b200_neox_free"
     _EVAL_SESSIONS, _INFER_SESSIONS = "b200_neox_evaluate_sessions", "b200_neox_infer_next_tokens"
+    _EVAL_RAGGED = "b200_neox_evaluate_ragged"
 
     BOT_TOKEN: Optional[bytes] = None       # the vocabulary entry bot_token_id() names (MPT, BLOOM); None: the model has no BOS token
     EOT_TOKEN: bytes = b"<|endoftext|>"     # the entry eot_token_id() names (gptneox lib.rs:376-378, gpt2 :353-355, gptj :329-331, mpt :277-279)

@@ -397,12 +397,13 @@ class _Generation:
 
 
 class _BatchedSessions:
-    """Batched decode over the sessions of one model (include/llm_b200.h: b200_model_evaluate_sessions / b200_neox_evaluate_sessions):
-    `_EVAL_SESSIONS` and `_INFER_SESSIONS` name the library's entry points, `_SESSION` the model's session class; the model keeps `L`, `_m` and
-    `hyperparameters`."""
-    _EVAL_SESSIONS, _INFER_SESSIONS = "", ""
+    """Batched steps over the sessions of one model (include/llm_b200.h: b200_model_evaluate_ragged / b200_neox_evaluate_ragged and the decode
+    steps b200_*_evaluate_sessions, b200_*_infer_next_tokens): `_EVAL_SESSIONS`, `_INFER_SESSIONS` and `_EVAL_RAGGED` name the library's entry
+    points, `_SESSION` the model's session class; the model keeps `L`, `_m`, `hyperparameters` and its context size."""
+    _EVAL_SESSIONS, _INFER_SESSIONS, _EVAL_RAGGED = "", "", ""
     _SESSION: type = type(None)
     MAX_SESSIONS = 64                           # B200_MAX_SESSIONS
+    MAX_BATCH_ROWS = 4096                       # B200_MAX_BATCH_ROWS: the tokens of one ragged step
 
     def _session_handles(self, sessions):
         return (C.c_void_p * max(1, len(sessions)))(*[s._s for s in sessions])
@@ -432,6 +433,66 @@ class _BatchedSessions:
         for i, s in enumerate(sessions):
             s._last_logits = None
         return out[:n]
+
+    def evaluate_ragged(self, sessions: Sequence["InferenceSession"], chunks, all_logits: bool = False) -> List[np.ndarray]:
+        """One step for several sessions of this model, each evaluating a chunk of its own: session i evaluates chunks[i] (1 to its n_batch ids)
+        at its own n_past, reading the weights once for all of them -- new sessions prefill while others decode.  Each session ends exactly as
+        after session.evaluate(chunks[i], all_logits) alone, bit for bit.  Returns one array per session: its last row [n_vocab], or with
+        all_logits every row [len(chunks[i]), n_vocab].  Refused as a whole, nothing changed (RuntimeError, or ContextFull when a chunk does not
+        fit): evaluate_sessions' refusals, an empty chunk or one longer than its session's n_batch, more than 4096 ids in all; TypeError for a
+        session that is not of this model's runtime.  See include/llm_b200.h."""
+        n = len(sessions)
+        if len(chunks) != n:
+            raise ValueError(f"{n} sessions, {len(chunks)} chunks")
+        arrs = [np.ascontiguousarray(c, np.int32).ravel() for c in chunks]
+        counts = np.array([a.size for a in arrs] or [0], np.int32)
+        toks = np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros(1, np.int32), np.int32)
+        self._own(sessions, "evaluate_ragged")
+        rows = int(counts[:n].sum()) if all_logits else n
+        out = np.empty((max(rows, 1), int(self.hyperparameters["n_vocab"])), np.float32)
+        _check(getattr(self.L, self._EVAL_RAGGED)(self._m, self._session_handles(sessions), n, counts.ctypes.data_as(C.c_void_p),
+                                                 toks.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p), 1 if all_logits else 0),
+               "evaluate_ragged")
+        for s in sessions:
+            s._last_logits = None
+        if not all_logits:
+            return [out[i] for i in range(n)]
+        ends = np.cumsum(counts[:n])
+        return [out[e - c:e] for e, c in zip(ends, counts[:n])]
+
+    def feed_prompts(self, sessions: Sequence["InferenceSession"], prompts) -> List[np.ndarray]:
+        """InferenceSession::feed_prompt for several sessions of this model: each prompt is cut into chunks of its own session's n_batch, and step
+        k evaluates chunk k of every session that still has one (evaluate_ragged), so each session ends bit-identical to feed_prompt alone.  A
+        step of more than 4096 ids is split across sessions; each session's chunks stay the same.  Returns each session's last_logits (an empty
+        prompt leaves its session untouched).  ContextFull, before anything is evaluated, when a prompt does not fit its session."""
+        n = len(sessions)
+        if len(prompts) != n:
+            raise ValueError(f"{n} sessions, {len(prompts)} prompts")
+        self._own(sessions, "feed_prompts")
+        ps = [np.ascontiguousarray(p, np.int32).ravel() for p in prompts]
+        cs = self.context_size
+        n_ctx = cs() if callable(cs) else cs
+        for s, p in zip(sessions, ps):
+            if s.n_past + p.size > n_ctx:              # feed_prompt's check (inference_session.rs:311-313), for every session first
+                raise ContextFull("feed_prompts")
+            if min(p.size, s.n_batch) > self.MAX_BATCH_ROWS:
+                raise ValueError(f"feed_prompts: a chunk of {s.n_batch} ids is more than one step takes ({self.MAX_BATCH_ROWS})")
+        done = [0] * n
+        while True:
+            step = [(i, ps[i][done[i]:done[i] + sessions[i].n_batch]) for i in range(n) if done[i] < ps[i].size]
+            if not step:
+                break
+            while step:
+                rows, k = 0, 0
+                while k < len(step) and rows + step[k][1].size <= self.MAX_BATCH_ROWS:
+                    rows += step[k][1].size
+                    k += 1
+                part, step = step[:k], step[k:]
+                got = self.evaluate_ragged([sessions[i] for i, _ in part], [c for _, c in part])
+                for (i, c), row in zip(part, got):
+                    done[i] += c.size
+                    sessions[i]._last_logits = row.copy()
+        return [s.last_logits for s in sessions]
 
     def infer_next_tokens(self, sessions: Sequence["InferenceSession"], params, rngs: Sequence[Rng]) -> List[int]:
         """infer_next_token for several sessions at once: session i samples from its last row with its own parameters and rngs[i], then one
@@ -524,6 +585,7 @@ class Llama(_BatchedSessions, _Native):
     `tensor_types`: {name: enum ggml_type} of 2-D weights whose type is not `wtype` (mixed-type files, b200_llama_new_typed)."""
     _HANDLE, _FREE = "_m", "b200_model_free"
     _EVAL_SESSIONS, _INFER_SESSIONS = "b200_model_evaluate_sessions", "b200_model_infer_next_tokens"
+    _EVAL_RAGGED = "b200_model_evaluate_ragged"
     tensor_types: Dict[str, int] = {}           # models loaded from a file or cut into shards: their types are in the C model
 
     def __init__(self, hyperparameters: Dict[str, int], params: ModelParameters = None, tensors: Dict[str, np.ndarray] = None,
@@ -656,6 +718,10 @@ class InferenceSession(_Generation, _Snapshots, _Native):
     @property
     def n_past(self) -> int:
         return self.L.b200_session_n_past(self._s)
+
+    @property
+    def n_batch(self) -> int:
+        return self.config.n_batch
 
     def top_k(self, k: int):
         """Sampler hand-off: (token ids, logits) of the k largest logits of the last evaluated row, selected on the device."""
